@@ -148,6 +148,20 @@ int opb_gather_features3d(const float* desc, const float* scores, int32_t dim, i
 int opb_ransac_pnp(const double* K, const double* pts2d, const double* pts3d, const int32_t* offsets, int32_t B, int32_t hypotheses,
                    double reproj_error, uint64_t seed, double* workspace, double* pose_out, int32_t* inlier_mask, int32_t* n_inliers,
                    void* stream);
+/* Matched 2D-3D pairs of B frames in the layout opb_ransac_pnp reads; replaces inference.py:147-152 / eval_utils.py:72-77
+ * (valid = matches0 > -1; mkpts2d = kpts2d[valid]; mkpts3d = kpts3d[matches0[valid]]; mconf = scores0[valid]).
+ *   matches0     device int64 [B, N]  (opb_forward's output; an entry outside [0, M) is not a match)
+ *   mscores0     device fp32  [B, N]  or NULL (then mconf must be NULL)
+ *   keypoints2d  device fp32  [B, N, 2]  (x, y; opb_sp_forward's keypoints with cap = N; rows of unmatched entries are never read)
+ *   keypoints3d  device fp32  [M, 3]
+ * Outputs (device, capacity B*N): pts2d f64 [B*N, 2], pts3d f64 [B*N, 3], mconf fp32 [B*N] or NULL,
+ * query_index int32 [B*N] or NULL (= n of each pair), offsets int32 [B+1] (frame b owns [offsets[b], offsets[b+1])).
+ * Pairs are frame-major and, within a frame, in ascending n: numpy boolean-mask order.  The values are exact (fp32 -> f64
+ * conversions, as numpy's astype(np.float64)).  Three launches, deterministic, no host synchronisation.  B*N < 2^31;
+ * matches0 / keypoints2d / pts2d / pts3d may be NULL when N = 0 (then offsets = 0). */
+int opb_gather_matches(const int64_t* matches0, const float* mscores0, const float* keypoints2d, const float* keypoints3d,
+                       int32_t B, int32_t N, int32_t M, double* pts2d, double* pts3d, float* mconf, int32_t* query_index,
+                       int32_t* offsets, void* stream);
 
 /* ---- adjacent producer: SuperPoint key-point extractor (SURVEY 8f N4) ----
  * Replaces SuperPoint.forward (reference src/models/extractors/SuperPoint/superpoint.py:140-197): shared VGG-style encoder

@@ -367,8 +367,124 @@ __global__ void __launch_bounds__(kRefineThreads) pnp_select_refine(const double
   }
 }
 
+// ---- matched pairs -> the ragged correspondence lists above (reference inference.py:147-152: valid = matches > -1;
+// mkpts2d = kpts2d[valid]; mkpts3d = kpts3d[matches[valid]]).  Three launches, no workspace: per-frame counts into
+// offsets[1..B], an in-place scan of offsets, then a per-frame ordered compaction (ascending n, numpy boolean-mask order).
+constexpr int kGatherThreads = 256;
+
+__device__ __forceinline__ bool is_match(int64_t m, int M) { return m >= 0 && m < (int64_t)M; }
+
+__global__ void __launch_bounds__(kGatherThreads) gather_count(const int64_t* __restrict__ matches0, int N, int M, int* __restrict__ offsets) {
+  __shared__ int cnt_w[kGatherThreads / 32];
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const int64_t* m0 = matches0 + (size_t)b * N;
+  int cnt = 0;
+  for (int n = tid; n < N; n += kGatherThreads) cnt += is_match(m0[n], M) ? 1 : 0;
+  for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
+  if ((tid & 31) == 0) cnt_w[tid >> 5] = cnt;
+  __syncthreads();
+  if (tid == 0) {
+    int c = 0;
+    for (int w = 0; w < kGatherThreads / 32; ++w) c += cnt_w[w];
+    offsets[b + 1] = c;
+    if (b == 0) offsets[0] = 0;
+  }
+}
+
+// one block: inclusive scan of offsets[1..B] in place (offsets[0] = 0), tiles of 1024 with a running carry
+constexpr int kScanThreads = 1024;
+__global__ void __launch_bounds__(kScanThreads) gather_scan(int B, int* __restrict__ offsets) {
+  __shared__ int warp_sum[kScanThreads / 32];
+  __shared__ int carry;
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  if (tid == 0) carry = 0;
+  for (int base = 0; base < B; base += kScanThreads) {
+    const int i = base + tid;
+    int v = i < B ? offsets[i + 1] : 0;
+    for (int o = 1; o < 32; o <<= 1) {
+      const int u = __shfl_up_sync(0xffffffffu, v, o);
+      if (lane >= o) v += u;
+    }
+    if (lane == 31) warp_sum[warp] = v;
+    __syncthreads();
+    if (warp == 0) {
+      int s = warp_sum[lane];
+      for (int o = 1; o < 32; o <<= 1) {
+        const int u = __shfl_up_sync(0xffffffffu, s, o);
+        if (lane >= o) s += u;
+      }
+      warp_sum[lane] = s;                            // inclusive prefix over warps
+    }
+    __syncthreads();
+    const int c = carry;
+    v += c + (warp > 0 ? warp_sum[warp - 1] : 0);
+    if (i < B) offsets[i + 1] = v;
+    __syncthreads();                                 // every thread has read carry and warp_sum
+    if (tid == kScanThreads - 1) carry = v;
+    __syncthreads();
+  }
+}
+
+// one block per frame: ordered compaction over tiles of kGatherThreads entries; keypoints2d rows are read for matches only
+__global__ void __launch_bounds__(kGatherThreads) gather_compact(const int64_t* __restrict__ matches0, const float* __restrict__ mscores0,
+                                                                 const float* __restrict__ kp2d, const float* __restrict__ kp3d, int N, int M,
+                                                                 const int* __restrict__ offsets, double* __restrict__ pts2d, double* __restrict__ pts3d,
+                                                                 float* __restrict__ mconf, int* __restrict__ query_index) {
+  __shared__ int warp_cnt[kGatherThreads / 32];
+  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const size_t row0 = (size_t)b * N;
+  int pos = offsets[b];
+  for (int base = 0; base < N; base += kGatherThreads) {
+    const int n = base + tid;
+    const int64_t m = n < N ? matches0[row0 + n] : -1;
+    const bool valid = is_match(m, M);
+    const unsigned ballot = __ballot_sync(0xffffffffu, valid);
+    if (lane == 0) warp_cnt[warp] = __popc(ballot);
+    __syncthreads();
+    int before = 0, total = 0;
+#pragma unroll
+    for (int w = 0; w < kGatherThreads / 32; ++w) {
+      const int c = warp_cnt[w];
+      before += w < warp ? c : 0;
+      total += c;
+    }
+    if (valid) {
+      const size_t o = (size_t)(pos + before + __popc(ballot & ((1u << lane) - 1u)));
+      const float* k2 = kp2d + (row0 + n) * 2;
+      const float* k3 = kp3d + (size_t)m * 3;
+      pts2d[o * 2 + 0] = (double)k2[0];
+      pts2d[o * 2 + 1] = (double)k2[1];
+      pts3d[o * 3 + 0] = (double)k3[0];
+      pts3d[o * 3 + 1] = (double)k3[1];
+      pts3d[o * 3 + 2] = (double)k3[2];
+      if (mconf) mconf[o] = mscores0[row0 + n];
+      if (query_index) query_index[o] = n;
+    }
+    pos += total;
+    __syncthreads();                                 // warp_cnt is rewritten by the next tile
+  }
+}
+
 }  // namespace
 }  // namespace opb
+
+extern "C" int opb_gather_matches(const int64_t* matches0, const float* mscores0, const float* keypoints2d, const float* keypoints3d,
+                                  int32_t B, int32_t N, int32_t M, double* pts2d, double* pts3d, float* mconf, int32_t* query_index,
+                                  int32_t* offsets, void* stream) {
+  if (B <= 0 || N < 0 || M <= 0 || !keypoints3d || !offsets || (int64_t)B * N > (int64_t)INT32_MAX) return OPB_E_INVALID;
+  if (N > 0 && (!matches0 || !keypoints2d || !pts2d || !pts3d)) return OPB_E_INVALID;
+  if (mconf && !mscores0) return OPB_E_INVALID;
+  cudaStream_t st = (cudaStream_t)stream;
+  if (N == 0) {
+    if (cudaMemsetAsync(offsets, 0, sizeof(int32_t) * ((size_t)B + 1), st) != cudaSuccess) return OPB_E_CUDA;
+    return OPB_OK;
+  }
+  opb::gather_count<<<(unsigned)B, opb::kGatherThreads, 0, st>>>(matches0, N, M, offsets);
+  opb::gather_scan<<<1, opb::kScanThreads, 0, st>>>(B, offsets);
+  opb::gather_compact<<<(unsigned)B, opb::kGatherThreads, 0, st>>>(matches0, mscores0, keypoints2d, keypoints3d, N, M, offsets, pts2d, pts3d,
+                                                                   mconf, query_index);
+  return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_E_CUDA;
+}
 
 extern "C" int opb_ransac_pnp(const double* K, const double* pts2d, const double* pts3d, const int32_t* offsets, int32_t B, int32_t hypotheses,
                               double reproj_error, uint64_t seed, double* workspace, double* pose_out, int32_t* inlier_mask, int32_t* n_inliers,

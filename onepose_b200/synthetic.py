@@ -193,6 +193,39 @@ def make_pnp_scene(seed: int, n: int, outlier_frac: float = 0.4, noise_px: float
     return K, uv, P, np.concatenate([R, t[:, None]], 1)
 
 
+def make_planted_scene(object_id: int, frame_ids, N: int, M: int, L: int = 8, unplanted=(), noise_px: float = 0.5, size: int = 512):
+    """An object and B frames that the matcher and the pose solver can both get right: ``make_object`` descriptors, M 3D points
+    (metres, ~10 cm across; keypoints3d fp32 [M,3]) and per frame a camera K, a ground-truth pose and ``make_frame`` query
+    descriptors whose planted column i sits at the projection of 3D point perm[i] (plus ``noise_px`` of pixel noise); unplanted
+    columns have key points uniform in the size x size crop.  Frames listed in ``unplanted`` get random descriptors only.
+    Returns a dict of numpy arrays: desc3d [256,M], desc2d_db [256,M*L], keypoints3d [M,3] f32, K [B,3,3] f64,
+    descriptors2d [B,256,N] f32, keypoints2d [B,N,2] f32, pose_gt [B,3,4] f64, n_planted [B]."""
+    db, leaves = make_object(object_id, M, L)
+    rs = np.random.RandomState(5000 + object_id)
+    P = (0.05 * rs.randn(M, 3)).astype(np.float32)
+    Ks, qs, kps, gts, npl = [], [], [], [], []
+    for f in frame_ids:
+        if f in unplanted:
+            q, perm = _unit_cols(np.random.RandomState(f).randn(db.shape[0], N)), np.zeros(0, np.int64)
+        else:
+            q, perm = make_frame(f, db, N)
+        frs = np.random.RandomState(7000 + f)
+        K = np.array([[600.0 + 50 * frs.rand(), 0, size / 2 + 5 * frs.randn()], [0, 600.0 + 50 * frs.rand(), size / 2 + 5 * frs.randn()],
+                      [0, 0, 1.0]])
+        w = frs.randn(3)
+        th = np.linalg.norm(w)
+        k = w / th
+        Kx = np.array([[0, -k[2], k[1]], [k[2], 0, -k[0]], [-k[1], k[0], 0]])
+        R = np.eye(3) + np.sin(th) * Kx + (1 - np.cos(th)) * Kx @ Kx
+        t = np.array([0.03 * frs.randn(), 0.03 * frs.randn(), 0.5 + 0.3 * frs.rand()])
+        kp = frs.rand(N, 2) * size
+        X = P[perm].astype(np.float64) @ R.T + t
+        kp[:len(perm)] = X[:, :2] / X[:, 2:3] * np.array([K[0, 0], K[1, 1]]) + np.array([K[0, 2], K[1, 2]]) + noise_px * frs.randn(len(perm), 2)
+        Ks.append(K); qs.append(q); kps.append(kp.astype(np.float32)); gts.append(np.concatenate([R, t[:, None]], 1)); npl.append(len(perm))
+    return {"desc3d": db, "desc2d_db": leaves, "keypoints3d": P, "K": np.stack(Ks), "descriptors2d": np.stack(qs),
+            "keypoints2d": np.stack(kps), "pose_gt": np.stack(gts), "n_planted": np.array(npl)}
+
+
 # ---------------------------------------------------------------------------------------------
 # SuperPoint extractor (SURVEY 8f N4): reference-shaped state dict and seeded grey images
 # ---------------------------------------------------------------------------------------------
