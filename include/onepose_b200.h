@@ -139,9 +139,13 @@ int opb_gather_features3d(const float* desc, const float* scores, int32_t dim, i
  *   K          device f64 [B, 9]   row-major camera matrices
  *   pts2d      device f64 [total, 2], pts3d device f64 [total, 3]  matched key points of all frames, concatenated
  *   offsets    device int32 [B+1]  frame b owns correspondences [offsets[b], offsets[b+1])
- *   hypotheses minimal samples per frame (P3P), reproj_error in pixels, seed of the sample generator (results are a
- *              deterministic function of it)
- *   workspace  device f64 [B * hypotheses * 13]
+ *   hypotheses minimal samples per frame (P3P), 1 .. 65535 * 128; reproj_error in pixels, > 0; seed of the sample generator
+ *              (results are a deterministic function of it)
+ *   workspace  device f64 [B * hypotheses * 13]: one record of 13 doubles per frame and hypothesis, frame-major
+ *              (record b * hypotheses + h): the inlier count of the hypothesis's best P3P pose, then that pose's R (9,
+ *              row-major) and t (3).  A record with count 0 (frame with fewer than 4 correspondences, or no P3P solution)
+ *              leaves its pose unwritten.  Sample h of frame b is three distinct indices drawn from
+ *              splitmix64(seed ^ (b << 40) ^ h) and its successors.
  * Outputs (device): pose f64 [B, 12] = row-major [R | t] (world -> camera), inlier_mask int32 [total], n_inliers int32 [B].
  * A frame with fewer than 4 correspondences or no model gets the identity pose and no inliers (the reference's cv2.error
  * branch).  Parity with the reference is on the pose (cm / degree), not on bits: OpenCV draws its own samples. */

@@ -6,8 +6,9 @@
 // The reference delegates the arithmetic to OpenCV; parity for this row is the pose itself (the reference's own metric is the
 // cm-degree error, src/evaluators/cmd_evaluator.py), not bits: OpenCV draws its minimal samples from its own RNG.  Algorithm:
 //   hypotheses  one thread per minimal sample: 3 correspondences -> P3P (Grunert's quartic, coefficients as in Haralick et al.
-//               1994; closed-form quartic roots + Newton polish) -> up to 4 poses, each scored by its inlier count over ALL
-//               correspondences of the frame (reprojection error < threshold, point in front of the camera), fp64;
+//               1994; closed-form quartic roots + Newton polish; the second depth ratio from the quadratic of one law-of-cosines
+//               equation, then Newton on the three distance equations) -> up to 4 poses, each scored by its inlier count over
+//               ALL correspondences of the frame (reprojection error < threshold, point in front of the camera), fp64;
 //   selection   per frame: hypothesis with the most inliers (lowest index wins ties: deterministic);
 //   refinement  Gauss-Newton on the reprojection error of the inlier set (6 DoF, left rotation update), inlier set re-evaluated
 //               between rounds (local optimisation) -- what OpenCV's final EPnP refit on the inliers approximates.
@@ -45,8 +46,12 @@ __device__ double cubic_largest_real(double a2, double a1, double a0) {
   return 2.0 * sqrt(-q) * cos(th / 3.0) - a2 / 3.0;
 }
 
-// real roots of A4 x^4 + ... + A0 (Ferrari via the resolvent cubic), polished by two Newton steps; returns their number
-__device__ int quartic_real_roots(double A4, double A3, double A2, double A1, double A0, double* x) {
+// real roots of A4 x^4 + ... + A0 (Ferrari via the resolvent cubic), polished by two Newton steps that are kept only when
+// they shrink |f|; returns their number.  A quadratic factor with a negative discriminant still yields its real part, flagged
+// in *approx (bit k for x[k]): a double root, as a symmetric P3P sample produces, lands there as often as not, because the
+// depressed coefficients lose most of their digits when the roots cluster (narrow views).  The caller verifies those.
+__device__ int quartic_real_roots(double A4, double A3, double A2, double A1, double A0, double* x, unsigned* approx) {
+  *approx = 0u;
   if (fabs(A4) < 1e-300) return 0;
   const double a = A3 / A4, b = A2 / A4, c = A1 / A4, d = A0 / A4;
   const double p = b - 3.0 * a * a / 8.0, q = c - a * b / 2.0 + a * a * a / 8.0;
@@ -69,13 +74,19 @@ __device__ int quartic_real_roots(double A4, double A3, double A2, double A1, do
       const double B = sg * s, C = (p + z - sg * q / s) / 2.0;   // y^2 + B y + C = 0
       const double disc = B * B - 4.0 * C;
       if (disc >= 0.0) { const double sd = sqrt(disc); y[n++] = (-B + sd) / 2.0; y[n++] = (-B - sd) / 2.0; }
+      else { *approx |= 1u << n; y[n++] = -B / 2.0; }
     }
   }
   for (int k = 0; k < n; ++k) {
     double v = y[k] - a / 4.0;
-    for (int it = 0; it < 2; ++it) {
-      const double f = (((A4 * v + A3) * v + A2) * v + A1) * v + A0, df = ((4.0 * A4 * v + 3.0 * A3) * v + 2.0 * A2) * v + A1;
-      if (df != 0.0) v -= f / df;
+    double f = (((A4 * v + A3) * v + A2) * v + A1) * v + A0;
+    for (int it = 0; it < 2; ++it) {   // near a double root f' ~ 0 and a full step can leave for another root
+      const double df = ((4.0 * A4 * v + 3.0 * A3) * v + 2.0 * A2) * v + A1;
+      if (df == 0.0) break;
+      const double vn = v - f / df, fn = (((A4 * vn + A3) * vn + A2) * vn + A1) * vn + A0;
+      if (!(fabs(fn) < fabs(f))) break;
+      v = vn;
+      f = fn;
     }
     x[k] = v;
   }
@@ -121,29 +132,74 @@ __device__ int p3p(const double P[3][3], const double j[3][3], Pose* out) {
   const double A1 = 4.0 * (-p * (1.0 + p) * cb + 2.0 * a2 / b2 * cg * cg * cb - (1.0 - q) * ca * cg);
   const double A0 = (1.0 + p) * (1.0 + p) - 4.0 * a2 / b2 * cg * cg;
   double v[4];
-  const int nr = quartic_real_roots(A4, A3, A2, A1, A0, v);
+  unsigned approx;
+  const int nr = quartic_real_roots(A4, A3, A2, A1, A0, v, &approx);
   double FP[9];
   if (!tri_frame(P, FP)) return 0;
+  double depths[4][3];
   int ns = 0;
-  for (int k = 0; k < nr; ++k) {
+  for (int k = 0; k < nr && ns < 4; ++k) {
     if (!(v[k] > 0.0)) continue;
-    const double den = 2.0 * (cg - v[k] * ca);
-    if (fabs(den) < 1e-12) continue;
-    const double u = ((-1.0 + p) * v[k] * v[k] - 2.0 * p * cb * v[k] + 1.0 + p) / den;
-    if (!(u > 0.0)) continue;
-    const double s1sq = c2 / (1.0 + u * u - 2.0 * u * cg);
-    if (!(s1sq > 0.0)) continue;
-    const double s[3] = {sqrt(s1sq), u * sqrt(s1sq), v[k] * sqrt(s1sq)};
-    double X[3][3];
-    for (int i = 0; i < 3; ++i)
-      for (int d = 0; d < 3; ++d) X[i][d] = s[i] * j[i][d];
-    double FX[9];
-    if (!tri_frame(X, FX)) continue;
-    Pose& o = out[ns];
-    for (int r = 0; r < 3; ++r)
-      for (int c = 0; c < 3; ++c) o.R[r * 3 + c] = FX[r * 3 + 0] * FP[c * 3 + 0] + FX[r * 3 + 1] * FP[c * 3 + 1] + FX[r * 3 + 2] * FP[c * 3 + 2];   // FX . FP^T
-    for (int r = 0; r < 3; ++r) o.t[r] = X[0][r] - (o.R[r * 3 + 0] * P[0][0] + o.R[r * 3 + 1] * P[0][1] + o.R[r * 3 + 2] * P[0][2]);
-    ++ns;
+    // depths (s0, u s0, v s0): s0 from the b^2 equation; u from the quadratic of the c^2 equation, u^2 - 2 cg u + 1 -
+    // (c2/b2) w = 0, the root that better satisfies the a^2 equation first.  (Grunert's linear back-substitution divides by
+    // cg - v ca, which vanishes at the true root of a sample symmetric about a plane through the camera centre; both roots
+    // then satisfy the a^2 equation and both are poses.)
+    const double w = 1.0 + v[k] * v[k] - 2.0 * v[k] * cb;
+    if (!(w > 0.0)) continue;
+    const double sd = sqrt(fmax(0.0, cg * cg - 1.0 + c2 / b2 * w));
+    double uc[2] = {cg + sd, cg - sd};
+    const double e0 = fabs(uc[0] * uc[0] + v[k] * v[k] - 2.0 * uc[0] * v[k] * ca - a2 / b2 * w);
+    const double e1 = fabs(uc[1] * uc[1] + v[k] * v[k] - 2.0 * uc[1] * v[k] * ca - a2 / b2 * w);
+    if (e1 < e0) { const double tmp = uc[0]; uc[0] = uc[1]; uc[1] = tmp; }
+    for (int m = 0; m < 2 && ns < 4; ++m) {
+      const bool verify = m == 1 || ((approx >> k) & 1u);   // a candidate that must prove itself a solution
+      if (!(uc[m] > 0.0)) continue;
+      const double s0 = sqrt(b2 / w);
+      double s[3] = {s0, uc[m] * s0, v[k] * s0};
+      // Newton on the three distance equations: the quartic root carries its conditioning into u and s, the depths'
+      // own system is well conditioned for any sample a P3P can solve
+      double F[3];
+      for (int it = 0; it < 6; ++it) {   // from a clustered-root start the quadratic phase takes a few steps
+        F[0] = s[1] * s[1] + s[2] * s[2] - 2.0 * s[1] * s[2] * ca - a2;
+        F[1] = s[0] * s[0] + s[2] * s[2] - 2.0 * s[0] * s[2] * cb - b2;
+        F[2] = s[0] * s[0] + s[1] * s[1] - 2.0 * s[0] * s[1] * cg - c2;
+        const double J[3][3] = {{0.0, 2.0 * (s[1] - s[2] * ca), 2.0 * (s[2] - s[1] * ca)},
+                                {2.0 * (s[0] - s[2] * cb), 0.0, 2.0 * (s[2] - s[0] * cb)},
+                                {2.0 * (s[0] - s[1] * cg), 2.0 * (s[1] - s[0] * cg), 0.0}};
+        const double C0 = J[1][1] * J[2][2] - J[1][2] * J[2][1], C1 = J[1][2] * J[2][0] - J[1][0] * J[2][2], C2 = J[1][0] * J[2][1] - J[1][1] * J[2][0];
+        const double det = J[0][0] * C0 + J[0][1] * C1 + J[0][2] * C2;
+        if (!(fabs(det) > 1e-300)) break;
+        // s -= J^-1 F (adjugate)
+        const double d0 = (C0 * F[0] + (J[0][2] * J[2][1] - J[0][1] * J[2][2]) * F[1] + (J[0][1] * J[1][2] - J[0][2] * J[1][1]) * F[2]) / det;
+        const double d1 = (C1 * F[0] + (J[0][0] * J[2][2] - J[0][2] * J[2][0]) * F[1] + (J[0][2] * J[1][0] - J[0][0] * J[1][2]) * F[2]) / det;
+        const double d2 = (C2 * F[0] + (J[0][1] * J[2][0] - J[0][0] * J[2][1]) * F[1] + (J[0][0] * J[1][1] - J[0][1] * J[1][0]) * F[2]) / det;
+        s[0] -= d0; s[1] -= d1; s[2] -= d2;
+      }
+      if (!(s[0] > 0.0 && s[1] > 0.0 && s[2] > 0.0)) continue;
+      if (verify) {
+        F[0] = s[1] * s[1] + s[2] * s[2] - 2.0 * s[1] * s[2] * ca - a2;
+        F[1] = s[0] * s[0] + s[2] * s[2] - 2.0 * s[0] * s[2] * cb - b2;
+        F[2] = s[0] * s[0] + s[1] * s[1] - 2.0 * s[0] * s[1] * cg - c2;
+        const double sm = fmax(s[0], fmax(s[1], s[2]));
+        if (!(fmax(fabs(F[0]), fmax(fabs(F[1]), fabs(F[2]))) <= 1e-12 * sm * sm)) continue;
+      }
+      bool dup = false;                                  // a double root is reported twice
+      const double smax = fmax(s[0], fmax(s[1], s[2]));
+      for (int o = 0; o < ns; ++o)
+        dup |= fmax(fabs(s[0] - depths[o][0]), fmax(fabs(s[1] - depths[o][1]), fabs(s[2] - depths[o][2]))) <= 1e-9 * smax;
+      if (dup) continue;
+      double X[3][3];
+      for (int i = 0; i < 3; ++i)
+        for (int d = 0; d < 3; ++d) X[i][d] = s[i] * j[i][d];
+      double FX[9];
+      if (!tri_frame(X, FX)) continue;
+      Pose& o = out[ns];
+      for (int r = 0; r < 3; ++r)
+        for (int c = 0; c < 3; ++c) o.R[r * 3 + c] = FX[r * 3 + 0] * FP[c * 3 + 0] + FX[r * 3 + 1] * FP[c * 3 + 1] + FX[r * 3 + 2] * FP[c * 3 + 2];   // FX . FP^T
+      for (int r = 0; r < 3; ++r) o.t[r] = X[0][r] - (o.R[r * 3 + 0] * P[0][0] + o.R[r * 3 + 1] * P[0][1] + o.R[r * 3 + 2] * P[0][2]);
+      for (int i = 0; i < 3; ++i) depths[ns][i] = s[i];
+      ++ns;
+    }
   }
   return ns;
 }
@@ -159,12 +215,14 @@ __device__ __forceinline__ bool reproj_inlier(const Pose& T, const double* Kc /*
 
 // hyp: [B][H] {count, pose(12)} as 13 doubles
 constexpr int kHypStride = 13;
+constexpr int kHypThreads = 128;
+constexpr int kMaxHypotheses = 65535 * kHypThreads;
 
-__global__ void __launch_bounds__(128) pnp_hypotheses(const double* __restrict__ Kmat /*[B][9]*/, const double* __restrict__ pts2d, const double* __restrict__ pts3d,
+__global__ void __launch_bounds__(kHypThreads, 4) pnp_hypotheses(const double* __restrict__ Kmat /*[B][9]*/, const double* __restrict__ pts2d, const double* __restrict__ pts3d,
                                                       const int* __restrict__ offsets, int H, double thr2, unsigned long long seed,
                                                       double* __restrict__ hyp) {
-  const int b = blockIdx.y;
-  const int h = blockIdx.x * blockDim.x + threadIdx.x;
+  const int b = blockIdx.x;                          // frames on x: any B; hypothesis blocks on y (at most 65535)
+  const int h = blockIdx.y * blockDim.x + threadIdx.x;
   if (h >= H) return;
   const int o0 = offsets[b], n = offsets[b + 1] - o0;
   double* out = hyp + ((size_t)b * H + h) * kHypStride;
@@ -489,12 +547,13 @@ extern "C" int opb_gather_matches(const int64_t* matches0, const float* mscores0
 extern "C" int opb_ransac_pnp(const double* K, const double* pts2d, const double* pts3d, const int32_t* offsets, int32_t B, int32_t hypotheses,
                               double reproj_error, uint64_t seed, double* workspace, double* pose_out, int32_t* inlier_mask, int32_t* n_inliers,
                               void* stream) {
-  if (!K || !pts2d || !pts3d || !offsets || !workspace || !pose_out || !inlier_mask || !n_inliers || B <= 0 || hypotheses <= 0 || !(reproj_error > 0.0))
+  if (!K || !pts2d || !pts3d || !offsets || !workspace || !pose_out || !inlier_mask || !n_inliers || B <= 0 || hypotheses <= 0 ||
+      hypotheses > opb::kMaxHypotheses || !(reproj_error > 0.0))
     return OPB_E_INVALID;
   cudaStream_t st = (cudaStream_t)stream;
   const double thr2 = reproj_error * reproj_error;
-  opb::pnp_hypotheses<<<dim3((unsigned)((hypotheses + 127) / 128), (unsigned)B), 128, 0, st>>>(K, pts2d, pts3d, offsets, hypotheses, thr2,
-                                                                                               (unsigned long long)seed, workspace);
+  opb::pnp_hypotheses<<<dim3((unsigned)B, (unsigned)((hypotheses + opb::kHypThreads - 1) / opb::kHypThreads)), opb::kHypThreads, 0, st>>>(
+      K, pts2d, pts3d, offsets, hypotheses, thr2, (unsigned long long)seed, workspace);
   opb::pnp_select_refine<<<(unsigned)B, opb::kRefineThreads, 0, st>>>(K, pts2d, pts3d, offsets, hypotheses, thr2, workspace, pose_out, inlier_mask, n_inliers);
   return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_E_CUDA;
 }
