@@ -81,6 +81,25 @@ int opb_forward(opb_matcher* m, const float* desc2d_query, const int32_t* n2d_le
                 int64_t* matches0, int64_t* matches1, float* mscores0, float* mscores1,
                 float* conf, void* stream);
 
+/* Several objects on one handle.  opb_add_object uploads an object's constants (arguments as opb_set_object) and returns its
+ * id in *object_id; its GNN prologue runs on its first use, once.  The registration is independent of opb_set_object's
+ * current object.  opb_finalize_weights keeps registered objects: their leaf logits and prologue are recomputed under the new
+ * weights on their next use.  opb_remove_object frees an object after the work in flight (it synchronises the device). */
+int opb_add_object(opb_matcher* m, const float* desc3d_db, const float* desc2d_db, int32_t M, int32_t L, void* stream,
+                   int32_t* object_id);
+int opb_remove_object(opb_matcher* m, int32_t object_id);
+
+/* opb_forward for frames of different objects in one call: frame b matches against object object_ids_host[b] (HOST int32
+ * [B], registered ids; every object of a call has the same L, M may differ).  desc2d_query / n2d_lengths as in opb_forward.
+ * Outputs (device): matches0 int64 [B,N], mscores0 fp32 [B,N], matches1 int64 [B,M_out], mscores1 fp32 [B,M_out], conf fp32
+ * [B,N,M_out] or NULL; M_out >= the largest M of the call.  Columns >= M_b of frame b (its object's M) are -1 in matches1 and
+ * 0 in mscores1 and conf.  A frame's results do not depend on the other frames of the call.  OPB_E_INVALID for an unknown
+ * id, objects with different L, M_out too small, B <= 0 or N <= 0.  The range guard reports as for opb_forward.
+ * Asynchronous on `stream`; no host synchronisation. */
+int opb_forward_objects(opb_matcher* m, const int32_t* object_ids_host, const float* desc2d_query, const int32_t* n2d_lengths,
+                        int32_t B, int32_t N, int32_t M_out, int64_t* matches0, int64_t* matches1, float* mscores0, float* mscores1,
+                        float* conf, void* stream);
+
 /* Same call with HOST buffers (pinned or pageable): H2D of the query descriptors (and lengths, may be NULL),
  * forward, D2H of matches/scores; returns after the stream has been synchronised.  The confidence matrix is
  * materialised on the device if conf_host is non-NULL (then also copied back) or materialize_conf != 0
@@ -115,7 +134,8 @@ int opb_get_profile_entry(opb_matcher* m, const char* prefix, double* ms, double
  * reference does (same results up to fp32 rounding; used by the tests). */
 int opb_set_hoist(opb_matcher* m, int32_t enable);
 
-/* Frames processed together through the GNN (workspace-size knob); 0 = default (32). */
+/* Frames processed together through the GNN (workspace-size knob); 0 = default (32).  At most 64: larger values return
+ * OPB_E_INVALID and leave the setting unchanged. */
 int opb_set_chunk_frames(opb_matcher* m, int32_t frames);
 
 /* ---- adjacent producers: the per-object feature files the path consumes (SURVEY 8f N2) ---- */
@@ -166,6 +186,14 @@ int opb_ransac_pnp(const double* K, const double* pts2d, const double* pts3d, co
 int opb_gather_matches(const int64_t* matches0, const float* mscores0, const float* keypoints2d, const float* keypoints3d,
                        int32_t B, int32_t N, int32_t M, double* pts2d, double* pts3d, float* mconf, int32_t* query_index,
                        int32_t* offsets, void* stream);
+/* The same for frames of different objects (opb_forward_objects' output):
+ *   keypoints3d  device fp32 [sum M, 3]  the objects' 3D key points, concatenated
+ *   kp3_first    device int32 [B]        first row of frame b's object in keypoints3d
+ *   kp3_count    device int32 [B]        its M: an entry m of frame b is a match iff 0 <= m < kp3_count[b]
+ * Other arguments, outputs and order as opb_gather_matches, which is this call with kp3_first = 0 and kp3_count = M. */
+int opb_gather_matches_objects(const int64_t* matches0, const float* mscores0, const float* keypoints2d, const float* keypoints3d,
+                               const int32_t* kp3_first, const int32_t* kp3_count, int32_t B, int32_t N, double* pts2d, double* pts3d,
+                               float* mconf, int32_t* query_index, int32_t* offsets, void* stream);
 
 /* ---- adjacent producer: SuperPoint key-point extractor (SURVEY 8f N4) ----
  * Replaces SuperPoint.forward (reference src/models/extractors/SuperPoint/superpoint.py:140-197): shared VGG-style encoder

@@ -43,6 +43,9 @@ SYMBOLS = {
     "opb_set_object": (C.c_int, [_P, _P, _P, _I, _I, _P]),
     "opb_reserve_workspace": (C.c_int, [_P, _I, _I]),
     "opb_forward": (C.c_int, [_P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P]),
+    "opb_add_object": (C.c_int, [_P, _P, _P, _I, _I, _P, C.POINTER(_I)]),
+    "opb_remove_object": (C.c_int, [_P, _I]),
+    "opb_forward_objects": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P]),
     "opb_forward_host": (C.c_int, [_P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _I, _P]),
     "opb_check_range": (C.c_int, [_P, _P]),
     "opb_poll_range": (C.c_int, [_P]),
@@ -57,6 +60,7 @@ SYMBOLS = {
     "opb_gather_features3d": (C.c_int, [_P, _P, _I, C.c_int64, _P, C.c_int64, _P, _P, C.c_int64, _P]),
     "opb_ransac_pnp": (C.c_int, [_P, _P, _P, _P, _I, _I, C.c_double, C.c_uint64, _P, _P, _P, _P, _P]),
     "opb_gather_matches": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P]),
+    "opb_gather_matches_objects": (C.c_int, [_P, _P, _P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P]),
     "opb_debug_set_pdl": (C.c_int, [_I]),
     "opb_debug_set_ws_fill": (C.c_int, [_I]),
     "opb_debug_set_kv_passes": (C.c_int, [_P, _I]),

@@ -40,6 +40,17 @@ struct AttnLayerW {       // one AttentionPropagation (reference GATs_SuperGlue.
   DevBuf b1;              // [256]
 };
 
+struct ObjectState {      // per-object constants: the handle's current object (opb_set_object) or one opb_add_object registration
+  int M = 0, Lf = 0, m_pad = 0;
+  DevBuf leaves;          // fp32 [M*Lf, 256] point-major
+  PlaneBuf db;            // [m_pad, 256]
+  DevBuf s2;              // [4][M*Lf]: leaf logits, valid while s2_ready (they depend on the weights)
+  PlaneBuf xo;            // [m_pad, 256]: 3D-point state entering layer 2 (object prologue), valid while prologue_ready
+  bool s2_ready = false;
+  bool prologue_ready = false;
+  void release() { leaves.release(); db.release(); s2.release(); xo.release(); }
+};
+
 }  // namespace opb
 
 using namespace opb;
@@ -59,15 +70,13 @@ struct opb_matcher {
   DevBuf bf;
   PlaneBuf eye;           // [256,256] identity, fp16-split (residual as an identity K-block of the mlp.3 GEMM)
   // per-object constants
-  int M = 0, Lf = 0, m_pad = 0;
-  DevBuf leaves;          // fp32 [M*Lf, 256] point-major
-  PlaneBuf db;            // [m_pad, 256]
-  DevBuf s2;              // [4][M*Lf]
-  PlaneBuf xo;            // [m_pad, 256]: 3D-point state entering layer 2 (object prologue), valid while prologue_ready
-  bool prologue_ready = false;
+  ObjectState cur;                              // opb_set_object's object (valid while object_ready)
+  std::map<int, ObjectState*> objects;          // opb_add_object registrations, by id
+  int next_object_id = 0;
   // workspace (chunk)
   int chunk_frames = 0;   // user override
-  int ws_frames = 0, ws_N = 0;
+  int ws_frames = 0, ws_N = 0, ws_m_pad = 0;
+  DevBuf tab;             // ChunkTable of the chunk in flight (written by assemble_layout)
   bool hoist = true;      // evaluate the frame-invariant layers once per object (object_prologue)
   int identity_diag = 1;  // residual identity K-block as N = 64 MMAs on the diagonal blocks (opb_debug_set_identity_diag)
   int kv_two_pass = 1;    // k,v projection as A_hi.(B_hi + B_lo): its output is one fp16 plane, the A_lo term is below that rounding
@@ -181,12 +190,14 @@ static int run_gemm(opb_matcher* m, const GemmProblem& p, cudaStream_t st, doubl
     prof_mark(m, st, name, 0.0);                                                                                    \
   } while (0)
 
-static int ensure_workspace(opb_matcher* m, int frames, int N) {
-  if (frames <= m->ws_frames && N <= m->ws_N) return 0;
-  frames = frames > m->ws_frames ? frames : m->ws_frames;
-  N = N > m->ws_N ? N : m->ws_N;
+// Sized for chunks of `frames` frames, N query points and 3D segments of m_pad rows (the largest object of a call); only grows.
+static int ensure_workspace(opb_matcher* m, int frames, int N, int m_pad) {
+  if (frames <= m->ws_frames && N <= m->ws_N && m_pad <= m->ws_m_pad) return 0;
+  frames = std::max(frames, m->ws_frames);
+  N = std::max(N, m->ws_N);
+  m_pad = std::max(m_pad, m->ws_m_pad);
   const int n_pad = round_up(N, kSegPad);
-  const size_t R = (size_t)n_pad + m->m_pad;
+  const size_t R = (size_t)n_pad + m_pad;
   const size_t rows = R * frames;
   const size_t S = 2 * (size_t)frames;
   CK(m, m->x.ensure(rows * kD));
@@ -203,44 +214,66 @@ static int ensure_workspace(opb_matcher* m, int frames, int N) {
   CK(m, m->mu.ensure(S * 512 * sizeof(float)));
   CK(m, m->rstd.ensure(S * 512 * sizeof(float)));
   CK(m, m->rowsum.ensure((size_t)frames * n_pad * sizeof(float)));
-  CK(m, m->rowsum_part.ensure((size_t)frames * (m->m_pad / 256) * 2 * n_pad * sizeof(float)));
-  CK(m, m->colsum_part.ensure((size_t)frames * (n_pad / 32) * m->m_pad * sizeof(float)));
-  CK(m, m->colsum.ensure((size_t)frames * m->m_pad * sizeof(float)));
+  CK(m, m->rowsum_part.ensure((size_t)frames * (m_pad / 256) * 2 * n_pad * sizeof(float)));
+  CK(m, m->colsum_part.ensure((size_t)frames * (n_pad / 32) * m_pad * sizeof(float)));
+  CK(m, m->colsum.ensure((size_t)frames * m_pad * sizeof(float)));
   CK(m, m->rowbest.ensure((size_t)frames * n_pad * sizeof(unsigned long long)));
-  CK(m, m->colbest.ensure((size_t)frames * m->m_pad * sizeof(unsigned long long)));
+  CK(m, m->colbest.ensure((size_t)frames * m_pad * sizeof(unsigned long long)));
   CK(m, m->range_flag.ensure(sizeof(int), true));
+  CK(m, m->tab.ensure(sizeof(ChunkTable)));
   if (m->cfg.with_linear_transform) {
-    CK(m, m->lin_a.ensure((size_t)frames * m->m_pad * kD));
-    CK(m, m->lin_b.ensure((size_t)frames * m->m_pad * kD));
+    CK(m, m->lin_a.ensure((size_t)frames * m_pad * kD));
+    CK(m, m->lin_b.ensure((size_t)frames * m_pad * kD));
   }
   // (re)allocation fills ran on the legacy stream: order them against the caller's (possibly non-blocking) stream once
   CK(m, cudaDeviceSynchronize());
   m->ws_frames = frames;
   m->ws_N = N;
+  m->ws_m_pad = m_pad;
   return 0;
 }
 
-// One GATs layer on the 3D-point segments of `x` (layout L).
-static int run_gats(opb_matcher* m, const Layout& L, XView x, int gi, cudaStream_t st) {
+static ChunkTable* tab_dev(const opb_matcher* m) { return m->tab.as<ChunkTable>(); }
+
+// Frame b of a chunk matches against its object's rows `o`.
+static void table_frame(ChunkTable& t, int b, const ObjectState& o, bool hoist) {
+  t.obj[b] = FrameObject{hoist ? o.xo.hi.as<__half>() : o.db.hi.as<__half>(), hoist ? o.xo.lo.as<__half>() : o.db.lo.as<__half>(),
+                         o.leaves.as<float>(), o.s2.as<float>()};
+  t.mlen[b] = o.M;
+}
+
+// GATs groups of a chunk: runs of consecutive frames of one object, cut at kGatsFramesPerWarp frames.  With one object these
+// are [0, 16), [16, 32), ...; frames of an object placed next to each other in a call share their leaf reads.
+static void make_groups(GatsGroups& g, const ObjectState* const* fobj, int fb) {
+  g.n = 0;
+  for (int b = 0; b < fb; ++b) {
+    if (b == 0 || fobj[b] != fobj[b - 1] || b - g.g[g.n - 1].b_begin == kGatsFramesPerWarp)
+      g.g[g.n++] = GatsGroup{fobj[b]->leaves.as<float>(), fobj[b]->s2.as<float>(), b, b, fobj[b]->M, 0};
+    g.g[g.n - 1].b_end = b + 1;
+  }
+}
+
+// One GATs layer on the 3D-point segments of `x` (layout L); frame b aggregates the leaves of its object (chunk table, already
+// on the device; `groups` for the 8-leaf kernel), `Lf` leaves per point.
+static int run_gats(opb_matcher* m, const Layout& L, XView x, int gi, int Lf, const GatsGroups& groups, cudaStream_t st) {
   const long long warps = (long long)L.M * L.B;
   if (warps == 0) return 0;
   const bool lin = m->cfg.with_linear_transform != 0;
   GatsOut out{lin ? m->lin_a.hi.as<__half>() : x.hi, lin ? m->lin_a.lo.as<__half>() : x.lo, lin ? 1 : 0};
-  const float* s2 = m->s2.as<float>() + (size_t)gi * m->M * m->Lf;
   const float* wa3 = m->wa3.as<float>() + gi * kD;
-  if (m->Lf == 8) {   // leaves loaded once per point and reused across 8 frames of the chunk (any B: one code path, frame-independent results)
-    const long long w8 = (long long)L.M * ((L.B + kGatsFramesPerWarp - 1) / kGatsFramesPerWarp);
+  const ChunkTable* tab = tab_dev(m);
+  if (Lf == 8) {   // leaves loaded once per point and reused across the frames of a group (frame-independent results)
+    const long long w8 = (long long)L.M * groups.n;
     LAUNCH(m, st, "gats_aggregate", gats_aggregate_frames8, dim3((unsigned)((w8 * 32 + 255) / 256)), dim3(256), 0, st, (const __half*)x.hi,
-           (const __half*)x.lo, L, (const float*)m->leaves.as<float>(), s2, wa3, (int)m->cfg.include_self, (int)m->cfg.additional, 0.2f, out);
+           (const __half*)x.lo, L, groups, gi, wa3, (int)m->cfg.include_self, (int)m->cfg.additional, 0.2f, out);
   } else {
     LAUNCH(m, st, "gats_aggregate", gats_aggregate, dim3((unsigned)((warps * 32 + 255) / 256)), dim3(256), 0, st, (const __half*)x.hi,
-           (const __half*)x.lo, L, (const float*)m->leaves.as<float>(), m->Lf, s2, wa3, (int)m->cfg.include_self, (int)m->cfg.additional, 0.2f,
-           out);
+           (const __half*)x.lo, L, tab, Lf, gi, wa3, (int)m->cfg.include_self, (int)m->cfg.additional, 0.2f, out);
   }
   if (!lin) return 0;
   // with_linear_transform (GATs.py:56-57,64-65): t = pre . W on the tensor cores over the compact 3D rows, then ELU (+ h3)
   Layout Lc{};
-  Lc.B = L.B; Lc.N = 0; Lc.M = L.M; Lc.n_pad = 0; Lc.m_pad = L.m_pad; Lc.R = L.m_pad;
+  Lc.B = L.B; Lc.N = 0; Lc.M = L.M; Lc.n_pad = 0; Lc.m_pad = L.m_pad; Lc.R = L.m_pad; Lc.mlen = L.mlen;
   GemmProblem p{};
   p.L = Lc; p.batch = 1; p.rows = Lc.rows();
   p.a1 = m->lin_a.c(kD); p.K1 = kD; p.b1 = m->wlin.c(kD, (size_t)gi * kD * kD); p.n_out = kD;
@@ -313,26 +346,44 @@ static int run_attn_layer(opb_matcher* m, const Layout& L, XView x, AttnLayerW& 
 
 // Object prologue: GNN layers 0 (GATs) and the 3D side of layer 1 (self-attention) depend only on the per-object
 // constants (reference GATs_SuperGlue.py:50-54 and :60-64 with src1 = desc3d_db), not on the query frame.  They are
-// evaluated ONCE PER OBJECT -- on a single copy of the object's rows, by the first opb_forward after opb_set_object /
-// opb_finalize_weights (it needs the chunk workspace) -- and shared by every frame of every later call, like the leaf
-// logits s2.  Result: m->xo = 3D-point state entering layer 2.
-static int object_prologue(opb_matcher* m, cudaStream_t st) {
+// evaluated ONCE PER OBJECT -- on a single copy of the object's rows, by the first call that uses the object after
+// opb_set_object / opb_add_object / opb_finalize_weights (it needs the chunk workspace) -- and shared by every frame of every
+// later call, like the leaf logits s2.  Result: o.xo = 3D-point state entering layer 2.
+static int object_prologue(opb_matcher* m, ObjectState& o, cudaStream_t st) {
   Layout Lo{};
-  Lo.B = 1; Lo.N = 0; Lo.M = m->M; Lo.n_pad = 0; Lo.m_pad = m->m_pad; Lo.R = m->m_pad;
+  Lo.B = 1; Lo.N = 0; Lo.M = o.M; Lo.n_pad = 0; Lo.m_pad = o.m_pad; Lo.R = o.m_pad;
+  ChunkTable t{};
+  table_frame(t, 0, o, /*hoist=*/false);
+  GatsGroups g{};
+  const ObjectState* one = &o;
+  make_groups(g, &one, 1);
   LAUNCH(m, st, "assemble_layout", assemble_layout, dim3(m->num_sms * 2, 1), dim3(256), 0, st, (const __half*)nullptr, (const __half*)nullptr,
-         (const __half*)m->db.hi.as<__half>(), (const __half*)m->db.lo.as<__half>(), m->xo.hi.as<__half>(), m->xo.lo.as<__half>(), Lo);
-  if (int rc = run_gats(m, Lo, m->xo.view(), 0, st)) return rc;
-  return run_attn_layer(m, Lo, m->xo.view(), m->attn[0], /*cross=*/0, st);
+         t, tab_dev(m), o.xo.hi.as<__half>(), o.xo.lo.as<__half>(), Lo);
+  if (int rc = run_gats(m, Lo, o.xo.view(), 0, o.Lf, g, st)) return rc;
+  return run_attn_layer(m, Lo, o.xo.view(), m->attn[0], /*cross=*/0, st);
 }
 
-// GNN + tail for `fb` frames starting at frame f0 of the call.
-static int forward_chunk(opb_matcher* m, const float* q_cf, const int* nlen, int N, int fb, int64_t* m0, int64_t* m1, float* s0, float* s1,
-                         float* conf, cudaStream_t st, int piece, int h2d_first) {
+// GNN + tail for the `fb` frames of a chunk; frame b matches against fobj[b].  Outputs: m1 / s1 rows and conf rows are M_out wide.
+static int forward_chunk(opb_matcher* m, const ObjectState* const* fobj, const float* q_cf, const int* nlen, int N, int fb, int M_out,
+                         int64_t* m0, int64_t* m1, float* s0, float* s1, float* conf, cudaStream_t st, int piece, int h2d_first) {
+  ChunkTable t{};
+  int m_max = 0, m_sum = 0;
+  bool uniform = true;
+  for (int b = 0; b < fb; ++b) {
+    table_frame(t, b, *fobj[b], m->hoist);
+    m_max = std::max(m_max, fobj[b]->M);
+    m_sum += fobj[b]->M;
+    uniform = uniform && fobj[b]->M == fobj[0]->M;
+  }
+  GatsGroups groups{};
+  make_groups(groups, fobj, fb);
+  const int Lf = fobj[0]->Lf;
   Layout L{};
-  L.B = fb; L.N = N; L.M = m->M; L.n_pad = round_up(N, kSegPad); L.m_pad = m->m_pad; L.R = L.n_pad + L.m_pad;
+  L.B = fb; L.N = N; L.M = m_max; L.n_pad = round_up(N, kSegPad); L.m_pad = round_up(m_max, kSegPad); L.R = L.n_pad + L.m_pad;
   L.nlen = nlen;
+  L.mlen = uniform ? nullptr : tab_dev(m)->mlen;     // device address of the table's mlen (written by assemble_layout)
   const int rows = L.rows();
-  const double valid_rows = (double)fb * (N + L.M);
+  const double valid_rows = (double)fb * N + m_sum;
   __half *xh = m->x.hi.as<__half>(), *xl = m->x.lo.as<__half>();
 
   int first_layer = 0;
@@ -351,21 +402,21 @@ static int forward_chunk(opb_matcher* m, const float* q_cf, const int* nlen, int
              (long long)kD * N, Lq.nlen, L.n_pad, xq.hi, xq.lo, (float*)nullptr, (long long)Lq.R, 0);
       if (int rc = run_attn_layer(m, Lq, xq, m->attn[0], 0, st)) return rc;
     }
-    // assemble the full layout: query rows from xq, 3D rows from the object prologue
+    // assemble the full layout: query rows from xq, 3D rows from each frame's object prologue
     LAUNCH(m, st, "assemble_layout", assemble_layout, dim3(m->num_sms * 2, fb), dim3(256), 0, st, (const __half*)m->xq.hi.as<__half>(),
-           (const __half*)m->xq.lo.as<__half>(), (const __half*)m->xo.hi.as<__half>(), (const __half*)m->xo.lo.as<__half>(), xh, xl, L);
+           (const __half*)m->xq.lo.as<__half>(), t, tab_dev(m), xh, xl, L);
     first_layer = 2;
   } else {
-    // inputs: query descriptors [fb,256,N] channel-first -> q segments; object rows -> d segments
+    // inputs: query descriptors [fb,256,N] channel-first -> q segments; each frame's object rows -> its d segment
     LAUNCH(m, st, "transpose_cf_to_rows", transpose_cf_to_rows<0>, dim3(L.n_pad / 32, fb), dim3(32, 8), 0, st, q_cf, N, N, (long long)kD * N, nlen,
            L.n_pad, xh, xl, (float*)nullptr, (long long)L.R, 0);
     LAUNCH(m, st, "assemble_layout", assemble_layout, dim3(m->num_sms * 2, fb), dim3(256), 0, st, (const __half*)nullptr, (const __half*)nullptr,
-           (const __half*)m->db.hi.as<__half>(), (const __half*)m->db.lo.as<__half>(), xh, xl, L);
+           t, tab_dev(m), xh, xl, L);
   }
 
   for (int layer = first_layer; layer < 12; ++layer) {
     if (layer % 3 == 0) {
-      if (int rc = run_gats(m, L, m->x.view(), layer / 3, st)) return rc;
+      if (int rc = run_gats(m, L, m->x.view(), layer / 3, Lf, groups, st)) return rc;
     } else {
       const int attn_idx = (layer / 3) * 2 + (layer % 3) - 1;
       if (int rc = run_attn_layer(m, L, m->x.view(), m->attn[attn_idx], (layer % 3 == 2) ? 1 : 0, st)) return rc;
@@ -390,15 +441,17 @@ static int forward_chunk(opb_matcher* m, const float* q_cf, const int* nlen, int
   ps.a_batch_rows = L.R; ps.b_batch_rows = L.R;
   ps.inv_scale = 1.f / m->cfg.scale_factor;
   ps.epi = EPI_SCORE_SUMS; ps.rowsum_part = m->rowsum_part.as<float>(); ps.colsum_part = m->colsum_part.as<float>();
-  if (int rc = run_gemm(m, ps, st, 2.0 * fb * (double)N * L.M * kD, "score_sums")) return rc;
+  if (int rc = run_gemm(m, ps, st, 2.0 * (double)N * m_sum * kD, "score_sums")) return rc;
   LAUNCH(m, st, "score_sums_finalize", score_sums_finalize, dim3((L.n_pad + L.m_pad + 255) / 256, fb), dim3(256), 0, st,
          (const float*)m->rowsum_part.as<float>(), (const float*)m->colsum_part.as<float>(), L, n_parts, q_groups, m->rowsum.as<float>(),
          m->colsum.as<float>(), m->rowbest.as<unsigned long long>(), m->colbest.as<unsigned long long>());
   ps.epi = EPI_SCORE_CONF; ps.inv_rowsum = m->rowsum.as<float>(); ps.inv_colsum = m->colsum.as<float>();
-  ps.conf = conf; ps.rowbest = m->rowbest.as<unsigned long long>(); ps.colbest = m->colbest.as<unsigned long long>();
+  ps.conf = conf; ps.conf_ld = M_out; ps.rowbest = m->rowbest.as<unsigned long long>(); ps.colbest = m->colbest.as<unsigned long long>();
   if (int rc = run_gemm(m, ps, st, 0.0, "score_conf")) return rc;      // recomputation: its FLOPs are not algorithmic
+  if (conf && M_out > L.m_pad)                                          // conf rows wider than this chunk's 3D segments
+    LAUNCH(m, st, "conf_fill_tail", conf_fill_tail, dim3(m->num_sms * 4), dim3(256), 0, st, conf, (long long)fb * N, M_out, L.m_pad);
   LAUNCH(m, st, "mutual_match", mutual_match, dim3(fb), dim3(256), 0, st, (const unsigned long long*)m->rowbest.as<unsigned long long>(),
-         (const unsigned long long*)m->colbest.as<unsigned long long>(), L, m->cfg.match_threshold, (const int*)m->range_flag.as<int>(),
+         (const unsigned long long*)m->colbest.as<unsigned long long>(), L, m->cfg.match_threshold, (const int*)m->range_flag.as<int>(), M_out,
          reinterpret_cast<long long*>(m0), reinterpret_cast<long long*>(m1), s0, s1);
   return 0;
 }
@@ -406,6 +459,94 @@ static int forward_chunk(opb_matcher* m, const float* q_cf, const int* nlen, int
 static int chunk_of(const opb_matcher* m, int B) {
   int chunk = m->chunk_frames > 0 ? m->chunk_frames : kDefaultChunk;
   return chunk > B ? B : chunk;
+}
+
+// Leaf logits of an object (frame-invariant, they depend on the weights): GATs.py:40,78 folded as s2 = leaves . (W a[:256]).
+// A plain launch: it also runs outside a forward (opb_set_object / opb_add_object), where it must not touch the profile of
+// the last forward; forward_frames counts and marks it itself.
+static int object_leaf_logits(opb_matcher* m, ObjectState& o, cudaStream_t st) {
+  CK(m, launch_k(gats_leaf_logits, dim3(m->num_sms * 4), dim3(256), 0, st, (const float*)o.leaves.as<float>(), (long long)o.M * o.Lf,
+                 (const float*)m->wa2.as<float>(), o.s2.as<float>()));
+  o.s2_ready = true;
+  return 0;
+}
+
+// Upload an object's constants into `o` (buffers only grow) and compute its leaf logits; its prologue runs on first use.
+static int load_object(opb_matcher* m, ObjectState& o, const float* desc3d_db, const float* desc2d_db, int M, int Lf, cudaStream_t st) {
+  const int m_pad = round_up(M, kSegPad);
+  o.M = M; o.Lf = Lf; o.m_pad = m_pad;
+  const long long n_leaf_rows = (long long)M * Lf;
+  o.leaves.grew = o.db.hi.grew = o.s2.grew = o.xo.hi.grew = false;
+  o.s2_ready = o.prologue_ready = false;
+  CK(m, o.leaves.ensure((size_t)n_leaf_rows * kD * sizeof(float)));
+  CK(m, o.db.ensure((size_t)m_pad * kD));
+  CK(m, o.s2.ensure((size_t)4 * n_leaf_rows * sizeof(float)));
+  CK(m, o.xo.ensure((size_t)m_pad * kD));
+  if (o.leaves.grew || o.db.hi.grew || o.s2.grew || o.xo.hi.grew) CK(m, cudaDeviceSynchronize());   // frees of the old buffers vs work in flight
+  launch_k(transpose_cf_to_rows<1>, dim3((unsigned)((n_leaf_rows + 31) / 32), 1), dim3(32, 8), 0, st, desc2d_db, (int)n_leaf_rows, (int)n_leaf_rows, 0ll,
+           (const int*)nullptr, (int)n_leaf_rows, (__half*)nullptr, (__half*)nullptr, o.leaves.as<float>(), 0ll, 0);
+  // rows [M, m_pad) of the object planes are written as zero by the transpose (MODE 0 pads to rows_out)
+  launch_k(transpose_cf_to_rows<0>, dim3(m_pad / 32, 1), dim3(32, 8), 0, st, desc3d_db, (int)M, (int)M, 0ll, (const int*)nullptr, m_pad,
+           o.db.hi.as<__half>(), o.db.lo.as<__half>(), (float*)nullptr, 0ll, 0);
+  CK(m, cudaGetLastError());
+  return object_leaf_logits(m, o, st);
+}
+
+static void invalidate_prologues(opb_matcher* m) {
+  m->cur.prologue_ready = false;
+  for (auto& kv : m->objects) kv.second->prologue_ready = false;
+}
+
+// The one forward of the handle: frame b of the call matches against fobj[b] (opb_forward: the current object everywhere).
+// m1 / s1 rows and conf rows are M_out >= max M_b wide.
+static int forward_frames(opb_matcher* m, ObjectState* const* fobj, const float* q, const int32_t* n2d_lengths, int B, int N, int M_out,
+                          int64_t* m0, int64_t* m1, float* s0, float* s1, float* conf, cudaStream_t st) {
+  int call_m_pad = 0;
+  for (int b = 0; b < B; ++b) call_m_pad = std::max(call_m_pad, fobj[b]->m_pad);
+  const int chunk = chunk_of(m, B);
+  if (int rc = ensure_workspace(m, chunk, N, call_m_pad)) return rc;   // no-op once opb_reserve_workspace / an earlier call has sized it
+  m->launches = 0;
+  if (m->profiling) {
+    m->ev_used = 0;
+    m->ev_flops.clear();
+    m->ev_name.clear();
+    if (!m->ev_fwd0) { cudaEventCreate(&m->ev_fwd0); cudaEventCreate(&m->ev_fwd1); }
+    cudaEventRecord(m->ev_fwd0, st);
+  }
+  // per-object work on first use: leaf logits after a weight reload, the prologue (once per object, shared by all later calls)
+  for (int b = 0; b < B; ++b) {
+    ObjectState& o = *fobj[b];
+    if (!o.s2_ready) {
+      if (int rc = object_leaf_logits(m, o, st)) return rc;
+      m->launches++;
+      prof_mark(m, st, "gats_leaf_logits", 0.0);
+    }
+    if (m->hoist && !o.prologue_ready) {
+      if (int rc = object_prologue(m, o, st)) return rc;
+      o.prologue_ready = true;
+    }
+  }
+  // granularity of the query-side layer-1 pass: the host-copy pieces when the queries stream in from the host, else the chunk
+  const int piece = m->h2d_pending > 0 ? std::min(chunk, kQPassFrames) : chunk;
+  const int ppc = (chunk + piece - 1) / piece;              // pieces per chunk
+  for (int f0 = 0, ci = 0; f0 < B; f0 += chunk, ++ci) {
+    const int fb = std::min(chunk, B - f0);
+    if (!m->hoist)                                          // per-frame evaluation consumes the whole chunk at once
+      for (int si = 0; si * piece < fb; ++si)
+        if (ci * ppc + si < m->h2d_pending) CK(m, cudaStreamWaitEvent(st, m->h2d_ev[ci * ppc + si], 0));
+    int rc = forward_chunk(m, fobj + f0, q + (size_t)f0 * kD * N, n2d_lengths ? n2d_lengths + f0 : nullptr, N, fb, M_out, m0 + (size_t)f0 * N,
+                           m1 + (size_t)f0 * M_out, s0 + (size_t)f0 * N, s1 + (size_t)f0 * M_out, conf ? conf + (size_t)f0 * N * M_out : nullptr,
+                           st, piece, ci * ppc);
+    if (rc) return rc;
+  }
+  // deferred range report: the flag travels to pinned host memory behind the call; opb_poll_range() reads it without blocking
+  CK(m, cudaMemcpyAsync(m->range_host, m->range_flag.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CK(m, cudaEventRecord(m->range_ev, st));
+  m->range_pending = true;
+  m->last_stream = st;
+  if (m->profiling) cudaEventRecord(m->ev_fwd1, st);
+  m->last_launches = m->launches;
+  return OPB_OK;
 }
 
 }  // namespace opb
@@ -445,11 +586,13 @@ void opb_destroy(opb_matcher* m) {
   cudaSetDevice(m->cfg.device);
   cudaDeviceSynchronize();
   for (auto& a : m->attn) { a.wqkv.release(); a.bqkv.release(); a.w0a.release(); a.w0m.release(); a.b0f.release(); a.w1.release(); a.b1.release(); }
-  DevBuf* bufs[] = {&m->wa2, &m->wa3, &m->bf, &m->leaves, &m->s2, &m->kvt, &m->hid, &m->kvpart, &m->kmean, &m->statpart,
+  DevBuf* bufs[] = {&m->wa2, &m->wa3, &m->bf, &m->kvt, &m->hid, &m->kvpart, &m->kmean, &m->statpart, &m->tab,
                     &m->mu, &m->rstd, &m->rowsum_part, &m->colsum_part, &m->rowsum, &m->colsum, &m->rowbest, &m->colbest, &m->range_flag,
                     &m->st_q, &m->st_m0, &m->st_m1, &m->st_s0, &m->st_s1, &m->st_conf, &m->st_len};
   for (auto* b : bufs) b->release();
-  PlaneBuf* pb[] = {&m->wf, &m->wlin, &m->db, &m->xo, &m->x, &m->qp, &m->pn, &m->g, &m->xq, &m->bd, &m->lin_a, &m->lin_b, &m->eye};
+  m->cur.release();
+  for (auto& kv : m->objects) { kv.second->release(); delete kv.second; }
+  PlaneBuf* pb[] = {&m->wf, &m->wlin, &m->x, &m->qp, &m->pn, &m->g, &m->xq, &m->bd, &m->lin_a, &m->lin_b, &m->eye};
   for (auto* b : pb) b->release();
   for (auto e : m->ev_pool) cudaEventDestroy(e);
   for (auto e : m->h2d_ev) cudaEventDestroy(e);
@@ -557,8 +700,9 @@ int opb_finalize_weights(opb_matcher* m) {
   if (int rc = upload_f32(m, m->wa3, wa3)) return rc;
   CK(m, cudaDeviceSynchronize());
   m->weights_ready = true;
-  m->object_ready = false;  // s2 and the prologue depend on the weights
-  m->prologue_ready = false;
+  m->object_ready = false;  // s2 and the prologue depend on the weights: the current object is set again, registered objects
+  invalidate_prologues(m);  // recompute theirs on their next use
+  for (auto& kv : m->objects) kv.second->s2_ready = false;
   return OPB_OK;
 }
 
@@ -569,34 +713,50 @@ int opb_set_object(opb_matcher* m, const float* desc3d_db, const float* desc2d_d
     return fail(m, OPB_E_INVALID, "set_object: need M > 0 and 1 <= num_leaf <= 32 (got M=%d, L=%d)", M, Lf);
   CK(m, cudaSetDevice(m->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
-  const int m_pad = round_up(M, kSegPad);
-  if (m_pad != m->m_pad) { m->ws_frames = 0; m->ws_N = 0; }  // workspace depends on m_pad
-  m->M = M; m->Lf = Lf; m->m_pad = m_pad;
-  const long long n_leaf_rows = (long long)M * Lf;
-  m->leaves.grew = m->db.hi.grew = m->db.lo.grew = m->s2.grew = m->xo.hi.grew = false;
-  m->prologue_ready = false;
-  CK(m, m->leaves.ensure((size_t)n_leaf_rows * kD * sizeof(float)));
-  CK(m, m->db.ensure((size_t)m_pad * kD));
-  CK(m, m->s2.ensure((size_t)4 * n_leaf_rows * sizeof(float)));
-  CK(m, m->xo.ensure((size_t)m_pad * kD));
-  if (m->leaves.grew || m->db.hi.grew || m->s2.grew || m->xo.hi.grew) CK(m, cudaDeviceSynchronize());   // frees of the old buffers vs work in flight
-  launch_k(transpose_cf_to_rows<1>, dim3((unsigned)((n_leaf_rows + 31) / 32), 1), dim3(32, 8), 0, st, desc2d_db, (int)n_leaf_rows, (int)n_leaf_rows, 0ll,
-           (const int*)nullptr, (int)n_leaf_rows, (__half*)nullptr, (__half*)nullptr, m->leaves.as<float>(), 0ll, 0);
-  // rows [M, m_pad) of the object planes are written as zero by the transpose (MODE 0 pads to rows_out)
-  launch_k(transpose_cf_to_rows<0>, dim3(m_pad / 32, 1), dim3(32, 8), 0, st, desc3d_db, (int)M, (int)M, 0ll, (const int*)nullptr, m_pad,
-           m->db.hi.as<__half>(), m->db.lo.as<__half>(), (float*)nullptr, 0ll, 0);
-  launch_k(gats_leaf_logits, dim3(m->num_sms * 4), dim3(256), 0, st, (const float*)m->leaves.as<float>(), n_leaf_rows, (const float*)m->wa2.as<float>(),
-           m->s2.as<float>());
-  CK(m, cudaGetLastError());
+  m->object_ready = false;
+  if (int rc = load_object(m, m->cur, desc3d_db, desc2d_db, M, Lf, st)) return rc;
   m->object_ready = true;
+  return OPB_OK;
+}
+
+int opb_add_object(opb_matcher* m, const float* desc3d_db, const float* desc2d_db, int32_t M, int32_t Lf, void* stream, int32_t* object_id) {
+  if (!m) return OPB_E_INVALID;
+  if (!m->weights_ready) return fail(m, OPB_E_STATE, "opb_add_object before opb_finalize_weights");
+  if (!desc3d_db || !desc2d_db || !object_id || M <= 0 || Lf <= 0 || Lf > 32)
+    return fail(m, OPB_E_INVALID, "add_object: need M > 0, 1 <= num_leaf <= 32 and an id pointer (got M=%d, L=%d)", M, Lf);
+  CK(m, cudaSetDevice(m->cfg.device));
+  auto* o = new ObjectState();
+  if (int rc = load_object(m, *o, desc3d_db, desc2d_db, M, Lf, (cudaStream_t)stream)) {
+    cudaDeviceSynchronize();
+    o->release();
+    delete o;
+    return rc;
+  }
+  const int id = m->next_object_id++;
+  m->objects[id] = o;
+  *object_id = id;
+  return OPB_OK;
+}
+
+int opb_remove_object(opb_matcher* m, int32_t object_id) {
+  if (!m) return OPB_E_INVALID;
+  auto it = m->objects.find(object_id);
+  if (it == m->objects.end()) return fail(m, OPB_E_INVALID, "remove_object: unknown object id %d", object_id);
+  CK(m, cudaSetDevice(m->cfg.device));
+  CK(m, cudaDeviceSynchronize());                  // calls in flight may still read the object's buffers
+  it->second->release();
+  delete it->second;
+  m->objects.erase(it);
   return OPB_OK;
 }
 
 int opb_reserve_workspace(opb_matcher* m, int32_t frames, int32_t N) {
   if (!m || frames <= 0 || N <= 0) return OPB_E_INVALID;
-  if (!m->object_ready) return fail(m, OPB_E_STATE, "opb_reserve_workspace needs an object (the workspace depends on M)");
+  if (!m->object_ready && m->objects.empty()) return fail(m, OPB_E_STATE, "opb_reserve_workspace needs an object (the workspace depends on M)");
   CK(m, cudaSetDevice(m->cfg.device));
-  return ensure_workspace(m, chunk_of(m, frames), N);
+  int m_pad = m->object_ready ? m->cur.m_pad : 0;   // sized for the largest object the handle knows
+  for (auto& kv : m->objects) m_pad = std::max(m_pad, kv.second->m_pad);
+  return ensure_workspace(m, chunk_of(m, frames), N, m_pad);
 }
 
 int opb_set_hoist(opb_matcher* m, int32_t enable) {
@@ -607,6 +767,8 @@ int opb_set_hoist(opb_matcher* m, int32_t enable) {
 
 int opb_set_chunk_frames(opb_matcher* m, int32_t frames) {
   if (!m || frames < 0) return OPB_E_INVALID;
+  if (frames > kMaxChunkFrames)            // the per-chunk object table (ChunkTable) is a kernel parameter of fixed size
+    return fail(m, OPB_E_INVALID, "opb_set_chunk_frames: at most %d frames per chunk (got %d)", kMaxChunkFrames, frames);
   m->chunk_frames = frames;
   return OPB_OK;
 }
@@ -617,41 +779,30 @@ int opb_forward(opb_matcher* m, const float* q, const int32_t* n2d_lengths, int3
   if (!m->weights_ready || !m->object_ready) return fail(m, OPB_E_STATE, "opb_forward needs weights and an object (finalize_weights, set_object)");
   if (!q || !m0 || !m1 || !s0 || !s1 || B <= 0 || N <= 0) return fail(m, OPB_E_INVALID, "opb_forward: bad argument (B=%d, N=%d)", B, N);
   CK(m, cudaSetDevice(m->cfg.device));
-  cudaStream_t st = (cudaStream_t)stream;
-  const int chunk = chunk_of(m, B);
-  if (int rc = ensure_workspace(m, chunk, N)) return rc;   // no-op once opb_reserve_workspace / an earlier call has sized it
-  m->launches = 0;
-  if (m->profiling) {
-    m->ev_used = 0;
-    m->ev_flops.clear();
-    m->ev_name.clear();
-    if (!m->ev_fwd0) { cudaEventCreate(&m->ev_fwd0); cudaEventCreate(&m->ev_fwd1); }
-    cudaEventRecord(m->ev_fwd0, st);
+  std::vector<ObjectState*> fobj((size_t)B, &m->cur);      // every frame uses the current object
+  return forward_frames(m, fobj.data(), q, n2d_lengths, B, N, m->cur.M, m0, m1, s0, s1, conf, (cudaStream_t)stream);
+}
+
+int opb_forward_objects(opb_matcher* m, const int32_t* object_ids_host, const float* q, const int32_t* n2d_lengths, int32_t B, int32_t N,
+                        int32_t M_out, int64_t* m0, int64_t* m1, float* s0, float* s1, float* conf, void* stream) {
+  if (!m) return OPB_E_INVALID;
+  if (!m->weights_ready) return fail(m, OPB_E_STATE, "opb_forward_objects needs weights (finalize_weights)");
+  if (!object_ids_host || !q || !m0 || !m1 || !s0 || !s1 || B <= 0 || N <= 0)
+    return fail(m, OPB_E_INVALID, "opb_forward_objects: bad argument (B=%d, N=%d)", B, N);
+  std::vector<ObjectState*> fobj((size_t)B);
+  int m_max = 0;
+  for (int b = 0; b < B; ++b) {
+    auto it = m->objects.find(object_ids_host[b]);
+    if (it == m->objects.end()) return fail(m, OPB_E_INVALID, "opb_forward_objects: unknown object id %d (frame %d)", object_ids_host[b], b);
+    fobj[b] = it->second;
+    if (fobj[b]->Lf != fobj[0]->Lf)
+      return fail(m, OPB_E_INVALID, "opb_forward_objects: frames %d and 0 use objects with different leaf counts (%d, %d)", b, fobj[b]->Lf,
+                  fobj[0]->Lf);
+    m_max = std::max(m_max, fobj[b]->M);
   }
-  if (m->hoist && !m->prologue_ready) {
-    if (int rc = object_prologue(m, st)) return rc;
-    m->prologue_ready = true;
-  }
-  // granularity of the query-side layer-1 pass: the host-copy pieces when the queries stream in from the host, else the chunk
-  const int piece = m->h2d_pending > 0 ? std::min(chunk, kQPassFrames) : chunk;
-  const int ppc = (chunk + piece - 1) / piece;              // pieces per chunk
-  for (int f0 = 0, ci = 0; f0 < B; f0 += chunk, ++ci) {
-    const int fb = std::min(chunk, B - f0);
-    if (!m->hoist)                                          // per-frame evaluation consumes the whole chunk at once
-      for (int si = 0; si * piece < fb; ++si)
-        if (ci * ppc + si < m->h2d_pending) CK(m, cudaStreamWaitEvent(st, m->h2d_ev[ci * ppc + si], 0));
-    int rc = forward_chunk(m, q + (size_t)f0 * kD * N, n2d_lengths ? n2d_lengths + f0 : nullptr, N, fb, m0 + (size_t)f0 * N, m1 + (size_t)f0 * m->M,
-                           s0 + (size_t)f0 * N, s1 + (size_t)f0 * m->M, conf ? conf + (size_t)f0 * N * m->M : nullptr, st, piece, ci * ppc);
-    if (rc) return rc;
-  }
-  // deferred range report: the flag travels to pinned host memory behind the call; opb_poll_range() reads it without blocking
-  CK(m, cudaMemcpyAsync(m->range_host, m->range_flag.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-  CK(m, cudaEventRecord(m->range_ev, st));
-  m->range_pending = true;
-  m->last_stream = st;
-  if (m->profiling) cudaEventRecord(m->ev_fwd1, st);
-  m->last_launches = m->launches;
-  return OPB_OK;
+  if (M_out < m_max) return fail(m, OPB_E_INVALID, "opb_forward_objects: M_out = %d is below the largest object of the call (M = %d)", M_out, m_max);
+  CK(m, cudaSetDevice(m->cfg.device));
+  return forward_frames(m, fobj.data(), q, n2d_lengths, B, N, M_out, m0, m1, s0, s1, conf, (cudaStream_t)stream);
 }
 
 int opb_set_profiling(opb_matcher* m, int32_t enable) {
@@ -716,7 +867,7 @@ int opb_forward_host(opb_matcher* m, const float* qh, const int32_t* n2d_lengths
   if (!qh || !m0h || !m1h || !s0h || !s1h || B <= 0 || N <= 0) return fail(m, OPB_E_INVALID, "opb_forward_host: bad argument");
   CK(m, cudaSetDevice(m->cfg.device));
   cudaStream_t st = (cudaStream_t)stream;
-  const size_t M = m->M;
+  const size_t M = m->cur.M;
   const bool want_conf = confh != nullptr || materialize_conf != 0;
   DevBuf* stg[] = {&m->st_q, &m->st_m0, &m->st_m1, &m->st_s0, &m->st_s1, &m->st_conf, &m->st_len};
   for (auto* b : stg) b->grew = false;
@@ -837,14 +988,14 @@ int opb_gather_features3d(const float* desc, const float* scores, int32_t dim, i
 int opb_debug_set_kv_passes(opb_matcher* m, int32_t passes) {
   if (!m || (passes != 2 && passes != 3)) return OPB_E_INVALID;
   m->kv_two_pass = passes == 2 ? 1 : 0;
-  m->prologue_ready = false;
+  invalidate_prologues(m);
   return OPB_OK;
 }
 
 int opb_debug_set_identity_diag(opb_matcher* m, int32_t enable) {
   if (!m) return OPB_E_INVALID;
   m->identity_diag = enable ? 1 : 0;
-  m->prologue_ready = false;
+  invalidate_prologues(m);
   return OPB_OK;
 }
 

@@ -20,13 +20,16 @@ constexpr float kProdInv = 1.0f / 4096.0f;
 
 // Activation layout of one forward chunk: frame b owns rows
 //   [b*R, b*R + n_pad)           query segment   (N valid)
-//   [b*R + n_pad, (b+1)*R)       3D-point segment (M valid)
+//   [b*R + n_pad, (b+1)*R)       3D-point segment (M_b valid: the rows of frame b's object)
 // with R = n_pad + m_pad, both multiples of kSegPad.  A "segment" is the unit of
 // InstanceNorm statistics and of the linear-attention KV state
 // (reference GATs_SuperGlue.py:126 and :77-78 reduce over the point dimension).
+// Frames of one chunk may use different objects: M is the largest M_b of the chunk, rows [M_b, m_pad) of a 3D segment are
+// zero and masked out of every reduction, as the query rows past n_of(b).
 struct Layout {
   int B, N, M, n_pad, m_pad, R;
   const int* nlen;   // device int32 [B]: valid query rows of each frame (ragged batch, every entry in [0, N]) or nullptr: N everywhere
+  const int* mlen;   // device int32 [B]: valid 3D rows of each frame (frames of different objects, entries in [1, M]) or nullptr: M everywhere
   __host__ __device__ int rows() const { return B * R; }
   __host__ __device__ int segs() const { return 2 * B; }
   __host__ __device__ int seg_of_row(int row) const {
@@ -38,7 +41,8 @@ struct Layout {
 #ifdef __CUDACC__
   // valid query rows of frame b / valid rows of a segment (device only: nlen lives in device memory)
   __device__ int n_of(int b) const { return nlen ? min(max(__ldg(nlen + b), 0), N) : N; }
-  __device__ int seg_valid(int seg) const { return (seg & 1) ? M : n_of(seg >> 1); }
+  __device__ int m_of(int b) const { return mlen ? __ldg(mlen + b) : M; }
+  __device__ int seg_valid(int seg) const { return (seg & 1) ? m_of(seg >> 1) : n_of(seg >> 1); }
 #endif
   // attention source segment: 'self' -> itself, 'cross' -> the other side of the frame
   // (reference GATs_SuperGlue.py:57-58, :62-63)

@@ -80,7 +80,8 @@ struct GemmProblem {
   float* colsum_part;               // [B][rows/32][m_pad]
   const float* inv_rowsum;          // [B][n_pad]
   const float* inv_colsum;          // [B][m_pad]
-  float* conf;                      // [B][N][M] or nullptr
+  float* conf;                      // [B][N][conf_ld] or nullptr; columns past frame b's L.m_of(b) are written as 0
+  int conf_ld;                      // columns of a conf row, >= L.M (0: L.M)
   unsigned long long* rowbest;      // [B][N]
   unsigned long long* colbest;      // [B][M]
 };

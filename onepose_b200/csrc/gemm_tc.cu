@@ -131,7 +131,8 @@ struct TcParams {
   const float* inv_rowsum;
   const float* inv_colsum;
   float* conf;
-  int conf_tma;          // 1: conf goes out through the 3-D tensor map (M % 4 == 0), 0: plain stores from the staged chunk
+  int conf_tma;          // 1: conf goes out through the 3-D tensor map (conf_ld % 4 == 0), 0: plain stores from the staged chunk
+  int conf_ld;           // columns of a conf row (GemmProblem::conf_ld)
   unsigned long long* rowbest;
   unsigned long long* colbest;
   // implicit-GEMM convolution (GemmProblem::taps) and the EPI_CONV geometry
@@ -610,7 +611,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
         // fixed shift  e = exp((cos - 1)/scale)  softmax(s,1)*softmax(s,2) = e^2 / (colsum*rowsum)  needs no running max.
         // Nothing is stored but the partial sums: row sums per (tile half, row) in registers; column sums over the warp's 32
         // rows by a transposing butterfly (31 shuffles per 32 x 32 block, no shared memory, no barriers).
-        const int Nz = p.L.n_of(z), M = p.L.M;
+        const int Nz = p.L.n_of(z), M = p.L.m_of(z);
         const int row = row0 + r_in_tile;                          // query index inside frame z
         const bool row_ok = row < Nz;
         const float ea = kProdInv * p.inv_scale * 1.4426950408889634f, eb = -p.inv_scale * 1.4426950408889634f;
@@ -645,7 +646,8 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
         // ---- dual-softmax tail, pass 2: conf = (e / rowsum) * (e / colsum) recomputed from the accumulator (the cos matrix is
         // never materialised), optional conf store, packed row / column arg-max (reference :218-220).  The 32-column chunk is
         // staged once in shared memory: it feeds the TMA store of conf and the per-column scan of the arg-max.
-        const int Nz = p.L.n_of(z), M = p.L.M;
+        // M: valid columns of frame z; conf rows are conf_ld wide (columns [M, conf_ld) hold 0), colbest rows L.M wide
+        const int Nz = p.L.n_of(z), M = p.L.m_of(z), ldm = p.conf_ld;
         const int row = row0 + r_in_tile;
         const bool row_ok = row < Nz;
         const float ea = kProdInv * p.inv_scale * 1.4426950408889634f, eb = -p.inv_scale * 1.4426950408889634f;
@@ -695,7 +697,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
           // column scan over the staged 128 x 32 chunk: thread (qq, cc) = rows [32 qq, +32) of column col0 + cc.  Fully unrolled
           // (invalid rows hold 0 and can never win): 32 independent shared-memory loads in flight instead of a latency chain.
           const int col = col0 + cc;
-          if (col < M) {
+          if (col < ldm) {                                          // columns >= M hold 0 and never win the column arg-max
             const int r_first = row0 + qq * 32;
             float cbest_v = 0.f;
             int cbest_r = -1;
@@ -706,13 +708,13 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
             for (int i = 0; i < 32; ++i)
               if (cv[i] > cbest_v) { cbest_v = cv[i]; cbest_r = r_first + i; }
             if (store_plain) {                                      // 32 consecutive columns of one row per warp instruction; rows
-              float* crow = p.conf + ((long long)z * p.L.N + r_first) * M + col;       // [Nz, N) of a ragged frame are written as 0
+              float* crow = p.conf + ((long long)z * p.L.N + r_first) * ldm + col;     // [Nz, N) of a ragged frame are written as 0
 #pragma unroll
-              for (int i = 0; i < 32; ++i, crow += M)    // a stepped pointer: offsets i * M would be hoisted out of the chunk
+              for (int i = 0; i < 32; ++i, crow += ldm)  // a stepped pointer: offsets i * M would be hoisted out of the chunk
                 if (r_first + i < p.L.N) *crow = cv[i];     // loop as 32 loop-invariant values and spilled
             }
             if (cbest_r >= 0)
-              atomicMax(p.colbest + (long long)z * M + col,
+              atomicMax(p.colbest + (long long)z * p.L.M + col,
                         ((unsigned long long)__float_as_uint(cbest_v) << 32) | (unsigned long long)(0xFFFFFFFFu - (unsigned)cbest_r));
           }
         }
@@ -941,6 +943,8 @@ int launch_gemm_tc(const GemmProblem& p, cudaStream_t stream) {
   if ((p.epi == EPI_QSCALE || p.epi == EPI_L2NORM) && !p.bias) return -1;
   const bool score = p.epi == EPI_SCORE_SUMS || p.epi == EPI_SCORE_CONF;
   int conf_tma = 0;
+  const int conf_ld = p.conf_ld ? p.conf_ld : p.L.M;
+  if (score && conf_ld < p.L.M) return -1;
   if (f32_out && (p.ldc % 4 || !p.c)) return -1;
   const long long a_rows = (long long)(p.batch - 1) * p.a_batch_rows + p.rows;
   const long long b1_rows = (long long)(p.batch - 1) * p.b_batch_rows + p.n_out;
@@ -971,8 +975,8 @@ int launch_gemm_tc(const GemmProblem& p, cudaStream_t stream) {
     mp.out_lo = mp.out_hi;
   } else if (score) {
     mp.out_f32 = mp.b1h; mp.out_hi = mp.b1h; mp.out_lo = mp.b1h;
-    if (p.epi == EPI_SCORE_CONF && p.conf && p.L.M % 4 == 0 && (reinterpret_cast<uintptr_t>(p.conf) & 15) == 0)
-      conf_tma = make_map3(&mp.out_f32, p.conf, p.L.M, p.L.N, p.batch) ? 1 : 0;
+    if (p.epi == EPI_SCORE_CONF && p.conf && conf_ld % 4 == 0 && (reinterpret_cast<uintptr_t>(p.conf) & 15) == 0)
+      conf_tma = make_map3(&mp.out_f32, p.conf, conf_ld, p.L.N, p.batch) ? 1 : 0;
   } else {
     ok = ok && make_map(&mp.out_hi, p.out.hi, out_rows, p.n_out, p.out.ld, 32, BM, false) && make_map(&mp.out_lo, p.out.lo, out_rows, p.n_out, p.out.ld, 32, BM, false);
     mp.out_f32 = mp.out_hi;
@@ -990,7 +994,7 @@ int launch_gemm_tc(const GemmProblem& p, cudaStream_t stream) {
   tp.seg_rows = (p.batch == 1 && p.L.R > 0 && p.L.rows() == p.rows) ? 1 : 0;
   tp.L = p.L; tp.bias = p.bias;
   tp.inv_scale = p.inv_scale; tp.rowsum_part = p.rowsum_part; tp.colsum_part = p.colsum_part; tp.inv_rowsum = p.inv_rowsum;
-  tp.inv_colsum = p.inv_colsum; tp.conf = p.conf; tp.conf_tma = conf_tma; tp.rowbest = p.rowbest; tp.colbest = p.colbest;
+  tp.inv_colsum = p.inv_colsum; tp.conf = p.conf; tp.conf_tma = conf_tma; tp.conf_ld = conf_ld; tp.rowbest = p.rowbest; tp.colbest = p.colbest;
   tp.mu = p.mu; tp.rstd = p.rstd;
   tp.kmean = p.kmean; tp.cross = p.cross; tp.statpart = p.statpart;
   if ((p.epi == EPI_QSCALE || p.b2_per_seg || p.epi == EPI_QKV || p.epi == EPI_F32_STATS || p.a_conv) && !tp.seg_rows) return -1;

@@ -51,16 +51,54 @@ __global__ void transpose_cf_to_rows(const float* __restrict__ in, int n, int n_
   }
 }
 
+// Per-chunk object table: which object each frame of the chunk matches against.  The host builds it for every chunk and
+// hands it to assemble_layout BY VALUE (no host synchronisation, no staging buffer that a later call could overwrite while
+// this one is in flight); assemble_layout also copies it into the workspace, where the later kernels of the chunk read it.
+constexpr int kMaxChunkFrames = 64;
+constexpr int kGatsFramesPerWarp = 16;   // leaf rows re-read once per 16 frames (8: 229 MB of leaf traffic per layer at B = 32, 16: 115 MB)
+struct FrameObject {
+  const __half* hi;       // the object's 3D rows [m_pad_obj, 256]: prologue state (hoisting) or raw db planes
+  const __half* lo;
+  const float* leaves;    // fp32 [M_b * L, 256] point-major
+  const float* s2;        // [4][M_b * L] leaf logits of the 4 GATs layers
+};
+struct ChunkTable {
+  FrameObject obj[kMaxChunkFrames];
+  int mlen[kMaxChunkFrames];              // M_b: valid 3D rows of frame b (= Layout::mlen)
+};
+// GATs groups of a chunk for gats_aggregate_frames8, passed BY VALUE (read from the constant bank, no dependent global loads
+// before the leaf rows): group g = frames [b_begin, b_end), a run of consecutive frames of one object, at most
+// kGatsFramesPerWarp long.
+struct GatsGroup {
+  const float* leaves;    // the object's leaves [M * 8, 256]
+  const float* s2;        // its leaf logits [4][M * 8]
+  int b_begin, b_end, M, pad;
+};
+struct GatsGroups {
+  GatsGroup g[kMaxChunkFrames];
+  int n;
+};
+
 // Assemble the activation layout of a chunk: frame b's query segment from the compact query buffer xq [B*n_pad, 256] and its
-// 3D-point segment from the per-object rows (object prologue or raw db planes).  One launch, 16-byte vectors.
+// 3D-point segment from its object's rows tab.obj[b] (rows [M_b, m_pad) are written as zero).  Block (0, 0) also stores the
+// table at tab_out.  One launch, 16-byte vectors.
 // grid (blocks, B)
-__global__ void assemble_layout(const __half* __restrict__ q_hi, const __half* __restrict__ q_lo, const __half* __restrict__ o_hi,
-                                const __half* __restrict__ o_lo, __half* __restrict__ x_hi, __half* __restrict__ x_lo, Layout L) {
+__global__ void assemble_layout(const __half* __restrict__ q_hi, const __half* __restrict__ q_lo, const __grid_constant__ ChunkTable tab,
+                                ChunkTable* __restrict__ tab_out, __half* __restrict__ x_hi, __half* __restrict__ x_lo, Layout L) {
   griddep_sync();
+  if (blockIdx.x == 0 && blockIdx.y == 0) {
+    const int* src = reinterpret_cast<const int*>(&tab);
+    int* dst = reinterpret_cast<int*>(tab_out);
+    for (int k = threadIdx.x; k < (int)(sizeof(ChunkTable) / sizeof(int)); k += blockDim.x) dst[k] = src[k];
+  }
+  const int b = blockIdx.y;
   const long long nq = q_hi ? (long long)L.n_pad * kD / 8 : 0;  // uint4 = 8 halves
   const long long nd = (long long)L.m_pad * kD / 8;
-  const long long dst0 = (long long)blockIdx.y * L.R * kD / 8;
-  const long long src_q0 = (long long)blockIdx.y * nq;
+  const long long nvalid = (long long)tab.mlen[b] * kD / 8;
+  const uint4* o_hi = reinterpret_cast<const uint4*>(tab.obj[b].hi);
+  const uint4* o_lo = reinterpret_cast<const uint4*>(tab.obj[b].lo);
+  const long long dst0 = (long long)b * L.R * kD / 8;
+  const long long src_q0 = (long long)b * nq;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < nq + nd; i += (long long)gridDim.x * blockDim.x) {
     if (i < nq) {
       reinterpret_cast<uint4*>(x_hi)[dst0 + i] = reinterpret_cast<const uint4*>(q_hi)[src_q0 + i];
@@ -68,8 +106,9 @@ __global__ void assemble_layout(const __half* __restrict__ q_hi, const __half* _
     } else {
       const long long j = i - nq;
       const long long d = dst0 + (long long)L.n_pad * kD / 8 + j;
-      reinterpret_cast<uint4*>(x_hi)[d] = reinterpret_cast<const uint4*>(o_hi)[j];
-      reinterpret_cast<uint4*>(x_lo)[d] = reinterpret_cast<const uint4*>(o_lo)[j];
+      const uint4 z = make_uint4(0u, 0u, 0u, 0u);
+      reinterpret_cast<uint4*>(x_hi)[d] = j < nvalid ? o_hi[j] : z;
+      reinterpret_cast<uint4*>(x_lo)[d] = j < nvalid ? o_lo[j] : z;
     }
   }
 }
@@ -154,10 +193,8 @@ __device__ __forceinline__ void gats_read_h3(const __half* x_hi, const __half* x
 }
 
 // Generic leaf count: warp per (point, frame); frames of one point are adjacent warps so the leaf rows are served from
-// L1/L2 after the first frame.
-__global__ void gats_aggregate(const __half* x_hi, const __half* x_lo, Layout L,
-                               const float* __restrict__ leaves, int n_leaf,
-                               const float* __restrict__ s2 /*[M*n_leaf] this layer*/,
+// L1/L2 after the first frame.  Frame b reads the leaves and the layer-`gi` leaf logits of its own object (tab->obj[b]).
+__global__ void gats_aggregate(const __half* x_hi, const __half* x_lo, Layout L, const ChunkTable* __restrict__ tab, int n_leaf, int gi,
                                const float* __restrict__ wa3 /*[256]*/, int include_self, int additional,
                                float alpha, GatsOut out) {
   griddep_sync();
@@ -167,6 +204,10 @@ __global__ void gats_aggregate(const __half* x_hi, const __half* x_lo, Layout L,
   if (warp >= total) return;
   const int b = (int)(warp % L.B);
   const int i = (int)(warp / L.B);
+  const int Mb = tab->mlen[b];
+  if (i >= Mb) return;
+  const float* __restrict__ leaves = tab->obj[b].leaves;
+  const float* __restrict__ s2 = tab->obj[b].s2 + (long long)gi * Mb * n_leaf;
   const long long row = (long long)b * L.R + L.n_pad + i;
   float h3[8];
   gats_read_h3(x_hi, x_lo, row, lane, h3);
@@ -212,21 +253,24 @@ __global__ void gats_aggregate(const __half* x_hi, const __half* x_lo, Layout L,
   gats_write_row(out, out.lin ? (long long)b * L.m_pad + i : row, lane, acc, h3, include_self, additional);
 }
 
-// Same layer, warp per (POINT, group of 8 frames): the point's 8 leaf rows and leaf logits are read once into registers and
-// reused for every frame of the group (the leaves are per-object constants; reference GATs.py:46 reshapes the same tensor for
-// every batch element).  Fast path for num_leaf == 8 (the released configuration, test_GATsSPG.yaml:5).
-constexpr int kGatsFramesPerWarp = 16;   // leaf rows re-read once per 16 frames (8: 229 MB of leaf traffic per layer at B = 32, 16: 115 MB)
+// Same layer, warp per (POINT, group of up to 16 consecutive frames of one object): the point's 8 leaf rows and leaf logits are
+// read once into registers and reused for every frame of the group (the leaves are per-object constants; reference GATs.py:46
+// reshapes the same tensor for every batch element).  Fast path for
+// num_leaf == 8 (the released configuration, test_GATsSPG.yaml:5).
 __global__ void __launch_bounds__(256, 2) gats_aggregate_frames8(const __half* x_hi, const __half* x_lo, Layout L,
-                                                              const float* __restrict__ leaves, const float* __restrict__ s2,
+                                                              const __grid_constant__ GatsGroups grp, int gi,
                                                               const float* __restrict__ wa3, int include_self, int additional, float alpha,
                                                               GatsOut out) {
   griddep_sync();
   const int lane = threadIdx.x & 31;
   const long long wid = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int n_groups = (L.B + kGatsFramesPerWarp - 1) / kGatsFramesPerWarp;   // frame groups: more warps in flight than points alone
+  const int n_groups = grp.n;                         // frame groups: more warps in flight than points alone
   const int i = (int)(wid / n_groups), fg = (int)(wid % n_groups);
-  if (i >= L.M) return;
-  const int b_begin = fg * kGatsFramesPerWarp, b_end = min(L.B, b_begin + kGatsFramesPerWarp);
+  const GatsGroup& G = grp.g[fg];
+  if (i >= G.M) return;
+  const int b_begin = G.b_begin, b_end = G.b_end;
+  const float* __restrict__ leaves = G.leaves;
+  const float* __restrict__ s2 = G.s2 + (long long)gi * G.M * 8;
   float4 lu[8], lv[8];
 #pragma unroll
   for (int c = 0; c < 8; ++c) {
@@ -308,6 +352,7 @@ __global__ void gats_lin_finish(const __half* __restrict__ t_hi, const __half* _
   const int c8 = (int)(idx & 31);
   const long long pr = idx >> 5;
   const int b = (int)(pr / L.M), i = (int)(pr % L.M);
+  if (i >= L.m_of(b)) return;                                              // pad rows of a smaller object stay zero
   const long long src = ((long long)b * L.m_pad + i) * kD + c8 * 8, dst = ((long long)b * L.R + L.n_pad + i) * kD + c8 * 8;
   const uint4 th = *reinterpret_cast<const uint4*>(t_hi + src), tlw = *reinterpret_cast<const uint4*>(t_lo + src);
   uint4 xh = *reinterpret_cast<const uint4*>(x_hi + dst), xl = *reinterpret_cast<const uint4*>(x_lo + dst);
@@ -452,28 +497,30 @@ __global__ void score_sums_finalize(const float* __restrict__ rowsum_part, const
     if (i < L.N) rowbest[(long long)b * L.N + i] = 0ull;
   } else if (i - L.n_pad < L.m_pad) {
     const int m = i - L.n_pad;
+    const int Mb = L.m_of(b);
     const int qv = (Nb + 31) / 32;                      // quarters that hold valid query rows
     float s = 0.f;
-    if (m < L.M)
+    if (m < Mb)
       for (int t = 0; t < qv && t < q_groups; ++t) s += colsum_part[((long long)b * q_groups + t) * L.m_pad + m];
-    inv_colsum[b * L.m_pad + m] = (m < L.M && qv > 0) ? 1.f / s : 0.f;
-    if (m < L.M) colbest[(long long)b * L.M + m] = 0ull;
+    inv_colsum[b * L.m_pad + m] = (m < Mb && qv > 0) ? 1.f / s : 0.f;
+    if (m < Mb) colbest[(long long)b * L.M + m] = 0ull;
   }
 }
 
 // Mutual nearest neighbour + threshold (reference GATs_SuperGlue.py:220-230).  rowbest / colbest hold packed
 // (conf bits << 32 | ~index): order-preserving for conf >= 0 with lowest-index-wins ties (torch.max returns the first maximum).
-// A frame with no valid query rows (ragged batch) or a raised range flag yields -1 / 0 everywhere.
+// A frame with no valid query rows (ragged batch) or a raised range flag yields -1 / 0 everywhere.  m1 / sc1 rows are
+// m_out >= L.M wide; columns past the frame's own M_b are -1 / 0.
 // One block per frame is plenty (N+M <= ~20k); grid (B), block 256.
 __global__ void mutual_match(const unsigned long long* __restrict__ rowbest, const unsigned long long* __restrict__ colbest, Layout L,
-                             float thr, const int* __restrict__ range_flag, long long* __restrict__ m0, long long* __restrict__ m1,
+                             float thr, const int* __restrict__ range_flag, int m_out, long long* __restrict__ m0, long long* __restrict__ m1,
                              float* __restrict__ sc0, float* __restrict__ sc1) {
   griddep_sync();
   const int b = blockIdx.x;
-  const int N = L.N, M = L.M, Nb = L.n_of(b);
+  const int N = L.N, M = L.m_of(b), Nb = L.n_of(b);
   const bool poisoned = *range_flag != 0 || Nb == 0;
   const unsigned long long* rb = rowbest + (long long)b * N;
-  const unsigned long long* cb = colbest + (long long)b * M;
+  const unsigned long long* cb = colbest + (long long)b * L.M;
   auto idx_of = [](unsigned long long p) { return (int)(0xFFFFFFFFu - (unsigned)(p & 0xFFFFFFFFull)); };
   auto val_of = [](unsigned long long p) { return __uint_as_float((unsigned)(p >> 32)); };
   for (int n = threadIdx.x; n < N; n += blockDim.x) {
@@ -488,10 +535,10 @@ __global__ void mutual_match(const unsigned long long* __restrict__ rowbest, con
     m0[(long long)b * N + n] = mm;
     sc0[(long long)b * N + n] = ms;
   }
-  for (int m = threadIdx.x; m < M; m += blockDim.x) {
+  for (int m = threadIdx.x; m < m_out; m += blockDim.x) {
     long long mm = -1ll;
     float ms1 = 0.f;
-    if (!poisoned) {
+    if (!poisoned && m < M) {
       const int i1 = idx_of(cb[m]);
       const int i0 = i1 >= 0 ? idx_of(rb[i1]) : -1;
       const bool mutual1 = i0 == m;
@@ -502,12 +549,20 @@ __global__ void mutual_match(const unsigned long long* __restrict__ rowbest, con
       ms1 = mutual1 ? ms0_i1 : 0.f;
       if (mutual1 && valid0_i1) mm = i1;
     }
-    m1[(long long)b * M + m] = mm;
-    sc1[(long long)b * M + m] = ms1;
+    m1[(long long)b * m_out + m] = mm;
+    sc1[(long long)b * m_out + m] = ms1;
   }
 }
 
 // conf rows of a poisoned call / of frames without valid queries are not touched here: pass 2 writes every element of conf.
+// ... up to the chunk's m_pad: when the conf rows are wider (a call whose largest object is in another chunk), this kernel
+// zeroes columns [c0, ld) of every row.  Grid-stride, block 256
+__global__ void conf_fill_tail(float* __restrict__ conf, long long rows, int ld, int c0) {
+  griddep_sync();
+  const int w = ld - c0;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < rows * w; i += (long long)gridDim.x * blockDim.x)
+    conf[(i / w) * ld + c0 + i % w] = 0.f;
+}
 
 // ---------------------------------------------------------------------------------------
 // Adjacent producers (offline feature files of an object, reference src/sfm/postprocess/feature_process.py:297-317 and

@@ -428,13 +428,18 @@ __global__ void __launch_bounds__(kRefineThreads) pnp_select_refine(const double
 // ---- matched pairs -> the ragged correspondence lists above (reference inference.py:147-152: valid = matches > -1;
 // mkpts2d = kpts2d[valid]; mkpts3d = kpts3d[matches[valid]]).  Three launches, no workspace: per-frame counts into
 // offsets[1..B], an in-place scan of offsets, then a per-frame ordered compaction (ascending n, numpy boolean-mask order).
+// Frames of different objects: frame b's 3D key points are rows [kp3_first[b], kp3_first[b] + kp3_count[b]) of the concatenated
+// keypoints3d; kp3_first == nullptr: one object of M rows for every frame.
 constexpr int kGatherThreads = 256;
 
 __device__ __forceinline__ bool is_match(int64_t m, int M) { return m >= 0 && m < (int64_t)M; }
+__device__ __forceinline__ int frame_kp3_count(const int* kp3_count, int b, int M) { return kp3_count ? kp3_count[b] : M; }
 
-__global__ void __launch_bounds__(kGatherThreads) gather_count(const int64_t* __restrict__ matches0, int N, int M, int* __restrict__ offsets) {
+__global__ void __launch_bounds__(kGatherThreads) gather_count(const int64_t* __restrict__ matches0, int N, int M_all,
+                                                               const int* __restrict__ kp3_count, int* __restrict__ offsets) {
   __shared__ int cnt_w[kGatherThreads / 32];
   const int b = blockIdx.x, tid = threadIdx.x;
+  const int M = frame_kp3_count(kp3_count, b, M_all);
   const int64_t* m0 = matches0 + (size_t)b * N;
   int cnt = 0;
   for (int n = tid; n < N; n += kGatherThreads) cnt += is_match(m0[n], M) ? 1 : 0;
@@ -485,11 +490,14 @@ __global__ void __launch_bounds__(kScanThreads) gather_scan(int B, int* __restri
 
 // one block per frame: ordered compaction over tiles of kGatherThreads entries; keypoints2d rows are read for matches only
 __global__ void __launch_bounds__(kGatherThreads) gather_compact(const int64_t* __restrict__ matches0, const float* __restrict__ mscores0,
-                                                                 const float* __restrict__ kp2d, const float* __restrict__ kp3d, int N, int M,
+                                                                 const float* __restrict__ kp2d, const float* __restrict__ kp3d_all, int N, int M_all,
+                                                                 const int* __restrict__ kp3_first, const int* __restrict__ kp3_count,
                                                                  const int* __restrict__ offsets, double* __restrict__ pts2d, double* __restrict__ pts3d,
                                                                  float* __restrict__ mconf, int* __restrict__ query_index) {
   __shared__ int warp_cnt[kGatherThreads / 32];
   const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const int M = frame_kp3_count(kp3_count, b, M_all);
+  const float* kp3d = kp3d_all + (kp3_first ? (size_t)kp3_first[b] * 3 : 0);
   const size_t row0 = (size_t)b * N;
   int pos = offsets[b];
   for (int base = 0; base < N; base += kGatherThreads) {
@@ -526,10 +534,10 @@ __global__ void __launch_bounds__(kGatherThreads) gather_compact(const int64_t* 
 }  // namespace
 }  // namespace opb
 
-extern "C" int opb_gather_matches(const int64_t* matches0, const float* mscores0, const float* keypoints2d, const float* keypoints3d,
-                                  int32_t B, int32_t N, int32_t M, double* pts2d, double* pts3d, float* mconf, int32_t* query_index,
-                                  int32_t* offsets, void* stream) {
-  if (B <= 0 || N < 0 || M <= 0 || !keypoints3d || !offsets || (int64_t)B * N > (int64_t)INT32_MAX) return OPB_E_INVALID;
+// The gather of both entry points: kp3_first / kp3_count == nullptr means one object of M key points for every frame.
+static int gather_matches_impl(const int64_t* matches0, const float* mscores0, const float* keypoints2d, const float* keypoints3d, int32_t B,
+                               int32_t N, int32_t M, const int32_t* kp3_first, const int32_t* kp3_count, double* pts2d, double* pts3d,
+                               float* mconf, int32_t* query_index, int32_t* offsets, void* stream) {
   if (N > 0 && (!matches0 || !keypoints2d || !pts2d || !pts3d)) return OPB_E_INVALID;
   if (mconf && !mscores0) return OPB_E_INVALID;
   cudaStream_t st = (cudaStream_t)stream;
@@ -537,11 +545,27 @@ extern "C" int opb_gather_matches(const int64_t* matches0, const float* mscores0
     if (cudaMemsetAsync(offsets, 0, sizeof(int32_t) * ((size_t)B + 1), st) != cudaSuccess) return OPB_E_CUDA;
     return OPB_OK;
   }
-  opb::gather_count<<<(unsigned)B, opb::kGatherThreads, 0, st>>>(matches0, N, M, offsets);
+  opb::gather_count<<<(unsigned)B, opb::kGatherThreads, 0, st>>>(matches0, N, M, kp3_count, offsets);
   opb::gather_scan<<<1, opb::kScanThreads, 0, st>>>(B, offsets);
-  opb::gather_compact<<<(unsigned)B, opb::kGatherThreads, 0, st>>>(matches0, mscores0, keypoints2d, keypoints3d, N, M, offsets, pts2d, pts3d,
-                                                                   mconf, query_index);
+  opb::gather_compact<<<(unsigned)B, opb::kGatherThreads, 0, st>>>(matches0, mscores0, keypoints2d, keypoints3d, N, M, kp3_first, kp3_count, offsets,
+                                                                   pts2d, pts3d, mconf, query_index);
   return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_E_CUDA;
+}
+
+extern "C" int opb_gather_matches(const int64_t* matches0, const float* mscores0, const float* keypoints2d, const float* keypoints3d,
+                                  int32_t B, int32_t N, int32_t M, double* pts2d, double* pts3d, float* mconf, int32_t* query_index,
+                                  int32_t* offsets, void* stream) {
+  if (B <= 0 || N < 0 || M <= 0 || !keypoints3d || !offsets || (int64_t)B * N > (int64_t)INT32_MAX) return OPB_E_INVALID;
+  return gather_matches_impl(matches0, mscores0, keypoints2d, keypoints3d, B, N, M, nullptr, nullptr, pts2d, pts3d, mconf, query_index, offsets,
+                             stream);
+}
+
+extern "C" int opb_gather_matches_objects(const int64_t* matches0, const float* mscores0, const float* keypoints2d, const float* keypoints3d,
+                                          const int32_t* kp3_first, const int32_t* kp3_count, int32_t B, int32_t N, double* pts2d, double* pts3d,
+                                          float* mconf, int32_t* query_index, int32_t* offsets, void* stream) {
+  if (B <= 0 || N < 0 || !keypoints3d || !kp3_first || !kp3_count || !offsets || (int64_t)B * N > (int64_t)INT32_MAX) return OPB_E_INVALID;
+  return gather_matches_impl(matches0, mscores0, keypoints2d, keypoints3d, B, N, 0, kp3_first, kp3_count, pts2d, pts3d, mconf, query_index, offsets,
+                             stream);
 }
 
 extern "C" int opb_ransac_pnp(const double* K, const double* pts2d, const double* pts3d, const int32_t* offsets, int32_t B, int32_t hypotheses,

@@ -111,6 +111,7 @@ class GATsSuperGlue(nn.Module):
         self._obj_copy = None          # private copy of the packed object (exact comparison on a key miss)
         self._chunk_frames = 0
         self._hoist = True
+        self._objects = {}             # registered object id -> M (add_object)
         self.last_batched = None       # batched outputs of the last forward (all B frames)
 
     # ------------------------------------------------------------------ handle / weights
@@ -135,6 +136,7 @@ class GATsSuperGlue(nn.Module):
         _lib.check(self._lib.opb_create(C.byref(cfg), C.byref(h)))
         self._handle, self._handle_device = h, device
         self._weights_key = self._obj_key = self._obj_ref = self._obj_copy = self._M = None
+        self._objects = {}             # registrations live on the handle
         if self._chunk_frames:
             _lib.check(self._lib.opb_set_chunk_frames(self._handle, self._chunk_frames), self._handle)
         if not self._hoist:
@@ -159,9 +161,9 @@ class GATsSuperGlue(nn.Module):
 
     def set_chunk_frames(self, frames: int):
         """Frames pushed through the GNN together (workspace-size knob of the C ABI)."""
-        self._chunk_frames = int(frames)
         if self._handle is not None:
-            _lib.check(self._lib.opb_set_chunk_frames(self._handle, self._chunk_frames), self._handle)
+            _lib.check(self._lib.opb_set_chunk_frames(self._handle, int(frames)), self._handle)
+        self._chunk_frames = int(frames)
 
     # ------------------------------------------------------------------ fast API
     def set_object(self, descriptors3d_db: torch.Tensor, descriptors2d_db: torch.Tensor, reserve=None):
@@ -219,6 +221,79 @@ class GATsSuperGlue(nn.Module):
         _lib.check(self._lib.opb_forward(self._handle, q.data_ptr(), lengths.data_ptr() if lengths is not None else None, B, N,
                                          m0.data_ptr(), m1.data_ptr(), s0.data_ptr(), s1.data_ptr(),
                                          conf.data_ptr() if conf is not None else None, st), self._handle)
+        return {"matches0": m0, "matches1": m1, "matching_scores0": s0, "matching_scores1": s1, "conf_matrix": conf}
+
+    # ------------------------------------------------------------------ several objects per call
+    def add_object(self, descriptors3d_db: torch.Tensor, descriptors2d_db: torch.Tensor) -> int:
+        """Register an object (descriptors3d_db [256, M], descriptors2d_db [256, M*L], CUDA fp32) next to the current one and
+        return its id for match_objects.  Its frame-invariant GNN layers run on its first use; reloading the weights keeps it."""
+        d3 = descriptors3d_db.float().contiguous()
+        d2 = descriptors2d_db.float().contiguous()
+        if not d3.is_cuda:
+            raise RuntimeError("onepose_b200 has no CPU path: tensors must be on a CUDA device")
+        self._ensure_handle(d3.device)
+        self._sync_weights()
+        M = d3.shape[1]
+        if M == 0 or d2.shape[1] % M:
+            raise ValueError(f"descriptors2d_db has {d2.shape[1]} columns, not a multiple of M={M}")
+        st = torch.cuda.current_stream(d3.device).cuda_stream
+        oid = C.c_int32()
+        _lib.check(self._lib.opb_add_object(self._handle, d3.data_ptr(), d2.data_ptr(), M, d2.shape[1] // M, st, C.byref(oid)),
+                   self._handle)
+        self._objects[oid.value] = M
+        return oid.value
+
+    def remove_object(self, object_id: int):
+        """Forget a registered object (waits for the calls in flight that may use it)."""
+        if self._handle is None:
+            raise ValueError(f"unknown object id {object_id}")
+        _lib.check(self._lib.opb_remove_object(self._handle, int(object_id)), self._handle)
+        self._objects.pop(int(object_id), None)
+
+    def match_objects(self, descriptors2d_query: torch.Tensor, object_ids, return_conf: bool = True, lengths: torch.Tensor | None = None,
+                      out: dict | None = None):
+        """B frames of registered objects in one call: frame b matches against object object_ids[b] (a host sequence of ids, or a
+        CPU tensor; objects of one call share L).  descriptors2d_query [B, 256, N] CUDA fp32, lengths and out as in match_frames.
+        Returns the batched dict of match_frames with the M-wide outputs (matches1, matching_scores1, conf_matrix) padded to the
+        largest M of the call -- or, when out["matches1"] is a 2-D [B', M_out] buffer, to its width M_out (fixed-width rows across
+        calls; M_out must cover the call's largest M).  Columns past frame b's own M are -1 / 0 / 0.  Other out buffers are flat
+        storage as in match_frames.  Asynchronous: no host synchronisation."""
+        if self._handle is None:
+            raise RuntimeError("no object registered: call add_object first")
+        self._sync_weights()
+        ids = [int(i) for i in (object_ids.tolist() if isinstance(object_ids, torch.Tensor) else object_ids)]
+        q = descriptors2d_query.float().contiguous()
+        B, _, N = q.shape
+        if len(ids) != B:
+            raise ValueError(f"object_ids has {len(ids)} entries for {B} frames")
+        for i in ids:
+            if i not in self._objects:
+                raise ValueError(f"unknown object id {i}")
+        M = max(self._objects[i] for i in ids)
+        if out is not None and "matches1" in out and out["matches1"].dim() == 2:
+            if out["matches1"].shape[1] < M:
+                raise ValueError(f"out['matches1'] is {out['matches1'].shape[1]} wide, below the call's largest M = {M}")
+            M = int(out["matches1"].shape[1])
+        dev = q.device
+
+        def buf(name, shape, dtype):
+            return _out_view(out, name, shape, dtype, dev)
+
+        m0 = buf("matches0", (B, N), torch.int64)
+        m1 = buf("matches1", (B, M), torch.int64)
+        s0 = buf("matching_scores0", (B, N), torch.float32)
+        s1 = buf("matching_scores1", (B, M), torch.float32)
+        conf = buf("conf_matrix", (B, N, M), torch.float32) if return_conf else None
+        if lengths is not None:
+            lengths = lengths.to(device=dev, dtype=torch.int32).contiguous()
+            if lengths.numel() != B:
+                raise ValueError("lengths must have one entry per frame")
+        ids_host = (C.c_int32 * B)(*ids)
+        st = torch.cuda.current_stream(dev).cuda_stream
+        _lib.check(self._lib.opb_poll_range(self._handle), self._handle)
+        _lib.check(self._lib.opb_forward_objects(self._handle, ids_host, q.data_ptr(), lengths.data_ptr() if lengths is not None else None,
+                                                 B, N, M, m0.data_ptr(), m1.data_ptr(), s0.data_ptr(), s1.data_ptr(),
+                                                 conf.data_ptr() if conf is not None else None, st), self._handle)
         return {"matches0": m0, "matches1": m1, "matching_scores0": s0, "matching_scores1": s1, "conf_matrix": conf}
 
     def match_frames_host(self, q_host: torch.Tensor, out: dict | None = None, lengths: torch.Tensor | None = None,

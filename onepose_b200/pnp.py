@@ -86,18 +86,56 @@ def gather_matches(matches0: torch.Tensor, keypoints2d: torch.Tensor, keypoints3
     return out
 
 
-def poses_from_matches(K: torch.Tensor, keypoints2d: torch.Tensor, keypoints3d: torch.Tensor, matches0: torch.Tensor,
-                       matching_scores0: torch.Tensor | None = None, reproj_error: float = 5.0, scale: float = 1000.0,
-                       hypotheses: int = DEFAULT_HYPOTHESES, seed: int = 0):
-    """Object pose of B frames from the matcher's output: ``gather_matches`` then ``ransac_pnp_batch``, all on the device and with
-    no host synchronisation (inference.py:147-155 for a batch).  K [3,3] (shared) or [B,3,3]; the other arguments as in
-    ``gather_matches``.  ``scale`` multiplies the 3D points before the solve and divides the translation after it, as
-    ``ransac_PnP(..., scale=1000)`` does in the reference.  A frame with fewer than 4 pairs, or no model, gets the identity pose
-    and 0 inliers.  Returns a dict: pose [B,3,4] and pose_homo [B,4,4] f64, n_inliers int32 [B], inlier_mask bool [B*N],
-    query_index, mconf and offsets (rows indexed as in ``gather_matches``)."""
-    g = gather_matches(matches0, keypoints2d, keypoints3d, matching_scores0)
-    B = int(matches0.shape[0])
+def gather_matches_objects(matches0: torch.Tensor, keypoints2d: torch.Tensor, keypoints3d, object_ids,
+                           matching_scores0: torch.Tensor | None = None):
+    """``gather_matches`` for frames of different objects (``GATsSuperGlue.match_objects``' output): frame b's matches index the
+    3D key points ``keypoints3d[object_ids[b]]`` (fp32 [M_b, 3] CUDA tensors; ``keypoints3d`` maps object id -> tensor, a dict
+    or a sequence indexed by id), an entry outside [0, M_b) is not a match.  ``object_ids`` is a host sequence (or CPU tensor).
+    Same outputs as ``gather_matches``.  The per-frame tables go to the device from pinned memory: no host synchronisation."""
+    lib = _lib.load()
     dev = matches0.device
+    if dev.type != "cuda":
+        raise RuntimeError("onepose_b200 has no CPU path: tensors must be on a CUDA device")
+    if matches0.dim() != 2:
+        raise ValueError("matches0 must be [B, N]")
+    B, N = matches0.shape
+    ids = [int(i) for i in (object_ids.tolist() if isinstance(object_ids, torch.Tensor) else object_ids)]
+    if len(ids) != B:
+        raise ValueError(f"object_ids has {len(ids)} entries for {B} frames")
+    first, parts, row = {}, [], 0                       # each object's key points once, in order of first appearance
+    for i in ids:
+        if i not in first:
+            k = keypoints3d[i].to(device=dev, dtype=torch.float32)
+            if k.dim() != 2 or k.shape[1] != 3 or k.shape[0] == 0:
+                raise ValueError(f"keypoints3d[{i}] must be [M, 3] with M > 0, got {tuple(k.shape)}")
+            first[i] = (row, int(k.shape[0]))
+            parts.append(k)
+            row += int(k.shape[0])
+    kp3 = torch.cat(parts, 0).contiguous()
+    tab = torch.tensor([first[i][0] for i in ids] + [first[i][1] for i in ids], dtype=torch.int32).pin_memory()
+    tab = tab.to(dev, non_blocking=True)
+    m0 = matches0.to(torch.int64).contiguous()
+    kp2 = keypoints2d.to(device=dev, dtype=torch.float32).contiguous()
+    if tuple(kp2.shape) != (B, N, 2):
+        raise ValueError(f"keypoints2d must be [B, N, 2] = {(B, N, 2)}, got {tuple(kp2.shape)}")
+    sc = None
+    if matching_scores0 is not None:
+        sc = matching_scores0.to(device=dev, dtype=torch.float32).contiguous()
+        if tuple(sc.shape) != (B, N):
+            raise ValueError("matching_scores0 must be [B, N] like matches0")
+    out = {"pts2d": torch.empty(B * N, 2, dtype=torch.float64, device=dev), "pts3d": torch.empty(B * N, 3, dtype=torch.float64, device=dev),
+           "mconf": torch.empty(B * N, dtype=torch.float32, device=dev) if sc is not None else None,
+           "query_index": torch.empty(B * N, dtype=torch.int32, device=dev), "offsets": torch.empty(B + 1, dtype=torch.int32, device=dev)}
+    st = torch.cuda.current_stream(dev).cuda_stream
+    with torch.cuda.device(dev):
+        _lib.check(lib.opb_gather_matches_objects(m0.data_ptr(), sc.data_ptr() if sc is not None else None, kp2.data_ptr(), kp3.data_ptr(),
+                                                  tab.data_ptr(), tab[B:].data_ptr(), B, N, out["pts2d"].data_ptr(), out["pts3d"].data_ptr(),
+                                                  out["mconf"].data_ptr() if sc is not None else None, out["query_index"].data_ptr(),
+                                                  out["offsets"].data_ptr(), st))
+    return out
+
+
+def _solve(K, g, B, dev, reproj_error, scale, hypotheses, seed):
     K = K.to(device=dev, dtype=torch.float64)
     if K.dim() == 2:
         K = K.expand(B, 3, 3)
@@ -109,6 +147,28 @@ def poses_from_matches(K: torch.Tensor, keypoints2d: torch.Tensor, keypoints3d: 
     pose_homo[:, 3, 3] = 1.0
     return {"pose": pose, "pose_homo": pose_homo, "n_inliers": cnt, "inlier_mask": mask, "query_index": g["query_index"],
             "mconf": g["mconf"], "offsets": g["offsets"]}
+
+
+def poses_from_matches_objects(K: torch.Tensor, keypoints2d: torch.Tensor, keypoints3d, object_ids, matches0: torch.Tensor,
+                               matching_scores0: torch.Tensor | None = None, reproj_error: float = 5.0, scale: float = 1000.0,
+                               hypotheses: int = DEFAULT_HYPOTHESES, seed: int = 0):
+    """``poses_from_matches`` for frames of different objects: ``gather_matches_objects`` then ``ransac_pnp_batch``; same
+    arguments and outputs, with ``keypoints3d`` / ``object_ids`` as in ``gather_matches_objects``.  No host synchronisation."""
+    g = gather_matches_objects(matches0, keypoints2d, keypoints3d, object_ids, matching_scores0)
+    return _solve(K, g, int(matches0.shape[0]), matches0.device, reproj_error, scale, hypotheses, seed)
+
+
+def poses_from_matches(K: torch.Tensor, keypoints2d: torch.Tensor, keypoints3d: torch.Tensor, matches0: torch.Tensor,
+                       matching_scores0: torch.Tensor | None = None, reproj_error: float = 5.0, scale: float = 1000.0,
+                       hypotheses: int = DEFAULT_HYPOTHESES, seed: int = 0):
+    """Object pose of B frames from the matcher's output: ``gather_matches`` then ``ransac_pnp_batch``, all on the device and with
+    no host synchronisation (inference.py:147-155 for a batch).  K [3,3] (shared) or [B,3,3]; the other arguments as in
+    ``gather_matches``.  ``scale`` multiplies the 3D points before the solve and divides the translation after it, as
+    ``ransac_PnP(..., scale=1000)`` does in the reference.  A frame with fewer than 4 pairs, or no model, gets the identity pose
+    and 0 inliers.  Returns a dict: pose [B,3,4] and pose_homo [B,4,4] f64, n_inliers int32 [B], inlier_mask bool [B*N],
+    query_index, mconf and offsets (rows indexed as in ``gather_matches``)."""
+    g = gather_matches(matches0, keypoints2d, keypoints3d, matching_scores0)
+    return _solve(K, g, int(matches0.shape[0]), matches0.device, reproj_error, scale, hypotheses, seed)
 
 
 def pose_errors(pose_pred: torch.Tensor, pose_gt: torch.Tensor):
