@@ -2,7 +2,6 @@
 // Host-side state: packed weights, per-object constants, chunk workspace, launch sequence.
 #include <algorithm>
 #include <cmath>
-#include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -48,17 +47,14 @@ struct ObjectState {      // per-object constants: the handle's current object (
   PlaneBuf xo;            // [m_pad, 256]: 3D-point state entering layer 2 (object prologue), valid while prologue_ready
   bool s2_ready = false;
   bool prologue_ready = false;
-  void release() { leaves.release(); db.release(); s2.release(); xo.release(); }
 };
 
 }  // namespace opb
 
 using namespace opb;
 
-struct opb_matcher {
+struct opb_matcher : Handle {
   opb_config cfg{};
-  std::string err;
-  std::map<std::string, std::vector<float>> host_w;
   bool weights_ready = false;
   bool object_ready = false;
   int num_sms = 132;      // multiprocessors of the device (opb_create reads it; 132 on an H100 SXM)
@@ -71,7 +67,7 @@ struct opb_matcher {
   PlaneBuf eye;           // [256,256] identity, fp16-split (residual as an identity K-block of the mlp.3 GEMM)
   // per-object constants
   ObjectState cur;                              // opb_set_object's object (valid while object_ready)
-  std::map<int, ObjectState*> objects;          // opb_add_object registrations, by id
+  std::map<int, ObjectState> objects;           // opb_add_object registrations, by id
   int next_object_id = 0;
   // workspace (chunk)
   int chunk_frames = 0;   // user override
@@ -93,102 +89,23 @@ struct opb_matcher {
   cudaStream_t copy_stream = nullptr;          // opb_forward_host: H2D of chunk i+1 overlaps the compute of chunk i
   std::vector<cudaEvent_t> h2d_ev;              // one per piece; consumed by the chunk loop of opb_forward
   int h2d_pending = 0;
-  // profiling (bench.py roofline leg)
-  bool profiling = false;
-  std::vector<cudaEvent_t> ev_pool;
-  size_t ev_used = 0;
-  std::vector<double> ev_flops;     // per profiled launch (0 for the helper kernels)
-  std::vector<std::string> ev_name; // per profiled launch; an event is recorded AFTER every launch, durations = consecutive differences
-  cudaEvent_t ev_fwd0 = nullptr, ev_fwd1 = nullptr;
-  int launches = 0;
-  int last_launches = 0;
+  int last_launches = 0;                        // launches of the last completed forward
+  ~opb_matcher() {
+    for (auto e : h2d_ev) cudaEventDestroy(e);
+    if (copy_stream) cudaStreamDestroy(copy_stream);
+    if (range_ev) cudaEventDestroy(range_ev);
+    if (range_host) cudaFreeHost(range_host);
+  }
 };
 
 namespace opb {
 
-int fail(opb_matcher* m, int code, const char* fmt, ...) {
-  char buf[512];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof buf, fmt, ap);
-  va_end(ap);
-  if (m) m->err = buf; else g_create_error = buf;
-  return code;
+// One GATsSPG GEMM; its profile name tells the epilogue and the shape (bench.py selects on "gemm epi1 ", ...).
+static int gemm(opb_matcher* m, const GemmProblem& p, cudaStream_t st, double flops, const char* what) {
+  char tag[96] = "";
+  if (m->timeline.on) snprintf(tag, sizeof tag, "gemm epi%d n%d k%d %s", p.epi, p.n_out, p.K1 + p.K2, what);
+  return run_gemm(m, p, st, flops, what, tag);
 }
-
-#define CK(m, expr)                                                                                   \
-  do {                                                                                                \
-    cudaError_t _e = (expr);                                                                          \
-    if (_e != cudaSuccess)                                                                            \
-      return fail(m, OPB_E_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); \
-  } while (0)
-
-// weight uploads are synchronous copies on the legacy stream; opb_finalize_weights ends with a device synchronisation so that
-// they are ordered against whatever (non-blocking) stream the caller uses afterwards
-static int upload_planes(opb_matcher* m, PlaneBuf& dst, const std::vector<double>& w, size_t off_elems = 0, size_t total_elems = 0) {
-  std::vector<__half> hi, lo;
-  split_host(w, hi, lo);
-  CK(m, dst.ensure(total_elems ? total_elems : w.size()));
-  CK(m, cudaMemcpy(dst.hi.as<__half>() + off_elems, hi.data(), hi.size() * sizeof(__half), cudaMemcpyHostToDevice));
-  CK(m, cudaMemcpy(dst.lo.as<__half>() + off_elems, lo.data(), lo.size() * sizeof(__half), cudaMemcpyHostToDevice));
-  return 0;
-}
-static int upload_f32(opb_matcher* m, DevBuf& dst, const std::vector<double>& w) {
-  std::vector<float> f(w.begin(), w.end());
-  CK(m, dst.ensure(f.size() * sizeof(float)));
-  CK(m, cudaMemcpy(dst.p, f.data(), f.size() * sizeof(float), cudaMemcpyHostToDevice));
-  return 0;
-}
-
-static const std::vector<float>* find_w(opb_matcher* m, const std::string& key, size_t n) {
-  auto it = m->host_w.find(key);
-  if (it == m->host_w.end()) { fail(m, OPB_E_STATE, "missing weight '%s'", key.c_str()); return nullptr; }
-  if (it->second.size() != n) {
-    fail(m, OPB_E_INVALID, "weight '%s' has %zu elements, expected %zu", key.c_str(), it->second.size(), n);
-    return nullptr;
-  }
-  return &it->second;
-}
-
-static cudaEvent_t next_event(opb_matcher* m) {
-  if (m->ev_used == m->ev_pool.size()) {
-    cudaEvent_t e;
-    cudaEventCreate(&e);
-    m->ev_pool.push_back(e);
-  }
-  return m->ev_pool[m->ev_used++];
-}
-
-// Profiling (bench.py roofline leg): one event after every launch on the stream; a launch's time is the difference to the
-// previous event (so it includes any launch gap in front of it).
-static void prof_mark(opb_matcher* m, cudaStream_t st, const char* name, double flops) {
-  if (!m->profiling) return;
-  cudaEventRecord(next_event(m), st);
-  m->ev_flops.push_back(flops);
-  m->ev_name.push_back(name);
-}
-
-// One launch of the wgmma GEMM core.  `flops` = algorithmic FLOPs.
-static int run_gemm(opb_matcher* m, const GemmProblem& p, cudaStream_t st, double flops, const char* what) {
-  const int rc = launch_gemm_tc(p, st);
-  if (m->profiling) {
-    char tag[96];
-    snprintf(tag, sizeof tag, "gemm epi%d n%d k%d %s", p.epi, p.n_out, p.K1 + p.K2, what);
-    prof_mark(m, st, tag, flops);
-  }
-  m->launches++;
-  if (rc != 0) return fail(m, rc == -1 ? OPB_E_INVALID : OPB_E_CUDA, "GEMM launch failed (%s, rc=%d): %s", what, rc,
-                           cudaGetErrorString(cudaGetLastError()));
-  return 0;
-}
-
-#define LAUNCH(m, st, name, ...)                                                                                    \
-  do {                                                                                                              \
-    cudaError_t _le = launch_k(__VA_ARGS__);                                                                        \
-    if (_le != cudaSuccess) return fail(m, OPB_E_CUDA, "launch of %s failed: %s", name, cudaGetErrorString(_le));    \
-    (m)->launches++;                                                                                                \
-    prof_mark(m, st, name, 0.0);                                                                                    \
-  } while (0)
 
 // Sized for chunks of `frames` frames, N query points and 3D segments of m_pad rows (the largest object of a call); only grows.
 static int ensure_workspace(opb_matcher* m, int frames, int N, int m_pad) {
@@ -278,7 +195,7 @@ static int run_gats(opb_matcher* m, const Layout& L, XView x, int gi, int Lf, co
   p.L = Lc; p.batch = 1; p.rows = Lc.rows();
   p.a1 = m->lin_a.c(kD); p.K1 = kD; p.b1 = m->wlin.c(kD, (size_t)gi * kD * kD); p.n_out = kD;
   p.epi = EPI_BIAS_PLANES; p.out = m->lin_b.m(kD);
-  if (int rc = run_gemm(m, p, st, 2.0 * L.B * (double)L.M * kD * kD, "gats.W")) return rc;
+  if (int rc = gemm(m, p, st, 2.0 * L.B * (double)L.M * kD * kD, "gats.W")) return rc;
   const long long n = (long long)L.B * L.M * 32;
   LAUNCH(m, st, "gats_lin_finish", gats_lin_finish, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, st, (const __half*)m->lin_b.hi.as<__half>(),
          (const __half*)m->lin_b.lo.as<__half>(), x.hi, x.lo, L, (int)(m->cfg.include_self && m->cfg.additional));
@@ -299,12 +216,10 @@ static int run_attn_layer(opb_matcher* m, const Layout& L, XView x, AttnLayerW& 
   pk.bias = W.bqkv.as<float>() + 256;
   pk.epi = EPI_QKV; pk.out = Planes{m->kvt.as<__half>(), m->kvt.as<__half>(), 512};
   pk.a_hi_only = m->kv_two_pass;
-  if (int rc = run_gemm(m, pk, st, 2.0 * valid_rows * 512 * kD, "kv_proj")) return rc;
+  if (int rc = gemm(m, pk, st, 2.0 * valid_rows * 512 * kD, "kv_proj")) return rc;
   // (2) linear-attention state of every segment (:71-78): per-row-group partial states on the tensor cores ...
   const KvGroups G = kv_groups_for(L, m->num_sms);
-  if (launch_kv_state_h(m->kvt.as<__half>(), L, G, m->kvpart.as<float>(), st)) return fail(m, OPB_E_CUDA, "kv_state_h launch failed");
-  m->launches++;
-  prof_mark(m, st, "kv_state_h", 0.0);
+  if (int rc = launched(m, st, "kv_state_h", launch_kv_state_h(m->kvt.as<__half>(), L, G, m->kvpart.as<float>(), st))) return rc;
   // ... reduced per segment into Kmean and the block-diagonal operand of the G fold (indexed by DESTINATION segment)
   LAUNCH(m, st, "kv_state_reduce", kv_state_reduce, dim3(S * kHeads, (kKVPartial + 255) / 256), dim3(256), 0, st, (const float*)m->kvpart.as<float>(), L,
          G, cross, m->kmean.as<float>(), m->bd.hi.as<__half>(), m->bd.lo.as<__half>());
@@ -313,7 +228,7 @@ static int run_attn_layer(opb_matcher* m, const Layout& L, XView x, AttnLayerW& 
   pq.L = L; pq.batch = 1; pq.rows = rows;
   pq.a1 = x.c(kD); pq.K1 = kD; pq.b1 = W.wqkv.c(kD); pq.n_out = 256; pq.bias = W.bqkv.as<float>();
   pq.epi = EPI_QSCALE; pq.kmean = m->kmean.as<float>(); pq.cross = cross; pq.out = m->qp.m(kD);
-  if (int rc = run_gemm(m, pq, st, 2.0 * valid_rows * 256 * kD, "q_proj")) return rc;
+  if (int rc = gemm(m, pq, st, 2.0 * valid_rows * 256 * kD, "q_proj")) return rc;
   // (4) dynamic weight G[s] = W0m . blockdiag(KVmean_src(s))^T  -- merge and the message half of mlp.0 folded into one
   //     per-segment [512, 256] weight (4 x 64x64x512 MACs per segment), as a batched wgmma GEMM over the segments
   GemmProblem pg{};
@@ -321,7 +236,7 @@ static int run_attn_layer(opb_matcher* m, const Layout& L, XView x, AttnLayerW& 
   pg.a1 = W.w0m.c(kD); pg.a_batch_rows = 0;
   pg.b1 = m->bd.c(kD); pg.b_batch_rows = kD;
   pg.epi = EPI_BIAS_PLANES; pg.out = m->g.m(kD);
-  if (int rc = run_gemm(m, pg, st, 2.0 * S * 512.0 * kD * kDh, "g_fold")) return rc;
+  if (int rc = gemm(m, pg, st, 2.0 * S * 512.0 * kD * kDh, "g_fold")) return rc;
   // (5) hidden = mlp.0([x ; message]) = [x | Q'] . [W0a | G_seg]^T + b   (:101,:113,:122); epilogue also emits the InstanceNorm
   //     partial sums (:126)
   GemmProblem p2{};
@@ -330,7 +245,7 @@ static int run_attn_layer(opb_matcher* m, const Layout& L, XView x, AttnLayerW& 
   p2.a2 = m->qp.c(kD); p2.K2 = kD; p2.b2 = m->g.c(kD); p2.b2_per_seg = 1;
   p2.n_out = 512; p2.bias = W.b0f.as<float>(); p2.c = m->hid.as<float>(); p2.ldc = 512;
   p2.epi = EPI_F32_STATS; p2.statpart = m->statpart.as<float>();
-  if (int rc = run_gemm(m, p2, st, 2.0 * valid_rows * 512 * 512, "mlp0")) return rc;
+  if (int rc = gemm(m, p2, st, 2.0 * valid_rows * 512 * 512, "mlp0")) return rc;
   // (6) InstanceNorm statistics per segment (:126)
   LAUNCH(m, st, "in_stats_final", in_stats_final, dim3(S, 16), dim3(32, kStatSlices), 0, st, (const float*)m->statpart.as<float>(), L, m->mu.as<float>(),
          m->rstd.as<float>());
@@ -341,7 +256,7 @@ static int run_attn_layer(opb_matcher* m, const Layout& L, XView x, AttnLayerW& 
   p3.epi = EPI_BIAS_PLANES; p3.out = x.m(kD);
   p3.a2 = x.c(kD); p3.K2 = kD; p3.b2 = m->eye.c(kD); p3.b2_lo_zero = 1; p3.b2_identity = m->identity_diag;
   p3.a_conv = 1; p3.a_raw = m->hid.as<float>(); p3.a_raw_ld = 512; p3.mu = m->mu.as<float>(); p3.rstd = m->rstd.as<float>();
-  return run_gemm(m, p3, st, 2.0 * valid_rows * 256 * 512, "mlp3");
+  return gemm(m, p3, st, 2.0 * valid_rows * 256 * 512, "mlp3");
 }
 
 // Object prologue: GNN layers 0 (GATs) and the 3D side of layer 1 (self-attention) depend only on the per-object
@@ -432,7 +347,7 @@ static int forward_chunk(opb_matcher* m, const ObjectState* const* fobj, const f
   pf.a1 = m->x.c(kD); pf.K1 = kD; pf.b1 = m->wf.c(kD); pf.n_out = 256;
   pf.bias = m->bf.as<float>();
   pf.epi = EPI_L2NORM; pf.out = m->pn.m(kD);       // F.normalize fused into the final_proj epilogue (:209-213)
-  if (int rc = run_gemm(m, pf, st, 2.0 * valid_rows * kD * kD, "final_proj")) return rc;
+  if (int rc = gemm(m, pf, st, 2.0 * valid_rows * kD * kD, "final_proj")) return rc;
   // dual softmax + arg-max as two passes of the batched score GEMM (one batch = one frame); the cos matrix is never stored
   const int n_parts = (L.m_pad / 256) * 2, q_groups = L.n_pad / 32;
   GemmProblem ps{};
@@ -441,13 +356,13 @@ static int forward_chunk(opb_matcher* m, const ObjectState* const* fobj, const f
   ps.a_batch_rows = L.R; ps.b_batch_rows = L.R;
   ps.inv_scale = 1.f / m->cfg.scale_factor;
   ps.epi = EPI_SCORE_SUMS; ps.rowsum_part = m->rowsum_part.as<float>(); ps.colsum_part = m->colsum_part.as<float>();
-  if (int rc = run_gemm(m, ps, st, 2.0 * (double)N * m_sum * kD, "score_sums")) return rc;
+  if (int rc = gemm(m, ps, st, 2.0 * (double)N * m_sum * kD, "score_sums")) return rc;
   LAUNCH(m, st, "score_sums_finalize", score_sums_finalize, dim3((L.n_pad + L.m_pad + 255) / 256, fb), dim3(256), 0, st,
          (const float*)m->rowsum_part.as<float>(), (const float*)m->colsum_part.as<float>(), L, n_parts, q_groups, m->rowsum.as<float>(),
          m->colsum.as<float>(), m->rowbest.as<unsigned long long>(), m->colbest.as<unsigned long long>());
   ps.epi = EPI_SCORE_CONF; ps.inv_rowsum = m->rowsum.as<float>(); ps.inv_colsum = m->colsum.as<float>();
   ps.conf = conf; ps.conf_ld = M_out; ps.rowbest = m->rowbest.as<unsigned long long>(); ps.colbest = m->colbest.as<unsigned long long>();
-  if (int rc = run_gemm(m, ps, st, 0.0, "score_conf")) return rc;      // recomputation: its FLOPs are not algorithmic
+  if (int rc = gemm(m, ps, st, 0.0, "score_conf")) return rc;      // recomputation: its FLOPs are not algorithmic
   if (conf && M_out > L.m_pad)                                          // conf rows wider than this chunk's 3D segments
     LAUNCH(m, st, "conf_fill_tail", conf_fill_tail, dim3(m->num_sms * 4), dim3(256), 0, st, conf, (long long)fb * N, M_out, L.m_pad);
   LAUNCH(m, st, "mutual_match", mutual_match, dim3(fb), dim3(256), 0, st, (const unsigned long long*)m->rowbest.as<unsigned long long>(),
@@ -462,13 +377,11 @@ static int chunk_of(const opb_matcher* m, int B) {
 }
 
 // Leaf logits of an object (frame-invariant, they depend on the weights): GATs.py:40,78 folded as s2 = leaves . (W a[:256]).
-// A plain launch: it also runs outside a forward (opb_set_object / opb_add_object), where it must not touch the profile of
-// the last forward; forward_frames counts and marks it itself.
-static int object_leaf_logits(opb_matcher* m, ObjectState& o, cudaStream_t st) {
-  CK(m, launch_k(gats_leaf_logits, dim3(m->num_sms * 4), dim3(256), 0, st, (const float*)o.leaves.as<float>(), (long long)o.M * o.Lf,
-                 (const float*)m->wa2.as<float>(), o.s2.as<float>()));
-  o.s2_ready = true;
-  return 0;
+// Not counted here: it also runs outside a forward (opb_set_object / opb_add_object), where it must not touch the profile of
+// the last forward; forward_frames counts it.
+static cudaError_t launch_leaf_logits(const opb_matcher* m, const ObjectState& o, cudaStream_t st) {
+  return launch_k(gats_leaf_logits, dim3(m->num_sms * 4), dim3(256), 0, st, (const float*)o.leaves.as<float>(), (long long)o.M * o.Lf,
+                  (const float*)m->wa2.as<float>(), o.s2.as<float>());
 }
 
 // Upload an object's constants into `o` (buffers only grow) and compute its leaf logits; its prologue runs on first use.
@@ -489,12 +402,14 @@ static int load_object(opb_matcher* m, ObjectState& o, const float* desc3d_db, c
   launch_k(transpose_cf_to_rows<0>, dim3(m_pad / 32, 1), dim3(32, 8), 0, st, desc3d_db, (int)M, (int)M, 0ll, (const int*)nullptr, m_pad,
            o.db.hi.as<__half>(), o.db.lo.as<__half>(), (float*)nullptr, 0ll, 0);
   CK(m, cudaGetLastError());
-  return object_leaf_logits(m, o, st);
+  CK(m, launch_leaf_logits(m, o, st));
+  o.s2_ready = true;
+  return 0;
 }
 
 static void invalidate_prologues(opb_matcher* m) {
   m->cur.prologue_ready = false;
-  for (auto& kv : m->objects) kv.second->prologue_ready = false;
+  for (auto& kv : m->objects) kv.second.prologue_ready = false;
 }
 
 // The one forward of the handle: frame b of the call matches against fobj[b] (opb_forward: the current object everywhere).
@@ -505,21 +420,13 @@ static int forward_frames(opb_matcher* m, ObjectState* const* fobj, const float*
   for (int b = 0; b < B; ++b) call_m_pad = std::max(call_m_pad, fobj[b]->m_pad);
   const int chunk = chunk_of(m, B);
   if (int rc = ensure_workspace(m, chunk, N, call_m_pad)) return rc;   // no-op once opb_reserve_workspace / an earlier call has sized it
-  m->launches = 0;
-  if (m->profiling) {
-    m->ev_used = 0;
-    m->ev_flops.clear();
-    m->ev_name.clear();
-    if (!m->ev_fwd0) { cudaEventCreate(&m->ev_fwd0); cudaEventCreate(&m->ev_fwd1); }
-    cudaEventRecord(m->ev_fwd0, st);
-  }
+  m->begin(st);
   // per-object work on first use: leaf logits after a weight reload, the prologue (once per object, shared by all later calls)
   for (int b = 0; b < B; ++b) {
     ObjectState& o = *fobj[b];
     if (!o.s2_ready) {
-      if (int rc = object_leaf_logits(m, o, st)) return rc;
-      m->launches++;
-      prof_mark(m, st, "gats_leaf_logits", 0.0);
+      if (int rc = launched(m, st, "gats_leaf_logits", launch_leaf_logits(m, o, st))) return rc;
+      o.s2_ready = true;
     }
     if (m->hoist && !o.prologue_ready) {
       if (int rc = object_prologue(m, o, st)) return rc;
@@ -544,7 +451,7 @@ static int forward_frames(opb_matcher* m, ObjectState* const* fobj, const float*
   CK(m, cudaEventRecord(m->range_ev, st));
   m->range_pending = true;
   m->last_stream = st;
-  if (m->profiling) cudaEventRecord(m->ev_fwd1, st);
+  m->timeline.finish(st);
   m->last_launches = m->launches;
   return OPB_OK;
 }
@@ -555,26 +462,19 @@ static int forward_frames(opb_matcher* m, ObjectState* const* fobj, const float*
 extern "C" {
 
 int opb_create(const opb_config* cfg, opb_matcher** out) {
-  if (!cfg || !out) return fail(nullptr, OPB_E_INVALID, "null argument");
+  if (!cfg || !out) return fail(g_create_error, OPB_E_INVALID, "null argument");
   if (cfg->descriptor_dim != kD || cfg->num_heads != kHeads)
-    return fail(nullptr, OPB_E_INVALID, "only descriptor_dim=256, num_heads=4 are supported (got %d, %d)", cfg->descriptor_dim, cfg->num_heads);
-  if (!(cfg->scale_factor > 0.f)) return fail(nullptr, OPB_E_INVALID, "scale_factor must be > 0");
-  int n_dev = 0;
-  cudaError_t e = cudaGetDeviceCount(&n_dev);
-  if (e != cudaSuccess || n_dev == 0)
-    return fail(nullptr, OPB_E_CUDA, "no CUDA device: %s (this library has no CPU path)", cudaGetErrorString(e));
-  if (cfg->device < 0 || cfg->device >= n_dev) return fail(nullptr, OPB_E_INVALID, "device %d out of range", cfg->device);
-  e = cudaSetDevice(cfg->device);
-  if (e != cudaSuccess) return fail(nullptr, OPB_E_CUDA, "cudaSetDevice: %s", cudaGetErrorString(e));
+    return fail(g_create_error, OPB_E_INVALID, "only descriptor_dim=256, num_heads=4 are supported (got %d, %d)", cfg->descriptor_dim,
+                cfg->num_heads);
+  if (!(cfg->scale_factor > 0.f)) return fail(g_create_error, OPB_E_INVALID, "scale_factor must be > 0");
   cudaDeviceProp prop;
-  cudaGetDeviceProperties(&prop, cfg->device);
-  if (prop.major != 9 || prop.minor != 0) return fail(nullptr, OPB_E_CUDA, "device is sm_%d%d; this library is built for sm_90a only", prop.major, prop.minor);
+  if (int rc = select_device(cfg->device, prop, g_create_error)) return rc;
   auto* m = new opb_matcher();
   m->cfg = *cfg;
   m->num_sms = prop.multiProcessorCount;
   if (cudaMallocHost(&m->range_host, sizeof(int)) != cudaSuccess || cudaEventCreateWithFlags(&m->range_ev, cudaEventDisableTiming) != cudaSuccess) {
     delete m;
-    return fail(nullptr, OPB_E_CUDA, "pinned flag / event allocation failed");
+    return fail(g_create_error, OPB_E_CUDA, "pinned flag / event allocation failed");
   }
   *m->range_host = 0;
   *out = m;
@@ -584,29 +484,14 @@ int opb_create(const opb_config* cfg, opb_matcher** out) {
 void opb_destroy(opb_matcher* m) {
   if (!m) return;
   cudaSetDevice(m->cfg.device);
-  cudaDeviceSynchronize();
-  for (auto& a : m->attn) { a.wqkv.release(); a.bqkv.release(); a.w0a.release(); a.w0m.release(); a.b0f.release(); a.w1.release(); a.b1.release(); }
-  DevBuf* bufs[] = {&m->wa2, &m->wa3, &m->bf, &m->kvt, &m->hid, &m->kvpart, &m->kmean, &m->statpart, &m->tab,
-                    &m->mu, &m->rstd, &m->rowsum_part, &m->colsum_part, &m->rowsum, &m->colsum, &m->rowbest, &m->colbest, &m->range_flag,
-                    &m->st_q, &m->st_m0, &m->st_m1, &m->st_s0, &m->st_s1, &m->st_conf, &m->st_len};
-  for (auto* b : bufs) b->release();
-  m->cur.release();
-  for (auto& kv : m->objects) { kv.second->release(); delete kv.second; }
-  PlaneBuf* pb[] = {&m->wf, &m->wlin, &m->x, &m->qp, &m->pn, &m->g, &m->xq, &m->bd, &m->lin_a, &m->lin_b, &m->eye};
-  for (auto* b : pb) b->release();
-  for (auto e : m->ev_pool) cudaEventDestroy(e);
-  for (auto e : m->h2d_ev) cudaEventDestroy(e);
-  if (m->copy_stream) cudaStreamDestroy(m->copy_stream);
-  if (m->ev_fwd0) { cudaEventDestroy(m->ev_fwd0); cudaEventDestroy(m->ev_fwd1); }
-  if (m->range_ev) cudaEventDestroy(m->range_ev);
-  if (m->range_host) cudaFreeHost(m->range_host);
+  cudaDeviceSynchronize();   // the frees of the handle's buffers come after the work in flight
   delete m;
 }
 
 const char* opb_last_error(const opb_matcher* m) { return m ? m->err.c_str() : g_create_error.c_str(); }
 
 int opb_load_weight(opb_matcher* m, const char* name, const float* data, size_t n) {
-  if (!m || !name || !data) return fail(m, OPB_E_INVALID, "null argument");
+  if (!m || !name || !data) return m ? fail(m, OPB_E_INVALID, "null argument") : fail(g_create_error, OPB_E_INVALID, "null argument");
   m->host_w[name] = std::vector<float>(data, data + n);
   m->weights_ready = false;
   return OPB_OK;
@@ -624,9 +509,9 @@ int opb_finalize_weights(opb_matcher* m) {
   for (int layer = 0; layer < 12; ++layer) {
     const std::string p = "gnn.layers." + std::to_string(layer);
     if (layer % 3 == 0) {
-      auto* W = find_w(m, p + ".W", kD * kD);
-      auto* a = find_w(m, p + ".a", 2 * kD);
-      if (!W || !a) return OPB_E_STATE;
+      auto* W = find_weight(m, p + ".W", kD * kD);
+      auto* a = find_weight(m, p + ".a", 2 * kD);
+      if (!W || !a) return m->find_code;
       const int gi = layer / 3;
       for (int c = 0; c < kD; ++c) {  // h @ W @ a[:256] = h . (W a[:256])   (GATs.py:40,78-80)
         double s2 = 0, s3 = 0;
@@ -648,17 +533,17 @@ int opb_finalize_weights(opb_matcher* m) {
     AttnLayerW& A = m->attn[ai++];
     const std::vector<float>*Wp[3], *bp[3];
     for (int j = 0; j < 3; ++j) {
-      Wp[j] = find_w(m, p + ".attn.proj." + std::to_string(j) + ".weight", kD * kD);
-      bp[j] = find_w(m, p + ".attn.proj." + std::to_string(j) + ".bias", kD);
-      if (!Wp[j] || !bp[j]) return OPB_E_STATE;
+      Wp[j] = find_weight(m, p + ".attn.proj." + std::to_string(j) + ".weight", kD * kD);
+      bp[j] = find_weight(m, p + ".attn.proj." + std::to_string(j) + ".bias", kD);
+      if (!Wp[j] || !bp[j]) return m->find_code;
     }
-    auto* Wm = find_w(m, p + ".attn.merge.weight", kD * kD);
-    auto* bm = find_w(m, p + ".attn.merge.bias", kD);
-    auto* W0 = find_w(m, p + ".mlp.0.weight", 512 * 512);
-    auto* b0 = find_w(m, p + ".mlp.0.bias", 512);
-    auto* W1 = find_w(m, p + ".mlp.3.weight", kD * 512);
-    auto* b1 = find_w(m, p + ".mlp.3.bias", kD);
-    if (!Wm || !bm || !W0 || !b0 || !W1 || !b1) return OPB_E_STATE;
+    auto* Wm = find_weight(m, p + ".attn.merge.weight", kD * kD);
+    auto* bm = find_weight(m, p + ".attn.merge.bias", kD);
+    auto* W0 = find_weight(m, p + ".mlp.0.weight", 512 * 512);
+    auto* b0 = find_weight(m, p + ".mlp.0.bias", 512);
+    auto* W1 = find_weight(m, p + ".mlp.3.weight", kD * 512);
+    auto* b1 = find_weight(m, p + ".mlp.3.bias", kD);
+    if (!Wm || !bm || !W0 || !b0 || !W1 || !b1) return m->find_code;
     std::vector<double> wqkv(768 * kD), bqkv(768);
     for (int j = 0; j < 3; ++j)
       for (int c = 0; c < kD; ++c) {
@@ -686,9 +571,9 @@ int opb_finalize_weights(opb_matcher* m) {
     if (int rc = upload_planes(m, A.w1, w1)) return rc;
     if (int rc = upload_f32(m, A.b1, b1d)) return rc;
   }
-  auto* Wf = find_w(m, "final_proj.weight", kD * kD);
-  auto* bfv = find_w(m, "final_proj.bias", kD);
-  if (!Wf || !bfv) return OPB_E_STATE;
+  auto* Wf = find_weight(m, "final_proj.weight", kD * kD);
+  auto* bfv = find_weight(m, "final_proj.bias", kD);
+  if (!Wf || !bfv) return m->find_code;
   if (int rc = upload_planes(m, m->wf, std::vector<double>(Wf->begin(), Wf->end()))) return rc;
   {
     std::vector<double> eye((size_t)kD * kD, 0.0);
@@ -702,7 +587,7 @@ int opb_finalize_weights(opb_matcher* m) {
   m->weights_ready = true;
   m->object_ready = false;  // s2 and the prologue depend on the weights: the current object is set again, registered objects
   invalidate_prologues(m);  // recompute theirs on their next use
-  for (auto& kv : m->objects) kv.second->s2_ready = false;
+  for (auto& kv : m->objects) kv.second.s2_ready = false;
   return OPB_OK;
 }
 
@@ -725,15 +610,14 @@ int opb_add_object(opb_matcher* m, const float* desc3d_db, const float* desc2d_d
   if (!desc3d_db || !desc2d_db || !object_id || M <= 0 || Lf <= 0 || Lf > 32)
     return fail(m, OPB_E_INVALID, "add_object: need M > 0, 1 <= num_leaf <= 32 and an id pointer (got M=%d, L=%d)", M, Lf);
   CK(m, cudaSetDevice(m->cfg.device));
-  auto* o = new ObjectState();
-  if (int rc = load_object(m, *o, desc3d_db, desc2d_db, M, Lf, (cudaStream_t)stream)) {
+  const int id = m->next_object_id;
+  ObjectState& o = m->objects[id];
+  if (int rc = load_object(m, o, desc3d_db, desc2d_db, M, Lf, (cudaStream_t)stream)) {
     cudaDeviceSynchronize();
-    o->release();
-    delete o;
+    m->objects.erase(id);
     return rc;
   }
-  const int id = m->next_object_id++;
-  m->objects[id] = o;
+  m->next_object_id++;
   *object_id = id;
   return OPB_OK;
 }
@@ -744,8 +628,6 @@ int opb_remove_object(opb_matcher* m, int32_t object_id) {
   if (it == m->objects.end()) return fail(m, OPB_E_INVALID, "remove_object: unknown object id %d", object_id);
   CK(m, cudaSetDevice(m->cfg.device));
   CK(m, cudaDeviceSynchronize());                  // calls in flight may still read the object's buffers
-  it->second->release();
-  delete it->second;
   m->objects.erase(it);
   return OPB_OK;
 }
@@ -755,7 +637,7 @@ int opb_reserve_workspace(opb_matcher* m, int32_t frames, int32_t N) {
   if (!m->object_ready && m->objects.empty()) return fail(m, OPB_E_STATE, "opb_reserve_workspace needs an object (the workspace depends on M)");
   CK(m, cudaSetDevice(m->cfg.device));
   int m_pad = m->object_ready ? m->cur.m_pad : 0;   // sized for the largest object the handle knows
-  for (auto& kv : m->objects) m_pad = std::max(m_pad, kv.second->m_pad);
+  for (auto& kv : m->objects) m_pad = std::max(m_pad, kv.second.m_pad);
   return ensure_workspace(m, chunk_of(m, frames), N, m_pad);
 }
 
@@ -794,7 +676,7 @@ int opb_forward_objects(opb_matcher* m, const int32_t* object_ids_host, const fl
   for (int b = 0; b < B; ++b) {
     auto it = m->objects.find(object_ids_host[b]);
     if (it == m->objects.end()) return fail(m, OPB_E_INVALID, "opb_forward_objects: unknown object id %d (frame %d)", object_ids_host[b], b);
-    fobj[b] = it->second;
+    fobj[b] = &it->second;
     if (fobj[b]->Lf != fobj[0]->Lf)
       return fail(m, OPB_E_INVALID, "opb_forward_objects: frames %d and 0 use objects with different leaf counts (%d, %d)", b, fobj[b]->Lf,
                   fobj[0]->Lf);
@@ -807,28 +689,27 @@ int opb_forward_objects(opb_matcher* m, const int32_t* object_ids_host, const fl
 
 int opb_set_profiling(opb_matcher* m, int32_t enable) {
   if (!m) return OPB_E_INVALID;
-  m->profiling = enable != 0;
-  m->ev_used = 0;
-  m->ev_flops.clear();
-  m->ev_name.clear();
+  m->timeline.on = enable != 0;
+  m->timeline.clear();
   return OPB_OK;
 }
 
 int opb_get_profile(opb_matcher* m, double* gemm_ms, double* gemm_flops, int32_t* gemm_launches, double* total_ms) {
-  if (!m || !m->ev_fwd1) return OPB_E_STATE;
-  CK(m, cudaEventSynchronize(m->ev_fwd1));
+  if (!m || !m->timeline.end) return OPB_E_STATE;
+  const Timeline& tl = m->timeline;
+  CK(m, cudaEventSynchronize(tl.end));
   double ms = 0, fl = 0;
   int n_gemm = 0;
   std::map<std::string, std::pair<double, std::pair<double, int>>> agg;
-  for (size_t i = 0; i < m->ev_flops.size(); ++i) {
+  for (size_t i = 0; i < tl.size(); ++i) {
     float t = 0;
-    CK(m, cudaEventElapsedTime(&t, i == 0 ? m->ev_fwd0 : m->ev_pool[i - 1], m->ev_pool[i]));
-    if (m->ev_name[i].compare(0, 4, "gemm") == 0) { ms += t; fl += m->ev_flops[i]; ++n_gemm; }
-    auto& a = agg[m->ev_name[i]];
-    a.first += t; a.second.first += m->ev_flops[i]; a.second.second++;
+    CK(m, tl.ms(i, &t));
+    if (tl.name[i].compare(0, 4, "gemm") == 0) { ms += t; fl += tl.flops[i]; ++n_gemm; }
+    auto& a = agg[tl.name[i]];
+    a.first += t; a.second.first += tl.flops[i]; a.second.second++;
   }
   float tot = 0;
-  CK(m, cudaEventElapsedTime(&tot, m->ev_fwd0, m->ev_fwd1));
+  CK(m, cudaEventElapsedTime(&tot, tl.start, tl.end));
   if (getenv("OPB_PROFILE_DUMP")) {   // measurement aid only: prints the table, selects nothing
     fprintf(stderr, "[opb profile] forward %.3f ms, GEMM %.3f ms in %d launches\n", tot, ms, n_gemm);
     for (auto& kv : agg)
@@ -843,16 +724,17 @@ int opb_get_profile(opb_matcher* m, double* gemm_ms, double* gemm_flops, int32_t
 }
 
 int opb_get_profile_entry(opb_matcher* m, const char* prefix, double* ms_out, double* flops_out, int32_t* launches_out) {
-  if (!m || !prefix || !m->ev_fwd1) return OPB_E_STATE;
-  CK(m, cudaEventSynchronize(m->ev_fwd1));
+  if (!m || !prefix || !m->timeline.end) return OPB_E_STATE;
+  const Timeline& tl = m->timeline;
+  CK(m, cudaEventSynchronize(tl.end));
   double ms = 0, fl = 0;
   int n = 0;
   const size_t pl = strlen(prefix);
-  for (size_t i = 0; i < m->ev_flops.size(); ++i) {
-    if (m->ev_name[i].compare(0, pl, prefix) != 0) continue;
+  for (size_t i = 0; i < tl.size(); ++i) {
+    if (tl.name[i].compare(0, pl, prefix) != 0) continue;
     float t = 0;
-    CK(m, cudaEventElapsedTime(&t, i == 0 ? m->ev_fwd0 : m->ev_pool[i - 1], m->ev_pool[i]));
-    ms += t; fl += m->ev_flops[i]; ++n;
+    CK(m, tl.ms(i, &t));
+    ms += t; fl += tl.flops[i]; ++n;
   }
   if (ms_out) *ms_out = ms;
   if (flops_out) *flops_out = fl;
@@ -1035,7 +917,7 @@ int opb_debug_kv_state_h(const void* kvh, int32_t frames, int32_t n, int32_t m_p
   }
   if (n_groups) *n_groups = frames * (G.gq + G.gd);
   if (!partial) return OPB_OK;                    // size query
-  return launch_kv_state_h((const __half*)kvh, L, G, partial, (cudaStream_t)stream) == 0 ? OPB_OK : OPB_E_CUDA;
+  return launch_kv_state_h((const __half*)kvh, L, G, partial, (cudaStream_t)stream) == cudaSuccess ? OPB_OK : OPB_E_CUDA;
 }
 
 int opb_debug_split(const float* x, void* hi, void* lo, size_t n, void* stream) {

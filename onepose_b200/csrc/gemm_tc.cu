@@ -32,6 +32,7 @@
 #include <tuple>
 
 #include "gemm_tc.cuh"
+#include "host_util.cuh"
 #include "tma.cuh"
 #include "wgmma.cuh"
 
@@ -904,7 +905,7 @@ int num_sms() {
 }
 
 template <int EPI, int ACV = ACV_NONE, bool HI = false, int BN_ = 256, bool DIAG = false>
-cudaError_t launch_variant(const cudaLaunchConfig_t& cfg, const Maps& mp, const TcParams& tp) {
+cudaError_t launch_variant(int grid, cudaStream_t stream, const Maps& mp, const TcParams& tp) {
   static bool attr_done = false;
   auto* kern = gemm_tc_kernel<EPI, ACV, HI, BN_, DIAG>;
   if (!attr_done) {
@@ -912,7 +913,7 @@ cudaError_t launch_variant(const cudaLaunchConfig_t& cfg, const Maps& mp, const 
     if (e != cudaSuccess) return e;
     attr_done = true;
   }
-  return cudaLaunchKernelEx(&cfg, kern, mp, tp);
+  return launch_k(kern, dim3(grid), dim3(kThreads), kSmemBytes, stream, mp, tp);
 }
 
 }  // namespace
@@ -1000,35 +1001,26 @@ int launch_gemm_tc(const GemmProblem& p, cudaStream_t stream) {
   if ((p.epi == EPI_QSCALE || p.b2_per_seg || p.epi == EPI_QKV || p.epi == EPI_F32_STATS || p.a_conv) && !tp.seg_rows) return -1;
   const int total_units = tp.m_tiles * tp.n_tiles * tp.batch;
   const int grid = total_units < num_sms() ? total_units : num_sms();
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(kThreads);
-  cfg.dynamicSmemBytes = kSmemBytes;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;
   cudaError_t le;
   if (p.a_conv) {
-    le = p.b2_identity ? launch_variant<EPI_BIAS_PLANES, ACV_NORM_RELU, false, 256, true>(cfg, mp, tp)
-                       : launch_variant<EPI_BIAS_PLANES, ACV_NORM_RELU>(cfg, mp, tp);
+    le = p.b2_identity ? launch_variant<EPI_BIAS_PLANES, ACV_NORM_RELU, false, 256, true>(grid, stream, mp, tp)
+                       : launch_variant<EPI_BIAS_PLANES, ACV_NORM_RELU>(grid, stream, mp, tp);
   } else {
     switch (p.epi) {
       case EPI_F32:
-        le = bn == 128 ? launch_variant<EPI_F32, ACV_NONE, false, 128>(cfg, mp, tp) : launch_variant<EPI_F32>(cfg, mp, tp);
+        le = bn == 128 ? launch_variant<EPI_F32, ACV_NONE, false, 128>(grid, stream, mp, tp) : launch_variant<EPI_F32>(grid, stream, mp, tp);
         break;
       case EPI_CONV:
-        le = bn == 64 ? launch_variant<EPI_CONV, ACV_NONE, false, 64>(cfg, mp, tp) : launch_variant<EPI_CONV, ACV_NONE, false, 128>(cfg, mp, tp);
+        le = bn == 64 ? launch_variant<EPI_CONV, ACV_NONE, false, 64>(grid, stream, mp, tp) : launch_variant<EPI_CONV, ACV_NONE, false, 128>(grid, stream, mp, tp);
         break;
-      case EPI_F32_STATS: le = launch_variant<EPI_F32_STATS>(cfg, mp, tp); break;
-      case EPI_QSCALE: le = launch_variant<EPI_QSCALE>(cfg, mp, tp); break;
-      case EPI_L2NORM: le = launch_variant<EPI_L2NORM>(cfg, mp, tp); break;
-      case EPI_SCORE_SUMS: le = launch_variant<EPI_SCORE_SUMS>(cfg, mp, tp); break;
-      case EPI_SCORE_CONF: le = launch_variant<EPI_SCORE_CONF>(cfg, mp, tp); break;
-      case EPI_QKV: le = p.a_hi_only ? launch_variant<EPI_QKV, ACV_NONE, true>(cfg, mp, tp) : launch_variant<EPI_QKV>(cfg, mp, tp); break;
+      case EPI_F32_STATS: le = launch_variant<EPI_F32_STATS>(grid, stream, mp, tp); break;
+      case EPI_QSCALE: le = launch_variant<EPI_QSCALE>(grid, stream, mp, tp); break;
+      case EPI_L2NORM: le = launch_variant<EPI_L2NORM>(grid, stream, mp, tp); break;
+      case EPI_SCORE_SUMS: le = launch_variant<EPI_SCORE_SUMS>(grid, stream, mp, tp); break;
+      case EPI_SCORE_CONF: le = launch_variant<EPI_SCORE_CONF>(grid, stream, mp, tp); break;
+      case EPI_QKV: le = p.a_hi_only ? launch_variant<EPI_QKV, ACV_NONE, true>(grid, stream, mp, tp) : launch_variant<EPI_QKV>(grid, stream, mp, tp); break;
       case EPI_BIAS_PLANES:
-        le = p.b2_identity ? launch_variant<EPI_BIAS_PLANES, ACV_NONE, false, 256, true>(cfg, mp, tp) : launch_variant<EPI_BIAS_PLANES>(cfg, mp, tp);
+        le = p.b2_identity ? launch_variant<EPI_BIAS_PLANES, ACV_NONE, false, 256, true>(grid, stream, mp, tp) : launch_variant<EPI_BIAS_PLANES>(grid, stream, mp, tp);
         break;
       default: return -1;
     }

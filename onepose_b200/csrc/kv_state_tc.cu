@@ -12,6 +12,7 @@
 
 #include "common.cuh"
 #include "gemm_tc.cuh"
+#include "host_util.cuh"
 #include "kv_state_tc.cuh"
 #include "tma.cuh"
 #include "wgmma.cuh"
@@ -174,23 +175,15 @@ KvGroups kv_groups_for(const Layout& L, int num_sms) {
   return G;
 }
 
-int launch_kv_state_h(const __half* kvh, const Layout& L, const KvGroups& G, float* partial, cudaStream_t stream) {
+cudaError_t launch_kv_state_h(const __half* kvh, const Layout& L, const KvGroups& G, float* partial, cudaStream_t stream) {
   static bool attr_done = false;
   if (!attr_done) {
-    if (cudaFuncSetAttribute(kv_state_h_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kHSmemBytes) != cudaSuccess) return -2;
+    const cudaError_t e = cudaFuncSetAttribute(kv_state_h_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kHSmemBytes);
+    if (e != cudaSuccess) return e;
     attr_done = true;
   }
   CUtensorMap map;
-  if (!make_tensor_map_2d(&map, kvh, L.rows(), 512, 512, 64, kHRows, false)) return -2;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((unsigned)(L.B * (G.gq + G.gd)));
-  cfg.blockDim = dim3(kHThreads);
-  cfg.dynamicSmemBytes = kHSmemBytes;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[0].val.programmaticStreamSerializationAllowed = 1;
-  cfg.attrs = attr; cfg.numAttrs = pdl_enabled() ? 1 : 0;
-  return cudaLaunchKernelEx(&cfg, kv_state_h_kernel, map, L, G, partial) == cudaSuccess ? 0 : -2;
+  if (!make_tensor_map_2d(&map, kvh, L.rows(), 512, 512, 64, kHRows, false)) return cudaErrorInvalidValue;
+  return launch_k(kv_state_h_kernel, dim3((unsigned)(L.B * (G.gq + G.gd))), dim3(kHThreads), kHSmemBytes, stream, map, L, G, partial);
 }
 }  // namespace opb

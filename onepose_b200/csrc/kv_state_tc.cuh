@@ -11,6 +11,6 @@ struct KvGroups {
 KvGroups kv_groups_for(const Layout& L, int num_sms);
 // kvh = fp16 [rows, 512] = 64 * [elu1(K) | V] with pad rows zero (written by the k,v GEMM, EPI_QKV).
 // partial: [B*(gq+gd)][4 heads][64*64 + 64] per-group sums (KV then Ksum), reduced per segment by kv_state_reduce.
-// Returns 0 or -2 (CUDA error).
-int launch_kv_state_h(const __half* kvh, const Layout& L, const KvGroups& G, float* partial, cudaStream_t stream);
+// A tensor map the driver rejects is reported as cudaErrorInvalidValue.
+cudaError_t launch_kv_state_h(const __half* kvh, const Layout& L, const KvGroups& G, float* partial, cudaStream_t stream);
 }  // namespace opb
