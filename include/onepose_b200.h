@@ -256,6 +256,26 @@ int opb_debug_set_conv_halo(int32_t mode);
 int opb_sp_debug_read(opb_superpoint* h, int32_t which, float* out, size_t capacity_elems, int64_t* n_elems, void* stream);
 
 /* ---- test hooks (used by tests/ and tools/ only; stable but not part of the drop-in surface) ---- */
+/* Stop the next opb_forward / opb_forward_objects right after step `step` of GNN layer `layer` of its first chunk; the call
+ * returns OPB_OK and its outputs are unspecified.  layer = -1 turns the hook off (default).  Steps of an attention layer (1, 2,
+ * 4, 5, 7, 8, 10, 11): 0 k,v projection, 1 state partials, 2 state reduce, 3 q projection, 4 G fold, 5 mlp.0, 6 InstanceNorm
+ * statistics, 7 mlp.3 (+ residual).  A GATs layer (0, 3, 6, 9): 0 aggregation, and with with_linear_transform 1 the W GEMM and
+ * its finish.  layer = 12, the tail: 0 final_proj + normalize, 1 score sums, 2 their finalize, 3 score conf.  With hoisting
+ * on, layer 1 is the compact query-side pass (its first sub-batch), and layers 16 / 17 are the object prologue's layers 0 and
+ * 1 (the first object whose prologue runs in the call).  A host-side check only: the launches are the same with the hook off. */
+int opb_debug_set_stop(opb_matcher* m, int32_t layer, int32_t step);
+/* Layout of the pass the last forward stopped in: layout[7] = {B, N, M, n_pad, m_pad, R, S}, rows = B * R, S = 2 B segments
+ * (frame b's query rows [b R, b R + n_pad), its 3D rows [b R + n_pad, (b + 1) R)).  OPB_E_STATE if the last forward did not
+ * stop. */
+int opb_debug_stopped_layout(const opb_matcher* m, int32_t* layout);
+/* Copy a buffer of the stopped pass to `out` (device): *n_elems = its size; OPB_E_INVALID when it exceeds capacity_elems.
+ * fp32 elements except 12 / 13:  0 X planes [rows, 256], (hi + lo) / 64;  1 kvt [rows, 512] = [elu(K) + 1 | V] (one fp16 plane
+ * / 64, head-contiguous channels h*64 + d);  2 Kmean [S, 256];  3 bd [S, 256, 256] (block-diagonal KVmean of the source
+ * segment, indexed by destination segment);  4 Q' [rows, 256];  5 G [S, 512, 256];  6 hid (mlp.0 output) [rows, 512];
+ * 7 InstanceNorm mean [S, 512];  8 its rstd [S, 512];  9 pn (normalized final_proj rows) [rows, 256];  10 inverse row sums
+ * [B, n_pad];  11 inverse column sums [B, m_pad];  12 packed row arg-max int64 [B, N];  13 packed column arg-max int64 [B, M]
+ * ((conf bits << 32) | ~index);  14 with_linear_transform only: the GATs rows before W [B * m_pad, 256]. */
+int opb_debug_read(opb_matcher* m, int32_t which, void* out, size_t capacity_elems, int64_t* n_elems, void* stream);
 /* Programmatic dependent launch on (default) / off for every launch of the library (A/B measurements). */
 int opb_debug_set_pdl(int32_t enable);
 /* byte >= 0: every workspace / object buffer allocated from now on is filled with `byte` (0xFF = NaN patterns) unless the

@@ -68,6 +68,9 @@ SYMBOLS = {
     "opb_debug_gemm": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
     "opb_debug_kv_state_h": (C.c_int, [_P, _I, _I, _I, _I, _P, C.POINTER(_I), _P]),
     "opb_debug_split": (C.c_int, [_P, _P, _P, C.c_size_t, _P]),
+    "opb_debug_set_stop": (C.c_int, [_P, _I, _I]),
+    "opb_debug_stopped_layout": (C.c_int, [_P, C.POINTER(_I)]),
+    "opb_debug_read": (C.c_int, [_P, _I, _P, C.c_size_t, C.POINTER(C.c_int64), _P]),
     # SuperPoint extractor
     "opb_sp_create": (C.c_int, [C.POINTER(OpbSpConfig), C.POINTER(_P)]),
     "opb_sp_destroy": (None, [_P]),

@@ -90,6 +90,11 @@ struct opb_matcher : Handle {
   std::vector<cudaEvent_t> h2d_ev;              // one per piece; consumed by the chunk loop of opb_forward
   int h2d_pending = 0;
   int last_launches = 0;                        // launches of the last completed forward
+  // test hook (opb_debug_set_stop / opb_debug_read): the next forward stops after step dbg_step of GNN layer dbg_layer
+  int dbg_layer = -1, dbg_step = 0;
+  bool dbg_stopped = false;                     // the last forward stopped there; dbg_L / dbg_x are the layout and X of that pass
+  Layout dbg_L{};
+  XView dbg_x{};
   ~opb_matcher() {
     for (auto e : h2d_ev) cudaEventDestroy(e);
     if (copy_stream) cudaStreamDestroy(copy_stream);
@@ -152,6 +157,22 @@ static int ensure_workspace(opb_matcher* m, int frames, int N, int m_pad) {
 
 static ChunkTable* tab_dev(const opb_matcher* m) { return m->tab.as<ChunkTable>(); }
 
+// Test hook: layer ids of opb_debug_set_stop.  0..11 are the GNN layers of a chunk, kTailLayer the tail; with hoisting, layer 1
+// is the compact query-side pass and the object prologue's layers 0 and 1 are kPrologueLayer + 0 / + 1.
+constexpr int kTailLayer = 12;
+constexpr int kPrologueLayer = 16;
+constexpr int kStopped = 1;      // internal return code of a forward that reached the stop (never returned by the C ABI)
+
+// True when the forward is to stop after step `step` of `layer`; then records the pass for opb_debug_read.  A host-side
+// comparison only: the launch sequence is the same with the hook off.
+static bool stop_here(opb_matcher* m, int layer, int step, const Layout& L, XView x) {
+  if (layer != m->dbg_layer || step != m->dbg_step) return false;
+  m->dbg_stopped = true;
+  m->dbg_L = L;
+  m->dbg_x = x;
+  return true;
+}
+
 // Frame b of a chunk matches against its object's rows `o`.
 static void table_frame(ChunkTable& t, int b, const ObjectState& o, bool hoist) {
   t.obj[b] = FrameObject{hoist ? o.xo.hi.as<__half>() : o.db.hi.as<__half>(), hoist ? o.xo.lo.as<__half>() : o.db.lo.as<__half>(),
@@ -172,7 +193,8 @@ static void make_groups(GatsGroups& g, const ObjectState* const* fobj, int fb) {
 
 // One GATs layer on the 3D-point segments of `x` (layout L); frame b aggregates the leaves of its object (chunk table, already
 // on the device; `groups` for the 8-leaf kernel), `Lf` leaves per point.
-static int run_gats(opb_matcher* m, const Layout& L, XView x, int gi, int Lf, const GatsGroups& groups, cudaStream_t st) {
+static int run_gats(opb_matcher* m, const Layout& L, XView x, int layer, int Lf, const GatsGroups& groups, cudaStream_t st) {
+  const int gi = (layer % kPrologueLayer) / 3;
   const long long warps = (long long)L.M * L.B;
   if (warps == 0) return 0;
   const bool lin = m->cfg.with_linear_transform != 0;
@@ -187,6 +209,7 @@ static int run_gats(opb_matcher* m, const Layout& L, XView x, int gi, int Lf, co
     LAUNCH(m, st, "gats_aggregate", gats_aggregate, dim3((unsigned)((warps * 32 + 255) / 256)), dim3(256), 0, st, (const __half*)x.hi,
            (const __half*)x.lo, L, tab, Lf, gi, wa3, (int)m->cfg.include_self, (int)m->cfg.additional, 0.2f, out);
   }
+  if (stop_here(m, layer, 0, L, x)) return kStopped;
   if (!lin) return 0;
   // with_linear_transform (GATs.py:56-57,64-65): t = pre . W on the tensor cores over the compact 3D rows, then ELU (+ h3)
   Layout Lc{};
@@ -199,12 +222,13 @@ static int run_gats(opb_matcher* m, const Layout& L, XView x, int gi, int Lf, co
   const long long n = (long long)L.B * L.M * 32;
   LAUNCH(m, st, "gats_lin_finish", gats_lin_finish, dim3((unsigned)((n + 255) / 256)), dim3(256), 0, st, (const __half*)m->lin_b.hi.as<__half>(),
          (const __half*)m->lin_b.lo.as<__half>(), x.hi, x.lo, L, (int)(m->cfg.include_self && m->cfg.additional));
+  if (stop_here(m, layer, 1, L, x)) return kStopped;
   return 0;
 }
 
 // One AttentionPropagation layer (reference GATs_SuperGlue.py:55-64, :104-113) on every segment of `x`:
 // both sides of all frames in ONE set of 8 launches (the layer's weights are shared by the two sides).
-static int run_attn_layer(opb_matcher* m, const Layout& L, XView x, AttnLayerW& W, int cross, cudaStream_t st) {
+static int run_attn_layer(opb_matcher* m, const Layout& L, XView x, int layer, AttnLayerW& W, int cross, cudaStream_t st) {
   const int rows = L.rows();
   const int S = L.segs();
   const double valid_rows = (double)L.B * (L.N + L.M);
@@ -217,18 +241,22 @@ static int run_attn_layer(opb_matcher* m, const Layout& L, XView x, AttnLayerW& 
   pk.epi = EPI_QKV; pk.out = Planes{m->kvt.as<__half>(), m->kvt.as<__half>(), 512};
   pk.a_hi_only = m->kv_two_pass;
   if (int rc = gemm(m, pk, st, 2.0 * valid_rows * 512 * kD, "kv_proj")) return rc;
+  if (stop_here(m, layer, 0, L, x)) return kStopped;
   // (2) linear-attention state of every segment (:71-78): per-row-group partial states on the tensor cores ...
   const KvGroups G = kv_groups_for(L, m->num_sms);
   if (int rc = launched(m, st, "kv_state_h", launch_kv_state_h(m->kvt.as<__half>(), L, G, m->kvpart.as<float>(), st))) return rc;
+  if (stop_here(m, layer, 1, L, x)) return kStopped;
   // ... reduced per segment into Kmean and the block-diagonal operand of the G fold (indexed by DESTINATION segment)
   LAUNCH(m, st, "kv_state_reduce", kv_state_reduce, dim3(S * kHeads, (kKVPartial + 255) / 256), dim3(256), 0, st, (const float*)m->kvpart.as<float>(), L,
          G, cross, m->kmean.as<float>(), m->bd.hi.as<__half>(), m->bd.lo.as<__half>());
+  if (stop_here(m, layer, 2, L, x)) return kStopped;
   // (3) q projection; epilogue: elu+1 and the per-head normaliser with the SOURCE segment's K mean -> Q' planes (:78-79)
   GemmProblem pq{};
   pq.L = L; pq.batch = 1; pq.rows = rows;
   pq.a1 = x.c(kD); pq.K1 = kD; pq.b1 = W.wqkv.c(kD); pq.n_out = 256; pq.bias = W.bqkv.as<float>();
   pq.epi = EPI_QSCALE; pq.kmean = m->kmean.as<float>(); pq.cross = cross; pq.out = m->qp.m(kD);
   if (int rc = gemm(m, pq, st, 2.0 * valid_rows * 256 * kD, "q_proj")) return rc;
+  if (stop_here(m, layer, 3, L, x)) return kStopped;
   // (4) dynamic weight G[s] = W0m . blockdiag(KVmean_src(s))^T  -- merge and the message half of mlp.0 folded into one
   //     per-segment [512, 256] weight (4 x 64x64x512 MACs per segment), as a batched wgmma GEMM over the segments
   GemmProblem pg{};
@@ -237,6 +265,7 @@ static int run_attn_layer(opb_matcher* m, const Layout& L, XView x, AttnLayerW& 
   pg.b1 = m->bd.c(kD); pg.b_batch_rows = kD;
   pg.epi = EPI_BIAS_PLANES; pg.out = m->g.m(kD);
   if (int rc = gemm(m, pg, st, 2.0 * S * 512.0 * kD * kDh, "g_fold")) return rc;
+  if (stop_here(m, layer, 4, L, x)) return kStopped;
   // (5) hidden = mlp.0([x ; message]) = [x | Q'] . [W0a | G_seg]^T + b   (:101,:113,:122); epilogue also emits the InstanceNorm
   //     partial sums (:126)
   GemmProblem p2{};
@@ -246,9 +275,11 @@ static int run_attn_layer(opb_matcher* m, const Layout& L, XView x, AttnLayerW& 
   p2.n_out = 512; p2.bias = W.b0f.as<float>(); p2.c = m->hid.as<float>(); p2.ldc = 512;
   p2.epi = EPI_F32_STATS; p2.statpart = m->statpart.as<float>();
   if (int rc = gemm(m, p2, st, 2.0 * valid_rows * 512 * 512, "mlp0")) return rc;
+  if (stop_here(m, layer, 5, L, x)) return kStopped;
   // (6) InstanceNorm statistics per segment (:126)
   LAUNCH(m, st, "in_stats_final", in_stats_final, dim3(S, 16), dim3(32, kStatSlices), 0, st, (const float*)m->statpart.as<float>(), L, m->mu.as<float>(),
          m->rstd.as<float>());
+  if (stop_here(m, layer, 6, L, x)) return kStopped;
   // (7) x <- x + mlp.3(ReLU(IN(hidden)))  (:122, :59/:64): the converters form hn inside the GEMM, the residual is an identity K-block
   GemmProblem p3{};
   p3.L = L; p3.batch = 1; p3.rows = rows;
@@ -256,7 +287,8 @@ static int run_attn_layer(opb_matcher* m, const Layout& L, XView x, AttnLayerW& 
   p3.epi = EPI_BIAS_PLANES; p3.out = x.m(kD);
   p3.a2 = x.c(kD); p3.K2 = kD; p3.b2 = m->eye.c(kD); p3.b2_lo_zero = 1; p3.b2_identity = m->identity_diag;
   p3.a_conv = 1; p3.a_raw = m->hid.as<float>(); p3.a_raw_ld = 512; p3.mu = m->mu.as<float>(); p3.rstd = m->rstd.as<float>();
-  return gemm(m, p3, st, 2.0 * valid_rows * 256 * 512, "mlp3");
+  if (int rc = gemm(m, p3, st, 2.0 * valid_rows * 256 * 512, "mlp3")) return rc;
+  return stop_here(m, layer, 7, L, x) ? kStopped : 0;
 }
 
 // Object prologue: GNN layers 0 (GATs) and the 3D side of layer 1 (self-attention) depend only on the per-object
@@ -274,8 +306,8 @@ static int object_prologue(opb_matcher* m, ObjectState& o, cudaStream_t st) {
   make_groups(g, &one, 1);
   LAUNCH(m, st, "assemble_layout", assemble_layout, dim3(m->num_sms * 2, 1), dim3(256), 0, st, (const __half*)nullptr, (const __half*)nullptr,
          t, tab_dev(m), o.xo.hi.as<__half>(), o.xo.lo.as<__half>(), Lo);
-  if (int rc = run_gats(m, Lo, o.xo.view(), 0, o.Lf, g, st)) return rc;
-  return run_attn_layer(m, Lo, o.xo.view(), m->attn[0], /*cross=*/0, st);
+  if (int rc = run_gats(m, Lo, o.xo.view(), kPrologueLayer + 0, o.Lf, g, st)) return rc;
+  return run_attn_layer(m, Lo, o.xo.view(), kPrologueLayer + 1, m->attn[0], /*cross=*/0, st);
 }
 
 // GNN + tail for the `fb` frames of a chunk; frame b matches against fobj[b].  Outputs: m1 / s1 rows and conf rows are M_out wide.
@@ -315,7 +347,7 @@ static int forward_chunk(opb_matcher* m, const ObjectState* const* fobj, const f
       XView xq = m->xq.view((size_t)p0 * L.n_pad);
       LAUNCH(m, st, "transpose_cf_to_rows", transpose_cf_to_rows<0>, dim3(L.n_pad / 32, sb), dim3(32, 8), 0, st, q_cf + (size_t)p0 * kD * N, N, N,
              (long long)kD * N, Lq.nlen, L.n_pad, xq.hi, xq.lo, (float*)nullptr, (long long)Lq.R, 0);
-      if (int rc = run_attn_layer(m, Lq, xq, m->attn[0], 0, st)) return rc;
+      if (int rc = run_attn_layer(m, Lq, xq, 1, m->attn[0], 0, st)) return rc;
     }
     // assemble the full layout: query rows from xq, 3D rows from each frame's object prologue
     LAUNCH(m, st, "assemble_layout", assemble_layout, dim3(m->num_sms * 2, fb), dim3(256), 0, st, (const __half*)m->xq.hi.as<__half>(),
@@ -331,10 +363,10 @@ static int forward_chunk(opb_matcher* m, const ObjectState* const* fobj, const f
 
   for (int layer = first_layer; layer < 12; ++layer) {
     if (layer % 3 == 0) {
-      if (int rc = run_gats(m, L, m->x.view(), layer / 3, Lf, groups, st)) return rc;
+      if (int rc = run_gats(m, L, m->x.view(), layer, Lf, groups, st)) return rc;
     } else {
       const int attn_idx = (layer / 3) * 2 + (layer % 3) - 1;
-      if (int rc = run_attn_layer(m, L, m->x.view(), m->attn[attn_idx], (layer % 3 == 2) ? 1 : 0, st)) return rc;
+      if (int rc = run_attn_layer(m, L, m->x.view(), layer, m->attn[attn_idx], (layer % 3 == 2) ? 1 : 0, st)) return rc;
     }
   }
 
@@ -348,6 +380,7 @@ static int forward_chunk(opb_matcher* m, const ObjectState* const* fobj, const f
   pf.bias = m->bf.as<float>();
   pf.epi = EPI_L2NORM; pf.out = m->pn.m(kD);       // F.normalize fused into the final_proj epilogue (:209-213)
   if (int rc = gemm(m, pf, st, 2.0 * valid_rows * kD * kD, "final_proj")) return rc;
+  if (stop_here(m, kTailLayer, 0, L, m->x.view())) return kStopped;
   // dual softmax + arg-max as two passes of the batched score GEMM (one batch = one frame); the cos matrix is never stored
   const int n_parts = (L.m_pad / 256) * 2, q_groups = L.n_pad / 32;
   GemmProblem ps{};
@@ -357,12 +390,15 @@ static int forward_chunk(opb_matcher* m, const ObjectState* const* fobj, const f
   ps.inv_scale = 1.f / m->cfg.scale_factor;
   ps.epi = EPI_SCORE_SUMS; ps.rowsum_part = m->rowsum_part.as<float>(); ps.colsum_part = m->colsum_part.as<float>();
   if (int rc = gemm(m, ps, st, 2.0 * (double)N * m_sum * kD, "score_sums")) return rc;
+  if (stop_here(m, kTailLayer, 1, L, m->x.view())) return kStopped;
   LAUNCH(m, st, "score_sums_finalize", score_sums_finalize, dim3((L.n_pad + L.m_pad + 255) / 256, fb), dim3(256), 0, st,
          (const float*)m->rowsum_part.as<float>(), (const float*)m->colsum_part.as<float>(), L, n_parts, q_groups, m->rowsum.as<float>(),
          m->colsum.as<float>(), m->rowbest.as<unsigned long long>(), m->colbest.as<unsigned long long>());
+  if (stop_here(m, kTailLayer, 2, L, m->x.view())) return kStopped;
   ps.epi = EPI_SCORE_CONF; ps.inv_rowsum = m->rowsum.as<float>(); ps.inv_colsum = m->colsum.as<float>();
   ps.conf = conf; ps.conf_ld = M_out; ps.rowbest = m->rowbest.as<unsigned long long>(); ps.colbest = m->colbest.as<unsigned long long>();
   if (int rc = gemm(m, ps, st, 0.0, "score_conf")) return rc;      // recomputation: its FLOPs are not algorithmic
+  if (stop_here(m, kTailLayer, 3, L, m->x.view())) return kStopped;
   if (conf && M_out > L.m_pad)                                          // conf rows wider than this chunk's 3D segments
     LAUNCH(m, st, "conf_fill_tail", conf_fill_tail, dim3(m->num_sms * 4), dim3(256), 0, st, conf, (long long)fb * N, M_out, L.m_pad);
   LAUNCH(m, st, "mutual_match", mutual_match, dim3(fb), dim3(256), 0, st, (const unsigned long long*)m->rowbest.as<unsigned long long>(),
@@ -412,6 +448,13 @@ static void invalidate_prologues(opb_matcher* m) {
   for (auto& kv : m->objects) kv.second.prologue_ready = false;
 }
 
+// A forward that reached the stop of opb_debug_set_stop: its buffers stay as they are for opb_debug_read.
+static int stopped(opb_matcher* m, cudaStream_t st) {
+  m->timeline.finish(st);
+  m->last_launches = m->launches;
+  return OPB_OK;
+}
+
 // The one forward of the handle: frame b of the call matches against fobj[b] (opb_forward: the current object everywhere).
 // m1 / s1 rows and conf rows are M_out >= max M_b wide.
 static int forward_frames(opb_matcher* m, ObjectState* const* fobj, const float* q, const int32_t* n2d_lengths, int B, int N, int M_out,
@@ -421,6 +464,7 @@ static int forward_frames(opb_matcher* m, ObjectState* const* fobj, const float*
   const int chunk = chunk_of(m, B);
   if (int rc = ensure_workspace(m, chunk, N, call_m_pad)) return rc;   // no-op once opb_reserve_workspace / an earlier call has sized it
   m->begin(st);
+  m->dbg_stopped = false;
   // per-object work on first use: leaf logits after a weight reload, the prologue (once per object, shared by all later calls)
   for (int b = 0; b < B; ++b) {
     ObjectState& o = *fobj[b];
@@ -429,7 +473,7 @@ static int forward_frames(opb_matcher* m, ObjectState* const* fobj, const float*
       o.s2_ready = true;
     }
     if (m->hoist && !o.prologue_ready) {
-      if (int rc = object_prologue(m, o, st)) return rc;
+      if (int rc = object_prologue(m, o, st)) return rc == kStopped ? stopped(m, st) : rc;
       o.prologue_ready = true;
     }
   }
@@ -444,7 +488,7 @@ static int forward_frames(opb_matcher* m, ObjectState* const* fobj, const float*
     int rc = forward_chunk(m, fobj + f0, q + (size_t)f0 * kD * N, n2d_lengths ? n2d_lengths + f0 : nullptr, N, fb, M_out, m0 + (size_t)f0 * N,
                            m1 + (size_t)f0 * M_out, s0 + (size_t)f0 * N, s1 + (size_t)f0 * M_out, conf ? conf + (size_t)f0 * N * M_out : nullptr,
                            st, piece, ci * ppc);
-    if (rc) return rc;
+    if (rc) return rc == kStopped ? stopped(m, st) : rc;
   }
   // deferred range report: the flag travels to pinned host memory behind the call; opb_poll_range() reads it without blocking
   CK(m, cudaMemcpyAsync(m->range_host, m->range_flag.p, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -878,6 +922,59 @@ int opb_debug_set_identity_diag(opb_matcher* m, int32_t enable) {
   if (!m) return OPB_E_INVALID;
   m->identity_diag = enable ? 1 : 0;
   invalidate_prologues(m);
+  return OPB_OK;
+}
+
+int opb_debug_set_stop(opb_matcher* m, int32_t layer, int32_t step) {
+  if (!m || layer < -1 || step < 0) return OPB_E_INVALID;
+  m->dbg_layer = layer;
+  m->dbg_step = step;
+  return OPB_OK;
+}
+
+int opb_debug_stopped_layout(const opb_matcher* m, int32_t* layout) {
+  if (!m || !layout || !m->dbg_stopped) return OPB_E_STATE;
+  const Layout& L = m->dbg_L;
+  const int32_t v[7] = {L.B, L.N, L.M, L.n_pad, L.m_pad, L.R, L.segs()};
+  for (int i = 0; i < 7; ++i) layout[i] = v[i];
+  return OPB_OK;
+}
+
+int opb_debug_read(opb_matcher* m, int32_t which, void* out, size_t capacity_elems, int64_t* n_elems, void* stream) {
+  if (!m || !out) return OPB_E_INVALID;
+  if (!m->dbg_stopped) return fail(m, OPB_E_STATE, "opb_debug_read: the last forward did not stop (opb_debug_set_stop)");
+  cudaStream_t st = (cudaStream_t)stream;
+  const Layout& L = m->dbg_L;
+  const size_t rows = (size_t)L.rows(), S = (size_t)L.segs();
+  const __half *hi = nullptr, *lo = nullptr;    // planes to join, or ...
+  const void* raw = nullptr;                    // ... 4- or 8-byte elements to copy
+  size_t n = 0, esize = sizeof(float);
+  switch (which) {
+    case 0: n = rows * kD; hi = m->dbg_x.hi; lo = m->dbg_x.lo; break;
+    case 1: n = rows * 512; hi = m->kvt.as<__half>(); break;
+    case 2: n = S * kD; raw = m->kmean.p; break;
+    case 3: n = S * kD * kD; hi = m->bd.hi.as<__half>(); lo = m->bd.lo.as<__half>(); break;
+    case 4: n = rows * kD; hi = m->qp.hi.as<__half>(); lo = m->qp.lo.as<__half>(); break;
+    case 5: n = S * 512 * kD; hi = m->g.hi.as<__half>(); lo = m->g.lo.as<__half>(); break;
+    case 6: n = rows * 512; raw = m->hid.p; break;
+    case 7: n = S * 512; raw = m->mu.p; break;
+    case 8: n = S * 512; raw = m->rstd.p; break;
+    case 9: n = rows * kD; hi = m->pn.hi.as<__half>(); lo = m->pn.lo.as<__half>(); break;
+    case 10: n = (size_t)L.B * L.n_pad; raw = m->rowsum.p; break;
+    case 11: n = (size_t)L.B * L.m_pad; raw = m->colsum.p; break;
+    case 12: n = (size_t)L.B * L.N; raw = m->rowbest.p; esize = 8; break;
+    case 13: n = (size_t)L.B * L.M; raw = m->colbest.p; esize = 8; break;
+    case 14:
+      if (!m->cfg.with_linear_transform) return fail(m, OPB_E_INVALID, "opb_debug_read: buffer 14 exists with with_linear_transform only");
+      n = (size_t)L.B * L.m_pad * kD; hi = m->lin_a.hi.as<__half>(); lo = m->lin_a.lo.as<__half>(); break;
+    default: return fail(m, OPB_E_INVALID, "opb_debug_read: unknown buffer %d", which);
+  }
+  if (n_elems) *n_elems = (int64_t)n;
+  if (n > capacity_elems) return fail(m, OPB_E_INVALID, "opb_debug_read: buffer %d has %zu elements, capacity %zu", which, n, capacity_elems);
+  if (n == 0) return OPB_OK;
+  if (raw) CK(m, cudaMemcpyAsync(out, raw, n * esize, cudaMemcpyDeviceToDevice, st));
+  else join_planes<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(hi, lo, (float*)out, (long long)n);
+  CK(m, cudaGetLastError());
   return OPB_OK;
 }
 

@@ -16,7 +16,7 @@ namespace opb {
 // Epilogue of the wgmma core (what happens to the accumulator tile before it leaves the SM):
 enum GemmEpilogue {
   EPI_F32 = 0,        // c[rows, ldc] fp32 = acc (+bias)
-  EPI_F32_STATS = 1,  // EPI_F32 + InstanceNorm partial sums (sum, sum^2 per 32-row quarter and column) -> statpart
+  EPI_F32_STATS = 1,  // EPI_F32 + InstanceNorm partials (sum, sum of squared deviations from the mean, per 32-row quarter and column) -> statpart
   EPI_QSCALE = 2,     // Q' = elu1(acc+bias) / (elu1(.) . Kmean_src + 1e-6/m_src) per head -> out planes   (n_out = 256)
   EPI_L2NORM = 5,     // F.normalize(acc + bias) over the 256 columns -> out planes                          (n_out = 256)
   // dual-softmax tail on the batched score GEMM (one batch = one frame; rows = queries, columns = 3D points):

@@ -554,18 +554,21 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
             tma_store_commit();
           }
           if (EPI == EPI_F32_STATS) {
-            // InstanceNorm partial sums straight from the staged tile: thread = (32-row quarter, column)
+            // InstanceNorm partials straight from the staged tile: thread = (32-row quarter, column); the sum and the sum of
+            // squared deviations from the quarter's mean, two passes over the 32 staged values (the one-pass sum(x^2) - n mean^2
+            // cancels catastrophically when a channel's mean is large against its spread)
             const int t = t_in_grp, qq = t >> 5, cc = t & 31;
-            float sum = 0.f, sq = 0.f;
             const int r_end = min(32, n_valid - qq * 32);
+            auto staged = [&](int i) { return *reinterpret_cast<const float*>(sb + stg_off(qq * 32 + i, cc >> 2) + (cc & 3) * 4); };
+            float sum = 0.f, m2 = 0.f;
+            for (int i = 0; i < r_end; ++i) sum += staged(i);
+            const float mq = r_end > 0 ? sum / (float)r_end : 0.f;
             for (int i = 0; i < r_end; ++i) {
-              const int r = qq * 32 + i;
-              const float x = *reinterpret_cast<const float*>(sb + stg_off(r, cc >> 2) + (cc & 3) * 4);
-              sum += x;
-              sq = fmaf(x, x, sq);
+              const float d = staged(i) - mq;
+              m2 = fmaf(d, d, m2);
             }
             float2* dst = reinterpret_cast<float2*>(p.statpart) + ((long long)(out_row0 / 32 + qq) * p.n_out + col0 + cc);
-            *dst = make_float2(sum, sq);
+            *dst = make_float2(sum, m2);
           }
         }
       } else if (EPI == EPI_QKV) {

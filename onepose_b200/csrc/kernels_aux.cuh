@@ -417,14 +417,19 @@ __global__ void kv_state_reduce(const float* __restrict__ partial, Layout L, KvG
 // ---------------------------------------------------------------------------------------
 // InstanceNorm1d(512) statistics over the valid rows of each segment
 // (reference GATs_SuperGlue.py:126: no affine, biased variance, eps 1e-5).
-// Stage 1: per 32-row quarter and channel: sum, sum of squares (fp32) -- written by the mlp.0 GEMM epilogue (EPI_F32_STATS).
-// Stage 2, here: per (segment, channel): fixed-order fp64 combine -> mean, rstd.
+// Stage 1: per 32-row quarter and channel: sum and sum of squared deviations from the quarter's mean (fp32) -- written by the
+// mlp.0 GEMM epilogue (EPI_F32_STATS).
+// Stage 2, here: per (segment, channel): fixed-order fp64 combine of the quarters -> mean, rstd.  The quarters' deviations
+// are taken about a shift common to the whole segment, K = quarter 0's mean (law of total variance, the parallel form of
+// Chan, Golub and LeVeque):  with u_t = s_t - n_t K,
+//   M2 = sum_t M2_t + sum_t u_t^2 / n_t - (sum_t u_t)^2 / n,   mean = K + (sum_t u_t) / n
+// -- plain sums, so the slices combine by addition and the loop has no division (n_t = 32 except in the last quarter).
 // grid (S, 16), block (32 channels, kStatSlices slices): the slices keep enough independent loads in flight that the kernel is
 // not a chain of dependent L2 round trips (8 slices: 17 us per launch at 224 quarters per segment)
 // ---------------------------------------------------------------------------------------
 constexpr int kStatSlices = 32;
 __global__ void __launch_bounds__(32 * kStatSlices) in_stats_final(const float* __restrict__ part, Layout L, float* __restrict__ mu, float* __restrict__ rstd) {
-  __shared__ double sh[kStatSlices][32][2];
+  __shared__ double sh[kStatSlices][32][3];
   griddep_sync();
   const int seg = blockIdx.x;
   const int c = blockIdx.y * 32 + threadIdx.x;
@@ -432,24 +437,31 @@ __global__ void __launch_bounds__(32 * kStatSlices) in_stats_final(const float* 
   const int q0 = L.seg_start(seg) / 32;
   const int valid = L.seg_valid(seg);
   const int nq = (valid + 31) / 32;
-  double s = 0.0, s2 = 0.0;
+  const float2* p = reinterpret_cast<const float2*>(part) + (long long)q0 * 512 + c;
+  const int n_last = valid - 32 * (nq - 1);                      // rows of the last quarter
+  const double K = nq > 0 ? (double)p[0].x / (double)(nq > 1 ? 32 : n_last) : 0.0;
+  const double inv_last = nq > 0 ? 1.0 / (double)n_last : 0.0;
+  double u = 0.0, uu = 0.0, m2 = 0.0;
   for (int t = slice; t < nq; t += kStatSlices) {
-    const float2 v = reinterpret_cast<const float2*>(part)[(long long)(q0 + t) * 512 + c];
-    s += (double)v.x;
-    s2 += (double)v.y;
+    const float2 v = p[(long long)t * 512];
+    const bool last = t == nq - 1;
+    const double ut = fma(-(double)(last ? n_last : 32), K, (double)v.x);
+    u += ut;
+    uu = fma(ut * ut, last ? inv_last : 1.0 / 32.0, uu);
+    m2 += (double)v.y;
   }
-  sh[slice][threadIdx.x][0] = s;
-  sh[slice][threadIdx.x][1] = s2;
+  sh[slice][threadIdx.x][0] = u;
+  sh[slice][threadIdx.x][1] = uu;
+  sh[slice][threadIdx.x][2] = m2;
   __syncthreads();
   if (slice == 0) {
-    s = 0.0; s2 = 0.0;
+    u = 0.0; uu = 0.0; m2 = 0.0;
 #pragma unroll
-    for (int k = 0; k < kStatSlices; ++k) { s += sh[k][threadIdx.x][0]; s2 += sh[k][threadIdx.x][1]; }
+    for (int k = 0; k < kStatSlices; ++k) { u += sh[k][threadIdx.x][0]; uu += sh[k][threadIdx.x][1]; m2 += sh[k][threadIdx.x][2]; }
     const double n = (double)(valid > 0 ? valid : 1);
-    const double mean = s / n;
-    double var = s2 / n - mean * mean;
+    double var = (m2 + uu - u * u / n) / n;
     if (var < 0.0) var = 0.0;
-    mu[seg * 512 + c] = (float)mean;
+    mu[seg * 512 + c] = (float)(K + u / n);
     rstd[seg * 512 + c] = (float)(1.0 / sqrt(var + 1e-5));
   }
 }
@@ -473,6 +485,11 @@ __global__ void range_check(const __half* __restrict__ x_hi, long long n_vec /* 
 __global__ void split_planes(const float* __restrict__ x, __half* __restrict__ hi, __half* __restrict__ lo, long long n) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i < n) split_f32(x[i], hi[i], lo[i]);
+}
+// planes -> fp32: (hi + lo) / 64; lo = nullptr reads a single fp16 plane (the k,v projection's output) as hi / 64
+__global__ void join_planes(const __half* __restrict__ hi, const __half* __restrict__ lo, float* __restrict__ x, long long n) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n) x[i] = lo ? join_f32(hi[i], lo[i]) : __half2float(hi[i]) * kPreInv;
 }
 
 // ---------------------------------------------------------------------------------------

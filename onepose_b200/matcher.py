@@ -341,6 +341,40 @@ class GATsSuperGlue(nn.Module):
     def launch_count(self) -> int:
         return int(self._lib.opb_last_launch_count(self._handle)) if self._handle is not None else 0
 
+    # ------------------------------------------------------------------ test hooks (opb_debug_set_stop / opb_debug_read)
+    DEBUG_BUFFERS = {"x": 0, "kvt": 1, "kmean": 2, "bd": 3, "qp": 4, "g": 5, "hid": 6, "mu": 7, "rstd": 8, "pn": 9,
+                     "inv_rowsum": 10, "inv_colsum": 11, "rowbest": 12, "colbest": 13, "gats_pre": 14}
+
+    def debug_stop_after(self, layer: int, step: int = 0):
+        """Stop the next call after step `step` of GNN layer `layer` (12 = tail, 16 / 17 = the object prologue's layers 0 / 1;
+        see opb_debug_set_stop); -1 runs everything."""
+        _lib.check(self._lib.opb_debug_set_stop(self._handle, int(layer), int(step)), self._handle)
+
+    def debug_layout(self) -> dict:
+        """Layout of the pass the last call stopped in: B, N, M, n_pad, m_pad, R, S."""
+        v = (C.c_int32 * 7)()
+        _lib.check(self._lib.opb_debug_stopped_layout(self._handle, v), self._handle)
+        return dict(zip(("B", "N", "M", "n_pad", "m_pad", "R", "S"), list(v)))
+
+    def debug_read(self, name: str) -> torch.Tensor:
+        """A buffer of the stopped pass (opb_debug_read), shaped: [rows, C] / [S, ...] / [B, ...] (int64 for the arg-maxes)."""
+        L = self.debug_layout()
+        rows, S, B = L["B"] * L["R"], L["S"], L["B"]
+        shapes = {"x": (rows, 256), "kvt": (rows, 512), "kmean": (S, 256), "bd": (S, 256, 256), "qp": (rows, 256), "g": (S, 512, 256),
+                  "hid": (rows, 512), "mu": (S, 512), "rstd": (S, 512), "pn": (rows, 256), "inv_rowsum": (B, L["n_pad"]),
+                  "inv_colsum": (B, L["m_pad"]), "rowbest": (B, L["N"]), "colbest": (B, L["M"]), "gats_pre": (B * L["m_pad"], 256)}
+        shape = shapes[name]
+        n_want = 1
+        for d in shape:
+            n_want *= d
+        dtype = torch.int64 if name in ("rowbest", "colbest") else torch.float32
+        out = torch.empty(max(n_want, 1), dtype=dtype, device=self._handle_device)
+        n = C.c_int64()
+        st = torch.cuda.current_stream(self._handle_device).cuda_stream
+        _lib.check(self._lib.opb_debug_read(self._handle, self.DEBUG_BUFFERS[name], out.data_ptr(), out.numel(), C.byref(n), st),
+                   self._handle)
+        return out[:n.value].view(shape)
+
     # ------------------------------------------------------------------ reference contract
     @staticmethod
     def _tensor_key(t: torch.Tensor):
