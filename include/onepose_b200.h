@@ -237,6 +237,19 @@ int opb_sp_describe(opb_superpoint* h, float* keypoints, float* scores, float* d
 /* Both halves with a caller-chosen capacity, no host synchronisation (cap >= max_keypoints makes it exact). */
 int opb_sp_forward(opb_superpoint* h, const float* image, int32_t B, int32_t H, int32_t W, float* keypoints, float* scores,
                    float* descriptors, int32_t* counts, int32_t cap, void* stream);
+/* Range guard of the fp16-split operand format (|x| < 1023 per plane element), as for the matcher.  conv1a and every 3x3
+ * convolution check what they split: a value at |x| >= 1023 (after the ReLU), or an inf / NaN image pixel, raises a flag.
+ * opb_sp_finalize_weights refuses (OPB_E_RANGE) a weight or bias that is not finite, or a weight of a tensor-core layer
+ * (all but conv1a) at |w| >= 1023; with those excluded no NaN can arise that the check would not see.  A call that raised
+ * the flag reports count 0 for every image, on the device and without blocking, and the error is delivered to the host
+ * lazily:
+ *   opb_sp_poll_range   never blocks: OPB_E_RANGE if a finished earlier call raised the flag, OPB_OK otherwise (also while
+ *                       the last call is still running).  opb_sp_detect (and so opb_sp_forward) calls it first, and returns
+ *                       its error without running;
+ *   opb_sp_check_range  waits for the last opb_sp_detect and reports.
+ * Reporting clears the flag. */
+int opb_sp_check_range(opb_superpoint* h, void* stream);
+int opb_sp_poll_range(opb_superpoint* h);
 int opb_sp_last_launch_count(const opb_superpoint* h);
 /* bench.py hooks: with profiling on, an event follows every launch of opb_sp_detect / opb_sp_describe; entry i = launch i
  * (name, milliseconds, algorithmic FLOPs of a convolution: 2 * interior pixels * C_out * 9 * C_in). */

@@ -80,6 +80,8 @@ SYMBOLS = {
     "opb_sp_detect": (C.c_int, [_P, _P, _I, _I, _I, _P, _P]),
     "opb_sp_describe": (C.c_int, [_P, _P, _P, _P, _P, _I, _P]),
     "opb_sp_forward": (C.c_int, [_P, _P, _I, _I, _I, _P, _P, _P, _P, _I, _P]),
+    "opb_sp_check_range": (C.c_int, [_P, _P]),
+    "opb_sp_poll_range": (C.c_int, [_P]),
     "opb_sp_last_launch_count": (C.c_int, [_P]),
     "opb_sp_set_profiling": (C.c_int, [_P, _I]),
     "opb_sp_get_profile": (C.c_int, [_P, _I, C.c_char_p, C.c_size_t, C.POINTER(C.c_double), C.POINTER(C.c_double)]),

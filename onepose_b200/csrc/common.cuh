@@ -17,6 +17,14 @@ constexpr int kSegPad = 256;   // segments are padded to this: 2 row tiles / one
 constexpr float kPre = 64.0f;
 constexpr float kPreInv = 1.0f / 64.0f;
 constexpr float kProdInv = 1.0f / 4096.0f;
+// Smallest pre-scaled value whose hi plane rounds to fp16 inf (65504 + half an ulp): a split of 64 x at or above it stores
+// hi = inf, lo = -inf, and the next product turns into NaN.
+constexpr float kSplitLimit = 65520.0f;
+// Range guard of the extractor's producers of split planes: `peak` is the largest pre-scaled |value| a thread split.  A
+// running fmaxf ignores NaN, so NaN is excluded where it could enter instead: the weights are checked on the host
+// (opb_sp_finalize_weights) and the image in sp_conv1a; from finite in-range operands a convolution can only produce finite
+// values, which the peak sees.
+__host__ __device__ __forceinline__ bool split_out_of_range(float peak) { return !(peak < kSplitLimit); }
 
 // Activation layout of one forward chunk: frame b owns rows
 //   [b*R, b*R + n_pad)           query segment   (N valid)

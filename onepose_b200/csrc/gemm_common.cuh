@@ -55,6 +55,7 @@ struct GemmProblem {
   // EPI_CONV: pixel-grid geometry (row r is pixel q = r % cv_ppad of its image; y = q / cv_w2, x = q % cv_w2; interior:
   // 1 <= y <= cv_h, 1 <= x <= cv_w) and the activation
   int cv_w2, cv_h, cv_w, cv_ppad, relu;
+  int* range_flag;       // EPI_CONV: set to 1 when an output leaves the split operand range (split_out_of_range), or nullptr
   int batch;
   long long a_batch_rows, b_batch_rows, c_batch_elems;
   Layout L;

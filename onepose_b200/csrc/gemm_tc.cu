@@ -140,6 +140,7 @@ struct TcParams {
   int taps, kb_per_tap;
   int tap_off[9];
   int cv_w2, cv_h, cv_w, cv_ppad, relu;
+  int* range_flag;       // GemmProblem::range_flag
   int halo;              // 3x3 convolution with one (BM + 2)-row A box per (kernel row, 64-channel block)
 };
 
@@ -740,6 +741,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
           row_ok = r_in_tile < n_valid;
         }
         const bool relu = EPI == EPI_CONV && p.relu;
+        float peak = 0.f;              // EPI_CONV range guard: the largest |output| of this thread's row (see split_out_of_range)
 #pragma unroll 1
         for (int c0 = c_begin; c0 < c_end; c0 += 32) {
           uint32_t v[32];
@@ -749,9 +751,11 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
             const float2 bb = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + col0) + j) : make_float2(0.f, 0.f);
             float2 sc = make_float2(fmaf(__uint_as_float(v[2 * j]), kPreInv, bb.x * kPre), fmaf(__uint_as_float(v[2 * j + 1]), kPreInv, bb.y * kPre));
             if (relu) sc = make_float2(fmaxf(sc.x, 0.f), fmaxf(sc.y, 0.f));
+            if (EPI == EPI_CONV) peak = fmaxf(peak, fmaxf(fabsf(sc.x), fabsf(sc.y)));
             return row_ok ? sc : make_float2(0.f, 0.f);
           });
         }
+        if (EPI == EPI_CONV && __any_sync(0xffffffffu, row_ok && split_out_of_range(peak)) && lane == 0 && p.range_flag) atomicOr(p.range_flag, 1);
       } else {
         // ---- planes out (row-major, 64 columns per chunk): EPI_QSCALE / EPI_L2NORM
         float inv_norm = 1.f;
@@ -993,7 +997,7 @@ int launch_gemm_tc(const GemmProblem& p, cudaStream_t stream) {
   tp.m_tiles = p.rows / BM; tp.n_tiles = p.n_out / bn; tp.batch = p.batch;
   tp.taps = p.taps; tp.kb_per_tap = p.kb_per_tap;
   for (int t = 0; t < 9; ++t) tp.tap_off[t] = p.tap_off[t];
-  tp.cv_w2 = p.cv_w2; tp.cv_h = p.cv_h; tp.cv_w = p.cv_w; tp.cv_ppad = p.cv_ppad; tp.relu = p.relu; tp.halo = halo;
+  tp.cv_w2 = p.cv_w2; tp.cv_h = p.cv_h; tp.cv_w = p.cv_w; tp.cv_ppad = p.cv_ppad; tp.relu = p.relu; tp.range_flag = p.range_flag; tp.halo = halo;
   tp.a_batch_rows = p.a_batch_rows; tp.b_batch_rows = p.b_batch_rows; tp.c_batch_rows = p.rows;
   tp.seg_rows = (p.batch == 1 && p.L.R > 0 && p.L.rows() == p.rows) ? 1 : 0;
   tp.L = p.L; tp.bias = p.bias;

@@ -10,6 +10,7 @@
 // again a valid zero-bordered input.  Arithmetic: the same 3-pass fp16-split product as the matcher (fp32 semantics; the
 // reference network is fp32).  Everything that is not a GEMM (first layer with one input channel, 2x2 pooling, 65-way softmax
 // + pixel shuffle, NMS, ordered key-point compaction, top-k, bilinear descriptor sampling) is a plain bandwidth-bound kernel.
+#include <cfloat>
 #include <cmath>
 #include <cstring>
 #include <string>
@@ -32,7 +33,8 @@ constexpr int kSelChunk = 2048;          // pixels per block of the key-point co
 // channels); writes the zero-bordered planes of the first GEMM layer.  img fp32 [B, H, W].
 // ------------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256) sp_conv1a(const float* __restrict__ img, int H, int W, int ppad, const float* __restrict__ w,
-                                                 const float* __restrict__ bias, __half* __restrict__ ohi, __half* __restrict__ olo) {
+                                                 const float* __restrict__ bias, __half* __restrict__ ohi, __half* __restrict__ olo,
+                                                 int* __restrict__ range_flag) {
   griddep_sync();
   // grid (chunks of 256 grid pixels, image); thread = (pixel, 4-channel group g): g is fixed per thread (256 % 16 == 0), so its
   // 4 x 9 weights and 4 biases live in registers; 16 lanes = one 128-byte plane row per store instruction.  All index math is
@@ -49,6 +51,8 @@ __global__ void __launch_bounds__(256) sp_conv1a(const float* __restrict__ img, 
   const float* im = img + (size_t)b * H * W;
   const unsigned w2 = (unsigned)(W + 2);
   const size_t row_base = (size_t)b * ppad;
+  float peak = 0.f;                 // range guard: the largest split value, and whether an image pixel is inf / NaN
+  bool bad_pixel = false;
 #pragma unroll 4
   for (int it = 0; it < 16; ++it) {
     const unsigned q = blockIdx.x * 256u + it * 16u + (threadIdx.x >> 4);
@@ -73,6 +77,7 @@ __global__ void __launch_bounds__(256) sp_conv1a(const float* __restrict__ img, 
             in[ky * 3 + kx] = (yy >= 0 && yy < H && xx >= 0 && xx < W) ? __ldg(im + yy * W + xx) : 0.f;
           }
       }
+      bad_pixel |= !(fabsf(in[4]) <= FLT_MAX);                   // every pixel is the centre of one grid row
       float v[4];
 #pragma unroll
       for (int e = 0; e < 4; ++e) {
@@ -80,6 +85,7 @@ __global__ void __launch_bounds__(256) sp_conv1a(const float* __restrict__ img, 
 #pragma unroll
         for (int k = 0; k < 9; ++k) acc = fmaf(wr[e][k], in[k], acc);
         v[e] = fmaxf(acc + br[e], 0.f) * kPre;
+        peak = fmaxf(peak, v[e]);
       }
 #pragma unroll
       for (int e = 0; e < 2; ++e) {
@@ -93,6 +99,7 @@ __global__ void __launch_bounds__(256) sp_conv1a(const float* __restrict__ img, 
     reinterpret_cast<uint2*>(ohi)[(row_base + q) * 16 + g] = oh;
     reinterpret_cast<uint2*>(olo)[(row_base + q) * 16 + g] = ol;
   }
+  if (__any_sync(0xffffffffu, bad_pixel || split_out_of_range(peak)) && (threadIdx.x & 31) == 0) atomicOr(range_flag, 1);   // every thread gets here
 }
 
 // ------------------------------------------------------------------------------------------------------------------
@@ -323,7 +330,8 @@ __global__ void __launch_bounds__(256) sp_compact(const float* __restrict__ nms,
 // (torch.topk, superpoint.py:72-76; equal scores: lower pixel index first).  Rank by counting: candidate i goes to position
 // #{j : key_j > key_i}; O(n^2) comparisons on at most a few 10^4 candidates.  Key points are (x, y) floats (superpoint.py:177).
 __global__ void __launch_bounds__(256) sp_emit(const int* __restrict__ cand_idx, const float* __restrict__ cand_score, const int* __restrict__ totals, int HW,
-                                               int W, int k, int cap, float* __restrict__ kpts, float* __restrict__ kscores, int* __restrict__ counts) {
+                                               int W, int k, int cap, const int* __restrict__ range_flag, float* __restrict__ kpts,
+                                               float* __restrict__ kscores, int* __restrict__ counts) {
   // key = (score bits, ~pixel index): scores are positive floats (> threshold >= 0 is not required: the sign bit is flipped
   // into an order-preserving unsigned), so one 64-bit compare orders by (score descending, index ascending)
   __shared__ unsigned long long tk[1024];
@@ -331,7 +339,7 @@ __global__ void __launch_bounds__(256) sp_emit(const int* __restrict__ cand_idx,
   const int b = blockIdx.y;
   const int total = totals[b];
   const int sel = (k >= 0 && total > k) ? k : total;
-  const int n_out = sel < cap ? sel : cap;
+  const int n_out = *range_flag ? 0 : (sel < cap ? sel : cap);     // a call that left the operand range emits nothing
   if (blockIdx.x == 0 && threadIdx.x == 0) counts[b] = n_out;
   const int i0 = blockIdx.x * 256;
   if (i0 >= total) return;
@@ -426,10 +434,10 @@ __global__ void __launch_bounds__(256) sp_sample(const float* __restrict__ ddesc
   for (int e = 0; e < 8; ++e) out[((long long)b * 256 + lane * 8 + e) * cap + i] = acc[e] * inv;
 }
 
-__global__ void sp_counts_out(const int* __restrict__ totals, int k, int n, int* __restrict__ counts) {
+__global__ void sp_counts_out(const int* __restrict__ totals, int k, int n, const int* __restrict__ range_flag, int* __restrict__ counts) {
   griddep_sync();
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i < n) counts[i] = (k >= 0 && totals[i] > k) ? k : totals[i];
+  if (i < n) counts[i] = *range_flag ? 0 : (k >= 0 && totals[i] > k) ? k : totals[i];
 }
 
 __global__ void sp_join_planes(const __half* __restrict__ hi, const __half* __restrict__ lo, float* __restrict__ out, long long n) {
@@ -457,15 +465,36 @@ struct opb_superpoint : Handle {
   int ws_B = 0, ws_H = 0, ws_W = 0;
   PlaneBuf arena[2];               // ping-pong activations
   DevBuf logits, ddesc, scores, nms, cand_idx, cand_score, blk_counts, totals;
+  // range guard (opb_sp_check_range): the device flag, its pinned copy written at the end of every opb_sp_detect
+  DevBuf range_flag;
+  int* range_host = nullptr;
+  cudaEvent_t range_ev = nullptr;
+  bool range_pending = false;
+  cudaStream_t last_stream = nullptr;
   int last_B = 0, last_H = 0, last_W = 0;
   int stop_after = -1;             // test hook: leave the encoder after layer i (opb_sp_debug_set_stop)
   int dbg_arena = 0, dbg_c = 0;
   long long dbg_rows = 0;
+  ~opb_superpoint() {
+    if (range_ev) cudaEventDestroy(range_ev);
+    if (range_host) cudaFreeHost(range_host);
+  }
 };
 
 namespace {
 
 thread_local std::string g_sp_create_error;
+
+// The range guard's premise (split_out_of_range): finite weights and biases, and weights that split (|64 w| < 65 520)
+template <typename V>
+int sp_check_weights(opb_superpoint* h, const std::string& name, const V& w, const V& b, bool split) {
+  for (const auto& x : w)
+    if (!std::isfinite((float)x) || (split && split_out_of_range(std::fabs((float)x) * kPre)))
+      return fail(h, OPB_E_RANGE, "%s.weight holds %g: weights must be finite%s", name.c_str(), (double)x, split ? " and within the fp16-split range (|w| < 1023)" : "");
+  for (const auto& x : b)
+    if (!std::isfinite((float)x)) return fail(h, OPB_E_RANGE, "%s.bias holds %g: biases must be finite", name.c_str(), (double)x);
+  return OPB_OK;
+}
 
 // Pack one or two conv layers [cout, cin, k, k] (k = 3 or 1) that share their input into the B operand [cout_total (padded to
 // cout_pad), taps*cin] with reduction index tap*cin + c (tap = ky*3 + kx), plus the bias.
@@ -480,6 +509,7 @@ int sp_pack(opb_superpoint* h, SpConv& L, const std::vector<std::string>& names,
     const auto* ww = find_weight(h, names[li] + ".weight", (size_t)cout * cin * taps);
     const auto* bb = find_weight(h, names[li] + ".bias", (size_t)cout);
     if (!ww || !bb) return h->find_code;
+    if (int rc = sp_check_weights(h, names[li], *ww, *bb, true)) return rc;
     for (int n = 0; n < cout; ++n) {
       for (int c = 0; c < cin; ++c)
         for (int t = 0; t < taps; ++t) w[(size_t)(row0 + n) * K + (size_t)t * cin + c] = (*ww)[((size_t)n * cin + c) * taps + t];
@@ -519,6 +549,7 @@ int sp_ensure_workspace(opb_superpoint* h, int B, int H, int W) {
   CK(h, h->cand_score.ensure(Bc * HW * sizeof(float)));
   CK(h, h->blk_counts.ensure((size_t)Bc * ((HW + kSelChunk - 1) / kSelChunk) * sizeof(int)));
   CK(h, h->totals.ensure((size_t)Bc * sizeof(int)));
+  CK(h, h->range_flag.ensure(sizeof(int), true));
   CK(h, cudaDeviceSynchronize());
   h->ws_B = Bc; h->ws_H = H; h->ws_W = W;
   return 0;
@@ -537,6 +568,7 @@ int sp_run_conv(opb_superpoint* h, const SpConv& L, const PlaneBuf& in, int in_l
   p.bias = L.b.as<float>();
   if (outp) {
     p.epi = EPI_CONV;
+    p.range_flag = h->range_flag.as<int>();
     p.out = outp->m(out_ld);
     p.cv_w2 = g.w + 2; p.cv_h = g.h; p.cv_w = g.w; p.cv_ppad = g.ppad; p.relu = relu;
     if (L.taps == 9) {
@@ -570,6 +602,11 @@ int opb_sp_create(const opb_sp_config* cfg, opb_superpoint** out) {
   if (int rc = select_device(cfg->device, prop, g_sp_create_error)) return rc;
   auto* h = new opb_superpoint();
   h->cfg = *cfg;
+  if (cudaMallocHost(&h->range_host, sizeof(int)) != cudaSuccess || cudaEventCreateWithFlags(&h->range_ev, cudaEventDisableTiming) != cudaSuccess) {
+    delete h;
+    return fail(g_sp_create_error, OPB_E_CUDA, "pinned flag / event allocation failed");
+  }
+  *h->range_host = 0;
   *out = h;
   return OPB_OK;
 }
@@ -595,6 +632,7 @@ int opb_sp_finalize_weights(opb_superpoint* h) {
   const auto* w1 = find_weight(h, "conv1a.weight", 64 * 9);
   const auto* b1 = find_weight(h, "conv1a.bias", 64);
   if (!w1 || !b1) return h->find_code;
+  if (int rc = sp_check_weights(h, "conv1a", *w1, *b1, false)) return rc;
   if (int rc = upload_f32(h, h->w1a, std::vector<double>(w1->begin(), w1->end()))) return rc;
   if (int rc = upload_f32(h, h->b1a, std::vector<double>(b1->begin(), b1->end()))) return rc;
   if (int rc = sp_pack(h, h->c1b, {"conv1b"}, 64, {64}, 3, 64, 64)) return rc;
@@ -619,6 +657,7 @@ int opb_sp_detect(opb_superpoint* h, const float* image, int32_t B, int32_t H, i
   if (!h->ready) return fail(h, OPB_E_STATE, "weights not finalized");
   if (H % 8 || W % 8) return fail(h, OPB_E_INVALID, "image size %dx%d: height and width must be multiples of 8 (three 2x2 poolings)", H, W);
   if ((long long)B * stage_of(H, W, 0).ppad > 0x7fffff00LL) return fail(h, OPB_E_INVALID, "batch too large for 32-bit row indices");
+  if (int rc = opb_sp_poll_range(h)) return rc;             // deferred report of a finished earlier call
   if (int rc = sp_ensure_workspace(h, B, H, W)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   h->begin(st);
@@ -634,7 +673,7 @@ int opb_sp_detect(opb_superpoint* h, const float* image, int32_t B, int32_t H, i
   };
   // ---- shared encoder (superpoint.py:142-152)
   LAUNCH(h, st, "sp_conv1a", sp_conv1a, dim3((s0.ppad + 255) / 256, B), dim3(256), 0, st, image, (int)H, (int)W, s0.ppad, (const float*)h->w1a.as<float>(),
-          (const float*)h->b1a.as<float>(), A.hi.as<__half>(), A.lo.as<__half>());
+          (const float*)h->b1a.as<float>(), A.hi.as<__half>(), A.lo.as<__half>(), h->range_flag.as<int>());
   if (stopped(0, 0, 64, s0)) return OPB_OK;
   if (int rc = sp_run_conv(h, h->c1b, A, 64, 0, &Bf, nullptr, 64, s0, B, 1, st, "conv1b")) return rc;
   if (stopped(1, 1, 64, s0)) return OPB_OK;
@@ -685,7 +724,13 @@ int opb_sp_detect(opb_superpoint* h, const float* image, int32_t B, int32_t H, i
           h->cfg.remove_borders, (const int*)h->blk_counts.as<int>(), h->cand_idx.as<int>(), h->cand_score.as<float>(), h->totals.as<int>());
   h->last_B = B; h->last_H = H; h->last_W = W;
   if (counts)     // number of key points opb_sp_describe will emit: min(total, max_keypoints)
-    LAUNCH(h, st, "sp_counts_out", sp_counts_out, dim3((B + 127) / 128), dim3(128), 0, st, (const int*)h->totals.as<int>(), h->cfg.max_keypoints, (int)B, counts);
+    LAUNCH(h, st, "sp_counts_out", sp_counts_out, dim3((B + 127) / 128), dim3(128), 0, st, (const int*)h->totals.as<int>(), h->cfg.max_keypoints, (int)B,
+           (const int*)h->range_flag.as<int>(), counts);
+  // deferred range report: every producer of split planes has run; the flag travels to pinned host memory behind the call
+  CK(h, cudaMemcpyAsync(h->range_host, h->range_flag.p, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CK(h, cudaEventRecord(h->range_ev, st));
+  h->range_pending = true;
+  h->last_stream = st;
   return OPB_OK;
 }
 
@@ -696,7 +741,7 @@ int opb_sp_describe(opb_superpoint* h, float* keypoints, float* scores, float* d
   const int B = h->last_B, H = h->last_H, W = h->last_W, HW = H * W;
   const Stage s3 = stage_of(H, W, 3);
   LAUNCH(h, st, "sp_emit", sp_emit, dim3((HW + 255) / 256, B), dim3(256), 0, st, (const int*)h->cand_idx.as<int>(), (const float*)h->cand_score.as<float>(),
-          (const int*)h->totals.as<int>(), HW, W, h->cfg.max_keypoints, (int)cap, keypoints, scores, counts);
+          (const int*)h->totals.as<int>(), HW, W, h->cfg.max_keypoints, (int)cap, (const int*)h->range_flag.as<int>(), keypoints, scores, counts);
   if (descriptors)
     LAUNCH(h, st, "sp_sample", sp_sample, dim3(((long long)cap * 32 + 255) / 256, B), dim3(256), 0, st, (const float*)h->ddesc.as<float>(), s3.h, s3.w, s3.ppad,
             (const float*)keypoints, (const int*)counts, (int)cap, h->cfg.align_corners, descriptors);
@@ -707,6 +752,31 @@ int opb_sp_forward(opb_superpoint* h, const float* image, int32_t B, int32_t H, 
                    int32_t* counts, int32_t cap, void* stream) {
   if (int rc = opb_sp_detect(h, image, B, H, W, nullptr, stream)) return rc;
   return opb_sp_describe(h, keypoints, scores, descriptors, counts, cap, stream);
+}
+
+// Consume the range flag.  After the event of the last opb_sp_detect has completed, the pinned copy is current.
+static int sp_consume_range_flag(opb_superpoint* h) {
+  h->range_pending = false;
+  if (*h->range_host == 0) return OPB_OK;
+  *h->range_host = 0;
+  CK(h, cudaMemsetAsync(h->range_flag.p, 0, sizeof(int), h->last_stream));
+  return fail(h, OPB_E_RANGE, "an activation left the fp16-split operand range (|x| >= 1023) or became NaN: the call reported no key "
+                              "points (count 0) for every image");
+}
+
+int opb_sp_check_range(opb_superpoint* h, void* stream) {
+  if (!h || !h->range_pending) return OPB_OK;
+  (void)stream;
+  CK(h, cudaEventSynchronize(h->range_ev));
+  return sp_consume_range_flag(h);
+}
+
+int opb_sp_poll_range(opb_superpoint* h) {
+  if (!h || !h->range_pending) return OPB_OK;
+  const cudaError_t q = cudaEventQuery(h->range_ev);
+  if (q == cudaErrorNotReady) return OPB_OK;               // the call is still running: report on a later poll / check
+  if (q != cudaSuccess) return fail(h, OPB_E_CUDA, "cudaEventQuery: %s", cudaGetErrorString(q));
+  return sp_consume_range_flag(h);
 }
 
 int opb_sp_last_launch_count(const opb_superpoint* h) { return h ? h->launches : 0; }

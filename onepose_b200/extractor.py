@@ -103,7 +103,9 @@ class SuperPoint(nn.Module):
     @torch.no_grad()
     def forward_padded(self, inp: torch.Tensor, cap: int | None = None, descriptors: bool = True):
         """Fixed-capacity outputs, no host synchronisation: keypoints [B, cap, 2], scores [B, cap], descriptors [B, 256, cap],
-        counts int32 [B] (entries >= counts[b] are unspecified).  cap defaults to max_keypoints (which must then be >= 0)."""
+        counts int32 [B] (entries >= counts[b] are unspecified).  cap defaults to max_keypoints (which must then be >= 0).
+        A call whose activations leave the operand range reports count 0 everywhere (see check_range); its error is raised by
+        check_range() or by a later call."""
         img, st = self._prepare(inp)
         B, _, H, W = img.shape
         if cap is None:
@@ -130,6 +132,7 @@ class SuperPoint(nn.Module):
         cnt = torch.empty(B, dtype=torch.int32, device=dev)
         _lib.check_sp(self._lib.opb_sp_detect(self._handle, img.data_ptr(), B, H, W, cnt.data_ptr(), st), self._handle, self._lib)
         n = [int(v) for v in cnt.cpu()]
+        self.check_range()                 # the read of the counts has synchronised: an out-of-range call raises here
         cap = max(max(n), 1)
         kp = torch.empty(B, cap, 2, dtype=torch.float32, device=dev)
         sc = torch.empty(B, cap, dtype=torch.float32, device=dev)
@@ -141,6 +144,12 @@ class SuperPoint(nn.Module):
             "scores": [sc[b, :n[b]] for b in range(B)],
             "descriptors": [de[b, :, :n[b]].contiguous() for b in range(B)],
         }
+
+    def check_range(self):
+        """Wait for the last call and raise OpbError(OPB_E_RANGE) if an activation left the fp16-split operand range
+        (|x| >= 1023) or became NaN; that call reported no key points.  Reporting clears the error."""
+        if self._handle is not None:
+            _lib.check_sp(self._lib.opb_sp_check_range(self._handle, None), self._handle, self._lib)
 
     # ------------------------------------------------------------------ measurement / test hooks
     def launch_count(self) -> int:

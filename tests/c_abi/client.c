@@ -22,6 +22,9 @@ int main(void) {
   printf("opb_create -> %d (%s)\n", rc, rc ? opb_last_error(NULL) : "ok");
   rc2 = opb_sp_create(&scfg, &s);
   printf("opb_sp_create -> %d (%s)\n", rc2, rc2 ? opb_sp_last_error(NULL) : "ok");
+  /* the range guards report nothing for a null handle or one that has not run yet */
+  if (opb_sp_poll_range(s) != OPB_OK || opb_sp_check_range(s, NULL) != OPB_OK) return 3;
+  if (opb_poll_range(m) != OPB_OK || opb_check_range(m, NULL) != OPB_OK) return 3;
   if (rc == OPB_OK && rc2 == OPB_OK) {            /* GPU box */
     opb_destroy(m);
     opb_sp_destroy(s);
