@@ -37,7 +37,7 @@ typedef struct opb_matcher opb_matcher; /* opaque */
 typedef struct opb_config {
   int32_t descriptor_dim;        /* 256 (only value supported)                         */
   int32_t num_heads;             /* 4   (GATs_SuperGlue.py:43)                          */
-  float scale_factor;            /* 0.07 (GATs_SuperGlue.py:217)                        */
+  float scale_factor;            /* 0.07 (GATs_SuperGlue.py:217); >= 2 log2(e) / 126    */
   float match_threshold;         /* 0.2  (GATs_SuperGlue.py:227)                        */
   int32_t include_self;          /* GATs.py:48                                          */
   int32_t additional;            /* GATs.py:61                                          */
@@ -75,7 +75,9 @@ int opb_reserve_workspace(opb_matcher* m, int32_t frames, int32_t N);
  * the reference).  n2d_lengths: device int32 [B] = valid query points of each frame (SuperPoint yields a different count per
  * frame, src/sfm/extract_features.py:19-24; columns >= n2d_lengths[b] of frame b are ignored) or NULL = N everywhere.
  * Outputs (device): matches0 int64 [B,N], matches1 int64 [B,M], mscores0 fp32 [B,N], mscores1 fp32 [B,M]; conf fp32 [B,N,M]
- * or NULL to skip materialising the confidence matrix.  Entries of a frame beyond its length are -1 / 0.
+ * or NULL to skip materialising the confidence matrix.  Entries of a frame beyond its length are -1 / 0.  A length of 0 is
+ * valid: that frame matches nothing (-1 / 0 everywhere, conf rows 0), its 3D points receive no cross-attention message, and
+ * the other frames of the call are unaffected.
  * Asynchronous on `stream`; no host synchronisation. */
 int opb_forward(opb_matcher* m, const float* desc2d_query, const int32_t* n2d_lengths, int32_t B, int32_t N,
                 int64_t* matches0, int64_t* matches1, float* mscores0, float* mscores1,
@@ -269,14 +271,23 @@ int opb_debug_set_conv_halo(int32_t mode);
 int opb_sp_debug_read(opb_superpoint* h, int32_t which, float* out, size_t capacity_elems, int64_t* n_elems, void* stream);
 
 /* ---- test hooks (used by tests/ and tools/ only; stable but not part of the drop-in surface) ---- */
-/* Stop the next opb_forward / opb_forward_objects right after step `step` of GNN layer `layer` of its first chunk; the call
- * returns OPB_OK and its outputs are unspecified.  layer = -1 turns the hook off (default).  Steps of an attention layer (1, 2,
+/* Stop the next opb_forward / opb_forward_objects right after step `step` of GNN layer `layer` of the chunk chosen by
+ * opb_debug_set_stop_pass (default: the first); the call returns OPB_OK and its outputs are unspecified.  layer = -1 turns the hook off (default).  Steps of an attention layer (1, 2,
  * 4, 5, 7, 8, 10, 11): 0 k,v projection, 1 state partials, 2 state reduce, 3 q projection, 4 G fold, 5 mlp.0, 6 InstanceNorm
  * statistics, 7 mlp.3 (+ residual).  A GATs layer (0, 3, 6, 9): 0 aggregation, and with with_linear_transform 1 the W GEMM and
  * its finish.  layer = 12, the tail: 0 final_proj + normalize, 1 score sums, 2 their finalize, 3 score conf.  With hoisting
- * on, layer 1 is the compact query-side pass (its first sub-batch), and layers 16 / 17 are the object prologue's layers 0 and
- * 1 (the first object whose prologue runs in the call).  A host-side check only: the launches are the same with the hook off. */
+ * on, layer 1 is the compact query-side pass (the sub-batch chosen by opb_debug_set_stop_pass), and layers 16 / 17 are the
+ * object prologue's layers 0 and 1 (the first object whose prologue runs in the call).  A host-side check only: the launches
+ * are the same with the hook off. */
 int opb_debug_set_stop(opb_matcher* m, int32_t layer, int32_t step);
+/* The pass later stops of opb_debug_set_stop apply to: chunk `chunk` of the call (chunks of opb_set_chunk_frames frames) and,
+ * for layer 1 with hoisting on, sub-batch `piece` of its query-side pass (16 frames each when the queries come from the host
+ * through opb_forward_host, else one per chunk).  The object prologue (layers 16 / 17) ignores both.  Default (0, 0).  A stop
+ * the call never reaches leaves the call complete, and opb_debug_read then returns OPB_E_STATE. */
+int opb_debug_set_stop_pass(opb_matcher* m, int32_t chunk, int32_t piece);
+/* The next forward runs the object prologue of every object of the handle again (with hoisting on), as after a weight reload:
+ * a stop at layer 16 / 17 then reaches the prologue of the call's first frame's object. */
+int opb_debug_invalidate_prologues(opb_matcher* m);
 /* Layout of the pass the last forward stopped in: layout[7] = {B, N, M, n_pad, m_pad, R, S}, rows = B * R, S = 2 B segments
  * (frame b's query rows [b R, b R + n_pad), its 3D rows [b R + n_pad, (b + 1) R)).  OPB_E_STATE if the last forward did not
  * stop. */

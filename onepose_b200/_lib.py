@@ -69,6 +69,8 @@ SYMBOLS = {
     "opb_debug_kv_state_h": (C.c_int, [_P, _I, _I, _I, _I, _P, C.POINTER(_I), _P]),
     "opb_debug_split": (C.c_int, [_P, _P, _P, C.c_size_t, _P]),
     "opb_debug_set_stop": (C.c_int, [_P, _I, _I]),
+    "opb_debug_set_stop_pass": (C.c_int, [_P, _I, _I]),
+    "opb_debug_invalidate_prologues": (C.c_int, [_P]),
     "opb_debug_stopped_layout": (C.c_int, [_P, C.POINTER(_I)]),
     "opb_debug_read": (C.c_int, [_P, _I, _P, C.c_size_t, C.POINTER(C.c_int64), _P]),
     # SuperPoint extractor

@@ -21,6 +21,7 @@ namespace opb {
 
 constexpr int kDefaultChunk = 32;   // frames pushed through the GNN together (measured: 4 -> 1340, 8 -> 1650, 16 -> 2390, 32 -> 2550 frames/s)
 constexpr int kQPassFrames = 16;    // granularity of the query-side layer-1 pass when the queries stream in from the host
+constexpr double kMinScaleFactor = 2.0 * 1.4426950408889634 / 126.0;   // ~0.0229: smallest scale_factor opb_create accepts
 
 static thread_local std::string g_create_error;
 static bool g_pdl = true;
@@ -92,6 +93,8 @@ struct opb_matcher : Handle {
   int last_launches = 0;                        // launches of the last completed forward
   // test hook (opb_debug_set_stop / opb_debug_read): the next forward stops after step dbg_step of GNN layer dbg_layer
   int dbg_layer = -1, dbg_step = 0;
+  int dbg_chunk = 0, dbg_piece = 0;             // ... in chunk dbg_chunk (and sub-batch dbg_piece of the hoisted query pass)
+  int pass_chunk = 0, pass_piece = -1;          // the pass being enqueued: its chunk, its query-pass sub-batch (-1: none)
   bool dbg_stopped = false;                     // the last forward stopped there; dbg_L / dbg_x are the layout and X of that pass
   Layout dbg_L{};
   XView dbg_x{};
@@ -163,10 +166,12 @@ constexpr int kTailLayer = 12;
 constexpr int kPrologueLayer = 16;
 constexpr int kStopped = 1;      // internal return code of a forward that reached the stop (never returned by the C ABI)
 
-// True when the forward is to stop after step `step` of `layer`; then records the pass for opb_debug_read.  A host-side
-// comparison only: the launch sequence is the same with the hook off.
+// True when the forward is to stop after step `step` of `layer` (of chunk dbg_chunk, and of sub-batch dbg_piece in the hoisted
+// query pass; the object prologue belongs to no chunk); then records the pass for opb_debug_read.  A host-side comparison only:
+// the launch sequence is the same with the hook off.
 static bool stop_here(opb_matcher* m, int layer, int step, const Layout& L, XView x) {
   if (layer != m->dbg_layer || step != m->dbg_step) return false;
+  if (layer < kPrologueLayer && (m->pass_chunk != m->dbg_chunk || (m->pass_piece >= 0 && m->pass_piece != m->dbg_piece))) return false;
   m->dbg_stopped = true;
   m->dbg_L = L;
   m->dbg_x = x;
@@ -347,7 +352,10 @@ static int forward_chunk(opb_matcher* m, const ObjectState* const* fobj, const f
       XView xq = m->xq.view((size_t)p0 * L.n_pad);
       LAUNCH(m, st, "transpose_cf_to_rows", transpose_cf_to_rows<0>, dim3(L.n_pad / 32, sb), dim3(32, 8), 0, st, q_cf + (size_t)p0 * kD * N, N, N,
              (long long)kD * N, Lq.nlen, L.n_pad, xq.hi, xq.lo, (float*)nullptr, (long long)Lq.R, 0);
-      if (int rc = run_attn_layer(m, Lq, xq, 1, m->attn[0], 0, st)) return rc;
+      m->pass_piece = si;
+      const int rc = run_attn_layer(m, Lq, xq, 1, m->attn[0], 0, st);
+      m->pass_piece = -1;
+      if (rc) return rc;
     }
     // assemble the full layout: query rows from xq, 3D rows from each frame's object prologue
     LAUNCH(m, st, "assemble_layout", assemble_layout, dim3(m->num_sms * 2, fb), dim3(256), 0, st, (const __half*)m->xq.hi.as<__half>(),
@@ -485,6 +493,7 @@ static int forward_frames(opb_matcher* m, ObjectState* const* fobj, const float*
     if (!m->hoist)                                          // per-frame evaluation consumes the whole chunk at once
       for (int si = 0; si * piece < fb; ++si)
         if (ci * ppc + si < m->h2d_pending) CK(m, cudaStreamWaitEvent(st, m->h2d_ev[ci * ppc + si], 0));
+    m->pass_chunk = ci;
     int rc = forward_chunk(m, fobj + f0, q + (size_t)f0 * kD * N, n2d_lengths ? n2d_lengths + f0 : nullptr, N, fb, M_out, m0 + (size_t)f0 * N,
                            m1 + (size_t)f0 * M_out, s0 + (size_t)f0 * N, s1 + (size_t)f0 * M_out, conf ? conf + (size_t)f0 * N * M_out : nullptr,
                            st, piece, ci * ppc);
@@ -510,7 +519,11 @@ int opb_create(const opb_config* cfg, opb_matcher** out) {
   if (cfg->descriptor_dim != kD || cfg->num_heads != kHeads)
     return fail(g_create_error, OPB_E_INVALID, "only descriptor_dim=256, num_heads=4 are supported (got %d, %d)", cfg->descriptor_dim,
                 cfg->num_heads);
-  if (!(cfg->scale_factor > 0.f)) return fail(g_create_error, OPB_E_INVALID, "scale_factor must be > 0");
+  // The tail's fixed shift e = exp((cos - 1) / scale) runs on ex2.approx.ftz, which flushes results below 2^-126 to zero: every
+  // cosine in [-1, 1] keeps e a normal fp32 value only when 2 log2(e) / scale <= 126.  Below that a query whose cosines are all
+  // low would get a zero row sum and a NaN conf row.
+  if (!((double)cfg->scale_factor >= kMinScaleFactor))
+    return fail(g_create_error, OPB_E_INVALID, "scale_factor must be >= 2 log2(e) / 126 = %.6f (got %g)", kMinScaleFactor, (double)cfg->scale_factor);
   cudaDeviceProp prop;
   if (int rc = select_device(cfg->device, prop, g_create_error)) return rc;
   auto* m = new opb_matcher();
@@ -929,6 +942,19 @@ int opb_debug_set_stop(opb_matcher* m, int32_t layer, int32_t step) {
   if (!m || layer < -1 || step < 0) return OPB_E_INVALID;
   m->dbg_layer = layer;
   m->dbg_step = step;
+  return OPB_OK;
+}
+
+int opb_debug_invalidate_prologues(opb_matcher* m) {
+  if (!m) return OPB_E_INVALID;
+  invalidate_prologues(m);
+  return OPB_OK;
+}
+
+int opb_debug_set_stop_pass(opb_matcher* m, int32_t chunk, int32_t piece) {
+  if (!m || chunk < 0 || piece < 0) return OPB_E_INVALID;
+  m->dbg_chunk = chunk;
+  m->dbg_piece = piece;
   return OPB_OK;
 }
 

@@ -819,7 +819,9 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
               }
             }
             const float dot = (dotp[0] + dotp[1]) + (dotp[2] + dotp[3]);
-            const float zf = 1.f / (dot + eps_m);
+            // a segment whose source has no valid rows (a frame without queries, in a cross layer) receives no message: Q' = 0.
+            // q / eps_m would leave the fp16-split range and turn the message into inf x 0 = NaN
+            const float zf = p.L.seg_valid(src) > 0 ? 1.f / (dot + eps_m) : 0.f;
 #pragma unroll
             for (int j = 0; j < 64; ++j) x[j] *= zf;
           } else {  // EPI_L2NORM

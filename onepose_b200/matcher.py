@@ -300,7 +300,8 @@ class GATsSuperGlue(nn.Module):
                           materialize_conf: bool = True):
         """End-to-end call on HOST buffers (bench.py e2e leg): pinned fp32 [B,256,N] in; matches /
         scores copied back to pinned host tensors.  conf_matrix is computed on the device and stays
-        there (the reference caller discards it: inference.py:146); materialize_conf=False skips it."""
+        there (the reference caller discards it: inference.py:146); materialize_conf=False skips it.  A host buffer
+        out["conf_matrix"] (fp32, B * N * M elements) receives a copy of it."""
         self._require_object()
         B, _, N = q_host.shape
         M = self._M
@@ -311,10 +312,14 @@ class GATsSuperGlue(nn.Module):
                    "matching_scores1": torch.empty(B, M, dtype=torch.float32, **pin)}
         if lengths is not None:
             lengths = lengths.to(device="cpu", dtype=torch.int32).contiguous()
+        conf = out.get("conf_matrix")
+        if conf is not None and (conf.is_cuda or conf.dtype != torch.float32 or conf.numel() < B * N * M or not conf.is_contiguous()):
+            raise ValueError(f"out['conf_matrix'] must be a contiguous fp32 host buffer with at least {B * N * M} elements")
         st = torch.cuda.current_stream(self._handle_device).cuda_stream
         _lib.check(self._lib.opb_forward_host(self._handle, q_host.data_ptr(), lengths.data_ptr() if lengths is not None else None, B, N,
                                               out["matches0"].data_ptr(), out["matches1"].data_ptr(), out["matching_scores0"].data_ptr(),
-                                              out["matching_scores1"].data_ptr(), None, int(bool(materialize_conf)), st), self._handle)
+                                              out["matching_scores1"].data_ptr(), conf.data_ptr() if conf is not None else None,
+                                              int(bool(materialize_conf)), st), self._handle)
         return out
 
     def check_range(self):
@@ -345,10 +350,16 @@ class GATsSuperGlue(nn.Module):
     DEBUG_BUFFERS = {"x": 0, "kvt": 1, "kmean": 2, "bd": 3, "qp": 4, "g": 5, "hid": 6, "mu": 7, "rstd": 8, "pn": 9,
                      "inv_rowsum": 10, "inv_colsum": 11, "rowbest": 12, "colbest": 13, "gats_pre": 14}
 
-    def debug_stop_after(self, layer: int, step: int = 0):
+    def debug_stop_after(self, layer: int, step: int = 0, chunk: int = 0, piece: int = 0):
         """Stop the next call after step `step` of GNN layer `layer` (12 = tail, 16 / 17 = the object prologue's layers 0 / 1;
-        see opb_debug_set_stop); -1 runs everything."""
+        see opb_debug_set_stop) in chunk `chunk`, and in sub-batch `piece` of the hoisted query pass (layer 1; see
+        opb_debug_set_stop_pass); -1 runs everything."""
+        _lib.check(self._lib.opb_debug_set_stop_pass(self._handle, int(chunk), int(piece)), self._handle)
         _lib.check(self._lib.opb_debug_set_stop(self._handle, int(layer), int(step)), self._handle)
+
+    def debug_invalidate_prologues(self):
+        """The next call runs every object's prologue again (opb_debug_invalidate_prologues)."""
+        _lib.check(self._lib.opb_debug_invalidate_prologues(self._handle), self._handle)
 
     def debug_layout(self) -> dict:
         """Layout of the pass the last call stopped in: B, N, M, n_pad, m_pad, R, S."""

@@ -160,3 +160,22 @@ def test_plain_c_client_links_and_runs(tmp_path):
     r = subprocess.run([str(exe)], capture_output=True, text=True, timeout=120)
     assert r.returncode == 0, r.stdout + r.stderr
     assert "opb_create ->" in r.stdout and "opb_sp_create ->" in r.stdout
+
+
+def test_scale_factor_below_the_tail_bound_is_refused():
+    """The tail's e = exp((cos - 1) / scale) stays a normal fp32 value (ex2.approx.ftz flushes below 2^-126) for every cosine only
+    when scale >= 2 log2(e) / 126 ~ 0.0229: below that opb_create refuses the config, with or without a GPU."""
+    import ctypes as C
+    lib = _lib.load()
+    bound = 2.0 * np.log2(np.e) / 126.0
+    h = C.c_void_p()
+    for scale in (0.0, -1.0, float("nan"), float(np.nextafter(np.float32(bound), np.float32(0)))):
+        cfg = _lib.OpbConfig(256, 4, scale, 0.2, 1, 0, 0, 0)
+        assert lib.opb_create(C.byref(cfg), C.byref(h)) == -1, scale
+        assert b"scale_factor" in lib.opb_last_error(None)
+    for scale in (float(np.nextafter(np.float32(bound), np.float32(1))), 0.07):
+        cfg = _lib.OpbConfig(256, 4, scale, 0.2, 1, 0, 0, 0)
+        rc = lib.opb_create(C.byref(cfg), C.byref(h))
+        assert rc != -1, (scale, lib.opb_last_error(None))
+        if rc == 0:
+            lib.opb_destroy(h)

@@ -4,7 +4,10 @@
   frames of objects of different sizes and every GraphAttentionLayer branch -- so a wrong reference cannot hide a wrong kernel.
 * Teeth: each planted defect moves its own stage by at least 10x that stage's bar, while the end-to-end conf moves by less
   than the 1e-4 bar of the parity tests (all but InstanceNorm statistics over the pad rows, which the end-to-end bar sees).
-  This is why the matcher's attention path is tested stage by stage."""
+  This is why the matcher's attention path is tested stage by stage.
+* Tail teeth: conf entries below 1e-4 written as 0, a column using its neighbour's inverse sum, and matching_scores1 taken from
+  the wrong row each move the entry-by-entry conf check or the exact mutual check by at least 10x.  Only the last one passes the
+  end-to-end bars (conf within 1e-4, decided arg-max); the test asserts each outcome."""
 import numpy as np
 import pytest
 import torch
@@ -123,3 +126,69 @@ def test_planted_defect_clears_its_stage_bar_but_not_the_end_to_end_bar(teeth_se
         assert dconf > 1e-4, f"{name}: no longer visible end to end ({dconf:.2e})"
     else:
         assert dconf < 1e-4, f"{name}: visible end to end ({dconf:.2e})"
+
+
+# ------------------------------------------------------------------------------------------------------------ tail teeth
+TAIL_DEFECTS = {"conf_zero_below_1e-4": ref.Defect(conf_zero_below=1e-4), "conf_neighbour_ics": ref.Defect(conf_neighbour_ics=True),
+                "ms1_wrong_row": ref.Defect(ms1_wrong_row=True)}
+# whether each defect passes the end-to-end bars: zeroing below 1e-4 keeps max|dconf| under the bar but moves the arg-max of
+# columns whose entries all lie below it; the wrong scores row touches neither conf nor the arg-maxes
+TAIL_DEFECT_PASSES_END_TO_END = {"conf_zero_below_1e-4": False, "conf_neighbour_ics": False, "ms1_wrong_row": True}
+
+
+@pytest.fixture(scope="module")
+def tail_setup():
+    """pn of the clean fp64 chain on two frames of one object (the fixture weights); its inverse sums and conf."""
+    sd = synthetic.make_state_dict(4)
+    P = oracle.params_from_numpy(sd, torch.float64)
+    data = synthetic.make_batch(9, [100, 101], 300, 700, 8)
+    objects = [(data["descriptors3d_db"][b], data["descriptors2d_db"][b]) for b in range(2)]
+    x, leaves_of, L = ref.assemble(data["descriptors2d_query"], objects)
+    pn = ref.final_proj(ref.gnn(x, leaves_of, P, HP, L), P)
+    return pn, L
+
+
+@pytest.mark.parametrize("name", list(TAIL_DEFECTS))
+def test_tail_defect_clears_the_conf_or_mutual_bar(tail_setup, name):
+    """Each tail defect moves the entry-by-entry conf check or the exact mutual check by at least 10x its bar; the end-to-end
+    bars (conf within 1e-4, arg-max where the fp64 decision is clear) are reported alongside."""
+    pn, L = tail_setup
+    d = TAIL_DEFECTS[name]
+    scale, thr = HP["scale_factor"], HP["match_threshold"]
+    ratio, dconf, argmax_bad = 0.0, 0.0, 0
+    for b in range(L.B):
+        cos = pn[L.seg_rows(2 * b)] @ pn[L.seg_rows(2 * b + 1)].T
+        e = torch.exp((cos - 1.0) / scale)
+        irs, ics = 1.0 / e.sum(1), 1.0 / e.sum(0)
+        clean = ref.conf_entries(e, irs, ics)
+        bad = ref.conf_entries(e, irs, ics, d).float()       # the device's conf is fp32
+        ratio = max(ratio, ref.bar_conf(bad, cos, irs, ics, scale))
+        m0, m1, s0, s1 = ref.mutual(bad, thr, d)
+        if ref.mutual_mismatches(m0, m1, s0, s1, bad, thr):
+            ratio = float("inf")
+        dconf = max(dconf, float((bad.double() - clean).abs().max()))
+        argmax_bad += ref.argmax_mismatches(bad.argmax(1), clean, 1) + ref.argmax_mismatches(bad.argmax(0), clean, 0)
+    e2e = dconf <= 1e-4 and argmax_bad == 0
+    print(f"{name}: conf / mutual check = {ratio:.3g} x its bar; end to end max|dconf| = {dconf:.2e}, decided arg-max "
+          f"mismatches = {argmax_bad} -> end-to-end bars {'pass' if e2e else 'fail'}")
+    assert ratio >= 10.0, f"{name}: the tail checks would not catch it ({ratio:.3g} x)"
+    assert e2e == TAIL_DEFECT_PASSES_END_TO_END[name], f"{name}: end-to-end bars {'pass' if e2e else 'fail'}"
+
+
+def test_clean_tail_meets_the_conf_bar_in_fp32(tail_setup):
+    """The clean conf rounded to fp32 (what the epilogue's last product does) stays far inside the per-entry bar, so the bar is
+    not met by accident of a loose reference."""
+    pn, L = tail_setup
+    scale = HP["scale_factor"]
+    for b in range(L.B):
+        cos = pn[L.seg_rows(2 * b)] @ pn[L.seg_rows(2 * b + 1)].T
+        e = torch.exp((cos - 1.0) / scale)
+        irs, ics = 1.0 / e.sum(1), 1.0 / e.sum(0)
+        assert ref.bar_conf(ref.conf_entries(e, irs, ics).float(), cos, irs, ics, scale) < 0.01
+
+
+def test_fp16_ulp_equals_numpy_spacing():
+    rs = np.random.RandomState(3)
+    v = np.concatenate([rs.randn(4000) * 10.0 ** rs.uniform(-9, 4, 4000), [0.0, 2.0 ** -14, 2.0 ** -15, 1.0, 2047.9, 65000.0]])
+    want = np.spacing(np.abs(v).astype(np.float16)).astype(np.float64)
+    assert np.array_equal(ref.fp16_ulp(torch.from_numpy(v)).numpy(), want)
