@@ -174,6 +174,37 @@ int opb_gather_features3d(const float* desc, const float* scores, int32_t dim, i
 int opb_ransac_pnp(const double* K, const double* pts2d, const double* pts3d, const int32_t* offsets, int32_t B, int32_t hypotheses,
                    double reproj_error, uint64_t seed, double* workspace, double* pose_out, int32_t* inlier_mask, int32_t* n_inliers,
                    void* stream);
+/* EPnP (Lepetit, Moreno-Noguer, Fua, IJCV 2009) on all correspondences of each frame: cv2.solvePnP(..., flags=SOLVEPNP_EPNP)
+ * for B frames, one block per frame, fp64, fixed-order reductions (deterministic).  K, pts2d, pts3d, offsets as for
+ * opb_ransac_pnp (used as given, no rounding).  Outputs (device): pose f64 [B, 12] row-major [R | t], status int32 [B] = 1 for
+ * a pose, 0 with the identity pose for a frame with fewer than 4 correspondences or a non-finite result (coincident or
+ * collinear points, or no candidate with solvable betas).  Control points: the centroid and the principal axes scaled by
+ * sqrt(lambda / n), each axis with its largest-magnitude component positive (on noisy data the answer depends on these
+ * signs; OpenCV takes its SVD's, so its pose can differ from this one by the noise's effect); for a planar set (third
+ * eigenvalue below 1e-10 of the first) the third control point sits at the first axis's length along the normal, and the
+ * null vector with the least weight on its columns comes first.  The null space of M^T M by Jacobi rotations; candidates for
+ * N = 1, 2, 3 null vectors, each refined by 5 Gauss-Newton steps on the four betas; R, t by Horn's quaternion; the lowest
+ * mean reprojection error wins, the first candidate on ties. */
+int opb_epnp(const double* K, const double* pts2d, const double* pts3d, const int32_t* offsets, int32_t B, double* pose_out,
+             int32_t* status, void* stream);
+/* EPnP-RANSAC: the reference's cv2.solvePnPRansac(..., flags=SOLVEPNP_EPNP) for B frames; same arguments, workspace records and
+ * outputs as opb_ransac_pnp, no host synchronisation.
+ *   inputs      every correspondence is rounded to fp32 first (as OpenCV converts its inputs); K is used as given;
+ *   hypotheses  sample h of frame b: r = splitmix64(seed ^ (b << 40) ^ h); index k (k = 0..4) is the next state modulo
+ *               n - k, increased by one for every earlier index it reaches (taken in ascending order), so the five are
+ *               distinct; EPnP on them (the routine of opb_epnp, one thread).  A frame of exactly 4 correspondences solves
+ *               P3P on correspondences 0-2 and keeps the solution that reprojects 3 best: OpenCV also fits a 4-point model
+ *               there (it returns a pose with 4 inliers where no 5-point sample exists: tests/golden/make_epnp.py);
+ *   count       inliers over all n by OpenCV's rule: squared reprojection error <= reproj_error^2, in fp64, with no depth
+ *               test (points behind the camera that project close enough count); a non-finite pose counts 0;
+ *   selection   most inliers, lowest index on ties (the arg-max of opb_ransac_pnp);
+ *   refit       EPnP (the block routine of opb_epnp) on the winning sample's inlier set, which is the reported inlier_mask.
+ * Fewer than 4 correspondences, or a best count below 4, gives the identity pose and no inliers.  OpenCV raises or returns
+ * false there instead, and the reference's ransac_PnP turns that into the same identity pose and empty inlier list.  OpenCV
+ * draws its samples from its own serial, adaptive sequence, so parity is on the pose, not on bits. */
+int opb_ransac_epnp(const double* K, const double* pts2d, const double* pts3d, const int32_t* offsets, int32_t B, int32_t hypotheses,
+                    double reproj_error, uint64_t seed, double* workspace, double* pose_out, int32_t* inlier_mask, int32_t* n_inliers,
+                    void* stream);
 /* Matched 2D-3D pairs of B frames in the layout opb_ransac_pnp reads; replaces inference.py:147-152 / eval_utils.py:72-77
  * (valid = matches0 > -1; mkpts2d = kpts2d[valid]; mkpts3d = kpts3d[matches0[valid]]; mconf = scores0[valid]).
  *   matches0     device int64 [B, N]  (opb_forward's output; an entry outside [0, M) is not a match)

@@ -59,6 +59,8 @@ SYMBOLS = {
     "opb_segmented_mean_scores_f64": (C.c_int, [_P, _P, _I, _P, _P]),
     "opb_gather_features3d": (C.c_int, [_P, _P, _I, C.c_int64, _P, C.c_int64, _P, _P, C.c_int64, _P]),
     "opb_ransac_pnp": (C.c_int, [_P, _P, _P, _P, _I, _I, C.c_double, C.c_uint64, _P, _P, _P, _P, _P]),
+    "opb_epnp": (C.c_int, [_P, _P, _P, _P, _I, _P, _P, _P]),
+    "opb_ransac_epnp": (C.c_int, [_P, _P, _P, _P, _I, _I, C.c_double, C.c_uint64, _P, _P, _P, _P, _P]),
     "opb_gather_matches": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P]),
     "opb_gather_matches_objects": (C.c_int, [_P, _P, _P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P]),
     "opb_debug_set_pdl": (C.c_int, [_I]),

@@ -282,8 +282,29 @@ __device__ void rodrigues_left(const double* w, Pose& T) {   // T <- exp([w]x) .
   for (int k = 0; k < 3; ++k) T.t[k] = tn[k];
 }
 
-// one block per frame: arg-max over hypotheses, local optimisation, outputs
+// block-wide arg-max over frame b's hypothesis records: the most inliers, the lowest index on ties.  Returns the count and
+// sets *best_h; every thread of the block gets the same answer.
 constexpr int kRefineThreads = 256;
+__device__ int best_hypothesis(const double* __restrict__ hyp, int b, int H, unsigned long long* best_key /*shared [kRefineThreads]*/, int* best_h) {
+  const int tid = threadIdx.x;
+  unsigned long long key = 0ull;
+  for (int h = tid; h < H; h += kRefineThreads) {
+    const unsigned long long c = (unsigned long long)hyp[((size_t)b * H + h) * kHypStride];
+    const unsigned long long k = (c << 32) | (unsigned long long)(0xFFFFFFFFu - (unsigned)h);
+    key = k > key ? k : key;
+  }
+  best_key[tid] = key;
+  __syncthreads();
+  for (int s = kRefineThreads / 2; s > 0; s >>= 1) {
+    if (tid < s && best_key[tid + s] > best_key[tid]) best_key[tid] = best_key[tid + s];
+    __syncthreads();
+  }
+  const unsigned long long bk = best_key[0];
+  *best_h = (int)(0xFFFFFFFFu - (unsigned)(bk & 0xFFFFFFFFull));
+  return (int)(bk >> 32);
+}
+
+// one block per frame: arg-max over hypotheses, local optimisation, outputs
 __global__ void __launch_bounds__(kRefineThreads) pnp_select_refine(const double* __restrict__ Kmat, const double* __restrict__ pts2d, const double* __restrict__ pts3d,
                                                                      const int* __restrict__ offsets, int H, double thr2, const double* __restrict__ hyp,
                                                                      double* __restrict__ pose_out /*[B][12]*/, int* __restrict__ inlier_mask,
@@ -298,20 +319,8 @@ __global__ void __launch_bounds__(kRefineThreads) pnp_select_refine(const double
   const double* K = Kmat + (size_t)b * 9;
   const double Kc[4] = {K[0], K[4], K[2], K[5]};
   // ---- best hypothesis: max count, lowest index
-  unsigned long long key = 0ull;
-  for (int h = tid; h < H; h += kRefineThreads) {
-    const unsigned long long c = (unsigned long long)hyp[((size_t)b * H + h) * kHypStride];
-    const unsigned long long k = (c << 32) | (unsigned long long)(0xFFFFFFFFu - (unsigned)h);
-    key = k > key ? k : key;
-  }
-  best_key[tid] = key;
-  __syncthreads();
-  for (int s = kRefineThreads / 2; s > 0; s >>= 1) {
-    if (tid < s && best_key[tid + s] > best_key[tid]) best_key[tid] = best_key[tid + s];
-    __syncthreads();
-  }
-  const unsigned long long bk = best_key[0];
-  const int best_cnt = (int)(bk >> 32), best_h = (int)(0xFFFFFFFFu - (unsigned)(bk & 0xFFFFFFFFull));
+  int best_h;
+  const int best_cnt = best_hypothesis(hyp, b, H, best_key, &best_h);
   if (tid == 0) {
     ok = best_cnt >= 4 ? 1 : 0;
     if (ok) {
@@ -423,6 +432,588 @@ __global__ void __launch_bounds__(kRefineThreads) pnp_select_refine(const double
       pose_out[(size_t)b * 12 + r * 4 + 3] = T.t[r];
     }
   }
+}
+
+// ---- EPnP (Lepetit, Moreno-Noguer, Fua, "EPnP: An Accurate O(n) Solution to the PnP Problem", IJCV 2009), fp64.
+// Control points: the centroid c0 and c0 + sqrt(lambda_k / n) e_k along the principal axes of the point set (largest first);
+// every point is an affine combination (the alphas) of them, so its camera coordinates are the same combination of the
+// control points' camera coordinates x (12 unknowns), and each correspondence gives two rows of M x = 0.  x lies near the span
+// of the eigenvectors v_0..v_3 of M^T M with the smallest eigenvalues; x = sum beta_k v_k, the betas from the six distance
+// constraints |c_a - c_b| (L [6x10] . products of the betas = rho), linearised for N = 1, 2, 3 vectors and refined by
+// Gauss-Newton; each candidate gives the points' camera coordinates (depth sign made positive) and R, t by absolute
+// orientation; the candidate with the lowest mean reprojection error wins, the first on ties.
+// Everything the candidates need from the points is a sum over them (kEpnpSums), so one routine serves a thread that loops
+// over a 5-point sample and a block that reduces over a frame.
+constexpr int kMtmSums = 78;                           // upper triangle of M^T M (12 x 12)
+constexpr int kEpnpSums = kMtmSums + 10 + 4;           // + upper triangle of alpha^T alpha (4 x 4) + alpha sums
+constexpr int kEpnpGnIters = 5;
+
+// symmetric eigenproblem by cyclic Jacobi rotations: A [N*N] row-major (its diagonal ends as the eigenvalues), V [N*N]
+// (columns = eigenvectors).  Fixed sweep order: deterministic.
+template <int N>
+__device__ void jacobi_eigen(double* A, double* V) {
+  for (int i = 0; i < N * N; ++i) V[i] = (i % (N + 1)) == 0 ? 1.0 : 0.0;
+  for (int sweep = 0; sweep < 32; ++sweep) {
+    double off = 0.0, dia = 0.0;
+    for (int p = 0; p < N; ++p) {
+      dia += A[p * N + p] * A[p * N + p];
+      for (int q = p + 1; q < N; ++q) off += A[p * N + q] * A[p * N + q];
+    }
+    if (!(off > 1e-34 * dia)) break;
+    for (int p = 0; p < N - 1; ++p)
+      for (int q = p + 1; q < N; ++q) {
+        const double apq = A[p * N + q];
+        if (apq == 0.0) continue;
+        const double th = (A[q * N + q] - A[p * N + p]) / (2.0 * apq);
+        const double t = fabs(th) > 1e150 ? 0.5 / th : (th >= 0.0 ? 1.0 : -1.0) / (fabs(th) + sqrt(th * th + 1.0));
+        const double c = 1.0 / sqrt(t * t + 1.0), s = t * c;
+        for (int k = 0; k < N; ++k) {               // A <- A J
+          const double akp = A[k * N + p], akq = A[k * N + q];
+          A[k * N + p] = c * akp - s * akq;
+          A[k * N + q] = s * akp + c * akq;
+        }
+        for (int k = 0; k < N; ++k) {               // A <- J^T A
+          const double apk = A[p * N + k], aqk = A[q * N + k];
+          A[p * N + k] = c * apk - s * aqk;
+          A[q * N + k] = s * apk + c * aqk;
+        }
+        for (int k = 0; k < N; ++k) {               // V <- V J
+          const double vkp = V[k * N + p], vkq = V[k * N + q];
+          V[k * N + p] = c * vkp - s * vkq;
+          V[k * N + q] = s * vkp + c * vkq;
+        }
+      }
+  }
+}
+
+// least squares min |A x - b| of a 6 x k system (k <= 5) by Householder QR; a [6*5] row-major (first k columns) and b are
+// destroyed.  False when a column is rank deficient.
+__device__ bool lstsq6(double* a, double* b, int k, double* x) {
+  for (int j = 0; j < k; ++j) {
+    double nrm = 0.0;
+    for (int r = j; r < 6; ++r) nrm += a[r * 5 + j] * a[r * 5 + j];
+    nrm = sqrt(nrm);
+    if (!(nrm > 0.0)) return false;
+    const double alpha = a[j * 5 + j] > 0.0 ? -nrm : nrm;
+    double v[6], vv = 0.0;
+    for (int r = j; r < 6; ++r) v[r] = a[r * 5 + j];
+    v[j] -= alpha;
+    for (int r = j; r < 6; ++r) vv += v[r] * v[r];
+    if (vv > 0.0) {
+      for (int c = j; c < k; ++c) {
+        double s = 0.0;
+        for (int r = j; r < 6; ++r) s += v[r] * a[r * 5 + c];
+        s *= 2.0 / vv;
+        for (int r = j; r < 6; ++r) a[r * 5 + c] -= s * v[r];
+      }
+      double s = 0.0;
+      for (int r = j; r < 6; ++r) s += v[r] * b[r];
+      s *= 2.0 / vv;
+      for (int r = j; r < 6; ++r) b[r] -= s * v[r];
+    }
+  }
+  for (int j = k - 1; j >= 0; --j) {
+    double s = b[j];
+    for (int c = j + 1; c < k; ++c) s -= a[j * 5 + c] * x[c];
+    x[j] = s / a[j * 5 + j];
+  }
+  return true;
+}
+
+constexpr double kEpnpFlat = 1e-10;                   // an axis whose eigenvalue is below this fraction of the largest is flat
+
+struct EpnpBasis {
+  double c[4][3];    // world control points
+  double ax[3][3];   // c[k+1] - c[0]
+  double il2[3];     // 1 / |ax_k|^2
+  int planar;        // the third axis is flat: its control point is placed at full length along the plane's normal
+};
+
+// centroid sum[3] and scatter sc[6] = {xx, xy, xz, yy, yz, zz} about the centroid of m points -> control points.
+// Each axis is an eigenvector of the scatter with its largest-magnitude component made positive (the first such component on
+// ties), so that the control points -- and, on noisy data, EPnP's algebraic least squares, which depends on them -- do not
+// depend on the sign an eigen-solver happens to return.  A flat third axis (a planar set) gets the length of the first, so
+// that its control point stays a distinct point: the points' coordinates along it are then (near) 0 and its camera
+// coordinates are fixed by the distance constraints alone.  False for coincident or collinear points.
+__device__ bool epnp_basis(const double* sum, const double* sc, int m, EpnpBasis& E) {
+  double A[9] = {sc[0], sc[1], sc[2], sc[1], sc[3], sc[4], sc[2], sc[4], sc[5]}, V[9];
+  jacobi_eigen<3>(A, V);
+  int ord[3] = {0, 1, 2};                              // descending eigenvalues
+  for (int i = 1; i < 3; ++i)
+    for (int j = i; j > 0 && A[ord[j] * 4] > A[ord[j - 1] * 4]; --j) { const int t = ord[j]; ord[j] = ord[j - 1]; ord[j - 1] = t; }
+  const double l0 = A[ord[0] * 4];
+  if (!(l0 > 0.0) || !(A[ord[1] * 4] > kEpnpFlat * l0)) return false;
+  E.planar = A[ord[2] * 4] > kEpnpFlat * l0 ? 0 : 1;
+  for (int d = 0; d < 3; ++d) E.c[0][d] = sum[d] / m;
+  for (int k = 0; k < 3; ++k) {
+    const double lam = (k == 2 && E.planar) ? l0 : A[ord[k] * 4];
+    int big = 0;
+    for (int d = 1; d < 3; ++d)
+      if (fabs(V[d * 3 + ord[k]]) > fabs(V[big * 3 + ord[k]])) big = d;
+    const double s = (V[big * 3 + ord[k]] < 0.0 ? -1.0 : 1.0) * sqrt(lam / m);
+    double l2 = 0.0;
+    for (int d = 0; d < 3; ++d) {
+      E.c[k + 1][d] = E.c[0][d] + s * V[d * 3 + ord[k]];
+      E.ax[k][d] = E.c[k + 1][d] - E.c[0][d];
+      l2 += E.ax[k][d] * E.ax[k][d];
+    }
+    if (!(l2 > 0.0)) return false;
+    E.il2[k] = 1.0 / l2;
+  }
+  return true;
+}
+
+__device__ __forceinline__ void epnp_alphas(const EpnpBasis& E, const double* p, double* a) {
+  const double d[3] = {p[0] - E.c[0][0], p[1] - E.c[0][1], p[2] - E.c[0][2]};
+  for (int k = 0; k < 3; ++k) a[k + 1] = (E.ax[k][0] * d[0] + E.ax[k][1] * d[1] + E.ax[k][2] * d[2]) * E.il2[k];
+  a[0] = 1.0 - a[1] - a[2] - a[3];
+}
+
+// one correspondence's contribution to the kEpnpSums sums
+__device__ __forceinline__ void epnp_accumulate(const double* a, const double* uv, const double* Kc, double* acc) {
+  double r1[12], r2[12];
+#pragma unroll
+  for (int j = 0; j < 4; ++j) {
+    r1[3 * j] = a[j] * Kc[0]; r1[3 * j + 1] = 0.0; r1[3 * j + 2] = a[j] * (Kc[2] - uv[0]);
+    r2[3 * j] = 0.0; r2[3 * j + 1] = a[j] * Kc[1]; r2[3 * j + 2] = a[j] * (Kc[3] - uv[1]);
+  }
+  int k = 0;
+#pragma unroll
+  for (int r = 0; r < 12; ++r)
+#pragma unroll
+    for (int c = r; c < 12; ++c) acc[k++] += r1[r] * r1[c] + r2[r] * r2[c];
+#pragma unroll
+  for (int r = 0; r < 4; ++r)
+#pragma unroll
+    for (int c = r; c < 4; ++c) acc[k++] += a[r] * a[c];
+#pragma unroll
+  for (int r = 0; r < 4; ++r) acc[k++] += a[r];
+}
+
+__device__ __forceinline__ void beta_products(const double* be, double* p) {
+  p[0] = be[0] * be[0]; p[1] = be[0] * be[1]; p[2] = be[1] * be[1]; p[3] = be[0] * be[2]; p[4] = be[1] * be[2];
+  p[5] = be[2] * be[2]; p[6] = be[0] * be[3]; p[7] = be[1] * be[3]; p[8] = be[2] * be[3]; p[9] = be[3] * be[3];
+}
+
+// beta0, beta1 from the linearised b00, b01, b11
+__device__ __forceinline__ void two_betas(double b00, double b01, double b11, double* be) {
+  if (b00 < 0.0) { be[0] = sqrt(-b00); be[1] = b11 < 0.0 ? sqrt(-b11) : 0.0; }
+  else { be[0] = sqrt(b00); be[1] = b11 > 0.0 ? sqrt(b11) : 0.0; }
+  if (b01 < 0.0) be[0] = -be[0];
+}
+
+// the three candidates' poses from the sums of m points
+__device__ void epnp_candidates(const double* sums, const EpnpBasis& E, int m, Pose* cand) {
+  double A[144], V[144];
+  {
+    int k = 0;
+    for (int r = 0; r < 12; ++r)
+      for (int c = r; c < 12; ++c) { A[r * 12 + c] = A[c * 12 + r] = sums[k]; ++k; }
+  }
+  jacobi_eigen<12>(A, V);
+  int ord[12];
+  for (int i = 0; i < 12; ++i) ord[i] = i;
+  for (int i = 1; i < 12; ++i)                          // ascending eigenvalues, stable
+    for (int j = i; j > 0 && A[ord[j] * 13] < A[ord[j - 1] * 13]; --j) { const int t = ord[j]; ord[j] = ord[j - 1]; ord[j - 1] = t; }
+  if (E.planar) {
+    // the flat axis's control point is unconstrained by M (its columns are (near) zero), so three of the four smallest
+    // eigenvalues belong to vectors that live on its columns and tie with the true one: the vector with the least weight
+    // there goes first (stable), the one the N = 1 .. 3 approximations build on
+    double w[4];
+    for (int k = 0; k < 4; ++k) w[k] = V[9 * 12 + ord[k]] * V[9 * 12 + ord[k]] + V[10 * 12 + ord[k]] * V[10 * 12 + ord[k]] + V[11 * 12 + ord[k]] * V[11 * 12 + ord[k]];
+    for (int i = 1; i < 4; ++i)
+      for (int j = i; j > 0 && w[j] < w[j - 1]; --j) {
+        const double tw = w[j]; w[j] = w[j - 1]; w[j - 1] = tw;
+        const int t = ord[j]; ord[j] = ord[j - 1]; ord[j - 1] = t;
+      }
+  }
+  double v[4][12];
+  for (int k = 0; k < 4; ++k)
+    for (int i = 0; i < 12; ++i) v[k][i] = V[i * 12 + ord[k]];
+  const int pa[6] = {0, 0, 0, 1, 1, 2}, pb[6] = {1, 2, 3, 2, 3, 3};
+  double L[6][10], rho[6];
+  for (int r = 0; r < 6; ++r) {
+    double dv[4][3];
+    for (int k = 0; k < 4; ++k)
+      for (int d = 0; d < 3; ++d) dv[k][d] = v[k][3 * pa[r] + d] - v[k][3 * pb[r] + d];
+    auto dot = [&](int i, int j) { return dv[i][0] * dv[j][0] + dv[i][1] * dv[j][1] + dv[i][2] * dv[j][2]; };
+    L[r][0] = dot(0, 0); L[r][1] = 2.0 * dot(0, 1); L[r][2] = dot(1, 1); L[r][3] = 2.0 * dot(0, 2); L[r][4] = 2.0 * dot(1, 2);
+    L[r][5] = dot(2, 2); L[r][6] = 2.0 * dot(0, 3); L[r][7] = 2.0 * dot(1, 3); L[r][8] = 2.0 * dot(2, 3); L[r][9] = dot(3, 3);
+    double r2 = 0.0;
+    for (int d = 0; d < 3; ++d) r2 += (E.c[pa[r]][d] - E.c[pb[r]][d]) * (E.c[pa[r]][d] - E.c[pb[r]][d]);
+    rho[r] = r2;
+  }
+  const double* G = sums + kMtmSums;                  // alpha^T alpha, upper triangle
+  const double* as = sums + kMtmSums + 10;            // alpha sums
+  double Gm[4][4];
+  {
+    int k = 0;
+    for (int r = 0; r < 4; ++r)
+      for (int c = r; c < 4; ++c) { Gm[r][c] = Gm[c][r] = G[k]; ++k; }
+  }
+  const int cols[3][5] = {{0, 1, 3, 6, 0}, {0, 1, 2, 0, 0}, {0, 1, 2, 3, 4}};
+  const int ncols[3] = {4, 3, 5};
+  for (int N = 0; N < 3; ++N) {
+    double a[30], bb[6], x[5] = {0, 0, 0, 0, 0}, be[4] = {0, 0, 0, 0};
+    for (int r = 0; r < 6; ++r) {
+      for (int c = 0; c < ncols[N]; ++c) a[r * 5 + c] = L[r][cols[N][c]];
+      bb[r] = rho[r];
+    }
+    if (!lstsq6(a, bb, ncols[N], x)) {                // no betas: the candidate is not a pose
+      for (int k = 0; k < 9; ++k) cand[N].R[k] = NAN;
+      for (int k = 0; k < 3; ++k) cand[N].t[k] = NAN;
+      continue;
+    }
+    {
+      if (N == 0) {
+        be[0] = sqrt(fabs(x[0]));
+        const double sg = x[0] < 0.0 ? -1.0 : 1.0;
+        for (int k = 1; k < 4; ++k) be[k] = sg * x[k] / be[0];
+      } else {
+        two_betas(x[0], x[1], x[2], be);
+        if (N == 2) be[2] = be[0] != 0.0 ? x[3] / be[0] : 0.0;
+      }
+    }
+    for (int it = 0; it < kEpnpGnIters; ++it) {         // Gauss-Newton on all four betas
+      double pr[10];
+      beta_products(be, pr);
+      for (int r = 0; r < 6; ++r) {
+        const double* l = L[r];
+        a[r * 5 + 0] = 2.0 * l[0] * be[0] + l[1] * be[1] + l[3] * be[2] + l[6] * be[3];
+        a[r * 5 + 1] = l[1] * be[0] + 2.0 * l[2] * be[1] + l[4] * be[2] + l[7] * be[3];
+        a[r * 5 + 2] = l[3] * be[0] + l[4] * be[1] + 2.0 * l[5] * be[2] + l[8] * be[3];
+        a[r * 5 + 3] = l[6] * be[0] + l[7] * be[1] + l[8] * be[2] + 2.0 * l[9] * be[3];
+        double s = 0.0;
+        for (int c = 0; c < 10; ++c) s += l[c] * pr[c];
+        bb[r] = rho[r] - s;
+      }
+      double d[5];
+      if (!lstsq6(a, bb, 4, d)) break;
+      for (int k = 0; k < 4; ++k) be[k] += d[k];
+    }
+    // camera control points, the sign that puts the points' depths (their sum) in front, centroids and the cross-covariance
+    // sum_i (pw_i - pw~)(pc_i - pc~)^T = sum_jk G_jk (cw_j - pw~)(cc_k - pc~)^T (alphas sum to 1) -> Horn's quaternion
+    double cc[4][3];
+    for (int j = 0; j < 4; ++j)
+      for (int d = 0; d < 3; ++d) cc[j][d] = be[0] * v[0][3 * j + d] + be[1] * v[1][3 * j + d] + be[2] * v[2][3 * j + d] + be[3] * v[3][3 * j + d];
+    double zs = 0.0;
+    for (int j = 0; j < 4; ++j) zs += as[j] * cc[j][2];
+    if (zs < 0.0)
+      for (int j = 0; j < 4; ++j)
+        for (int d = 0; d < 3; ++d) cc[j][d] = -cc[j][d];
+    double pw[3], pc[3];
+    for (int d = 0; d < 3; ++d) {
+      double sw = 0.0, sc = 0.0;
+      for (int j = 0; j < 4; ++j) { sw += as[j] * E.c[j][d]; sc += as[j] * cc[j][d]; }
+      pw[d] = sw / m;
+      pc[d] = sc / m;
+    }
+    double S[3][3] = {};
+    for (int j = 0; j < 4; ++j)
+      for (int k = 0; k < 4; ++k)
+        for (int r = 0; r < 3; ++r)
+          for (int c = 0; c < 3; ++c) S[r][c] += Gm[j][k] * (E.c[j][r] - pw[r]) * (cc[k][c] - pc[c]);
+    double Nq[16] = {S[0][0] + S[1][1] + S[2][2], S[1][2] - S[2][1], S[2][0] - S[0][2], S[0][1] - S[1][0],
+                     S[1][2] - S[2][1], S[0][0] - S[1][1] - S[2][2], S[0][1] + S[1][0], S[2][0] + S[0][2],
+                     S[2][0] - S[0][2], S[0][1] + S[1][0], -S[0][0] + S[1][1] - S[2][2], S[1][2] + S[2][1],
+                     S[0][1] - S[1][0], S[2][0] + S[0][2], S[1][2] + S[2][1], -S[0][0] - S[1][1] + S[2][2]};
+    double Vq[16];
+    jacobi_eigen<4>(Nq, Vq);
+    int top = 0;
+    for (int i = 1; i < 4; ++i)
+      if (Nq[i * 5] > Nq[top * 5]) top = i;
+    const double w = Vq[0 * 4 + top], x1 = Vq[1 * 4 + top], y = Vq[2 * 4 + top], z = Vq[3 * 4 + top];
+    double* R = cand[N].R;
+    R[0] = w * w + x1 * x1 - y * y - z * z; R[1] = 2.0 * (x1 * y - w * z);           R[2] = 2.0 * (x1 * z + w * y);
+    R[3] = 2.0 * (x1 * y + w * z);           R[4] = w * w - x1 * x1 + y * y - z * z; R[5] = 2.0 * (y * z - w * x1);
+    R[6] = 2.0 * (x1 * z - w * y);           R[7] = 2.0 * (y * z + w * x1);           R[8] = w * w - x1 * x1 - y * y + z * z;
+    for (int r = 0; r < 3; ++r) cand[N].t[r] = pc[r] - (R[r * 3] * pw[0] + R[r * 3 + 1] * pw[1] + R[r * 3 + 2] * pw[2]);
+  }
+}
+
+__device__ __forceinline__ double reproj_dist(const Pose& T, const double* Kc, const double* p3, const double* p2) {
+  const double x = T.R[0] * p3[0] + T.R[1] * p3[1] + T.R[2] * p3[2] + T.t[0];
+  const double y = T.R[3] * p3[0] + T.R[4] * p3[1] + T.R[5] * p3[2] + T.t[1];
+  const double z = T.R[6] * p3[0] + T.R[7] * p3[1] + T.R[8] * p3[2] + T.t[2];
+  const double du = Kc[0] * x / z + Kc[2] - p2[0], dv = Kc[1] * y / z + Kc[3] - p2[1];
+  return sqrt(du * du + dv * dv);
+}
+
+// the lowest error sum (mean x m), the first on ties; a non-finite error never wins
+__device__ __forceinline__ int epnp_pick(const double* err) {
+  int best = 0;
+  double be = isfinite(err[0]) ? err[0] : INFINITY;
+  for (int c = 1; c < 3; ++c)
+    if (isfinite(err[c]) && err[c] < be) { be = err[c]; best = c; }
+  return best;
+}
+
+__device__ __forceinline__ bool pose_finite(const Pose& T) {
+  bool f = true;
+  for (int k = 0; k < 9; ++k) f &= isfinite(T.R[k]);
+  for (int k = 0; k < 3; ++k) f &= isfinite(T.t[k]);
+  return f;
+}
+
+// OpenCV's RANSAC inlier rule: squared reprojection error <= thr^2, no depth test
+__device__ __forceinline__ bool epnp_inlier(const Pose& T, const double* Kc, const double* p3, const double* p2, double thr2) {
+  const double x = T.R[0] * p3[0] + T.R[1] * p3[1] + T.R[2] * p3[2] + T.t[0];
+  const double y = T.R[3] * p3[0] + T.R[4] * p3[1] + T.R[5] * p3[2] + T.t[1];
+  const double z = T.R[6] * p3[0] + T.R[7] * p3[1] + T.R[8] * p3[2] + T.t[2];
+  const double du = Kc[0] * x / z + Kc[2] - p2[0], dv = Kc[1] * y / z + Kc[3] - p2[1];
+  return du * du + dv * dv <= thr2;
+}
+
+// correspondence i of a frame, rounded to fp32 first when kRound (as OpenCV's solvePnPRansac converts its inputs)
+template <bool kRound>
+__device__ __forceinline__ void load_pair(const double* pts2d, const double* pts3d, size_t i, double* p2, double* p3) {
+  for (int d = 0; d < 2; ++d) p2[d] = kRound ? (double)(float)pts2d[i * 2 + d] : pts2d[i * 2 + d];
+  for (int d = 0; d < 3; ++d) p3[d] = kRound ? (double)(float)pts3d[i * 3 + d] : pts3d[i * 3 + d];
+}
+
+// EPnP of m <= 5 points by one thread (the RANSAC hypotheses)
+__device__ bool epnp_points(const double (*P)[3], const double (*uv)[2], int m, const double* Kc, Pose& out) {
+  double sum[3] = {0, 0, 0}, sc[6] = {0, 0, 0, 0, 0, 0};
+  for (int i = 0; i < m; ++i)
+    for (int d = 0; d < 3; ++d) sum[d] += P[i][d];
+  const double c0[3] = {sum[0] / m, sum[1] / m, sum[2] / m};
+  for (int i = 0; i < m; ++i) {
+    const double d[3] = {P[i][0] - c0[0], P[i][1] - c0[1], P[i][2] - c0[2]};
+    sc[0] += d[0] * d[0]; sc[1] += d[0] * d[1]; sc[2] += d[0] * d[2]; sc[3] += d[1] * d[1]; sc[4] += d[1] * d[2]; sc[5] += d[2] * d[2];
+  }
+  EpnpBasis E;
+  if (!epnp_basis(sum, sc, m, E)) return false;
+  double acc[kEpnpSums];
+  for (int k = 0; k < kEpnpSums; ++k) acc[k] = 0.0;
+  for (int i = 0; i < m; ++i) {
+    double a[4];
+    epnp_alphas(E, P[i], a);
+    epnp_accumulate(a, uv[i], Kc, acc);
+  }
+  Pose cand[3];
+  epnp_candidates(acc, E, m, cand);
+  double err[3] = {0, 0, 0};
+  for (int i = 0; i < m; ++i)
+    for (int c = 0; c < 3; ++c) err[c] += reproj_dist(cand[c], Kc, P[i], uv[i]);
+  out = cand[epnp_pick(err)];
+  return pose_finite(out);
+}
+
+// block-wide fixed-order sum of K per-thread values into out[K] (shared); every thread returns with out complete
+constexpr int kEpnpThreads = kRefineThreads;
+template <int K>
+__device__ void block_sum(double* v, double (*red)[kEpnpThreads / 32], double* out) {
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+#pragma unroll
+  for (int k = 0; k < K; ++k) {
+    double s = v[k];
+    for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+    if (lane == 0) red[k][warp] = s;
+  }
+  __syncthreads();
+  for (int k = tid; k < K; k += kEpnpThreads) {
+    double s = 0.0;
+    for (int w = 0; w < kEpnpThreads / 32; ++w) s += red[k][w];
+    out[k] = s;
+  }
+  __syncthreads();
+}
+
+struct EpnpShared {
+  double red[kEpnpSums][kEpnpThreads / 32];
+  double sums[kEpnpSums];
+  EpnpBasis E;
+  Pose cand[3];
+  int ok;
+};
+
+// EPnP of the frame's correspondences i in [0, n) with use(i) by the whole block; the pose lands in *out (shared).  Returns
+// the number of points used, or 0 for a degenerate set (then, as with fewer than 4 points, *out is not written).
+template <bool kRound, class Use>
+__device__ int epnp_block(const double* pts2d, const double* pts3d, int n, const double* Kc, Use use, EpnpShared& sh, Pose* out) {
+  const int tid = threadIdx.x;
+  double v[4] = {0, 0, 0, 0};
+  for (int i = tid; i < n; i += kEpnpThreads) {
+    if (!use(i)) continue;
+    double p2[2], p3[3];
+    load_pair<kRound>(pts2d, pts3d, i, p2, p3);
+    v[0] += p3[0]; v[1] += p3[1]; v[2] += p3[2]; v[3] += 1.0;
+  }
+  block_sum<4>(v, sh.red, sh.sums);
+  const int m = (int)sh.sums[3];
+  if (m < 4) return m;
+  const double sum[3] = {sh.sums[0], sh.sums[1], sh.sums[2]};
+  const double c0[3] = {sum[0] / m, sum[1] / m, sum[2] / m};
+  double sc[6] = {0, 0, 0, 0, 0, 0};
+  for (int i = tid; i < n; i += kEpnpThreads) {
+    if (!use(i)) continue;
+    double p2[2], p3[3];
+    load_pair<kRound>(pts2d, pts3d, i, p2, p3);
+    const double d[3] = {p3[0] - c0[0], p3[1] - c0[1], p3[2] - c0[2]};
+    sc[0] += d[0] * d[0]; sc[1] += d[0] * d[1]; sc[2] += d[0] * d[2]; sc[3] += d[1] * d[1]; sc[4] += d[1] * d[2]; sc[5] += d[2] * d[2];
+  }
+  block_sum<6>(sc, sh.red, sh.sums);
+  if (tid == 0) sh.ok = epnp_basis(sum, sh.sums, m, sh.E) ? 1 : 0;
+  __syncthreads();
+  if (!sh.ok) return 0;
+  double acc[kEpnpSums];
+#pragma unroll
+  for (int k = 0; k < kEpnpSums; ++k) acc[k] = 0.0;
+  for (int i = tid; i < n; i += kEpnpThreads) {
+    if (!use(i)) continue;
+    double p2[2], p3[3], a[4];
+    load_pair<kRound>(pts2d, pts3d, i, p2, p3);
+    epnp_alphas(sh.E, p3, a);
+    epnp_accumulate(a, p2, Kc, acc);
+  }
+  block_sum<kEpnpSums>(acc, sh.red, sh.sums);
+  if (tid == 0) epnp_candidates(sh.sums, sh.E, m, sh.cand);
+  __syncthreads();
+  double err[3] = {0, 0, 0};
+  for (int i = tid; i < n; i += kEpnpThreads) {
+    if (!use(i)) continue;
+    double p2[2], p3[3];
+    load_pair<kRound>(pts2d, pts3d, i, p2, p3);
+    for (int c = 0; c < 3; ++c) err[c] += reproj_dist(sh.cand[c], Kc, p3, p2);
+  }
+  block_sum<3>(err, sh.red, sh.sums);
+  if (tid == 0) *out = sh.cand[epnp_pick(sh.sums)];
+  __syncthreads();
+  return m;
+}
+
+__device__ __forceinline__ void write_pose(const Pose& T, double* dst) {
+  for (int r = 0; r < 3; ++r) {
+    for (int k = 0; k < 3; ++k) dst[r * 4 + k] = T.R[r * 3 + k];
+    dst[r * 4 + 3] = T.t[r];
+  }
+}
+__device__ __forceinline__ void write_identity(double* dst) {
+  for (int k = 0; k < 12; ++k) dst[k] = (k == 0 || k == 5 || k == 10) ? 1.0 : 0.0;
+}
+
+// one block per frame: EPnP on all of its correspondences (cv2.solvePnP(..., flags=SOLVEPNP_EPNP) for B frames)
+__global__ void __launch_bounds__(kEpnpThreads) epnp_frames(const double* __restrict__ Kmat, const double* __restrict__ pts2d, const double* __restrict__ pts3d,
+                                                            const int* __restrict__ offsets, double* __restrict__ pose_out, int* __restrict__ status) {
+  __shared__ EpnpShared sh;
+  __shared__ Pose T;
+  const int b = blockIdx.x;
+  const int o0 = offsets[b], n = offsets[b + 1] - o0;
+  const double* K = Kmat + (size_t)b * 9;
+  const double Kc[4] = {K[0], K[4], K[2], K[5]};
+  const int m = n >= 4 ? epnp_block<false>(pts2d + (size_t)o0 * 2, pts3d + (size_t)o0 * 3, n, Kc, [](int) { return true; }, sh, &T) : 0;
+  if (threadIdx.x == 0) {
+    const bool ok = m >= 4 && pose_finite(T);
+    if (ok) write_pose(T, pose_out + (size_t)b * 12);
+    else write_identity(pose_out + (size_t)b * 12);
+    status[b] = ok ? 1 : 0;
+  }
+}
+
+// EPnP-RANSAC hypotheses: one thread per sample of five distinct correspondences (fp32-rounded), EPnP on them, inliers over
+// all n by OpenCV's rule; a frame of exactly 4 correspondences uses P3P on 0-2, the solution that best reprojects 3
+__global__ void __launch_bounds__(kHypThreads) epnp_hypotheses(const double* __restrict__ Kmat, const double* __restrict__ pts2d, const double* __restrict__ pts3d,
+                                                               const int* __restrict__ offsets, int H, double thr2, unsigned long long seed,
+                                                               double* __restrict__ hyp) {
+  const int b = blockIdx.x;
+  const int h = blockIdx.y * blockDim.x + threadIdx.x;
+  if (h >= H) return;
+  const int o0 = offsets[b], n = offsets[b + 1] - o0;
+  double* out = hyp + ((size_t)b * H + h) * kHypStride;
+  out[0] = 0.0;
+  if (n < 4) return;
+  const double* K = Kmat + (size_t)b * 9;
+  const double Kc[4] = {K[0], K[4], K[2], K[5]};
+  const double* f2 = pts2d + (size_t)o0 * 2;
+  const double* f3 = pts3d + (size_t)o0 * 3;
+  Pose T;
+  bool ok = false;
+  if (n == 4) {
+    double P[4][3], uv[4][2], j[3][3];
+    for (int k = 0; k < 4; ++k) load_pair<true>(f2, f3, k, uv[k], P[k]);
+    for (int k = 0; k < 3; ++k) {
+      j[k][0] = (uv[k][0] - Kc[2]) / Kc[0]; j[k][1] = (uv[k][1] - Kc[3]) / Kc[1]; j[k][2] = 1.0;
+      normalize3(j[k]);
+    }
+    Pose sol[4];
+    const int ns = p3p(P, j, sol);
+    double be = INFINITY;
+    for (int s = 0; s < ns; ++s) {
+      const double e = reproj_dist(sol[s], Kc, P[3], uv[3]);
+      if (e < be) { be = e; T = sol[s]; ok = true; }
+    }
+  } else {
+    // five distinct indices: the k-th draw modulo n - k, shifted past the earlier indices in ascending order
+    uint64_t r = mix64(seed ^ ((uint64_t)b << 40) ^ (uint64_t)h);
+    int idx[5], srt[5];
+    idx[0] = srt[0] = (int)(r % (uint64_t)n);
+    for (int k = 1; k < 5; ++k) {
+      r = mix64(r);
+      int v = (int)(r % (uint64_t)(n - k));
+      for (int e = 0; e < k; ++e)
+        if (v >= srt[e]) ++v;
+      idx[k] = v;
+      int e = k;                                         // insert into the sorted list
+      for (; e > 0 && srt[e - 1] > v; --e) srt[e] = srt[e - 1];
+      srt[e] = v;
+    }
+    double P[5][3], uv[5][2];
+    for (int k = 0; k < 5; ++k) load_pair<true>(f2, f3, idx[k], uv[k], P[k]);
+    ok = epnp_points(P, uv, 5, Kc, T);
+  }
+  if (!ok || !pose_finite(T)) return;
+  int cnt = 0;
+  for (int i = 0; i < n; ++i) {
+    double p2[2], p3[3];
+    load_pair<true>(f2, f3, i, p2, p3);
+    cnt += epnp_inlier(T, Kc, p3, p2, thr2) ? 1 : 0;
+  }
+  if (cnt == 0) return;
+  out[0] = (double)cnt;
+  for (int k = 0; k < 9; ++k) out[1 + k] = T.R[k];
+  for (int k = 0; k < 3; ++k) out[10 + k] = T.t[k];
+}
+
+// one block per frame: the best hypothesis, its inlier set (the reported mask), EPnP on that set
+__global__ void __launch_bounds__(kEpnpThreads) epnp_select_refit(const double* __restrict__ Kmat, const double* __restrict__ pts2d, const double* __restrict__ pts3d,
+                                                                  const int* __restrict__ offsets, int H, double thr2, const double* __restrict__ hyp,
+                                                                  double* __restrict__ pose_out, int* __restrict__ inlier_mask, int* __restrict__ n_inliers) {
+  __shared__ unsigned long long best_key[kRefineThreads];
+  __shared__ EpnpShared sh;
+  __shared__ Pose W, T;
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const int o0 = offsets[b], n = offsets[b + 1] - o0;
+  const double* K = Kmat + (size_t)b * 9;
+  const double Kc[4] = {K[0], K[4], K[2], K[5]};
+  const double* f2 = pts2d + (size_t)o0 * 2;
+  const double* f3 = pts3d + (size_t)o0 * 3;
+  int best_h;
+  const int best_cnt = best_hypothesis(hyp, b, H, best_key, &best_h);
+  if (best_cnt >= 4) {
+    if (tid == 0) {
+      const double* src = hyp + ((size_t)b * H + best_h) * kHypStride;
+      for (int k = 0; k < 9; ++k) W.R[k] = src[1 + k];
+      for (int k = 0; k < 3; ++k) W.t[k] = src[10 + k];
+    }
+    __syncthreads();
+    const Pose Wl = W;
+    auto use = [&](int i) {
+      double p2[2], p3[3];
+      load_pair<true>(f2, f3, i, p2, p3);
+      return epnp_inlier(Wl, Kc, p3, p2, thr2);
+    };
+    for (int i = tid; i < n; i += kEpnpThreads) inlier_mask[o0 + i] = use(i) ? 1 : 0;
+    const int m = epnp_block<true>(pts2d + (size_t)o0 * 2, pts3d + (size_t)o0 * 3, n, Kc, use, sh, &T);
+    if (tid == 0) {                                    // a degenerate inlier set keeps the hypothesis's pose
+      write_pose(m >= 4 && pose_finite(T) ? T : W, pose_out + (size_t)b * 12);
+      n_inliers[b] = best_cnt;                         // the mask's count: the same test as the hypothesis's
+    }
+    return;
+  }
+  // no model: identity pose, no inliers
+  if (tid < 12) pose_out[(size_t)b * 12 + tid] = (tid == 0 || tid == 5 || tid == 10) ? 1.0 : 0.0;
+  for (int i = tid; i < n; i += kEpnpThreads) inlier_mask[o0 + i] = 0;
+  if (tid == 0) n_inliers[b] = 0;
 }
 
 // ---- matched pairs -> the ragged correspondence lists above (reference inference.py:147-152: valid = matches > -1;
@@ -579,5 +1170,27 @@ extern "C" int opb_ransac_pnp(const double* K, const double* pts2d, const double
   opb::pnp_hypotheses<<<dim3((unsigned)B, (unsigned)((hypotheses + opb::kHypThreads - 1) / opb::kHypThreads)), opb::kHypThreads, 0, st>>>(
       K, pts2d, pts3d, offsets, hypotheses, thr2, (unsigned long long)seed, workspace);
   opb::pnp_select_refine<<<(unsigned)B, opb::kRefineThreads, 0, st>>>(K, pts2d, pts3d, offsets, hypotheses, thr2, workspace, pose_out, inlier_mask, n_inliers);
+  return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_E_CUDA;
+}
+
+extern "C" int opb_epnp(const double* K, const double* pts2d, const double* pts3d, const int32_t* offsets, int32_t B, double* pose_out,
+                        int32_t* status, void* stream) {
+  if (!K || !pts2d || !pts3d || !offsets || !pose_out || !status || B <= 0) return OPB_E_INVALID;
+  opb::epnp_frames<<<(unsigned)B, opb::kEpnpThreads, 0, (cudaStream_t)stream>>>(K, pts2d, pts3d, offsets, pose_out, status);
+  return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_E_CUDA;
+}
+
+extern "C" int opb_ransac_epnp(const double* K, const double* pts2d, const double* pts3d, const int32_t* offsets, int32_t B, int32_t hypotheses,
+                               double reproj_error, uint64_t seed, double* workspace, double* pose_out, int32_t* inlier_mask, int32_t* n_inliers,
+                               void* stream) {
+  if (!K || !pts2d || !pts3d || !offsets || !workspace || !pose_out || !inlier_mask || !n_inliers || B <= 0 || hypotheses <= 0 ||
+      hypotheses > opb::kMaxHypotheses || !(reproj_error > 0.0))
+    return OPB_E_INVALID;
+  cudaStream_t st = (cudaStream_t)stream;
+  const double thr2 = reproj_error * reproj_error;
+  opb::epnp_hypotheses<<<dim3((unsigned)B, (unsigned)((hypotheses + opb::kHypThreads - 1) / opb::kHypThreads)), opb::kHypThreads, 0, st>>>(
+      K, pts2d, pts3d, offsets, hypotheses, thr2, (unsigned long long)seed, workspace);
+  opb::epnp_select_refit<<<(unsigned)B, opb::kEpnpThreads, 0, st>>>(K, pts2d, pts3d, offsets, hypotheses, thr2, workspace, pose_out, inlier_mask,
+                                                                    n_inliers);
   return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_E_CUDA;
 }

@@ -4,7 +4,8 @@
 return triple ``(pose [3,4], pose_homo [4,4], inliers)`` as numpy, identity pose and ``[]`` when no pose can be estimated);
 ``ransac_pnp_batch`` solves many frames in one launch and keeps everything on the device.  The arithmetic is
 ``csrc/pnp_ransac.cu`` (P3P minimal samples, inlier counting over all correspondences, Gauss-Newton refinement on the
-inliers) behind ``opb_ransac_pnp``.  The reference delegates to ``cv2.solvePnPRansac`` (EPnP, 10000 iterations, 5 px);
+inliers) behind ``opb_ransac_pnp``; ``method="epnp"`` selects the reference's own estimator instead (``opb_ransac_epnp``:
+five-point EPnP samples, OpenCV's inlier rule, an EPnP refit on the inliers), and ``epnp_batch`` is ``cv2.solvePnP(EPNP)``.  The reference delegates to ``cv2.solvePnPRansac`` (EPnP, 10000 iterations, 5 px);
 parity is on the pose (the reference's cm-degree metric), not on bits -- OpenCV draws its own random samples.
 
 ``gather_matches`` turns the matcher's ``matches0`` into those correspondence lists on the device (``opb_gather_matches``; the
@@ -20,13 +21,19 @@ import torch
 from . import _lib
 
 DEFAULT_HYPOTHESES = 4096      # minimal samples per frame: P(no all-inlier sample) < 1e-9 down to 15 % inliers
+EPNP_HYPOTHESES = 10000        # the reference's iterationsCount: five-point samples need more draws than three-point ones
+METHODS = ("p3p", "epnp")
 
 
-def ransac_pnp_batch(K: torch.Tensor, pts2d: torch.Tensor, pts3d: torch.Tensor, offsets: torch.Tensor, reproj_error: float = 5.0,
-                     hypotheses: int = DEFAULT_HYPOTHESES, seed: int = 0):
-    """K [B,3,3], pts2d [total,2], pts3d [total,3], offsets [B+1] (frame b owns [offsets[b], offsets[b+1])) -- CUDA tensors
-    (any float dtype; computed in fp64).  Returns (pose [B,3,4] f64, inlier_mask [total] bool, n_inliers [B] int32), on the device."""
-    lib = _lib.load()
+def _hypotheses(method, hypotheses):
+    if method not in METHODS:
+        raise ValueError(f"method must be one of {METHODS}, got {method!r}")
+    if hypotheses is None:
+        return DEFAULT_HYPOTHESES if method == "p3p" else EPNP_HYPOTHESES
+    return int(hypotheses)
+
+
+def _frames(K, pts2d, pts3d, offsets):
     dev = pts2d.device
     if dev.type != "cuda":
         raise RuntimeError("onepose_b200 has no CPU path: tensors must be on a CUDA device")
@@ -35,6 +42,33 @@ def ransac_pnp_batch(K: torch.Tensor, pts2d: torch.Tensor, pts3d: torch.Tensor, 
     p2 = pts2d.to(torch.float64).contiguous()
     p3 = pts3d.to(torch.float64).contiguous()
     off = offsets.to(device=dev, dtype=torch.int32).contiguous()
+    return dev, B, K, p2, p3, off
+
+
+def epnp_batch(K: torch.Tensor, pts2d: torch.Tensor, pts3d: torch.Tensor, offsets: torch.Tensor):
+    """EPnP on every correspondence of each frame -- ``cv2.solvePnP(..., flags=SOLVEPNP_EPNP)`` for B frames in one launch.
+    Arguments as in ``ransac_pnp_batch``.  Returns (pose [B,3,4] f64, status [B] int32) on the device: status 1 for a pose,
+    0 (and the identity pose) for a frame with fewer than 4 pairs or a degenerate point set.  No host synchronisation."""
+    lib = _lib.load()
+    dev, B, K, p2, p3, off = _frames(K, pts2d, pts3d, offsets)
+    pose = torch.empty(B, 12, dtype=torch.float64, device=dev)
+    status = torch.empty(B, dtype=torch.int32, device=dev)
+    st = torch.cuda.current_stream(dev).cuda_stream
+    with torch.cuda.device(dev):
+        _lib.check(lib.opb_epnp(K.data_ptr(), p2.data_ptr(), p3.data_ptr(), off.data_ptr(), B, pose.data_ptr(), status.data_ptr(), st))
+    return pose.reshape(B, 3, 4), status
+
+
+def ransac_pnp_batch(K: torch.Tensor, pts2d: torch.Tensor, pts3d: torch.Tensor, offsets: torch.Tensor, reproj_error: float = 5.0,
+                     hypotheses: int | None = None, seed: int = 0, method: str = "p3p"):
+    """K [B,3,3], pts2d [total,2], pts3d [total,3], offsets [B+1] (frame b owns [offsets[b], offsets[b+1])) -- CUDA tensors
+    (any float dtype; computed in fp64).  Returns (pose [B,3,4] f64, inlier_mask [total] bool, n_inliers [B] int32), on the device.
+    ``method`` picks the estimator: "p3p" (default: P3P samples, Gauss-Newton on the inliers; ``hypotheses=None`` = 4096) or
+    "epnp" (the reference's cv2.solvePnPRansac(EPNP): five-point EPnP samples on fp32-rounded inputs, OpenCV's inlier rule, an
+    EPnP refit on the best sample's inliers; ``hypotheses=None`` = 10000).  The two return different poses."""
+    hypotheses = _hypotheses(method, hypotheses)
+    lib = _lib.load()
+    dev, B, K, p2, p3, off = _frames(K, pts2d, pts3d, offsets)
     total = int(p2.shape[0])
     ws = torch.empty(B * hypotheses * 13, dtype=torch.float64, device=dev)
     pose = torch.empty(B, 12, dtype=torch.float64, device=dev)
@@ -42,8 +76,9 @@ def ransac_pnp_batch(K: torch.Tensor, pts2d: torch.Tensor, pts3d: torch.Tensor, 
     cnt = torch.empty(B, dtype=torch.int32, device=dev)
     st = torch.cuda.current_stream(dev).cuda_stream
     with torch.cuda.device(dev):
-        _lib.check(lib.opb_ransac_pnp(K.data_ptr(), p2.data_ptr(), p3.data_ptr(), off.data_ptr(), B, int(hypotheses), float(reproj_error),
-                                      int(seed) & 0xFFFFFFFFFFFFFFFF, ws.data_ptr(), pose.data_ptr(), mask.data_ptr(), cnt.data_ptr(), st))
+        fn = lib.opb_ransac_pnp if method == "p3p" else lib.opb_ransac_epnp
+        _lib.check(fn(K.data_ptr(), p2.data_ptr(), p3.data_ptr(), off.data_ptr(), B, int(hypotheses), float(reproj_error),
+                      int(seed) & 0xFFFFFFFFFFFFFFFF, ws.data_ptr(), pose.data_ptr(), mask.data_ptr(), cnt.data_ptr(), st))
     return pose.reshape(B, 3, 4), mask[:total].bool(), cnt
 
 
@@ -135,12 +170,12 @@ def gather_matches_objects(matches0: torch.Tensor, keypoints2d: torch.Tensor, ke
     return out
 
 
-def _solve(K, g, B, dev, reproj_error, scale, hypotheses, seed):
+def _solve(K, g, B, dev, reproj_error, scale, hypotheses, seed, method):
     K = K.to(device=dev, dtype=torch.float64)
     if K.dim() == 2:
         K = K.expand(B, 3, 3)
     pose, mask, cnt = ransac_pnp_batch(K, g["pts2d"], g["pts3d"] * scale, g["offsets"], reproj_error=reproj_error,
-                                       hypotheses=hypotheses, seed=seed)
+                                       hypotheses=hypotheses, seed=seed, method=method)
     pose[:, :, 3] /= scale
     pose_homo = torch.zeros(B, 4, 4, dtype=torch.float64, device=dev)
     pose_homo[:, :3] = pose
@@ -151,24 +186,26 @@ def _solve(K, g, B, dev, reproj_error, scale, hypotheses, seed):
 
 def poses_from_matches_objects(K: torch.Tensor, keypoints2d: torch.Tensor, keypoints3d, object_ids, matches0: torch.Tensor,
                                matching_scores0: torch.Tensor | None = None, reproj_error: float = 5.0, scale: float = 1000.0,
-                               hypotheses: int = DEFAULT_HYPOTHESES, seed: int = 0):
+                               hypotheses: int | None = None, seed: int = 0, method: str = "p3p"):
     """``poses_from_matches`` for frames of different objects: ``gather_matches_objects`` then ``ransac_pnp_batch``; same
     arguments and outputs, with ``keypoints3d`` / ``object_ids`` as in ``gather_matches_objects``.  No host synchronisation."""
+    hypotheses = _hypotheses(method, hypotheses)
     g = gather_matches_objects(matches0, keypoints2d, keypoints3d, object_ids, matching_scores0)
-    return _solve(K, g, int(matches0.shape[0]), matches0.device, reproj_error, scale, hypotheses, seed)
+    return _solve(K, g, int(matches0.shape[0]), matches0.device, reproj_error, scale, hypotheses, seed, method)
 
 
 def poses_from_matches(K: torch.Tensor, keypoints2d: torch.Tensor, keypoints3d: torch.Tensor, matches0: torch.Tensor,
                        matching_scores0: torch.Tensor | None = None, reproj_error: float = 5.0, scale: float = 1000.0,
-                       hypotheses: int = DEFAULT_HYPOTHESES, seed: int = 0):
+                       hypotheses: int | None = None, seed: int = 0, method: str = "p3p"):
     """Object pose of B frames from the matcher's output: ``gather_matches`` then ``ransac_pnp_batch``, all on the device and with
     no host synchronisation (inference.py:147-155 for a batch).  K [3,3] (shared) or [B,3,3]; the other arguments as in
     ``gather_matches``.  ``scale`` multiplies the 3D points before the solve and divides the translation after it, as
     ``ransac_PnP(..., scale=1000)`` does in the reference.  A frame with fewer than 4 pairs, or no model, gets the identity pose
-    and 0 inliers.  Returns a dict: pose [B,3,4] and pose_homo [B,4,4] f64, n_inliers int32 [B], inlier_mask bool [B*N],
-    query_index, mconf and offsets (rows indexed as in ``gather_matches``)."""
+    and 0 inliers.  ``method`` / ``hypotheses`` as in ``ransac_pnp_batch``.  Returns a dict: pose [B,3,4] and pose_homo [B,4,4]
+    f64, n_inliers int32 [B], inlier_mask bool [B*N], query_index, mconf and offsets (rows indexed as in ``gather_matches``)."""
+    hypotheses = _hypotheses(method, hypotheses)
     g = gather_matches(matches0, keypoints2d, keypoints3d, matching_scores0)
-    return _solve(K, g, int(matches0.shape[0]), matches0.device, reproj_error, scale, hypotheses, seed)
+    return _solve(K, g, int(matches0.shape[0]), matches0.device, reproj_error, scale, hypotheses, seed, method)
 
 
 def pose_errors(pose_pred: torch.Tensor, pose_gt: torch.Tensor):
@@ -195,10 +232,12 @@ def cm_degree(rot_err: torch.Tensor, trans_err: torch.Tensor, thresholds=(1, 3, 
     return {f"{t}cm@{t}degree": float(((rot < t) & (trans < t)).double().mean()) for t in thresholds}
 
 
-def ransac_PnP(K, pts_2d, pts_3d, scale=1, device=None):
+def ransac_PnP(K, pts_2d, pts_3d, scale=1, device=None, method="p3p"):
     """Drop-in for the reference ``ransac_PnP`` (eval_utils.py:18-42): numpy in, numpy out.
     ``scale`` only conditions OpenCV's EPnP in the reference (points x scale, translation / scale): applied and undone here
-    too so that the argument keeps its meaning.  Returns (pose [3,4], pose_homo [4,4], inliers [k,1] int32 or [])."""
+    too so that the argument keeps its meaning.  ``method="epnp"`` runs the reference's estimator (EPnP-RANSAC, 10000
+    samples), the default "p3p" the project's own.  Returns (pose [3,4], pose_homo [4,4], inliers [k,1] int32 or [])."""
+    _hypotheses(method, None)
     dev = torch.device(device if device is not None else "cuda")
     pts_2d = np.ascontiguousarray(np.asarray(pts_2d, dtype=np.float64)).reshape(-1, 2)
     pts_3d = np.ascontiguousarray(np.asarray(pts_3d, dtype=np.float64)).reshape(-1, 3) * scale
@@ -206,7 +245,7 @@ def ransac_PnP(K, pts_2d, pts_3d, scale=1, device=None):
     if n < 4:                                                   # cv2.error branch of the reference (:40-42)
         return np.eye(4)[:3], np.eye(4), []
     pose, mask, cnt = ransac_pnp_batch(torch.from_numpy(np.asarray(K, dtype=np.float64))[None].to(dev), torch.from_numpy(pts_2d).to(dev),
-                                       torch.from_numpy(pts_3d).to(dev), torch.tensor([0, n], dtype=torch.int32, device=dev))
+                                       torch.from_numpy(pts_3d).to(dev), torch.tensor([0, n], dtype=torch.int32, device=dev), method=method)
     if int(cnt[0]) == 0:
         return np.eye(4)[:3], np.eye(4), []
     pose = pose[0].cpu().numpy()
