@@ -205,6 +205,41 @@ int opb_epnp(const double* K, const double* pts2d, const double* pts3d, const in
 int opb_ransac_epnp(const double* K, const double* pts2d, const double* pts3d, const int32_t* offsets, int32_t B, int32_t hypotheses,
                     double reproj_error, uint64_t seed, double* workspace, double* pose_out, int32_t* inlier_mask, int32_t* n_inliers,
                     void* stream);
+/* EPnP-RANSAC as OpenCV runs it: cv2.solvePnPRansac(..., iterationsCount=hypotheses, confidence, flags=SOLVEPNP_EPNP) for B
+ * frames, with OpenCV's sample sequence and stopping rule; no host synchronisation.  Arguments as opb_ransac_epnp without the
+ * seed (OpenCV's generator starts from the same state on every call), plus:
+ *   confidence  0 .. 1 (OpenCV's run() asserts 0 < confidence < 1; 0 and 1 follow RANSACUpdateNumIters' clamped formula:
+ *               0 stops after the first winning sample; 1 lowers the budget to at most
+ *               cvRound(log(DBL_MIN) / log(1 - (1 - outlier ratio)^5)), e.g. about 8700 at 40 % outliers)
+ *   workspace   device f64 [B * (hypotheses * 13 + 16)]
+ *   iterations  device int32 [B] out: the iter at which OpenCV's loop exits (0 for frames of fewer than 6 pairs)
+ * Per frame, as RANSACPointSetRegistrator::run (calib3d/src/ptsetreg.cpp) with PnPRansacCallback:
+ *   samples     cv::RNG from state 2^64 - 1: state = (uint32)state * 4164903690 + (state >> 32), index = (uint32)state % n;
+ *               five per sample, an index equal to an earlier one of the same sample drawn again; sample i of a frame is the
+ *               i-th subset OpenCV draws for its n;
+ *   model       EPnP on the five fp32-rounded pairs (the routine of opb_ransac_epnp); no finite pose = no model;
+ *   count       OpenCV's fp32 error: the projection in fp64 rounded to fp32, the squared distance in fp32, <= (float)thr^2;
+ *   loop        sample i wins when its count > max(best, 4) (the earliest wins a tie); each win lowers the budget to
+ *               RANSACUpdateNumIters(confidence, outlier ratio, 5, budget); the loop exits at iter >= budget;
+ *   result      the winner's inlier set is inlier_mask (n_inliers its count), the pose EPnP on it.  No winner: the identity
+ *               pose and no inliers.  Frames of 4 or 5 pairs are solved once from all of them, every pair an inlier and no
+ *               refit, as solvePnPRansac does when npoints == model_points: 4 pairs by the 4-pair model of opb_ransac_epnp
+ *               (P3P on 0-2, the solution that best reprojects 3; solvePnP(P3P)), 5 by the per-thread EPnP on all five
+ *               (solvePnP(EPNP)).  Fewer than 4 pairs get the identity pose.
+ * Samples are evaluated in waves of W per frame (W chosen from B to fill the device); a frame skips every wave after the one
+ * its loop ends in, so a call costs the waves of its slowest frame, at most ceil(hypotheses / W).  Results past the exit are
+ * discarded, so the outputs do not depend on W. */
+int opb_ransac_epnp_cv(const double* K, const double* pts2d, const double* pts3d, const int32_t* offsets, int32_t B, int32_t hypotheses,
+                       double reproj_error, double confidence, double* workspace, double* pose_out, int32_t* inlier_mask,
+                       int32_t* n_inliers, int32_t* iterations, void* stream);
+/* Test hooks of opb_ransac_epnp_cv.  opb_debug_set_cv_wave: W for later calls (0 = chosen from B).  opb_debug_set_cv_trace:
+ * device buffers later calls fill (NULL to stop): samples int32 [B][capacity][5] and counts int32 [B][capacity] for every
+ * sample i < capacity the loop evaluates (count -1: no model), winner int32 [B] (-1: none).  opb_debug_cv_subsets: the first
+ * count samples of a frame of n >= 5 pairs into out int32 [count][5], by the device's generator, drawn `chunk` at a time
+ * (as the waves draw them). */
+int opb_debug_set_cv_wave(int32_t wave);
+int opb_debug_set_cv_trace(int32_t* samples, int32_t* counts, int32_t* winner, int32_t capacity);
+int opb_debug_cv_subsets(int32_t n, int32_t count, int32_t chunk, int32_t* out, void* stream);
 /* Matched 2D-3D pairs of B frames in the layout opb_ransac_pnp reads; replaces inference.py:147-152 / eval_utils.py:72-77
  * (valid = matches0 > -1; mkpts2d = kpts2d[valid]; mkpts3d = kpts3d[matches0[valid]]; mconf = scores0[valid]).
  *   matches0     device int64 [B, N]  (opb_forward's output; an entry outside [0, M) is not a match)

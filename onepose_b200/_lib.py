@@ -61,6 +61,10 @@ SYMBOLS = {
     "opb_ransac_pnp": (C.c_int, [_P, _P, _P, _P, _I, _I, C.c_double, C.c_uint64, _P, _P, _P, _P, _P]),
     "opb_epnp": (C.c_int, [_P, _P, _P, _P, _I, _P, _P, _P]),
     "opb_ransac_epnp": (C.c_int, [_P, _P, _P, _P, _I, _I, C.c_double, C.c_uint64, _P, _P, _P, _P, _P]),
+    "opb_ransac_epnp_cv": (C.c_int, [_P, _P, _P, _P, _I, _I, C.c_double, C.c_double, _P, _P, _P, _P, _P, _P]),
+    "opb_debug_set_cv_wave": (C.c_int, [_I]),
+    "opb_debug_set_cv_trace": (C.c_int, [_P, _P, _P, _I]),
+    "opb_debug_cv_subsets": (C.c_int, [_I, _I, _I, _P, _P]),
     "opb_gather_matches": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P]),
     "opb_gather_matches_objects": (C.c_int, [_P, _P, _P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P]),
     "opb_debug_set_pdl": (C.c_int, [_I]),

@@ -14,6 +14,7 @@
 //               between rounds (local optimisation) -- what OpenCV's final EPnP refit on the inliers approximates.
 // One launch handles B frames (ragged correspondence lists, offsets[B+1]); everything stays on the device.
 #include <cuda_runtime.h>
+#include <float.h>
 #include <math.h>
 #include <stdint.h>
 
@@ -910,6 +911,25 @@ __global__ void __launch_bounds__(kEpnpThreads) epnp_frames(const double* __rest
   }
 }
 
+// the model of a frame of exactly 4 correspondences (fp32-rounded): P3P on 0-2, the solution that best reprojects 3
+__device__ __forceinline__ bool four_pair_model(const double* f2, const double* f3, const double* Kc, Pose& T) {
+  double P[4][3], uv[4][2], j[3][3];
+  for (int k = 0; k < 4; ++k) load_pair<true>(f2, f3, k, uv[k], P[k]);
+  for (int k = 0; k < 3; ++k) {
+    j[k][0] = (uv[k][0] - Kc[2]) / Kc[0]; j[k][1] = (uv[k][1] - Kc[3]) / Kc[1]; j[k][2] = 1.0;
+    normalize3(j[k]);
+  }
+  Pose sol[4];
+  const int ns = p3p(P, j, sol);
+  double be = INFINITY;
+  bool ok = false;
+  for (int s = 0; s < ns; ++s) {
+    const double e = reproj_dist(sol[s], Kc, P[3], uv[3]);
+    if (e < be) { be = e; T = sol[s]; ok = true; }
+  }
+  return ok;
+}
+
 // EPnP-RANSAC hypotheses: one thread per sample of five distinct correspondences (fp32-rounded), EPnP on them, inliers over
 // all n by OpenCV's rule; a frame of exactly 4 correspondences uses P3P on 0-2, the solution that best reprojects 3
 __global__ void __launch_bounds__(kHypThreads) epnp_hypotheses(const double* __restrict__ Kmat, const double* __restrict__ pts2d, const double* __restrict__ pts3d,
@@ -929,19 +949,7 @@ __global__ void __launch_bounds__(kHypThreads) epnp_hypotheses(const double* __r
   Pose T;
   bool ok = false;
   if (n == 4) {
-    double P[4][3], uv[4][2], j[3][3];
-    for (int k = 0; k < 4; ++k) load_pair<true>(f2, f3, k, uv[k], P[k]);
-    for (int k = 0; k < 3; ++k) {
-      j[k][0] = (uv[k][0] - Kc[2]) / Kc[0]; j[k][1] = (uv[k][1] - Kc[3]) / Kc[1]; j[k][2] = 1.0;
-      normalize3(j[k]);
-    }
-    Pose sol[4];
-    const int ns = p3p(P, j, sol);
-    double be = INFINITY;
-    for (int s = 0; s < ns; ++s) {
-      const double e = reproj_dist(sol[s], Kc, P[3], uv[3]);
-      if (e < be) { be = e; T = sol[s]; ok = true; }
-    }
+    ok = four_pair_model(f2, f3, Kc, T);
   } else {
     // five distinct indices: the k-th draw modulo n - k, shifted past the earlier indices in ascending order
     uint64_t r = mix64(seed ^ ((uint64_t)b << 40) ^ (uint64_t)h);
@@ -1014,6 +1022,341 @@ __global__ void __launch_bounds__(kEpnpThreads) epnp_select_refit(const double* 
   if (tid < 12) pose_out[(size_t)b * 12 + tid] = (tid == 0 || tid == 5 || tid == 10) ? 1.0 : 0.0;
   for (int i = tid; i < n; i += kEpnpThreads) inlier_mask[o0 + i] = 0;
   if (tid == 0) n_inliers[b] = 0;
+}
+
+// ---- EPnP-RANSAC as OpenCV runs it (RANSACPointSetRegistrator::run, calib3d/src/ptsetreg.cpp): OpenCV's sample sequence,
+// its fp32 inlier count and its confidence-driven stopping rule, evaluated in waves of W samples per frame.
+//   cv_scan (wave -1)  per frame: the state below, and wave 0's samples;
+//   cv_wave (wave w)   one thread per sample w*W + h below the frame's budget: EPnP (epnp_points) and the fp32 count;
+//   cv_scan (wave w)   per frame, in sample order: the loop's bookkeeping, then wave w+1's samples unless the loop ended;
+//   cv_select_refit    the winner's inlier set as the mask, EPnP on it.
+// A frame whose loop ended skips every later launch at its first instruction.
+constexpr unsigned kMwcA = 4164903690u;                // cv::RNG's multiplier (CV_RNG_COEFF)
+constexpr int kCvModelPoints = 5;
+constexpr int kCvScanThreads = 32;
+
+struct CvState {                                       // per frame, 16 doubles at the end of the workspace
+  double pose[12];                                     // the winning sample's R (9) and t (3)
+  unsigned long long rng;                              // cv::RNG state after the samples drawn so far
+  int niters;                                          // the loop's budget (only ever lowered)
+  int iter;                                            // the iter at which the loop exited, once done
+  int best;                                            // maxGoodCount
+  int winner;                                          // index of the winning sample, -1 for none
+  int done;
+  int pad;
+};
+static_assert(sizeof(CvState) == 16 * sizeof(double), "CvState is 16 doubles");
+
+__device__ __forceinline__ unsigned mwc_next(unsigned long long& s) {   // cv::RNG::next
+  s = (unsigned long long)(unsigned)s * kMwcA + (s >> 32);
+  return (unsigned)s;
+}
+
+// x % n for 32-bit x by a 64-bit reciprocal m = 2^64 / n rounded up (Lemire, Kaser, Kurz 2019): exact for every 32-bit x, n
+__device__ __forceinline__ unsigned fast_mod(unsigned x, unsigned long long m, unsigned n) { return (unsigned)__umul64hi(m * x, n); }
+__host__ __device__ __forceinline__ unsigned long long fast_mod_m(unsigned n) { return ~0ull / n + 1; }
+
+// getSubset with the default checkSubset: five indices uniform(0, n), an index repeating an earlier one of the sample redrawn.
+// Five distinct draws in a row (the common case for large n) take one branch-free pass.
+__device__ __forceinline__ void cv_subset(unsigned long long& s, unsigned n, unsigned long long m, int* idx) {
+  unsigned long long t = s;
+  int v[kCvModelPoints];
+#pragma unroll
+  for (int k = 0; k < kCvModelPoints; ++k) v[k] = (int)fast_mod(mwc_next(t), m, n);
+  bool distinct = true;
+#pragma unroll
+  for (int a = 0; a < kCvModelPoints; ++a)
+#pragma unroll
+    for (int c = a + 1; c < kCvModelPoints; ++c) distinct &= v[a] != v[c];
+  if (distinct) {
+    s = t;
+#pragma unroll
+    for (int k = 0; k < kCvModelPoints; ++k) idx[k] = v[k];
+    return;
+  }
+  for (int i = 0; i < kCvModelPoints; ++i) {
+    int u;
+    bool rep;
+    do {
+      u = (int)fast_mod(mwc_next(s), m, n);
+      rep = false;
+      for (int e = 0; e < i; ++e) rep |= idx[e] == u;
+    } while (rep);
+    idx[i] = u;
+  }
+}
+
+// RANSACUpdateNumIters: clamps, DBL_MIN guards and cvRound (round half to even) as OpenCV has them
+__device__ int cv_update_num_iters(double p, double ep, int model_points, int max_iters) {
+  p = fmin(fmax(p, 0.0), 1.0);
+  ep = fmin(fmax(ep, 0.0), 1.0);
+  double num = fmax(1.0 - p, DBL_MIN);
+  double denom = 1.0 - pow(1.0 - ep, (double)model_points);
+  if (denom < DBL_MIN) return 0;
+  num = log(num);
+  denom = log(denom);
+  return denom >= 0.0 || -num >= max_iters * (-denom) ? max_iters : __double2int_rn(num / denom);
+}
+
+// PnPRansacCallback::computeError of one fp32-rounded pair: projectPoints in fp64 (x * (1/z), then * f + c; OpenCV's
+// distortion and tilt terms are exact no-ops for zero coefficients) rounded to fp32, the squared distance in fp32.  Explicit
+// roundings: no FMA contraction, as in OpenCV's x86 build, and the same value in every kernel that asks.
+__device__ __forceinline__ float cv_error(const Pose& T, const double* Kc, const double* p3, const double* p2) {
+  double X[3];
+#pragma unroll
+  for (int r = 0; r < 3; ++r)
+    X[r] = __dadd_rn(__dadd_rn(__dadd_rn(__dmul_rn(T.R[r * 3], p3[0]), __dmul_rn(T.R[r * 3 + 1], p3[1])), __dmul_rn(T.R[r * 3 + 2], p3[2])), T.t[r]);
+  const double iz = X[2] != 0.0 ? __ddiv_rn(1.0, X[2]) : 1.0;
+  const float u = (float)__dadd_rn(__dmul_rn(__dmul_rn(X[0], iz), Kc[0]), Kc[2]);
+  const float v = (float)__dadd_rn(__dmul_rn(__dmul_rn(X[1], iz), Kc[1]), Kc[3]);
+  const float du = __fsub_rn((float)p2[0], u), dv = __fsub_rn((float)p2[1], v);
+  return __fadd_rn(__fmul_rn(du, du), __fmul_rn(dv, dv));
+}
+
+constexpr unsigned long long kMwcM = (unsigned long long)kMwcA * 4294967296ull - 1ull;   // the LCG modulus of the MWC
+
+__device__ __forceinline__ unsigned long long mwc_mulmod(unsigned long long x, unsigned long long y) {
+  return (unsigned long long)(((unsigned __int128)x * y) % kMwcM);
+}
+
+// `count` consecutive samples from generator state s (updated), by one warp: every lane calls with the same arguments.
+// The MWC step is state -> state * kMwcA mod kMwcM on residues, so lane l jumps 5 l steps ahead and draws the five indices a
+// sample takes when it needs no redraw; the samples before the first lane that saw a repeat are OpenCV's, and that lane's
+// sample is drawn serially (with its redraws) before the next 32.  fresh: s is the start state 2^64 - 1, which, like the
+// state after it, lies above the modulus (its low word is not its residue's): the first sample is drawn serially.
+// Sample h goes to dst[h * stride .. + 4] (and trace[(trace_first + h) * 5 ..] while below trace_cap).
+__device__ void warp_draw(unsigned long long& s, bool fresh, unsigned n, int count, int* dst, int stride, int* trace, int trace_first,
+                          int trace_cap) {
+  const int lane = threadIdx.x & 31;
+  const unsigned long long m = fast_mod_m(n);
+  auto put = [&](int h, const int* idx) {
+    for (int k = 0; k < kCvModelPoints; ++k) dst[(size_t)h * stride + k] = idx[k];
+    if (trace && trace_first + h < trace_cap)
+      for (int k = 0; k < kCvModelPoints; ++k) trace[(size_t)(trace_first + h) * kCvModelPoints + k] = idx[k];
+  };
+  int h = 0;
+  if (fresh && count > 0) {
+    int idx[kCvModelPoints];
+    cv_subset(s, n, m, idx);
+    if (lane == 0) put(0, idx);
+    h = 1;
+  }
+  unsigned long long jump = 1, sq = kMwcA;             // kMwcA^(5 lane) mod kMwcM
+  for (int e = kCvModelPoints * lane; e; e >>= 1) {
+    if (e & 1) jump = mwc_mulmod(jump, sq);
+    sq = mwc_mulmod(sq, sq);
+  }
+  while (h < count) {
+    const unsigned long long start = mwc_mulmod(s, jump);
+    unsigned long long t = start;
+    int v[kCvModelPoints];
+#pragma unroll
+    for (int k = 0; k < kCvModelPoints; ++k) v[k] = (int)fast_mod(mwc_next(t), m, n);
+    bool distinct = true;
+#pragma unroll
+    for (int a = 0; a < kCvModelPoints; ++a)
+#pragma unroll
+      for (int c = a + 1; c < kCvModelPoints; ++c) distinct &= v[a] != v[c];
+    const int avail = min(32, count - h);
+    const unsigned bad = __ballot_sync(0xffffffffu, lane < avail && !distinct);
+    const int k = bad ? __ffs(bad) - 1 : avail;
+    if (lane < k) put(h + lane, v);
+    if (k == avail) {
+      s = __shfl_sync(0xffffffffu, t, k - 1);
+      h += k;
+    } else {
+      unsigned long long u = __shfl_sync(0xffffffffu, start, k);
+      int idx[kCvModelPoints];
+      cv_subset(u, n, m, idx);
+      if (lane == 0) put(h + k, idx);
+      s = u;
+      h += k + 1;
+    }
+  }
+}
+
+// samples first .. first + W - 1 of frame b, those below its budget, into the wave's records (one warp)
+__device__ void draw_wave(CvState& S, double* r, int n, int W, int first, int b, int* trace_samples, int trace_cap) {
+  const int count = min(W, S.niters - first);
+  unsigned long long s = S.rng;
+  if (count > 0)
+    warp_draw(s, first == 0, (unsigned)n, count, reinterpret_cast<int*>(r), kHypStride * 2, trace_samples + (trace_samples ? (size_t)b * trace_cap * kCvModelPoints : 0),
+              first, trace_cap);
+  if ((threadIdx.x & 31) == 0) S.rng = s;
+}
+
+// wave < 0: initialise frame b's state and draw wave 0.  wave >= 0: run the loop over wave w's counts, then draw wave w+1.
+// A frame of 4 or 5 pairs (model_points == npoints in solvePnPRansac) has one model, of every pair, and no loop.
+// One warp per frame: the loop reads 32 counts at a time and finds the next sample that wins or ends the loop by a ballot
+// (wins are rare); every lane keeps the same copy of the loop's state.  Lane 0 draws the samples.
+__global__ void __launch_bounds__(kCvScanThreads) epnp_cv_scan(const int* __restrict__ offsets, int H, int W, int wave, double confidence,
+                                                              CvState* __restrict__ st, double* __restrict__ rec, int* __restrict__ trace_samples,
+                                                              int trace_cap) {
+  const int b = blockIdx.x, lane = threadIdx.x;
+  CvState& S = st[b];
+  const int n = offsets[b + 1] - offsets[b];
+  double* r = rec + (size_t)b * W * kHypStride;
+  if (wave >= 0 && n > kCvModelPoints) {
+    if (S.done) return;
+    const int base = wave * W;
+    int niters = S.niters, best = S.best, winner = S.winner, done = 0, iter = 0;
+    for (int h0 = 0; h0 < W && !done; h0 += kCvScanThreads) {
+      const int h = h0 + lane;
+      const int c = h < W ? (int)r[(size_t)h * kHypStride] : -1;
+      int from = 0;                                    // lanes below it are done with
+      while (true) {
+        const bool event = lane >= from && h < W && (c > max(best, kCvModelPoints - 1) || base + h + 1 >= niters);
+        const unsigned mask = __ballot_sync(0xffffffffu, event);
+        if (!mask) break;
+        const int e = __ffs(mask) - 1, i = base + h0 + e;
+        const int ce = __shfl_sync(0xffffffffu, c, e);
+        if (ce > max(best, kCvModelPoints - 1)) {      // strict: the earliest sample wins a tie
+          best = ce;
+          winner = i;
+          if (lane < 12) S.pose[lane] = r[(size_t)(h0 + e) * kHypStride + 1 + lane];
+          niters = cv_update_num_iters(confidence, (double)(n - ce) / n, kCvModelPoints, niters);
+        }
+        if (i + 1 >= niters) { done = 1; iter = i + 1; break; }
+        from = e + 1;
+      }
+    }
+    if (lane == 0) {
+      S.niters = niters;
+      S.best = best;
+      S.winner = winner;
+      S.done = done;
+      S.iter = iter;
+    }
+    if (done) return;
+    __syncwarp();
+    draw_wave(S, r, n, W, base + W, b, trace_samples, trace_cap);
+    return;
+  }
+  if (wave < 0) {
+    if (lane == 0) {
+      S.rng = ~0ull;                                   // run() builds RNG rng((uint64)-1) on every call
+      S.niters = n <= kCvModelPoints ? 1 : H;          // 4 or 5 pairs: one model, sample 0 = every pair in order
+      S.iter = 0;
+      S.best = 0;
+      S.winner = -1;
+      S.done = n < 4 ? 1 : 0;
+      if (n >= 4 && n <= kCvModelPoints) {
+        int* si = reinterpret_cast<int*>(r);
+        for (int k = 0; k < kCvModelPoints; ++k) si[k] = k;
+      }
+    }
+    if (n <= kCvModelPoints) return;
+    __syncwarp();                                      // lane 0's state is visible to the warp
+    draw_wave(S, r, n, W, 0, b, trace_samples, trace_cap);
+    return;
+  }
+  if (lane != 0 || S.done) return;                     // wave >= 0, 4 or 5 pairs: take the one model
+  const int c = (int)r[0];
+  if (c >= 0) {
+    S.winner = 0;
+    S.best = n;
+    for (int k = 0; k < 12; ++k) S.pose[k] = r[1 + k];
+  }
+  S.done = 1;
+}
+
+// one thread per sample of the wave: its five indices (written over by its record), EPnP, OpenCV's count.  Record count -1:
+// no model (OpenCV's runKernel failing), which never wins.  Samples at or past the frame's budget are not needed.
+__global__ void __launch_bounds__(kHypThreads) epnp_cv_wave(const double* __restrict__ Kmat, const double* __restrict__ pts2d, const double* __restrict__ pts3d,
+                                                            const int* __restrict__ offsets, int W, int wave, float thr2f, const CvState* __restrict__ st,
+                                                            double* __restrict__ rec, int* __restrict__ trace_counts, int trace_cap) {
+  const int b = blockIdx.x;
+  const int h = blockIdx.y * blockDim.x + threadIdx.x;
+  if (h >= W) return;
+  const CvState& S = st[b];
+  const int i = wave * W + h;
+  if (S.done || i >= S.niters) return;
+  const int o0 = offsets[b], n = offsets[b + 1] - o0;
+  const double* K = Kmat + (size_t)b * 9;
+  const double Kc[4] = {K[0], K[4], K[2], K[5]};
+  const double* f2 = pts2d + (size_t)o0 * 2;
+  const double* f3 = pts3d + (size_t)o0 * 3;
+  double* out = rec + ((size_t)b * W + h) * kHypStride;
+  Pose T;
+  bool ok;
+  if (n == 4) {
+    ok = four_pair_model(f2, f3, Kc, T);
+  } else {
+    const int* si = reinterpret_cast<const int*>(out);
+    double P[5][3], uv[5][2];
+    for (int k = 0; k < 5; ++k) load_pair<true>(f2, f3, si[k], uv[k], P[k]);
+    ok = epnp_points(P, uv, 5, Kc, T);
+  }
+  int cnt = -1;
+  if (ok && pose_finite(T)) {
+    cnt = 0;
+    for (int j = 0; j < n; ++j) {
+      double p2[2], p3[3];
+      load_pair<true>(f2, f3, j, p2, p3);
+      cnt += cv_error(T, Kc, p3, p2) <= thr2f ? 1 : 0;
+    }
+  }
+  out[0] = (double)cnt;
+  for (int k = 0; k < 9; ++k) out[1 + k] = T.R[k];
+  for (int k = 0; k < 3; ++k) out[10 + k] = T.t[k];
+  if (trace_counts && i < trace_cap) trace_counts[(size_t)b * trace_cap + i] = cnt;
+}
+
+// one block per frame: the winner's inlier set as the mask, EPnP on it, the iteration count.  A frame of 4 or 5 pairs keeps
+// its one model (solvePnP(P3P) / solvePnP(EPNP) on every pair in solvePnPRansac), every pair an inlier, with no refit.
+__global__ void __launch_bounds__(kEpnpThreads) epnp_cv_select_refit(const double* __restrict__ Kmat, const double* __restrict__ pts2d, const double* __restrict__ pts3d,
+                                                                     const int* __restrict__ offsets, float thr2f, const CvState* __restrict__ st,
+                                                                     double* __restrict__ pose_out, int* __restrict__ inlier_mask, int* __restrict__ n_inliers,
+                                                                     int* __restrict__ iterations, int* __restrict__ trace_winner) {
+  __shared__ EpnpShared sh;
+  __shared__ Pose T;
+  const int b = blockIdx.x, tid = threadIdx.x;
+  const int o0 = offsets[b], n = offsets[b + 1] - o0;
+  const CvState& S = st[b];
+  const int winner = S.winner;
+  if (tid == 0) {
+    iterations[b] = S.iter;
+    if (trace_winner) trace_winner[b] = winner;
+  }
+  if (winner < 0) {                                    // no model: identity pose, no inliers (run() returns false)
+    if (tid < 12) pose_out[(size_t)b * 12 + tid] = (tid == 0 || tid == 5 || tid == 10) ? 1.0 : 0.0;
+    for (int i = tid; i < n; i += kEpnpThreads) inlier_mask[o0 + i] = 0;
+    if (tid == 0) n_inliers[b] = 0;
+    return;
+  }
+  const double* K = Kmat + (size_t)b * 9;
+  const double Kc[4] = {K[0], K[4], K[2], K[5]};
+  const double* f2 = pts2d + (size_t)o0 * 2;
+  const double* f3 = pts3d + (size_t)o0 * 3;
+  Pose Wl;
+  for (int k = 0; k < 9; ++k) Wl.R[k] = S.pose[k];
+  for (int k = 0; k < 3; ++k) Wl.t[k] = S.pose[9 + k];
+  if (n <= kCvModelPoints) {
+    for (int i = tid; i < n; i += kEpnpThreads) inlier_mask[o0 + i] = 1;
+    if (tid == 0) {
+      write_pose(Wl, pose_out + (size_t)b * 12);
+      n_inliers[b] = n;
+    }
+    return;
+  }
+  auto use = [&](int i) {
+    double p2[2], p3[3];
+    load_pair<true>(f2, f3, i, p2, p3);
+    return cv_error(Wl, Kc, p3, p2) <= thr2f;
+  };
+  for (int i = tid; i < n; i += kEpnpThreads) inlier_mask[o0 + i] = use(i) ? 1 : 0;
+  const int m = epnp_block<true>(f2, f3, n, Kc, use, sh, &T);
+  if (tid == 0) {                                      // a degenerate inlier set keeps the winner's pose
+    write_pose(m >= 4 && pose_finite(T) ? T : Wl, pose_out + (size_t)b * 12);
+    n_inliers[b] = S.best;                             // the mask's count: the same test as the winner's
+  }
+}
+
+// the first `count` samples of a frame of n pairs, by the generator epnp_cv_scan uses (one warp), in calls of `chunk`
+__global__ void epnp_cv_subsets(int n, int count, int chunk, int* __restrict__ out) {
+  unsigned long long s = ~0ull;
+  for (int i = 0; i < count; i += chunk)
+    warp_draw(s, i == 0, (unsigned)n, min(chunk, count - i), out + (size_t)i * kCvModelPoints, kCvModelPoints, nullptr, 0, 0);
 }
 
 // ---- matched pairs -> the ragged correspondence lists above (reference inference.py:147-152: valid = matches > -1;
@@ -1192,5 +1535,74 @@ extern "C" int opb_ransac_epnp(const double* K, const double* pts2d, const doubl
       K, pts2d, pts3d, offsets, hypotheses, thr2, (unsigned long long)seed, workspace);
   opb::epnp_select_refit<<<(unsigned)B, opb::kEpnpThreads, 0, st>>>(K, pts2d, pts3d, offsets, hypotheses, thr2, workspace, pose_out, inlier_mask,
                                                                     n_inliers);
+  return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_E_CUDA;
+}
+
+// test hooks of opb_ransac_epnp_cv (host-side settings read at launch; the launch sequence does not change)
+static int g_cv_wave = 0;                               // samples per frame and wave; 0 = chosen from B
+static int32_t* g_cv_trace_samples = nullptr;
+static int32_t* g_cv_trace_counts = nullptr;
+static int32_t* g_cv_trace_winner = nullptr;
+static int g_cv_trace_cap = 0;
+
+extern "C" int opb_debug_set_cv_wave(int32_t wave) {
+  if (wave < 0) return OPB_E_INVALID;
+  g_cv_wave = wave;
+  return OPB_OK;
+}
+
+extern "C" int opb_debug_set_cv_trace(int32_t* samples, int32_t* counts, int32_t* winner, int32_t capacity) {
+  if (capacity < 0 || ((samples || counts) && capacity == 0)) return OPB_E_INVALID;
+  g_cv_trace_samples = samples;
+  g_cv_trace_counts = counts;
+  g_cv_trace_winner = winner;
+  g_cv_trace_cap = capacity;
+  return OPB_OK;
+}
+
+extern "C" int opb_debug_cv_subsets(int32_t n, int32_t count, int32_t chunk, int32_t* out, void* stream) {
+  if (n < 5 || count <= 0 || chunk <= 0 || !out) return OPB_E_INVALID;
+  opb::epnp_cv_subsets<<<1, 32, 0, (cudaStream_t)stream>>>(n, count, chunk, out);
+  return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_E_CUDA;
+}
+
+// samples per frame and wave: B x W about one 128-thread block per SM.  A wave's time is one thread's EPnP latency (about
+// 2.5 ms on an H100) up to roughly that many threads, and grows with the thread count beyond it (tools/epnp_cv_bench.py,
+// DESIGN 5.4): smaller waves add waves without saving time, larger ones evaluate samples the loop may never need.  Whole
+// blocks, at most the budget.
+static int cv_wave_size(int B, int H) {
+  int w = g_cv_wave;
+  if (w == 0) {
+    int dev = 0, sms = 132;
+    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) sms = 132;
+    const int target = sms * opb::kHypThreads;
+    w = (target / B + opb::kHypThreads - 1) / opb::kHypThreads * opb::kHypThreads;
+    w = w < opb::kHypThreads ? opb::kHypThreads : w;
+  }
+  return w < H ? w : H;
+}
+
+extern "C" int opb_ransac_epnp_cv(const double* K, const double* pts2d, const double* pts3d, const int32_t* offsets, int32_t B, int32_t hypotheses,
+                                  double reproj_error, double confidence, double* workspace, double* pose_out, int32_t* inlier_mask,
+                                  int32_t* n_inliers, int32_t* iterations, void* stream) {
+  if (!K || !pts2d || !pts3d || !offsets || !workspace || !pose_out || !inlier_mask || !n_inliers || !iterations || B <= 0 || hypotheses <= 0 ||
+      hypotheses > opb::kMaxHypotheses || !(reproj_error > 0.0) || !(confidence >= 0.0 && confidence <= 1.0))
+    return OPB_E_INVALID;
+  cudaStream_t st = (cudaStream_t)stream;
+  const float thr2f = (float)(reproj_error * reproj_error);   // findInliers: (float)(thresh * thresh)
+  const int W = cv_wave_size(B, hypotheses);
+  const int waves = (hypotheses + W - 1) / W;
+  opb::CvState* state = reinterpret_cast<opb::CvState*>(workspace + (size_t)B * hypotheses * opb::kHypStride);
+  int* ts = g_cv_trace_samples;
+  int* tc = g_cv_trace_counts;
+  const int cap = g_cv_trace_cap;
+  opb::epnp_cv_scan<<<(unsigned)B, opb::kCvScanThreads, 0, st>>>(offsets, hypotheses, W, -1, confidence, state, workspace, ts, cap);
+  for (int w = 0; w < waves; ++w) {
+    opb::epnp_cv_wave<<<dim3((unsigned)B, (unsigned)((W + opb::kHypThreads - 1) / opb::kHypThreads)), opb::kHypThreads, 0, st>>>(
+        K, pts2d, pts3d, offsets, W, w, thr2f, state, workspace, tc, cap);
+    opb::epnp_cv_scan<<<(unsigned)B, opb::kCvScanThreads, 0, st>>>(offsets, hypotheses, W, w, confidence, state, workspace, ts, cap);
+  }
+  opb::epnp_cv_select_refit<<<(unsigned)B, opb::kEpnpThreads, 0, st>>>(K, pts2d, pts3d, offsets, thr2f, state, pose_out, inlier_mask, n_inliers,
+                                                                       iterations, g_cv_trace_winner);
   return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_E_CUDA;
 }

@@ -6,7 +6,9 @@ return triple ``(pose [3,4], pose_homo [4,4], inliers)`` as numpy, identity pose
 ``csrc/pnp_ransac.cu`` (P3P minimal samples, inlier counting over all correspondences, Gauss-Newton refinement on the
 inliers) behind ``opb_ransac_pnp``; ``method="epnp"`` selects the reference's own estimator instead (``opb_ransac_epnp``:
 five-point EPnP samples, OpenCV's inlier rule, an EPnP refit on the inliers), and ``epnp_batch`` is ``cv2.solvePnP(EPNP)``.  The reference delegates to ``cv2.solvePnPRansac`` (EPnP, 10000 iterations, 5 px);
-parity is on the pose (the reference's cm-degree metric), not on bits -- OpenCV draws its own random samples.
+parity is on the pose (the reference's cm-degree metric), not on bits -- OpenCV draws its own random samples.  With
+``confidence=c`` as well (``opb_ransac_epnp_cv``) the loop is OpenCV's own: its sample sequence, its fp32 inlier count and its
+stopping rule, so a frame stops after the samples OpenCV would draw (about 145 at 50 % inliers and c = 0.99).
 
 ``gather_matches`` turns the matcher's ``matches0`` into those correspondence lists on the device (``opb_gather_matches``; the
 reference's ``valid = matches > -1; mkpts2d = kpts2d[valid]; mkpts3d = kpts3d[matches[valid]]``, inference.py:147-152) and
@@ -25,9 +27,14 @@ EPNP_HYPOTHESES = 10000        # the reference's iterationsCount: five-point sam
 METHODS = ("p3p", "epnp")
 
 
-def _hypotheses(method, hypotheses):
+def _hypotheses(method, hypotheses, confidence=None):
     if method not in METHODS:
         raise ValueError(f"method must be one of {METHODS}, got {method!r}")
+    if confidence is not None:
+        if method != "epnp":
+            raise ValueError("confidence is OpenCV's EPnP-RANSAC stopping rule: it needs method=\"epnp\"")
+        if not 0.0 <= float(confidence) <= 1.0:
+            raise ValueError(f"confidence must be in [0, 1], got {confidence!r}")
     if hypotheses is None:
         return DEFAULT_HYPOTHESES if method == "p3p" else EPNP_HYPOTHESES
     return int(hypotheses)
@@ -60,21 +67,40 @@ def epnp_batch(K: torch.Tensor, pts2d: torch.Tensor, pts3d: torch.Tensor, offset
 
 
 def ransac_pnp_batch(K: torch.Tensor, pts2d: torch.Tensor, pts3d: torch.Tensor, offsets: torch.Tensor, reproj_error: float = 5.0,
-                     hypotheses: int | None = None, seed: int = 0, method: str = "p3p"):
+                     hypotheses: int | None = None, seed: int = 0, method: str = "p3p", confidence: float | None = None,
+                     iterations_out: torch.Tensor | None = None):
     """K [B,3,3], pts2d [total,2], pts3d [total,3], offsets [B+1] (frame b owns [offsets[b], offsets[b+1])) -- CUDA tensors
     (any float dtype; computed in fp64).  Returns (pose [B,3,4] f64, inlier_mask [total] bool, n_inliers [B] int32), on the device.
     ``method`` picks the estimator: "p3p" (default: P3P samples, Gauss-Newton on the inliers; ``hypotheses=None`` = 4096) or
     "epnp" (the reference's cv2.solvePnPRansac(EPNP): five-point EPnP samples on fp32-rounded inputs, OpenCV's inlier rule, an
-    EPnP refit on the best sample's inliers; ``hypotheses=None`` = 10000).  The two return different poses."""
-    hypotheses = _hypotheses(method, hypotheses)
+    EPnP refit on the best sample's inliers; ``hypotheses=None`` = 10000).  The two return different poses.
+    ``confidence`` (``method="epnp"`` only; a ValueError otherwise) runs OpenCV's loop, cv2.solvePnPRansac(...,
+    iterationsCount=hypotheses, confidence=confidence, flags=SOLVEPNP_EPNP): OpenCV's sample sequence (``seed`` plays no part),
+    its fp32 inlier count, and a frame stops when OpenCV's would.  ``iterations_out``, an int32 [B] device tensor, then receives
+    the number of samples each frame's loop ran (0 for frames of fewer than 6 pairs)."""
+    hypotheses = _hypotheses(method, hypotheses, confidence)
     lib = _lib.load()
     dev, B, K, p2, p3, off = _frames(K, pts2d, pts3d, offsets)
     total = int(p2.shape[0])
-    ws = torch.empty(B * hypotheses * 13, dtype=torch.float64, device=dev)
     pose = torch.empty(B, 12, dtype=torch.float64, device=dev)
     mask = torch.zeros(max(total, 1), dtype=torch.int32, device=dev)
     cnt = torch.empty(B, dtype=torch.int32, device=dev)
     st = torch.cuda.current_stream(dev).cuda_stream
+    if confidence is not None:
+        it = iterations_out
+        if it is None:
+            it = torch.empty(B, dtype=torch.int32, device=dev)
+        elif it.device != dev or it.dtype != torch.int32 or tuple(it.shape) != (B,) or not it.is_contiguous():
+            raise ValueError(f"iterations_out must be a contiguous int32 [{B}] tensor on {dev}")
+        ws = torch.empty(B * (hypotheses * 13 + 16), dtype=torch.float64, device=dev)
+        with torch.cuda.device(dev):
+            _lib.check(lib.opb_ransac_epnp_cv(K.data_ptr(), p2.data_ptr(), p3.data_ptr(), off.data_ptr(), B, int(hypotheses),
+                                              float(reproj_error), float(confidence), ws.data_ptr(), pose.data_ptr(), mask.data_ptr(),
+                                              cnt.data_ptr(), it.data_ptr(), st))
+        return pose.reshape(B, 3, 4), mask[:total].bool(), cnt
+    if iterations_out is not None:
+        raise ValueError("iterations_out is filled by the confidence mode only")
+    ws = torch.empty(B * hypotheses * 13, dtype=torch.float64, device=dev)
     with torch.cuda.device(dev):
         fn = lib.opb_ransac_pnp if method == "p3p" else lib.opb_ransac_epnp
         _lib.check(fn(K.data_ptr(), p2.data_ptr(), p3.data_ptr(), off.data_ptr(), B, int(hypotheses), float(reproj_error),
@@ -170,42 +196,47 @@ def gather_matches_objects(matches0: torch.Tensor, keypoints2d: torch.Tensor, ke
     return out
 
 
-def _solve(K, g, B, dev, reproj_error, scale, hypotheses, seed, method):
+def _solve(K, g, B, dev, reproj_error, scale, hypotheses, seed, method, confidence):
     K = K.to(device=dev, dtype=torch.float64)
     if K.dim() == 2:
         K = K.expand(B, 3, 3)
+    its = torch.empty(B, dtype=torch.int32, device=dev) if confidence is not None else None
     pose, mask, cnt = ransac_pnp_batch(K, g["pts2d"], g["pts3d"] * scale, g["offsets"], reproj_error=reproj_error,
-                                       hypotheses=hypotheses, seed=seed, method=method)
+                                       hypotheses=hypotheses, seed=seed, method=method, confidence=confidence, iterations_out=its)
     pose[:, :, 3] /= scale
     pose_homo = torch.zeros(B, 4, 4, dtype=torch.float64, device=dev)
     pose_homo[:, :3] = pose
     pose_homo[:, 3, 3] = 1.0
-    return {"pose": pose, "pose_homo": pose_homo, "n_inliers": cnt, "inlier_mask": mask, "query_index": g["query_index"],
-            "mconf": g["mconf"], "offsets": g["offsets"]}
+    out = {"pose": pose, "pose_homo": pose_homo, "n_inliers": cnt, "inlier_mask": mask, "query_index": g["query_index"],
+           "mconf": g["mconf"], "offsets": g["offsets"]}
+    if its is not None:
+        out["iterations"] = its
+    return out
 
 
 def poses_from_matches_objects(K: torch.Tensor, keypoints2d: torch.Tensor, keypoints3d, object_ids, matches0: torch.Tensor,
                                matching_scores0: torch.Tensor | None = None, reproj_error: float = 5.0, scale: float = 1000.0,
-                               hypotheses: int | None = None, seed: int = 0, method: str = "p3p"):
+                               hypotheses: int | None = None, seed: int = 0, method: str = "p3p", confidence: float | None = None):
     """``poses_from_matches`` for frames of different objects: ``gather_matches_objects`` then ``ransac_pnp_batch``; same
     arguments and outputs, with ``keypoints3d`` / ``object_ids`` as in ``gather_matches_objects``.  No host synchronisation."""
-    hypotheses = _hypotheses(method, hypotheses)
+    hypotheses = _hypotheses(method, hypotheses, confidence)
     g = gather_matches_objects(matches0, keypoints2d, keypoints3d, object_ids, matching_scores0)
-    return _solve(K, g, int(matches0.shape[0]), matches0.device, reproj_error, scale, hypotheses, seed, method)
+    return _solve(K, g, int(matches0.shape[0]), matches0.device, reproj_error, scale, hypotheses, seed, method, confidence)
 
 
 def poses_from_matches(K: torch.Tensor, keypoints2d: torch.Tensor, keypoints3d: torch.Tensor, matches0: torch.Tensor,
                        matching_scores0: torch.Tensor | None = None, reproj_error: float = 5.0, scale: float = 1000.0,
-                       hypotheses: int | None = None, seed: int = 0, method: str = "p3p"):
+                       hypotheses: int | None = None, seed: int = 0, method: str = "p3p", confidence: float | None = None):
     """Object pose of B frames from the matcher's output: ``gather_matches`` then ``ransac_pnp_batch``, all on the device and with
     no host synchronisation (inference.py:147-155 for a batch).  K [3,3] (shared) or [B,3,3]; the other arguments as in
     ``gather_matches``.  ``scale`` multiplies the 3D points before the solve and divides the translation after it, as
     ``ransac_PnP(..., scale=1000)`` does in the reference.  A frame with fewer than 4 pairs, or no model, gets the identity pose
-    and 0 inliers.  ``method`` / ``hypotheses`` as in ``ransac_pnp_batch``.  Returns a dict: pose [B,3,4] and pose_homo [B,4,4]
-    f64, n_inliers int32 [B], inlier_mask bool [B*N], query_index, mconf and offsets (rows indexed as in ``gather_matches``)."""
-    hypotheses = _hypotheses(method, hypotheses)
+    and 0 inliers.  ``method`` / ``hypotheses`` / ``confidence`` as in ``ransac_pnp_batch``.  Returns a dict: pose [B,3,4] and
+    pose_homo [B,4,4] f64, n_inliers int32 [B], inlier_mask bool [B*N], query_index, mconf and offsets (rows indexed as in
+    ``gather_matches``), and with ``confidence`` also iterations int32 [B] (the samples each frame's loop ran)."""
+    hypotheses = _hypotheses(method, hypotheses, confidence)
     g = gather_matches(matches0, keypoints2d, keypoints3d, matching_scores0)
-    return _solve(K, g, int(matches0.shape[0]), matches0.device, reproj_error, scale, hypotheses, seed, method)
+    return _solve(K, g, int(matches0.shape[0]), matches0.device, reproj_error, scale, hypotheses, seed, method, confidence)
 
 
 def pose_errors(pose_pred: torch.Tensor, pose_gt: torch.Tensor):
@@ -232,12 +263,13 @@ def cm_degree(rot_err: torch.Tensor, trans_err: torch.Tensor, thresholds=(1, 3, 
     return {f"{t}cm@{t}degree": float(((rot < t) & (trans < t)).double().mean()) for t in thresholds}
 
 
-def ransac_PnP(K, pts_2d, pts_3d, scale=1, device=None, method="p3p"):
+def ransac_PnP(K, pts_2d, pts_3d, scale=1, device=None, method="p3p", confidence=None):
     """Drop-in for the reference ``ransac_PnP`` (eval_utils.py:18-42): numpy in, numpy out.
     ``scale`` only conditions OpenCV's EPnP in the reference (points x scale, translation / scale): applied and undone here
     too so that the argument keeps its meaning.  ``method="epnp"`` runs the reference's estimator (EPnP-RANSAC, 10000
-    samples), the default "p3p" the project's own.  Returns (pose [3,4], pose_homo [4,4], inliers [k,1] int32 or [])."""
-    _hypotheses(method, None)
+    samples), the default "p3p" the project's own; ``method="epnp", confidence=0.99`` is the reference's call itself, OpenCV's
+    loop with its default confidence.  Returns (pose [3,4], pose_homo [4,4], inliers [k,1] int32 or [])."""
+    _hypotheses(method, None, confidence)
     dev = torch.device(device if device is not None else "cuda")
     pts_2d = np.ascontiguousarray(np.asarray(pts_2d, dtype=np.float64)).reshape(-1, 2)
     pts_3d = np.ascontiguousarray(np.asarray(pts_3d, dtype=np.float64)).reshape(-1, 3) * scale
@@ -245,7 +277,8 @@ def ransac_PnP(K, pts_2d, pts_3d, scale=1, device=None, method="p3p"):
     if n < 4:                                                   # cv2.error branch of the reference (:40-42)
         return np.eye(4)[:3], np.eye(4), []
     pose, mask, cnt = ransac_pnp_batch(torch.from_numpy(np.asarray(K, dtype=np.float64))[None].to(dev), torch.from_numpy(pts_2d).to(dev),
-                                       torch.from_numpy(pts_3d).to(dev), torch.tensor([0, n], dtype=torch.int32, device=dev), method=method)
+                                       torch.from_numpy(pts_3d).to(dev), torch.tensor([0, n], dtype=torch.int32, device=dev), method=method,
+                                       confidence=confidence)
     if int(cnt[0]) == 0:
         return np.eye(4)[:3], np.eye(4), []
     pose = pose[0].cpu().numpy()
