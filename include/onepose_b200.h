@@ -12,6 +12,20 @@
  *
  * Pointer ownership: inputs are borrowed and never written; outputs are caller
  * allocated (device memory unless the name says _host).
+ *
+ * Streams and devices:
+ *   - A handle (opb_matcher, opb_superpoint) owns one workspace and its objects.
+ *     The library orders the calls of one handle across streams: a call on
+ *     another stream than the handle's previous call first makes its stream wait
+ *     for that call (cudaStreamWaitEvent; the host does not block).  Callers
+ *     still order their own buffers (inputs, outputs) against their streams.
+ *   - A handle's work runs on its own device (the `device` of its config); its
+ *     inputs and outputs must live there.  Every handle entry point leaves the
+ *     caller's current device as it found it.
+ *   - The handle-free entry points (features3d producers, RANSAC-PnP, EPnP,
+ *     gather) run on the caller's current device and stream.
+ *   - Calls on different handles may run concurrently, from different threads;
+ *     one handle is used by one thread at a time.
  */
 #ifndef ONEPOSE_B200_H_
 #define ONEPOSE_B200_H_
@@ -114,8 +128,8 @@ int opb_forward_host(opb_matcher* m, const float* desc2d_query_host, const int32
  * range (or a NaN) reports "no match" (-1 / 0) for every point on the device, and the error is delivered to the host lazily:
  *   opb_poll_range   never blocks: OPB_E_RANGE if a finished earlier call raised the flag, OPB_OK otherwise (also while
  *                    the last call is still running);
- *   opb_check_range  waits for the last opb_forward and reports.  opb_forward_host calls it itself.
- * Reporting clears the flag. */
+ *   opb_check_range  waits for the handle's last call and reports.  opb_forward_host calls it itself.
+ * Reporting clears the flag; the clearing is ordered before the handle's next call, on whatever stream. */
 int opb_check_range(opb_matcher* m, void* stream);
 int opb_poll_range(opb_matcher* m);
 
@@ -314,8 +328,8 @@ int opb_sp_forward(opb_superpoint* h, const float* image, int32_t B, int32_t H, 
  *   opb_sp_poll_range   never blocks: OPB_E_RANGE if a finished earlier call raised the flag, OPB_OK otherwise (also while
  *                       the last call is still running).  opb_sp_detect (and so opb_sp_forward) calls it first, and returns
  *                       its error without running;
- *   opb_sp_check_range  waits for the last opb_sp_detect and reports.
- * Reporting clears the flag. */
+ *   opb_sp_check_range  waits for the handle's last call and reports.
+ * Reporting clears the flag; the clearing is ordered before the handle's next call, on whatever stream. */
 int opb_sp_check_range(opb_superpoint* h, void* stream);
 int opb_sp_poll_range(opb_superpoint* h);
 int opb_sp_last_launch_count(const opb_superpoint* h);

@@ -82,9 +82,7 @@ struct opb_matcher : Handle {
   DevBuf hid, kvpart, kmean, statpart, mu, rstd, rowsum_part, colsum_part, rowsum, colsum, rowbest, colbest;
   DevBuf range_flag;
   int* range_host = nullptr;                    // pinned copy of the flag, written at the end of every opb_forward
-  cudaEvent_t range_ev = nullptr;
   bool range_pending = false;
-  cudaStream_t last_stream = nullptr;
   // host-call staging
   DevBuf st_q, st_m0, st_m1, st_s0, st_s1, st_conf, st_len;
   cudaStream_t copy_stream = nullptr;          // opb_forward_host: H2D of chunk i+1 overlaps the compute of chunk i
@@ -101,7 +99,6 @@ struct opb_matcher : Handle {
   ~opb_matcher() {
     for (auto e : h2d_ev) cudaEventDestroy(e);
     if (copy_stream) cudaStreamDestroy(copy_stream);
-    if (range_ev) cudaEventDestroy(range_ev);
     if (range_host) cudaFreeHost(range_host);
   }
 };
@@ -499,11 +496,10 @@ static int forward_frames(opb_matcher* m, ObjectState* const* fobj, const float*
                            st, piece, ci * ppc);
     if (rc) return rc == kStopped ? stopped(m, st) : rc;
   }
-  // deferred range report: the flag travels to pinned host memory behind the call; opb_poll_range() reads it without blocking
+  // deferred range report: the flag travels to pinned host memory behind the call (current once the handle's event, recorded
+  // behind it, has completed); opb_poll_range() reads it without blocking
   CK(m, cudaMemcpyAsync(m->range_host, m->range_flag.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-  CK(m, cudaEventRecord(m->range_ev, st));
   m->range_pending = true;
-  m->last_stream = st;
   m->timeline.finish(st);
   m->last_launches = m->launches;
   return OPB_OK;
@@ -526,21 +522,22 @@ int opb_create(const opb_config* cfg, opb_matcher** out) {
     return fail(g_create_error, OPB_E_INVALID, "scale_factor must be >= 2 log2(e) / 126 = %.6f (got %g)", kMinScaleFactor, (double)cfg->scale_factor);
   cudaDeviceProp prop;
   if (int rc = select_device(cfg->device, prop, g_create_error)) return rc;
+  DeviceGuard dg(cfg->device);
+  if (dg.err) return fail(g_create_error, OPB_E_CUDA, "cudaSetDevice: %s", cudaGetErrorString(dg.err));
   auto* m = new opb_matcher();
   m->cfg = *cfg;
   m->num_sms = prop.multiProcessorCount;
-  if (cudaMallocHost(&m->range_host, sizeof(int)) != cudaSuccess || cudaEventCreateWithFlags(&m->range_ev, cudaEventDisableTiming) != cudaSuccess) {
+  if (int rc = create_handle_state(m, cfg->device, &m->range_host, g_create_error)) {
     delete m;
-    return fail(g_create_error, OPB_E_CUDA, "pinned flag / event allocation failed");
+    return rc;
   }
-  *m->range_host = 0;
   *out = m;
   return OPB_OK;
 }
 
 void opb_destroy(opb_matcher* m) {
   if (!m) return;
-  cudaSetDevice(m->cfg.device);
+  DeviceGuard dg(m->device);
   cudaDeviceSynchronize();   // the frees of the handle's buffers come after the work in flight
   delete m;
 }
@@ -556,7 +553,9 @@ int opb_load_weight(opb_matcher* m, const char* name, const float* data, size_t 
 
 int opb_finalize_weights(opb_matcher* m) {
   if (!m) return OPB_E_INVALID;
-  CK(m, cudaSetDevice(m->cfg.device));
+  DeviceGuard dg(m->device);
+  CK(m, dg.err);
+  CK(m, m->drain());          // the uploads below are host copies: calls in flight may still read the old weights
   // head-contiguous channel order: new c' = h*64 + d  <-  reference c = d*4 + h (GATs_SuperGlue.py:97)
   int perm[kD];
   for (int h = 0; h < kHeads; ++h)
@@ -653,10 +652,11 @@ int opb_set_object(opb_matcher* m, const float* desc3d_db, const float* desc2d_d
   if (!m->weights_ready) return fail(m, OPB_E_STATE, "opb_set_object before opb_finalize_weights");
   if (!desc3d_db || !desc2d_db || M <= 0 || Lf <= 0 || Lf > 32)
     return fail(m, OPB_E_INVALID, "set_object: need M > 0 and 1 <= num_leaf <= 32 (got M=%d, L=%d)", M, Lf);
-  CK(m, cudaSetDevice(m->cfg.device));
-  cudaStream_t st = (cudaStream_t)stream;
+  DeviceGuard dg(m->device);
+  CK(m, dg.err);
+  const cudaStream_t st = (cudaStream_t)stream;
   m->object_ready = false;
-  if (int rc = load_object(m, m->cur, desc3d_db, desc2d_db, M, Lf, st)) return rc;
+  if (int rc = ordered(m, st, [&] { return load_object(m, m->cur, desc3d_db, desc2d_db, M, Lf, st); })) return rc;
   m->object_ready = true;
   return OPB_OK;
 }
@@ -666,10 +666,12 @@ int opb_add_object(opb_matcher* m, const float* desc3d_db, const float* desc2d_d
   if (!m->weights_ready) return fail(m, OPB_E_STATE, "opb_add_object before opb_finalize_weights");
   if (!desc3d_db || !desc2d_db || !object_id || M <= 0 || Lf <= 0 || Lf > 32)
     return fail(m, OPB_E_INVALID, "add_object: need M > 0, 1 <= num_leaf <= 32 and an id pointer (got M=%d, L=%d)", M, Lf);
-  CK(m, cudaSetDevice(m->cfg.device));
+  DeviceGuard dg(m->device);
+  CK(m, dg.err);
+  const cudaStream_t st = (cudaStream_t)stream;
   const int id = m->next_object_id;
   ObjectState& o = m->objects[id];
-  if (int rc = load_object(m, o, desc3d_db, desc2d_db, M, Lf, (cudaStream_t)stream)) {
+  if (int rc = ordered(m, st, [&] { return load_object(m, o, desc3d_db, desc2d_db, M, Lf, st); })) {
     cudaDeviceSynchronize();
     m->objects.erase(id);
     return rc;
@@ -683,7 +685,8 @@ int opb_remove_object(opb_matcher* m, int32_t object_id) {
   if (!m) return OPB_E_INVALID;
   auto it = m->objects.find(object_id);
   if (it == m->objects.end()) return fail(m, OPB_E_INVALID, "remove_object: unknown object id %d", object_id);
-  CK(m, cudaSetDevice(m->cfg.device));
+  DeviceGuard dg(m->device);
+  CK(m, dg.err);
   CK(m, cudaDeviceSynchronize());                  // calls in flight may still read the object's buffers
   m->objects.erase(it);
   return OPB_OK;
@@ -692,7 +695,8 @@ int opb_remove_object(opb_matcher* m, int32_t object_id) {
 int opb_reserve_workspace(opb_matcher* m, int32_t frames, int32_t N) {
   if (!m || frames <= 0 || N <= 0) return OPB_E_INVALID;
   if (!m->object_ready && m->objects.empty()) return fail(m, OPB_E_STATE, "opb_reserve_workspace needs an object (the workspace depends on M)");
-  CK(m, cudaSetDevice(m->cfg.device));
+  DeviceGuard dg(m->device);
+  CK(m, dg.err);
   int m_pad = m->object_ready ? m->cur.m_pad : 0;   // sized for the largest object the handle knows
   for (auto& kv : m->objects) m_pad = std::max(m_pad, kv.second.m_pad);
   return ensure_workspace(m, chunk_of(m, frames), N, m_pad);
@@ -717,9 +721,11 @@ int opb_forward(opb_matcher* m, const float* q, const int32_t* n2d_lengths, int3
   if (!m) return OPB_E_INVALID;
   if (!m->weights_ready || !m->object_ready) return fail(m, OPB_E_STATE, "opb_forward needs weights and an object (finalize_weights, set_object)");
   if (!q || !m0 || !m1 || !s0 || !s1 || B <= 0 || N <= 0) return fail(m, OPB_E_INVALID, "opb_forward: bad argument (B=%d, N=%d)", B, N);
-  CK(m, cudaSetDevice(m->cfg.device));
+  DeviceGuard dg(m->device);
+  CK(m, dg.err);
+  const cudaStream_t st = (cudaStream_t)stream;
   std::vector<ObjectState*> fobj((size_t)B, &m->cur);      // every frame uses the current object
-  return forward_frames(m, fobj.data(), q, n2d_lengths, B, N, m->cur.M, m0, m1, s0, s1, conf, (cudaStream_t)stream);
+  return ordered(m, st, [&] { return forward_frames(m, fobj.data(), q, n2d_lengths, B, N, m->cur.M, m0, m1, s0, s1, conf, st); });
 }
 
 int opb_forward_objects(opb_matcher* m, const int32_t* object_ids_host, const float* q, const int32_t* n2d_lengths, int32_t B, int32_t N,
@@ -740,8 +746,10 @@ int opb_forward_objects(opb_matcher* m, const int32_t* object_ids_host, const fl
     m_max = std::max(m_max, fobj[b]->M);
   }
   if (M_out < m_max) return fail(m, OPB_E_INVALID, "opb_forward_objects: M_out = %d is below the largest object of the call (M = %d)", M_out, m_max);
-  CK(m, cudaSetDevice(m->cfg.device));
-  return forward_frames(m, fobj.data(), q, n2d_lengths, B, N, M_out, m0, m1, s0, s1, conf, (cudaStream_t)stream);
+  DeviceGuard dg(m->device);
+  CK(m, dg.err);
+  const cudaStream_t st = (cudaStream_t)stream;
+  return ordered(m, st, [&] { return forward_frames(m, fobj.data(), q, n2d_lengths, B, N, M_out, m0, m1, s0, s1, conf, st); });
 }
 
 int opb_set_profiling(opb_matcher* m, int32_t enable) {
@@ -753,6 +761,8 @@ int opb_set_profiling(opb_matcher* m, int32_t enable) {
 
 int opb_get_profile(opb_matcher* m, double* gemm_ms, double* gemm_flops, int32_t* gemm_launches, double* total_ms) {
   if (!m || !m->timeline.end) return OPB_E_STATE;
+  DeviceGuard dg(m->device);
+  CK(m, dg.err);
   const Timeline& tl = m->timeline;
   CK(m, cudaEventSynchronize(tl.end));
   double ms = 0, fl = 0;
@@ -782,6 +792,8 @@ int opb_get_profile(opb_matcher* m, double* gemm_ms, double* gemm_flops, int32_t
 
 int opb_get_profile_entry(opb_matcher* m, const char* prefix, double* ms_out, double* flops_out, int32_t* launches_out) {
   if (!m || !prefix || !m->timeline.end) return OPB_E_STATE;
+  DeviceGuard dg(m->device);
+  CK(m, dg.err);
   const Timeline& tl = m->timeline;
   CK(m, cudaEventSynchronize(tl.end));
   double ms = 0, fl = 0;
@@ -804,8 +816,9 @@ int opb_forward_host(opb_matcher* m, const float* qh, const int32_t* n2d_lengths
   if (!m) return OPB_E_INVALID;
   if (!m->object_ready) return fail(m, OPB_E_STATE, "opb_forward_host needs an object");
   if (!qh || !m0h || !m1h || !s0h || !s1h || B <= 0 || N <= 0) return fail(m, OPB_E_INVALID, "opb_forward_host: bad argument");
-  CK(m, cudaSetDevice(m->cfg.device));
-  cudaStream_t st = (cudaStream_t)stream;
+  DeviceGuard dg(m->device);
+  CK(m, dg.err);
+  const cudaStream_t st = (cudaStream_t)stream;
   const size_t M = m->cur.M;
   const bool want_conf = confh != nullptr || materialize_conf != 0;
   DevBuf* stg[] = {&m->st_q, &m->st_m0, &m->st_m1, &m->st_s0, &m->st_s1, &m->st_conf, &m->st_len};
@@ -829,40 +842,50 @@ int opb_forward_host(opb_matcher* m, const float* qh, const int32_t* n2d_lengths
     CK(m, cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
     m->h2d_ev.push_back(e);
   }
-  CK(m, cudaEventRecord(m->h2d_ev[n_ev], st));                           // staging buffer reuse: wait for earlier work on `st`
-  CK(m, cudaStreamWaitEvent(m->copy_stream, m->h2d_ev[n_ev], 0));
-  if (n2d_lengths_host) CK(m, cudaMemcpyAsync(m->st_len.p, n2d_lengths_host, (size_t)B * sizeof(int32_t), cudaMemcpyHostToDevice, m->copy_stream));
-  for (int ci = 0; ci < n_chunks; ++ci) {
-    const int c0 = ci * chunk, cb = std::min(chunk, B - c0);
-    for (int si = 0; si < ppc; ++si) {
-      const int f0 = c0 + si * piece, fb = std::min(piece, c0 + cb - f0);
-      if (fb > 0) {
-        const size_t off = (size_t)f0 * kD * N;
-        CK(m, cudaMemcpyAsync(m->st_q.as<float>() + off, qh + off, (size_t)fb * kD * N * sizeof(float), cudaMemcpyHostToDevice, m->copy_stream));
+  const int rc = ordered(m, st, [&] {
+    CK(m, cudaEventRecord(m->h2d_ev[n_ev], st));                         // staging buffer reuse: wait for earlier work on `st`
+    CK(m, cudaStreamWaitEvent(m->copy_stream, m->h2d_ev[n_ev], 0));
+    if (n2d_lengths_host) CK(m, cudaMemcpyAsync(m->st_len.p, n2d_lengths_host, (size_t)B * sizeof(int32_t), cudaMemcpyHostToDevice, m->copy_stream));
+    for (int ci = 0; ci < n_chunks; ++ci) {
+      const int c0 = ci * chunk, cb = std::min(chunk, B - c0);
+      for (int si = 0; si < ppc; ++si) {
+        const int f0 = c0 + si * piece, fb = std::min(piece, c0 + cb - f0);
+        if (fb > 0) {
+          const size_t off = (size_t)f0 * kD * N;
+          CK(m, cudaMemcpyAsync(m->st_q.as<float>() + off, qh + off, (size_t)fb * kD * N * sizeof(float), cudaMemcpyHostToDevice, m->copy_stream));
+        }
+        CK(m, cudaEventRecord(m->h2d_ev[ci * ppc + si], m->copy_stream));
       }
-      CK(m, cudaEventRecord(m->h2d_ev[ci * ppc + si], m->copy_stream));
     }
-  }
-  m->h2d_pending = n_ev;
-  const int frc = opb_forward(m, m->st_q.as<float>(), n2d_lengths_host ? m->st_len.as<int32_t>() : nullptr, B, N, m->st_m0.as<int64_t>(),
-                              m->st_m1.as<int64_t>(), m->st_s0.as<float>(), m->st_s1.as<float>(), want_conf ? m->st_conf.as<float>() : nullptr, stream);
-  m->h2d_pending = 0;
-  if (frc) return frc;
-  CK(m, cudaMemcpyAsync(m0h, m->st_m0.p, (size_t)B * N * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-  CK(m, cudaMemcpyAsync(m1h, m->st_m1.p, (size_t)B * M * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-  CK(m, cudaMemcpyAsync(s0h, m->st_s0.p, (size_t)B * N * sizeof(float), cudaMemcpyDeviceToHost, st));
-  CK(m, cudaMemcpyAsync(s1h, m->st_s1.p, (size_t)B * M * sizeof(float), cudaMemcpyDeviceToHost, st));
-  if (confh) CK(m, cudaMemcpyAsync(confh, m->st_conf.p, (size_t)B * N * M * sizeof(float), cudaMemcpyDeviceToHost, st));
+    m->h2d_pending = n_ev;
+    const int frc = opb_forward(m, m->st_q.as<float>(), n2d_lengths_host ? m->st_len.as<int32_t>() : nullptr, B, N, m->st_m0.as<int64_t>(),
+                                m->st_m1.as<int64_t>(), m->st_s0.as<float>(), m->st_s1.as<float>(), want_conf ? m->st_conf.as<float>() : nullptr, stream);
+    m->h2d_pending = 0;
+    if (frc) return frc;
+    CK(m, cudaMemcpyAsync(m0h, m->st_m0.p, (size_t)B * N * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    CK(m, cudaMemcpyAsync(m1h, m->st_m1.p, (size_t)B * M * sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+    CK(m, cudaMemcpyAsync(s0h, m->st_s0.p, (size_t)B * N * sizeof(float), cudaMemcpyDeviceToHost, st));
+    CK(m, cudaMemcpyAsync(s1h, m->st_s1.p, (size_t)B * M * sizeof(float), cudaMemcpyDeviceToHost, st));
+    if (confh) CK(m, cudaMemcpyAsync(confh, m->st_conf.p, (size_t)B * N * M * sizeof(float), cudaMemcpyDeviceToHost, st));
+    return (int)OPB_OK;
+  });
+  if (rc) return rc;
   CK(m, cudaStreamSynchronize(st));
   return opb_check_range(m, stream);
 }
 
-// Consume the range flag.  After a synchronisation of the stream the pinned copy written behind the last opb_forward is current.
+// Consume the range flag.  Once the handle's event has completed, the pinned copy written behind the last opb_forward is
+// current.  The reset of the device flag is a call of the handle like any other: the next call, on whatever stream, comes after it.
 static int consume_range_flag(opb_matcher* m) {
   m->range_pending = false;
   if (*m->range_host == 0) return OPB_OK;
   *m->range_host = 0;
-  CK(m, cudaMemsetAsync(m->range_flag.p, 0, sizeof(int), m->last_stream));
+  const cudaStream_t st = m->ev_stream;
+  if (int rc = ordered(m, st, [&] {
+        CK(m, cudaMemsetAsync(m->range_flag.p, 0, sizeof(int), st));
+        return (int)OPB_OK;
+      }))
+    return rc;
   return fail(m, OPB_E_RANGE, "an activation left the fp16-split operand range (|x| >= 1023) or became NaN: the matches of that call were "
                               "reported as -1 (no match)");
 }
@@ -870,13 +893,17 @@ static int consume_range_flag(opb_matcher* m) {
 int opb_check_range(opb_matcher* m, void* stream) {
   if (!m || !m->range_flag.p || !m->range_pending) return OPB_OK;
   (void)stream;
-  CK(m, cudaEventSynchronize(m->range_ev));
+  DeviceGuard dg(m->device);
+  CK(m, dg.err);
+  CK(m, cudaEventSynchronize(m->ev));
   return consume_range_flag(m);
 }
 
 int opb_poll_range(opb_matcher* m) {
   if (!m || !m->range_pending) return OPB_OK;
-  const cudaError_t q = cudaEventQuery(m->range_ev);
+  DeviceGuard dg(m->device);
+  CK(m, dg.err);
+  const cudaError_t q = cudaEventQuery(m->ev);
   if (q == cudaErrorNotReady) return OPB_OK;               // the call is still running: report on a later poll / check
   if (q != cudaSuccess) return fail(m, OPB_E_CUDA, "cudaEventQuery: %s", cudaGetErrorString(q));
   return consume_range_flag(m);
@@ -998,10 +1025,14 @@ int opb_debug_read(opb_matcher* m, int32_t which, void* out, size_t capacity_ele
   if (n_elems) *n_elems = (int64_t)n;
   if (n > capacity_elems) return fail(m, OPB_E_INVALID, "opb_debug_read: buffer %d has %zu elements, capacity %zu", which, n, capacity_elems);
   if (n == 0) return OPB_OK;
-  if (raw) CK(m, cudaMemcpyAsync(out, raw, n * esize, cudaMemcpyDeviceToDevice, st));
-  else join_planes<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(hi, lo, (float*)out, (long long)n);
-  CK(m, cudaGetLastError());
-  return OPB_OK;
+  DeviceGuard dg(m->device);
+  CK(m, dg.err);
+  return ordered(m, st, [&] {
+    if (raw) CK(m, cudaMemcpyAsync(out, raw, n * esize, cudaMemcpyDeviceToDevice, st));
+    else join_planes<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(hi, lo, (float*)out, (long long)n);
+    CK(m, cudaGetLastError());
+    return (int)OPB_OK;
+  });
 }
 
 int opb_debug_set_ws_fill(int32_t byte) {

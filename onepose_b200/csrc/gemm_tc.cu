@@ -915,17 +915,25 @@ int num_sms() {
 
 template <int EPI, int ACV = ACV_NONE, bool HI = false, int BN_ = 256, bool DIAG = false>
 cudaError_t launch_variant(int grid, cudaStream_t stream, const Maps& mp, const TcParams& tp) {
-  static bool attr_done = false;
   auto* kern = gemm_tc_kernel<EPI, ACV, HI, BN_, DIAG>;
-  if (!attr_done) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemBytes);
-    if (e != cudaSuccess) return e;
-    attr_done = true;
-  }
+  if (cudaError_t e = ensure_smem_limit((const void*)kern, kSmemBytes)) return e;
   return launch_k(kern, dim3(grid), dim3(kThreads), kSmemBytes, stream, mp, tp);
 }
 
 }  // namespace
+
+cudaError_t ensure_smem_limit(const void* func, int bytes) {
+  static std::map<std::pair<const void*, int>, int> done;   // (kernel, device) -> limit set
+  static std::mutex mu;
+  int dev = 0;
+  if (cudaError_t e = cudaGetDevice(&dev)) return e;
+  std::lock_guard<std::mutex> lk(mu);
+  int& set = done[{func, dev}];
+  if (bytes <= set) return cudaSuccess;
+  if (cudaError_t e = cudaFuncSetAttribute(func, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes)) return e;
+  set = bytes;
+  return cudaSuccess;
+}
 
 void set_conv_halo_mode(int mode) { g_conv_halo = mode ? 1 : 0; }
 

@@ -11,6 +11,9 @@ int launch_gemm_tc(const GemmProblem& p, cudaStream_t stream);
 // 2-D row-major tensor map [rows, ld] (columns used: `cols`), box = box_cols x box_rows; swizzle follows the box row width
 // (128 B -> SWIZZLE_128B, 64 B -> SWIZZLE_64B).  Cached per (pointer, shape, box, dtype).
 bool make_tensor_map_2d(CUtensorMap* out, const void* ptr, long long rows, long long cols, long long ld, int box_cols, int box_rows, bool f32);
+// Raises the dynamic shared-memory limit of kernel `func` to `bytes` on the current device.  The attribute belongs to a device's
+// context, so it is set once per (kernel, device) -- again only for a larger size; thread-safe.
+cudaError_t ensure_smem_limit(const void* func, int bytes);
 // Programmatic dependent launch switch shared by every launch site (default on; opb_debug_set_pdl).
 bool pdl_enabled();
 void set_pdl_enabled(bool on);

@@ -134,6 +134,26 @@ struct Timeline {
   }
 };
 
+// Makes `device` the current device for the guard's lifetime and gives the caller's current device back afterwards.  Every
+// entry point of a handle runs under one, so a handle's work lands on its own device whatever device the caller has current.
+struct DeviceGuard {
+  int prev = -1;                 // caller's device to restore; -1: nothing to restore
+  cudaError_t err = cudaSuccess;
+  explicit DeviceGuard(int device) {
+    int cur = 0;
+    err = cudaGetDevice(&cur);
+    if (err == cudaSuccess && cur != device) {
+      err = cudaSetDevice(device);
+      if (err == cudaSuccess) prev = cur;
+    }
+  }
+  DeviceGuard(const DeviceGuard&) = delete;
+  DeviceGuard& operator=(const DeviceGuard&) = delete;
+  ~DeviceGuard() {
+    if (prev >= 0) cudaSetDevice(prev);
+  }
+};
+
 // State every handle of the library has; opb_matcher and opb_superpoint derive from it.
 struct Handle {
   std::string err;                                     // message of the last failed call (opb_last_error / opb_sp_last_error)
@@ -141,6 +161,28 @@ struct Handle {
   int find_code = 0;                                   // code of the last failed find_weight
   int launches = 0;                                    // counted launches since begin()
   Timeline timeline;
+  int device = 0;                                      // the handle's device: its memory lives there and its work runs there
+  // Calls of one handle share its workspace and object buffers, so they are ordered across the caller's streams: every call that
+  // enqueues work records `ev` on its stream when it ends (enqueued()), and a call on another stream first makes its stream wait
+  // for that event (enter()) -- a device-side wait, the host does not block.  `ev` also tells when the last call has finished
+  // (the range reports wait for it).
+  cudaEvent_t ev = nullptr;
+  cudaStream_t ev_stream = nullptr;                    // stream `ev` was last recorded on
+  bool ev_recorded = false;
+  Handle() = default;
+  Handle(const Handle&) = delete;
+  Handle& operator=(const Handle&) = delete;
+  ~Handle() {
+    if (ev) cudaEventDestroy(ev);
+  }
+  cudaError_t enter(cudaStream_t st) const { return ev_recorded && st != ev_stream ? cudaStreamWaitEvent(st, ev, 0) : cudaSuccess; }
+  cudaError_t enqueued(cudaStream_t st) {
+    ev_stream = st;
+    ev_recorded = true;
+    return cudaEventRecord(ev, st);
+  }
+  // Host-side wait for the last call (before host copies that overwrite buffers it may still read).
+  cudaError_t drain() const { return ev_recorded ? cudaEventSynchronize(ev) : cudaSuccess; }
   void begin(cudaStream_t st) {
     launches = 0;
     timeline.begin(st);
@@ -179,6 +221,18 @@ inline int fail(Handle* h, int code, const char* fmt, ...) {
     if (_e != cudaSuccess)                                                                            \
       return fail(h, OPB_E_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); \
   } while (0)
+
+// Runs `enqueue()` -- the part of a call that enqueues work for handle `h` on `st` -- after the handle's previous call, and
+// records the handle's event behind it (Handle::enter / enqueued).
+template <typename F>
+inline int ordered(Handle* h, cudaStream_t st, F&& enqueue) {
+  CK(h, h->enter(st));
+  const int rc = enqueue();
+  const cudaError_t e = h->enqueued(st);
+  if (rc) return rc;
+  CK(h, e);
+  return OPB_OK;
+}
 
 // Result of a counted launch of kernel `name`: a failure becomes the handle's error, a success is counted and profiled.
 inline int launched(Handle* h, cudaStream_t st, const char* name, cudaError_t e) {
@@ -234,8 +288,8 @@ inline int upload_f32(Handle* h, DevBuf& dst, const std::vector<double>& w) {
   return 0;
 }
 
-// create: `device` must be an sm_90 device; it becomes the current device and `prop` its properties.  Messages go to `err`,
-// the create-error string of the handle kind.
+// create: `device` must be an sm_90 device; `prop` receives its properties.  The caller's current device is left as it is (the
+// create functions make `device` current with a DeviceGuard).  Messages go to `err`, the create-error string of the handle kind.
 inline int select_device(int device, cudaDeviceProp& prop, std::string& err) {
   int n_dev = 0;
   cudaError_t e = cudaGetDeviceCount(&n_dev);
@@ -245,8 +299,15 @@ inline int select_device(int device, cudaDeviceProp& prop, std::string& err) {
   if (e != cudaSuccess) return fail(err, OPB_E_CUDA, "cudaGetDeviceProperties: %s", cudaGetErrorString(e));
   if (prop.major != 9 || prop.minor != 0)
     return fail(err, OPB_E_CUDA, "device %d is sm_%d%d; this library is built for sm_90a only", device, prop.major, prop.minor);
-  e = cudaSetDevice(device);
-  if (e != cudaSuccess) return fail(err, OPB_E_CUDA, "cudaSetDevice: %s", cudaGetErrorString(e));
+  return OPB_OK;
+}
+
+// The rest of a handle's creation on its (already current) device: the order event and the pinned copy of the range flag.
+inline int create_handle_state(Handle* h, int device, int** range_host, std::string& err) {
+  h->device = device;
+  if (cudaMallocHost(range_host, sizeof(int)) != cudaSuccess || cudaEventCreateWithFlags(&h->ev, cudaEventDisableTiming) != cudaSuccess)
+    return fail(err, OPB_E_CUDA, "pinned flag / event allocation failed");
+  **range_host = 0;
   return OPB_OK;
 }
 

@@ -176,12 +176,7 @@ KvGroups kv_groups_for(const Layout& L, int num_sms) {
 }
 
 cudaError_t launch_kv_state_h(const __half* kvh, const Layout& L, const KvGroups& G, float* partial, cudaStream_t stream) {
-  static bool attr_done = false;
-  if (!attr_done) {
-    const cudaError_t e = cudaFuncSetAttribute(kv_state_h_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kHSmemBytes);
-    if (e != cudaSuccess) return e;
-    attr_done = true;
-  }
+  if (const cudaError_t e = ensure_smem_limit((const void*)kv_state_h_kernel, kHSmemBytes)) return e;
   CUtensorMap map;
   if (!make_tensor_map_2d(&map, kvh, L.rows(), 512, 512, 64, kHRows, false)) return cudaErrorInvalidValue;
   return launch_k(kv_state_h_kernel, dim3((unsigned)(L.B * (G.gq + G.gd))), dim3(kHThreads), kHSmemBytes, stream, map, L, G, partial);

@@ -465,18 +465,16 @@ struct opb_superpoint : Handle {
   int ws_B = 0, ws_H = 0, ws_W = 0;
   PlaneBuf arena[2];               // ping-pong activations
   DevBuf logits, ddesc, scores, nms, cand_idx, cand_score, blk_counts, totals;
-  // range guard (opb_sp_check_range): the device flag, its pinned copy written at the end of every opb_sp_detect
+  // range guard (opb_sp_check_range): the device flag, its pinned copy written at the end of every opb_sp_detect (current once
+  // the handle's event has completed)
   DevBuf range_flag;
   int* range_host = nullptr;
-  cudaEvent_t range_ev = nullptr;
   bool range_pending = false;
-  cudaStream_t last_stream = nullptr;
   int last_B = 0, last_H = 0, last_W = 0;
   int stop_after = -1;             // test hook: leave the encoder after layer i (opb_sp_debug_set_stop)
   int dbg_arena = 0, dbg_c = 0;
   long long dbg_rows = 0;
   ~opb_superpoint() {
-    if (range_ev) cudaEventDestroy(range_ev);
     if (range_host) cudaFreeHost(range_host);
   }
 };
@@ -600,20 +598,21 @@ int opb_sp_create(const opb_sp_config* cfg, opb_superpoint** out) {
     return fail(g_sp_create_error, OPB_E_NOT_IMPLEMENTED, "nms_radius %d: the tiled NMS supports 0..6", cfg->nms_radius);
   cudaDeviceProp prop;
   if (int rc = select_device(cfg->device, prop, g_sp_create_error)) return rc;
+  DeviceGuard dg(cfg->device);
+  if (dg.err) return fail(g_sp_create_error, OPB_E_CUDA, "cudaSetDevice: %s", cudaGetErrorString(dg.err));
   auto* h = new opb_superpoint();
   h->cfg = *cfg;
-  if (cudaMallocHost(&h->range_host, sizeof(int)) != cudaSuccess || cudaEventCreateWithFlags(&h->range_ev, cudaEventDisableTiming) != cudaSuccess) {
+  if (int rc = create_handle_state(h, cfg->device, &h->range_host, g_sp_create_error)) {
     delete h;
-    return fail(g_sp_create_error, OPB_E_CUDA, "pinned flag / event allocation failed");
+    return rc;
   }
-  *h->range_host = 0;
   *out = h;
   return OPB_OK;
 }
 
 void opb_sp_destroy(opb_superpoint* h) {
   if (!h) return;
-  cudaSetDevice(h->cfg.device);
+  DeviceGuard dg(h->device);
   cudaDeviceSynchronize();   // the frees of the handle's buffers come after the work in flight
   delete h;
 }
@@ -629,6 +628,9 @@ int opb_sp_load_weight(opb_superpoint* h, const char* name, const float* data, s
 
 int opb_sp_finalize_weights(opb_superpoint* h) {
   if (!h) return OPB_E_INVALID;
+  DeviceGuard dg(h->device);
+  CK(h, dg.err);
+  CK(h, h->drain());          // the uploads below are host copies: calls in flight may still read the old weights
   const auto* w1 = find_weight(h, "conv1a.weight", 64 * 9);
   const auto* b1 = find_weight(h, "conv1a.bias", 64);
   if (!w1 || !b1) return h->find_code;
@@ -652,14 +654,8 @@ int opb_sp_finalize_weights(opb_superpoint* h) {
   return OPB_OK;
 }
 
-int opb_sp_detect(opb_superpoint* h, const float* image, int32_t B, int32_t H, int32_t W, int32_t* counts, void* stream) {
-  if (!h || !image || B <= 0 || H <= 0 || W <= 0) return h ? fail(h, OPB_E_INVALID, "bad argument") : OPB_E_INVALID;
-  if (!h->ready) return fail(h, OPB_E_STATE, "weights not finalized");
-  if (H % 8 || W % 8) return fail(h, OPB_E_INVALID, "image size %dx%d: height and width must be multiples of 8 (three 2x2 poolings)", H, W);
-  if ((long long)B * stage_of(H, W, 0).ppad > 0x7fffff00LL) return fail(h, OPB_E_INVALID, "batch too large for 32-bit row indices");
-  if (int rc = opb_sp_poll_range(h)) return rc;             // deferred report of a finished earlier call
-  if (int rc = sp_ensure_workspace(h, B, H, W)) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
+// The work of opb_sp_detect, enqueued on `st` (arguments checked, workspace sized).
+static int sp_detect(opb_superpoint* h, const float* image, int B, int H, int W, int32_t* counts, cudaStream_t st) {
   h->begin(st);
   const Stage s0 = stage_of(H, W, 0), s1 = stage_of(H, W, 1), s2 = stage_of(H, W, 2), s3 = stage_of(H, W, 3);
   PlaneBuf& A = h->arena[0];
@@ -709,11 +705,7 @@ int opb_sp_detect(opb_superpoint* h, const float* image, int32_t B, int32_t H, i
   {
     const int r = h->cfg.nms_radius, D = kNmsTile + 10 * r;
     const size_t smem = (size_t)6 * D * D * sizeof(float);
-    static size_t smem_set = 0;
-    if (smem > smem_set) {
-      CK(h, cudaFuncSetAttribute(sp_nms, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      smem_set = smem;
-    }
+    CK(h, ensure_smem_limit((const void*)sp_nms, (int)smem));
     LAUNCH(h, st, "sp_nms", sp_nms, dim3((W + kNmsTile - 1) / kNmsTile, (H + kNmsTile - 1) / kNmsTile, B), dim3(512), smem, st,
             (const float*)h->scores.as<float>(), (int)H, (int)W, r, h->nms.as<float>());
   }
@@ -728,24 +720,39 @@ int opb_sp_detect(opb_superpoint* h, const float* image, int32_t B, int32_t H, i
            (const int*)h->range_flag.as<int>(), counts);
   // deferred range report: every producer of split planes has run; the flag travels to pinned host memory behind the call
   CK(h, cudaMemcpyAsync(h->range_host, h->range_flag.p, sizeof(int), cudaMemcpyDeviceToHost, st));
-  CK(h, cudaEventRecord(h->range_ev, st));
   h->range_pending = true;
-  h->last_stream = st;
   return OPB_OK;
+}
+
+int opb_sp_detect(opb_superpoint* h, const float* image, int32_t B, int32_t H, int32_t W, int32_t* counts, void* stream) {
+  if (!h || !image || B <= 0 || H <= 0 || W <= 0) return h ? fail(h, OPB_E_INVALID, "bad argument") : OPB_E_INVALID;
+  if (!h->ready) return fail(h, OPB_E_STATE, "weights not finalized");
+  if (H % 8 || W % 8) return fail(h, OPB_E_INVALID, "image size %dx%d: height and width must be multiples of 8 (three 2x2 poolings)", H, W);
+  if ((long long)B * stage_of(H, W, 0).ppad > 0x7fffff00LL) return fail(h, OPB_E_INVALID, "batch too large for 32-bit row indices");
+  DeviceGuard dg(h->device);
+  CK(h, dg.err);
+  if (int rc = opb_sp_poll_range(h)) return rc;             // deferred report of a finished earlier call
+  if (int rc = sp_ensure_workspace(h, B, H, W)) return rc;
+  const cudaStream_t st = (cudaStream_t)stream;
+  return ordered(h, st, [&] { return sp_detect(h, image, B, H, W, counts, st); });
 }
 
 int opb_sp_describe(opb_superpoint* h, float* keypoints, float* scores, float* descriptors, int32_t* counts, int32_t cap, void* stream) {
   if (!h || !keypoints || !scores || !counts || cap <= 0) return h ? fail(h, OPB_E_INVALID, "bad argument") : OPB_E_INVALID;
   if (!h->last_B) return fail(h, OPB_E_STATE, "opb_sp_describe without a preceding opb_sp_detect");
-  cudaStream_t st = (cudaStream_t)stream;
+  DeviceGuard dg(h->device);
+  CK(h, dg.err);
+  const cudaStream_t st = (cudaStream_t)stream;
   const int B = h->last_B, H = h->last_H, W = h->last_W, HW = H * W;
   const Stage s3 = stage_of(H, W, 3);
-  LAUNCH(h, st, "sp_emit", sp_emit, dim3((HW + 255) / 256, B), dim3(256), 0, st, (const int*)h->cand_idx.as<int>(), (const float*)h->cand_score.as<float>(),
-          (const int*)h->totals.as<int>(), HW, W, h->cfg.max_keypoints, (int)cap, (const int*)h->range_flag.as<int>(), keypoints, scores, counts);
-  if (descriptors)
-    LAUNCH(h, st, "sp_sample", sp_sample, dim3(((long long)cap * 32 + 255) / 256, B), dim3(256), 0, st, (const float*)h->ddesc.as<float>(), s3.h, s3.w, s3.ppad,
-            (const float*)keypoints, (const int*)counts, (int)cap, h->cfg.align_corners, descriptors);
-  return OPB_OK;
+  return ordered(h, st, [&] {
+    LAUNCH(h, st, "sp_emit", sp_emit, dim3((HW + 255) / 256, B), dim3(256), 0, st, (const int*)h->cand_idx.as<int>(), (const float*)h->cand_score.as<float>(),
+            (const int*)h->totals.as<int>(), HW, W, h->cfg.max_keypoints, (int)cap, (const int*)h->range_flag.as<int>(), keypoints, scores, counts);
+    if (descriptors)
+      LAUNCH(h, st, "sp_sample", sp_sample, dim3(((long long)cap * 32 + 255) / 256, B), dim3(256), 0, st, (const float*)h->ddesc.as<float>(), s3.h, s3.w, s3.ppad,
+              (const float*)keypoints, (const int*)counts, (int)cap, h->cfg.align_corners, descriptors);
+    return (int)OPB_OK;
+  });
 }
 
 int opb_sp_forward(opb_superpoint* h, const float* image, int32_t B, int32_t H, int32_t W, float* keypoints, float* scores, float* descriptors,
@@ -754,12 +761,18 @@ int opb_sp_forward(opb_superpoint* h, const float* image, int32_t B, int32_t H, 
   return opb_sp_describe(h, keypoints, scores, descriptors, counts, cap, stream);
 }
 
-// Consume the range flag.  After the event of the last opb_sp_detect has completed, the pinned copy is current.
+// Consume the range flag.  Once the handle's event has completed, the pinned copy of the last opb_sp_detect is current.  The
+// reset of the device flag is a call of the handle like any other: the next call, on whatever stream, comes after it.
 static int sp_consume_range_flag(opb_superpoint* h) {
   h->range_pending = false;
   if (*h->range_host == 0) return OPB_OK;
   *h->range_host = 0;
-  CK(h, cudaMemsetAsync(h->range_flag.p, 0, sizeof(int), h->last_stream));
+  const cudaStream_t st = h->ev_stream;
+  if (int rc = ordered(h, st, [&] {
+        CK(h, cudaMemsetAsync(h->range_flag.p, 0, sizeof(int), st));
+        return (int)OPB_OK;
+      }))
+    return rc;
   return fail(h, OPB_E_RANGE, "an activation left the fp16-split operand range (|x| >= 1023) or became NaN: the call reported no key "
                               "points (count 0) for every image");
 }
@@ -767,13 +780,17 @@ static int sp_consume_range_flag(opb_superpoint* h) {
 int opb_sp_check_range(opb_superpoint* h, void* stream) {
   if (!h || !h->range_pending) return OPB_OK;
   (void)stream;
-  CK(h, cudaEventSynchronize(h->range_ev));
+  DeviceGuard dg(h->device);
+  CK(h, dg.err);
+  CK(h, cudaEventSynchronize(h->ev));
   return sp_consume_range_flag(h);
 }
 
 int opb_sp_poll_range(opb_superpoint* h) {
   if (!h || !h->range_pending) return OPB_OK;
-  const cudaError_t q = cudaEventQuery(h->range_ev);
+  DeviceGuard dg(h->device);
+  CK(h, dg.err);
+  const cudaError_t q = cudaEventQuery(h->ev);
   if (q == cudaErrorNotReady) return OPB_OK;               // the call is still running: report on a later poll / check
   if (q != cudaSuccess) return fail(h, OPB_E_CUDA, "cudaEventQuery: %s", cudaGetErrorString(q));
   return sp_consume_range_flag(h);
@@ -791,6 +808,7 @@ int opb_sp_get_profile(opb_superpoint* h, int32_t index, char* name, size_t name
   if (!h || index < 0) return OPB_E_INVALID;
   const Timeline& tl = h->timeline;
   if ((size_t)index >= tl.size()) return OPB_E_INVALID;
+  DeviceGuard dg(h->device);
   cudaEventSynchronize(tl.ev[index]);
   float t = 0.f;
   tl.ms(index, &t);
@@ -824,19 +842,21 @@ int opb_sp_debug_read(opb_superpoint* h, int32_t which, float* out, size_t capac
     case 1: n = (size_t)B * H * W; src = h->nms.p; break;                          // after NMS
     case 2: n = (size_t)B * s3.ppad * 128; src = h->logits.p; break;               // convPb output rows [B*P3, 128] (65 valid)
     case 3: n = (size_t)B * s3.ppad * 256; src = h->ddesc.p; break;                // convDb output rows [B*P3, 256]
-    case 4: {                                                                      // activation planes of the last layer run (stop hook)
-      n = (size_t)h->dbg_rows * h->dbg_c;
-      if (n_elems) *n_elems = (int64_t)n;
-      if (n > capacity_elems) return OPB_E_INVALID;
-      const PlaneBuf& a = h->arena[h->dbg_arena];
-      sp_join_planes<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(a.hi.as<__half>(), a.lo.as<__half>(), out, (long long)n);
-      return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_E_CUDA;
-    }
+    case 4: n = (size_t)h->dbg_rows * h->dbg_c; break;                             // activation planes of the last layer run (stop hook)
     default: return OPB_E_INVALID;
   }
   if (n_elems) *n_elems = (int64_t)n;
   if (n > capacity_elems) return OPB_E_INVALID;
-  return cudaMemcpyAsync(out, src, n * sizeof(float), cudaMemcpyDeviceToDevice, st) == cudaSuccess ? OPB_OK : OPB_E_CUDA;
+  DeviceGuard dg(h->device);
+  if (dg.err) return OPB_E_CUDA;
+  return ordered(h, st, [&] {
+    if (which == 4) {
+      const PlaneBuf& a = h->arena[h->dbg_arena];
+      sp_join_planes<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(a.hi.as<__half>(), a.lo.as<__half>(), out, (long long)n);
+      return cudaGetLastError() == cudaSuccess ? (int)OPB_OK : (int)OPB_E_CUDA;
+    }
+    return cudaMemcpyAsync(out, src, n * sizeof(float), cudaMemcpyDeviceToDevice, st) == cudaSuccess ? (int)OPB_OK : (int)OPB_E_CUDA;
+  });
 }
 
 }  // extern "C"

@@ -191,6 +191,11 @@ class GATsSuperGlue(nn.Module):
         if self._handle is None or self._M is None:
             raise RuntimeError("no object set: call set_object(descriptors3d_db, descriptors2d_db) first (or use forward(data))")
 
+    def _check_device(self, q: torch.Tensor):
+        """The handle's work runs on its own device, so the queries (and every buffer of the call) must live there."""
+        if q.device != self._handle_device:
+            raise ValueError(f"descriptors2d_query is on {q.device}, the matcher's objects and workspace are on {self._handle_device}")
+
     def match_frames(self, descriptors2d_query: torch.Tensor, return_conf: bool = True, lengths: torch.Tensor | None = None,
                      out: dict | None = None):
         """B frames of the current object.  descriptors2d_query [B, 256, N] CUDA fp32; lengths (optional) CUDA int32 [B] =
@@ -200,6 +205,7 @@ class GATsSuperGlue(nn.Module):
         out (optional): flat CUDA buffers {"matches0", "matches1": int64, "matching_scores0", "matching_scores1", "conf_matrix":
         fp32} at least as large as the results; the returned tensors are views of them (a serving loop allocates once)."""
         self._require_object()
+        self._check_device(descriptors2d_query)
         q = descriptors2d_query.float().contiguous()
         B, _, N = q.shape
         M = self._M
@@ -260,6 +266,7 @@ class GATsSuperGlue(nn.Module):
         storage as in match_frames.  Asynchronous: no host synchronisation."""
         if self._handle is None:
             raise RuntimeError("no object registered: call add_object first")
+        self._check_device(descriptors2d_query)
         self._sync_weights()
         ids = [int(i) for i in (object_ids.tolist() if isinstance(object_ids, torch.Tensor) else object_ids)]
         q = descriptors2d_query.float().contiguous()
