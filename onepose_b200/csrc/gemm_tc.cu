@@ -109,8 +109,6 @@ __device__ __forceinline__ uint32_t stg64_off(int r, int j) { return (uint32_t)(
 struct TcParams {
   int K1, K2;            // reduction split (multiples of BK)
   int b2_per_seg;
-  int b2_lo_zero;        // skip the A_hi . B_lo pass of the K2 block (identity K-block: B_lo == 0)
-  int b2_identity;       // K2 block = identity: diagonal 64 x 64 blocks as N = 64 MMAs (GemmProblem::b2_identity)
   int n_out;
   int m_tiles, n_tiles, batch;
   long long a_batch_rows, b_batch_rows;
@@ -162,18 +160,25 @@ enum { ACV_NONE = 0, ACV_NORM_RELU = 1 };
 // HI: the A operand enters with its hi plane only (k,v projection, GemmProblem::a_hi_only): two passes, A_hi + B_hi + B_lo per stage.
 // BN_: column-tile width (256 for every matcher GEMM; 64 / 128 for the narrow convolution layers of the extractor: the stage
 // shrinks and the ring deepens to three / four stages).
-// DIAG: the K2 block is the identity (GemmProblem::b2_identity) and runs as N = 64 MMAs on the diagonal blocks.  Those MMAs
-// write 32-register slices of the m64n256 accumulator, which makes ptxas serialise every wgmma of the kernel, so the slices
-// live in an instantiation of their own and the other variants keep back-to-back MMAs.
-template <int EPI, int ACV = ACV_NONE, bool HI = false, int BN_ = 256, bool DIAG = false>
+// K2B: what the K2 block's B operand is (the residual GEMM's identity: GemmProblem::b2_lo_zero / b2_identity).
+//   K2_LO_ZERO  its lo plane is zero: the A_hi.B_lo pass of those k-blocks is not issued (it would add exact zeros)
+//   K2_DIAG     the identity, run as N = 64 MMAs on the diagonal blocks.  Those MMAs write 32-register slices of the m64n256
+//               accumulator, which makes ptxas serialise every wgmma of the kernel, so the slices live in an instantiation of
+//               their own and the other variants keep back-to-back MMAs.
+// Both are template properties so that the other variants' k-blocks are one branch-free chain of MMAs: a branch between two
+// wgmmas makes ptxas insert a warpgroup.arrive in front of the MMAs that follow it.
+enum { K2_FULL = 0, K2_LO_ZERO = 1, K2_DIAG = 2 };
+
+template <int EPI, int ACV = ACV_NONE, bool HI = false, int BN_ = 256, int K2B = K2_FULL>
 __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_constant__ Maps maps, TcParams p) {
   constexpr int BN = BN_;
+  constexpr bool DIAG = K2B == K2_DIAG;
   constexpr int kBBytes = BN * BK * 2;             // one plane of the B tile
   constexpr int kBOff = HI ? kABytes : 2 * kABytes;      // offset of the B planes inside a stage
   constexpr int kStageBytes = kBOff + 2 * kBBytes;
   constexpr int kStages = kRingBytes / kStageBytes;      // BN 256: 2, BN 128: 3, BN 64: 4
   constexpr int kDiagBBytes = 64 * BK * 2;         // a 64 x 64 diagonal block of the identity
-  static_assert(!DIAG || (BN_ == 256 && EPI == EPI_BIAS_PLANES), "identity K-block: residual GEMMs only");
+  static_assert(K2B == K2_FULL || (BN_ == 256 && EPI == EPI_BIAS_PLANES), "identity K-block: residual GEMMs only");
   static_assert(EPI == EPI_CONV ? BN_ == 64 || BN_ == 128 : EPI == EPI_F32 ? BN_ == 128 || BN_ == 256 : BN_ == 256,
                 "tile widths: EPI_CONV 64 / 128, EPI_F32 128 / 256, every other epilogue 256");
   static_assert(BN_ == 256 || ACV == ACV_NONE && !HI, "narrow tiles: no converter, both A planes");
@@ -444,7 +449,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
           }
           const uint32_t sa_h = smem_u32(st) + a_off;
           const uint32_t sa_l = sa_h + kABytes, sb_h = smem_u32(st) + kBOff, sb_l = sb_h + kBBytes;
-          const bool skip_lo = p.b2_lo_zero && kb >= nkb1;          // B_lo == 0: the A_hi.B_lo pass adds exact zeros
+          const bool skip_lo = K2B == K2_LO_ZERO && kb >= nkb1;     // B_lo == 0: the A_hi.B_lo pass adds exact zeros
           wgmma_fence();
           if (DIAG && kb >= nkb1) {
             // identity K-block j: only output columns [64 j, 64 j + 64) receive anything -> N = 64 MMAs on that slice of the
@@ -913,9 +918,9 @@ int num_sms() {
   return n;
 }
 
-template <int EPI, int ACV = ACV_NONE, bool HI = false, int BN_ = 256, bool DIAG = false>
+template <int EPI, int ACV = ACV_NONE, bool HI = false, int BN_ = 256, int K2B = K2_FULL>
 cudaError_t launch_variant(int grid, cudaStream_t stream, const Maps& mp, const TcParams& tp) {
-  auto* kern = gemm_tc_kernel<EPI, ACV, HI, BN_, DIAG>;
+  auto* kern = gemm_tc_kernel<EPI, ACV, HI, BN_, K2B>;
   if (cudaError_t e = ensure_smem_limit((const void*)kern, kSmemBytes)) return e;
   return launch_k(kern, dim3(grid), dim3(kThreads), kSmemBytes, stream, mp, tp);
 }
@@ -1001,9 +1006,12 @@ int launch_gemm_tc(const GemmProblem& p, cudaStream_t stream) {
   }
   if (!ok) return -2;
   TcParams tp{};
-  tp.K1 = p.K1; tp.K2 = p.K2; tp.b2_per_seg = p.b2_per_seg; tp.b2_lo_zero = p.b2_lo_zero; tp.n_out = p.n_out;
-  tp.b2_identity = p.b2_identity;
+  tp.K1 = p.K1; tp.K2 = p.K2; tp.b2_per_seg = p.b2_per_seg; tp.n_out = p.n_out;
   if (p.b2_identity && (!p.b2_lo_zero || p.b2_per_seg || p.K2 != p.n_out || p.n_out != BN || p.K1 <= 0 || bn != BN)) return -1;
+  // the K2 block variants exist for the residual GEMMs: mlp.3 (converted A) with the identity as N = 64 MMAs or as a zero-lo
+  // block, any other EPI_BIAS_PLANES GEMM with the identity as N = 64 MMAs
+  if (p.b2_lo_zero && (p.epi != EPI_BIAS_PLANES || !p.K2 || !(p.a_conv || p.b2_identity))) return -1;
+  const int k2b = p.b2_identity ? K2_DIAG : p.b2_lo_zero ? K2_LO_ZERO : K2_FULL;
   tp.m_tiles = p.rows / BM; tp.n_tiles = p.n_out / bn; tp.batch = p.batch;
   tp.taps = p.taps; tp.kb_per_tap = p.kb_per_tap;
   for (int t = 0; t < 9; ++t) tp.tap_off[t] = p.tap_off[t];
@@ -1020,8 +1028,9 @@ int launch_gemm_tc(const GemmProblem& p, cudaStream_t stream) {
   const int grid = total_units < num_sms() ? total_units : num_sms();
   cudaError_t le;
   if (p.a_conv) {
-    le = p.b2_identity ? launch_variant<EPI_BIAS_PLANES, ACV_NORM_RELU, false, 256, true>(grid, stream, mp, tp)
-                       : launch_variant<EPI_BIAS_PLANES, ACV_NORM_RELU>(grid, stream, mp, tp);
+    le = k2b == K2_DIAG      ? launch_variant<EPI_BIAS_PLANES, ACV_NORM_RELU, false, 256, K2_DIAG>(grid, stream, mp, tp)
+         : k2b == K2_LO_ZERO ? launch_variant<EPI_BIAS_PLANES, ACV_NORM_RELU, false, 256, K2_LO_ZERO>(grid, stream, mp, tp)
+                             : launch_variant<EPI_BIAS_PLANES, ACV_NORM_RELU>(grid, stream, mp, tp);
   } else {
     switch (p.epi) {
       case EPI_F32:
@@ -1037,7 +1046,8 @@ int launch_gemm_tc(const GemmProblem& p, cudaStream_t stream) {
       case EPI_SCORE_CONF: le = launch_variant<EPI_SCORE_CONF>(grid, stream, mp, tp); break;
       case EPI_QKV: le = p.a_hi_only ? launch_variant<EPI_QKV, ACV_NONE, true>(grid, stream, mp, tp) : launch_variant<EPI_QKV>(grid, stream, mp, tp); break;
       case EPI_BIAS_PLANES:
-        le = p.b2_identity ? launch_variant<EPI_BIAS_PLANES, ACV_NONE, false, 256, true>(grid, stream, mp, tp) : launch_variant<EPI_BIAS_PLANES>(grid, stream, mp, tp);
+        le = k2b == K2_DIAG ? launch_variant<EPI_BIAS_PLANES, ACV_NONE, false, 256, K2_DIAG>(grid, stream, mp, tp)
+                            : launch_variant<EPI_BIAS_PLANES>(grid, stream, mp, tp);
         break;
       default: return -1;
     }
