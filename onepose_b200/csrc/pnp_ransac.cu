@@ -28,11 +28,46 @@ struct Pose {
   double t[3];
 };
 
+// frame b of a batch: correspondences [o0, o0 + n) of the ragged lists, its intrinsics and its first 2D / 3D point
+struct Frame {
+  int o0, n;
+  double Kc[4];   // fx, fy, cx, cy
+  const double* p2;
+  const double* p3;
+};
+
+__device__ __forceinline__ Frame frame_view(int b, const double* Kmat /*[B][9]*/, const double* pts2d, const double* pts3d, const int* offsets) {
+  const int o0 = offsets[b];
+  const double* K = Kmat + (size_t)b * 9;
+  return {o0, offsets[b + 1] - o0, {K[0], K[4], K[2], K[5]}, pts2d + (size_t)o0 * 2, pts3d + (size_t)o0 * 3};
+}
+
 __device__ __forceinline__ uint64_t mix64(uint64_t z) {   // splitmix64 finaliser
   z += 0x9E3779B97F4A7C15ull;
   z = (z ^ (z >> 30)) * 0xBF58476D1CE4E5B9ull;
   z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
   return z ^ (z >> 31);
+}
+
+// K distinct indices in [0, n) for sample h of frame b: the k-th splitmix64 draw modulo n - k, shifted past the earlier
+// indices in ascending order.  K is a compile-time constant so that the loops unroll and the sorted list stays in registers.
+template <int K>
+__device__ __forceinline__ void sample_distinct(unsigned long long seed, int b, int h, int n, int* idx) {
+  uint64_t r = mix64(seed ^ ((uint64_t)b << 40) ^ (uint64_t)h);
+  int srt[K];
+#pragma unroll
+  for (int k = 0; k < K; ++k) {
+    if (k > 0) r = mix64(r);
+    int v = (int)(r % (uint64_t)(n - k));
+#pragma unroll
+    for (int e = 0; e < k; ++e)
+      if (v >= srt[e]) ++v;
+    idx[k] = v;
+    srt[k] = v;                                          // insert into the sorted list
+#pragma unroll
+    for (int e = k; e > 0; --e)
+      if (srt[e - 1] > srt[e]) { const int t = srt[e]; srt[e] = srt[e - 1]; srt[e - 1] = t; }
+  }
 }
 
 // largest real root of z^3 + a2 z^2 + a1 z + a0
@@ -102,6 +137,11 @@ __device__ __forceinline__ bool normalize3(double* a) {
   if (!(n > 1e-12)) return false;
   a[0] /= n; a[1] /= n; a[2] /= n;
   return true;
+}
+// unit bearing (camera frame) of pixel p2
+__device__ __forceinline__ void bearing(const double* Kc, const double* p2, double* j) {
+  j[0] = (p2[0] - Kc[2]) / Kc[0]; j[1] = (p2[1] - Kc[3]) / Kc[1]; j[2] = 1.0;
+  normalize3(j);
 }
 // orthonormal frame of a triangle: columns e1 = (Q1-Q0)^, e3 = (e1 x (Q2-Q0))^, e2 = e3 x e1; F row-major [3][3] with columns e1,e2,e3
 __device__ bool tri_frame(const double Q[3][3], double F[9]) {
@@ -205,19 +245,46 @@ __device__ int p3p(const double P[3][3], const double j[3][3], Pose* out) {
   return ns;
 }
 
-__device__ __forceinline__ bool reproj_inlier(const Pose& T, const double* Kc /*fx,fy,cx,cy*/, const double* p3, const double* p2, double thr2) {
-  const double x = T.R[0] * p3[0] + T.R[1] * p3[1] + T.R[2] * p3[2] + T.t[0];
-  const double y = T.R[3] * p3[0] + T.R[4] * p3[1] + T.R[5] * p3[2] + T.t[1];
-  const double z = T.R[6] * p3[0] + T.R[7] * p3[1] + T.R[8] * p3[2] + T.t[2];
-  if (!(z > 1e-9)) return false;
-  const double du = Kc[0] * x / z + Kc[2] - p2[0], dv = Kc[1] * y / z + Kc[3] - p2[1];
+// world point p3 in the camera frame of T
+__device__ __forceinline__ void to_camera(const Pose& T, const double* p3, double* X) {
+#pragma unroll
+  for (int r = 0; r < 3; ++r) X[r] = T.R[r * 3] * p3[0] + T.R[r * 3 + 1] * p3[1] + T.R[r * 3 + 2] * p3[2] + T.t[r];
+}
+
+// squared reprojection error of the correspondence p3 -> p2 under T, in fp64
+__device__ __forceinline__ double reproj_err2(const Pose& T, const double* Kc /*fx,fy,cx,cy*/, const double* p3, const double* p2) {
+  double X[3];
+  to_camera(T, p3, X);
+  const double du = Kc[0] * X[0] / X[2] + Kc[2] - p2[0], dv = Kc[1] * X[1] / X[2] + Kc[3] - p2[1];
+  return du * du + dv * dv;
+}
+
+// the P3P path's inlier rule: in front of the camera and squared reprojection error < thr^2.  Not written on reproj_err2:
+// that form costs both P3P kernels registers and spills.
+__device__ __forceinline__ bool reproj_inlier(const Pose& T, const double* Kc, const double* p3, const double* p2, double thr2) {
+  double X[3];
+  to_camera(T, p3, X);
+  if (!(X[2] > 1e-9)) return false;
+  const double du = Kc[0] * X[0] / X[2] + Kc[2] - p2[0], dv = Kc[1] * X[1] / X[2] + Kc[3] - p2[1];
   return du * du + dv * dv < thr2;
 }
 
-// hyp: [B][H] {count, pose(12)} as 13 doubles
+// hyp: [B][H] records {count, R (9), t (3)} as 13 doubles (the workspace layout of include/onepose_b200.h)
 constexpr int kHypStride = 13;
 constexpr int kHypThreads = 128;
 constexpr int kMaxHypotheses = 65535 * kHypThreads;
+
+__device__ __forceinline__ void store_record(double* rec, double count, const Pose& T) {
+  rec[0] = count;
+  for (int k = 0; k < 9; ++k) rec[1 + k] = T.R[k];
+  for (int k = 0; k < 3; ++k) rec[10 + k] = T.t[k];
+}
+__device__ __forceinline__ Pose load_record(const double* rec) {   // the record's pose; its count is rec[0]
+  Pose T;
+  for (int k = 0; k < 9; ++k) T.R[k] = rec[1 + k];
+  for (int k = 0; k < 3; ++k) T.t[k] = rec[10 + k];
+  return T;
+}
 
 __global__ void __launch_bounds__(kHypThreads, 4) pnp_hypotheses(const double* __restrict__ Kmat /*[B][9]*/, const double* __restrict__ pts2d, const double* __restrict__ pts3d,
                                                       const int* __restrict__ offsets, int H, double thr2, unsigned long long seed,
@@ -225,42 +292,29 @@ __global__ void __launch_bounds__(kHypThreads, 4) pnp_hypotheses(const double* _
   const int b = blockIdx.x;                          // frames on x: any B; hypothesis blocks on y (at most 65535)
   const int h = blockIdx.y * blockDim.x + threadIdx.x;
   if (h >= H) return;
-  const int o0 = offsets[b], n = offsets[b + 1] - o0;
+  const Frame f = frame_view(b, Kmat, pts2d, pts3d, offsets);
   double* out = hyp + ((size_t)b * H + h) * kHypStride;
   out[0] = 0.0;
-  if (n < 4) return;
-  const double* K = Kmat + (size_t)b * 9;
-  const double Kc[4] = {K[0], K[4], K[2], K[5]};
-  // three distinct correspondences
-  uint64_t r = mix64(seed ^ ((uint64_t)b << 40) ^ (uint64_t)h);
+  if (f.n < 4) return;
   int idx[3];
-  idx[0] = (int)(r % (uint64_t)n);
-  r = mix64(r);
-  idx[1] = (int)(r % (uint64_t)(n - 1));
-  if (idx[1] >= idx[0]) ++idx[1];
-  r = mix64(r);
-  idx[2] = (int)(r % (uint64_t)(n - 2));
-  { const int lo = min(idx[0], idx[1]), hi = max(idx[0], idx[1]); if (idx[2] >= lo) ++idx[2]; if (idx[2] >= hi) ++idx[2]; }
+  sample_distinct<3>(seed, b, h, f.n, idx);
   double P[3][3], j[3][3];
   for (int k = 0; k < 3; ++k) {
-    const double* p3 = pts3d + (size_t)(o0 + idx[k]) * 3;
-    const double* p2 = pts2d + (size_t)(o0 + idx[k]) * 2;
+    const double* p3 = f.p3 + (size_t)idx[k] * 3;
     P[k][0] = p3[0]; P[k][1] = p3[1]; P[k][2] = p3[2];
-    j[k][0] = (p2[0] - Kc[2]) / Kc[0]; j[k][1] = (p2[1] - Kc[3]) / Kc[1]; j[k][2] = 1.0;
-    normalize3(j[k]);
+    bearing(f.Kc, f.p2 + (size_t)idx[k] * 2, j[k]);
   }
   Pose sol[4];
   const int ns = p3p(P, j, sol);
   int best = -1, best_cnt = 0;
   for (int s = 0; s < ns; ++s) {
     int cnt = 0;
-    for (int i = 0; i < n; ++i) cnt += reproj_inlier(sol[s], Kc, pts3d + (size_t)(o0 + i) * 3, pts2d + (size_t)(o0 + i) * 2, thr2) ? 1 : 0;
+    // indexed from the batch's arrays: from the frame's base pointers this loop runs about 1 % slower on an H100
+    for (int i = 0; i < f.n; ++i) cnt += reproj_inlier(sol[s], f.Kc, pts3d + (size_t)(f.o0 + i) * 3, pts2d + (size_t)(f.o0 + i) * 2, thr2) ? 1 : 0;
     if (cnt > best_cnt) { best_cnt = cnt; best = s; }
   }
   if (best < 0) return;
-  out[0] = (double)best_cnt;
-  for (int k = 0; k < 9; ++k) out[1 + k] = sol[best].R[k];
-  for (int k = 0; k < 3; ++k) out[10 + k] = sol[best].t[k];
+  store_record(out, (double)best_cnt, sol[best]);
 }
 
 __device__ void rodrigues_left(const double* w, Pose& T) {   // T <- exp([w]x) . T (rotation and translation), small-angle safe
@@ -305,6 +359,35 @@ __device__ int best_hypothesis(const double* __restrict__ hyp, int b, int H, uns
   return (int)(bk >> 32);
 }
 
+// block-wide sum of one int per thread, returned to every thread
+template <int kThreads>
+__device__ __forceinline__ int block_count(int c, int* red /*shared [kThreads / 32]*/) {
+  for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = c;
+  __syncthreads();
+  int s = 0;
+  for (int w = 0; w < kThreads / 32; ++w) s += red[w];
+  return s;
+}
+
+__device__ __forceinline__ void write_pose(const Pose& T, double* dst) {
+  for (int r = 0; r < 3; ++r) {
+    for (int k = 0; k < 3; ++k) dst[r * 4 + k] = T.R[r * 3 + k];
+    dst[r * 4 + 3] = T.t[r];
+  }
+}
+__device__ __forceinline__ void write_identity(double* dst) {
+  for (int k = 0; k < 12; ++k) dst[k] = (k == 0 || k == 5 || k == 10) ? 1.0 : 0.0;
+}
+// a frame without a model, by its whole block: identity pose, no inliers (the reference's except-branch result)
+__device__ __forceinline__ void write_no_model(int b, const Frame& f, double* pose_out, int* inlier_mask, int* n_inliers) {
+  for (int i = threadIdx.x; i < f.n; i += kRefineThreads) inlier_mask[f.o0 + i] = 0;
+  if (threadIdx.x == 0) {
+    write_identity(pose_out + (size_t)b * 12);
+    n_inliers[b] = 0;
+  }
+}
+
 // one block per frame: arg-max over hypotheses, local optimisation, outputs
 __global__ void __launch_bounds__(kRefineThreads) pnp_select_refine(const double* __restrict__ Kmat, const double* __restrict__ pts2d, const double* __restrict__ pts3d,
                                                                      const int* __restrict__ offsets, int H, double thr2, const double* __restrict__ hyp,
@@ -312,44 +395,33 @@ __global__ void __launch_bounds__(kRefineThreads) pnp_select_refine(const double
                                                                      int* __restrict__ n_inliers /*[B]*/) {
   __shared__ unsigned long long best_key[kRefineThreads];
   __shared__ double red[27][kRefineThreads / 32];
+  __shared__ int cnt_w[kRefineThreads / 32];
   __shared__ Pose T;
   __shared__ double delta[6];
-  __shared__ int ok;
   const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const int o0 = offsets[b], n = offsets[b + 1] - o0;
-  const double* K = Kmat + (size_t)b * 9;
-  const double Kc[4] = {K[0], K[4], K[2], K[5]};
+  const Frame f = frame_view(b, Kmat, pts2d, pts3d, offsets);
   // ---- best hypothesis: max count, lowest index
   int best_h;
-  const int best_cnt = best_hypothesis(hyp, b, H, best_key, &best_h);
-  if (tid == 0) {
-    ok = best_cnt >= 4 ? 1 : 0;
-    if (ok) {
-      const double* src = hyp + ((size_t)b * H + best_h) * kHypStride;
-      for (int k = 0; k < 9; ++k) T.R[k] = src[1 + k];
-      for (int k = 0; k < 3; ++k) T.t[k] = src[10 + k];
-    }
-  }
-  __syncthreads();
-  if (!ok) {                                       // no model: identity pose, no inliers (the reference's except-branch result)
-    if (tid < 12) pose_out[(size_t)b * 12 + tid] = (tid == 0 || tid == 5 || tid == 10) ? 1.0 : 0.0;
-    for (int i = tid; i < n; i += kRefineThreads) inlier_mask[o0 + i] = 0;
-    if (tid == 0) n_inliers[b] = 0;
+  if (best_hypothesis(hyp, b, H, best_key, &best_h) < 4) {
+    write_no_model(b, f, pose_out, inlier_mask, n_inliers);
     return;
   }
+  if (tid == 0) T = load_record(hyp + ((size_t)b * H + best_h) * kHypStride);
+  __syncthreads();
   // ---- Gauss-Newton on the inliers of the current pose; the inlier set is re-evaluated every round
   for (int it = 0; it < 10; ++it) {
     double acc[27];
 #pragma unroll
     for (int k = 0; k < 27; ++k) acc[k] = 0.0;
     const Pose Tl = T;
-    for (int i = tid; i < n; i += kRefineThreads) {
-      const double* p3 = pts3d + (size_t)(o0 + i) * 3;
-      const double* p2 = pts2d + (size_t)(o0 + i) * 2;
-      if (!reproj_inlier(Tl, Kc, p3, p2, thr2)) continue;
-      const double x = Tl.R[0] * p3[0] + Tl.R[1] * p3[1] + Tl.R[2] * p3[2] + Tl.t[0];
-      const double y = Tl.R[3] * p3[0] + Tl.R[4] * p3[1] + Tl.R[5] * p3[2] + Tl.t[1];
-      const double z = Tl.R[6] * p3[0] + Tl.R[7] * p3[1] + Tl.R[8] * p3[2] + Tl.t[2];
+    for (int i = tid; i < f.n; i += kRefineThreads) {
+      const double* p3 = f.p3 + (size_t)i * 3;
+      const double* p2 = f.p2 + (size_t)i * 2;
+      if (!reproj_inlier(Tl, f.Kc, p3, p2, thr2)) continue;
+      double X[3];
+      to_camera(Tl, p3, X);
+      const double x = X[0], y = X[1], z = X[2];
+      const double* Kc = f.Kc;
       const double iz = 1.0 / z;
       const double ru = Kc[0] * x * iz + Kc[2] - p2[0], rv = Kc[1] * y * iz + Kc[3] - p2[1];
       // d(proj)/dX, X' = exp(w) X + dt  =>  dX/dw = -[X]x, dX/dt = I
@@ -367,6 +439,7 @@ __global__ void __launch_bounds__(kRefineThreads) pnp_select_refine(const double
 #pragma unroll
       for (int r = 0; r < 6; ++r) acc[21 + r] += Ju[r] * ru + Jv[r] * rv;
     }
+    // block_sum<27> gives the same sums in the same order, but costs this kernel two registers: thread 0 sums here
 #pragma unroll
     for (int k = 0; k < 27; ++k) {
       double v = acc[k];
@@ -415,23 +488,15 @@ __global__ void __launch_bounds__(kRefineThreads) pnp_select_refine(const double
   }
   // ---- outputs
   int cnt = 0;
-  for (int i = tid; i < n; i += kRefineThreads) {
-    const int in = reproj_inlier(T, Kc, pts3d + (size_t)(o0 + i) * 3, pts2d + (size_t)(o0 + i) * 2, thr2) ? 1 : 0;
-    inlier_mask[o0 + i] = in;
+  for (int i = tid; i < f.n; i += kRefineThreads) {
+    const int in = reproj_inlier(T, f.Kc, f.p3 + (size_t)i * 3, f.p2 + (size_t)i * 2, thr2) ? 1 : 0;
+    inlier_mask[f.o0 + i] = in;
     cnt += in;
   }
-  for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-  __shared__ int cnt_w[kRefineThreads / 32];
-  if (lane == 0) cnt_w[warp] = cnt;
-  __syncthreads();
+  cnt = block_count<kRefineThreads>(cnt, cnt_w);
   if (tid == 0) {
-    int c = 0;
-    for (int w = 0; w < kRefineThreads / 32; ++w) c += cnt_w[w];
-    n_inliers[b] = c;
-    for (int r = 0; r < 3; ++r) {
-      for (int k = 0; k < 3; ++k) pose_out[(size_t)b * 12 + r * 4 + k] = T.R[r * 3 + k];
-      pose_out[(size_t)b * 12 + r * 4 + 3] = T.t[r];
-    }
+    n_inliers[b] = cnt;
+    write_pose(T, pose_out + (size_t)b * 12);
   }
 }
 
@@ -732,12 +797,9 @@ __device__ void epnp_candidates(const double* sums, const EpnpBasis& E, int m, P
   }
 }
 
+// the reprojection distance that picks an EPnP candidate
 __device__ __forceinline__ double reproj_dist(const Pose& T, const double* Kc, const double* p3, const double* p2) {
-  const double x = T.R[0] * p3[0] + T.R[1] * p3[1] + T.R[2] * p3[2] + T.t[0];
-  const double y = T.R[3] * p3[0] + T.R[4] * p3[1] + T.R[5] * p3[2] + T.t[1];
-  const double z = T.R[6] * p3[0] + T.R[7] * p3[1] + T.R[8] * p3[2] + T.t[2];
-  const double du = Kc[0] * x / z + Kc[2] - p2[0], dv = Kc[1] * y / z + Kc[3] - p2[1];
-  return sqrt(du * du + dv * dv);
+  return sqrt(reproj_err2(T, Kc, p3, p2));
 }
 
 // the lowest error sum (mean x m), the first on ties; a non-finite error never wins
@@ -758,11 +820,7 @@ __device__ __forceinline__ bool pose_finite(const Pose& T) {
 
 // OpenCV's RANSAC inlier rule: squared reprojection error <= thr^2, no depth test
 __device__ __forceinline__ bool epnp_inlier(const Pose& T, const double* Kc, const double* p3, const double* p2, double thr2) {
-  const double x = T.R[0] * p3[0] + T.R[1] * p3[1] + T.R[2] * p3[2] + T.t[0];
-  const double y = T.R[3] * p3[0] + T.R[4] * p3[1] + T.R[5] * p3[2] + T.t[1];
-  const double z = T.R[6] * p3[0] + T.R[7] * p3[1] + T.R[8] * p3[2] + T.t[2];
-  const double du = Kc[0] * x / z + Kc[2] - p2[0], dv = Kc[1] * y / z + Kc[3] - p2[1];
-  return du * du + dv * dv <= thr2;
+  return reproj_err2(T, Kc, p3, p2) <= thr2;
 }
 
 // correspondence i of a frame, rounded to fp32 first when kRound (as OpenCV's solvePnPRansac converts its inputs)
@@ -772,16 +830,19 @@ __device__ __forceinline__ void load_pair(const double* pts2d, const double* pts
   for (int d = 0; d < 3; ++d) p3[d] = kRound ? (double)(float)pts3d[i * 3 + d] : pts3d[i * 3 + d];
 }
 
+// point p's contribution to the scatter sc[6] = {xx, xy, xz, yy, yz, zz} about c0
+__device__ __forceinline__ void add_scatter(const double* p, const double* c0, double* sc) {
+  const double d[3] = {p[0] - c0[0], p[1] - c0[1], p[2] - c0[2]};
+  sc[0] += d[0] * d[0]; sc[1] += d[0] * d[1]; sc[2] += d[0] * d[2]; sc[3] += d[1] * d[1]; sc[4] += d[1] * d[2]; sc[5] += d[2] * d[2];
+}
+
 // EPnP of m <= 5 points by one thread (the RANSAC hypotheses)
 __device__ bool epnp_points(const double (*P)[3], const double (*uv)[2], int m, const double* Kc, Pose& out) {
   double sum[3] = {0, 0, 0}, sc[6] = {0, 0, 0, 0, 0, 0};
   for (int i = 0; i < m; ++i)
     for (int d = 0; d < 3; ++d) sum[d] += P[i][d];
   const double c0[3] = {sum[0] / m, sum[1] / m, sum[2] / m};
-  for (int i = 0; i < m; ++i) {
-    const double d[3] = {P[i][0] - c0[0], P[i][1] - c0[1], P[i][2] - c0[2]};
-    sc[0] += d[0] * d[0]; sc[1] += d[0] * d[1]; sc[2] += d[0] * d[2]; sc[3] += d[1] * d[1]; sc[4] += d[1] * d[2]; sc[5] += d[2] * d[2];
-  }
+  for (int i = 0; i < m; ++i) add_scatter(P[i], c0, sc);
   EpnpBasis E;
   if (!epnp_basis(sum, sc, m, E)) return false;
   double acc[kEpnpSums];
@@ -850,8 +911,7 @@ __device__ int epnp_block(const double* pts2d, const double* pts3d, int n, const
     if (!use(i)) continue;
     double p2[2], p3[3];
     load_pair<kRound>(pts2d, pts3d, i, p2, p3);
-    const double d[3] = {p3[0] - c0[0], p3[1] - c0[1], p3[2] - c0[2]};
-    sc[0] += d[0] * d[0]; sc[1] += d[0] * d[1]; sc[2] += d[0] * d[2]; sc[3] += d[1] * d[1]; sc[4] += d[1] * d[2]; sc[5] += d[2] * d[2];
+    add_scatter(p3, c0, sc);
   }
   block_sum<6>(sc, sh.red, sh.sums);
   if (tid == 0) sh.ok = epnp_basis(sum, sh.sums, m, sh.E) ? 1 : 0;
@@ -883,14 +943,22 @@ __device__ int epnp_block(const double* pts2d, const double* pts3d, int n, const
   return m;
 }
 
-__device__ __forceinline__ void write_pose(const Pose& T, double* dst) {
-  for (int r = 0; r < 3; ++r) {
-    for (int k = 0; k < 3; ++k) dst[r * 4 + k] = T.R[r * 3 + k];
-    dst[r * 4 + 3] = T.t[r];
+// the end of both EPnP selectors: the winner's pose W, its inlier set (inlier(p3, p2) on the fp32-rounded pairs) as the mask,
+// EPnP on that set; a degenerate set keeps W.  count: the mask's count, which the winner's own count is (the same test).
+template <class Inlier>
+__device__ __forceinline__ void refit_tail(int b, const Frame& f, const Pose& W, Inlier inlier, int count, EpnpShared& sh, Pose* T,
+                                           double* pose_out, int* inlier_mask, int* n_inliers) {
+  auto use = [&](int i) {
+    double p2[2], p3[3];
+    load_pair<true>(f.p2, f.p3, i, p2, p3);
+    return inlier(p3, p2);
+  };
+  for (int i = threadIdx.x; i < f.n; i += kEpnpThreads) inlier_mask[f.o0 + i] = use(i) ? 1 : 0;
+  const int m = epnp_block<true>(f.p2, f.p3, f.n, f.Kc, use, sh, T);
+  if (threadIdx.x == 0) {
+    write_pose(m >= 4 && pose_finite(*T) ? *T : W, pose_out + (size_t)b * 12);
+    n_inliers[b] = count;
   }
-}
-__device__ __forceinline__ void write_identity(double* dst) {
-  for (int k = 0; k < 12; ++k) dst[k] = (k == 0 || k == 5 || k == 10) ? 1.0 : 0.0;
 }
 
 // one block per frame: EPnP on all of its correspondences (cv2.solvePnP(..., flags=SOLVEPNP_EPNP) for B frames)
@@ -899,10 +967,8 @@ __global__ void __launch_bounds__(kEpnpThreads) epnp_frames(const double* __rest
   __shared__ EpnpShared sh;
   __shared__ Pose T;
   const int b = blockIdx.x;
-  const int o0 = offsets[b], n = offsets[b + 1] - o0;
-  const double* K = Kmat + (size_t)b * 9;
-  const double Kc[4] = {K[0], K[4], K[2], K[5]};
-  const int m = n >= 4 ? epnp_block<false>(pts2d + (size_t)o0 * 2, pts3d + (size_t)o0 * 3, n, Kc, [](int) { return true; }, sh, &T) : 0;
+  const Frame f = frame_view(b, Kmat, pts2d, pts3d, offsets);
+  const int m = f.n >= 4 ? epnp_block<false>(f.p2, f.p3, f.n, f.Kc, [](int) { return true; }, sh, &T) : 0;
   if (threadIdx.x == 0) {
     const bool ok = m >= 4 && pose_finite(T);
     if (ok) write_pose(T, pose_out + (size_t)b * 12);
@@ -915,10 +981,7 @@ __global__ void __launch_bounds__(kEpnpThreads) epnp_frames(const double* __rest
 __device__ __forceinline__ bool four_pair_model(const double* f2, const double* f3, const double* Kc, Pose& T) {
   double P[4][3], uv[4][2], j[3][3];
   for (int k = 0; k < 4; ++k) load_pair<true>(f2, f3, k, uv[k], P[k]);
-  for (int k = 0; k < 3; ++k) {
-    j[k][0] = (uv[k][0] - Kc[2]) / Kc[0]; j[k][1] = (uv[k][1] - Kc[3]) / Kc[1]; j[k][2] = 1.0;
-    normalize3(j[k]);
-  }
+  for (int k = 0; k < 3; ++k) bearing(Kc, uv[k], j[k]);
   Pose sol[4];
   const int ns = p3p(P, j, sol);
   double be = INFINITY;
@@ -938,48 +1001,30 @@ __global__ void __launch_bounds__(kHypThreads) epnp_hypotheses(const double* __r
   const int b = blockIdx.x;
   const int h = blockIdx.y * blockDim.x + threadIdx.x;
   if (h >= H) return;
-  const int o0 = offsets[b], n = offsets[b + 1] - o0;
+  const Frame f = frame_view(b, Kmat, pts2d, pts3d, offsets);
   double* out = hyp + ((size_t)b * H + h) * kHypStride;
   out[0] = 0.0;
-  if (n < 4) return;
-  const double* K = Kmat + (size_t)b * 9;
-  const double Kc[4] = {K[0], K[4], K[2], K[5]};
-  const double* f2 = pts2d + (size_t)o0 * 2;
-  const double* f3 = pts3d + (size_t)o0 * 3;
+  if (f.n < 4) return;
   Pose T;
   bool ok = false;
-  if (n == 4) {
-    ok = four_pair_model(f2, f3, Kc, T);
+  if (f.n == 4) {
+    ok = four_pair_model(f.p2, f.p3, f.Kc, T);
   } else {
-    // five distinct indices: the k-th draw modulo n - k, shifted past the earlier indices in ascending order
-    uint64_t r = mix64(seed ^ ((uint64_t)b << 40) ^ (uint64_t)h);
-    int idx[5], srt[5];
-    idx[0] = srt[0] = (int)(r % (uint64_t)n);
-    for (int k = 1; k < 5; ++k) {
-      r = mix64(r);
-      int v = (int)(r % (uint64_t)(n - k));
-      for (int e = 0; e < k; ++e)
-        if (v >= srt[e]) ++v;
-      idx[k] = v;
-      int e = k;                                         // insert into the sorted list
-      for (; e > 0 && srt[e - 1] > v; --e) srt[e] = srt[e - 1];
-      srt[e] = v;
-    }
+    int idx[5];
+    sample_distinct<5>(seed, b, h, f.n, idx);
     double P[5][3], uv[5][2];
-    for (int k = 0; k < 5; ++k) load_pair<true>(f2, f3, idx[k], uv[k], P[k]);
-    ok = epnp_points(P, uv, 5, Kc, T);
+    for (int k = 0; k < 5; ++k) load_pair<true>(f.p2, f.p3, idx[k], uv[k], P[k]);
+    ok = epnp_points(P, uv, 5, f.Kc, T);
   }
   if (!ok || !pose_finite(T)) return;
   int cnt = 0;
-  for (int i = 0; i < n; ++i) {
+  for (int i = 0; i < f.n; ++i) {
     double p2[2], p3[3];
-    load_pair<true>(f2, f3, i, p2, p3);
-    cnt += epnp_inlier(T, Kc, p3, p2, thr2) ? 1 : 0;
+    load_pair<true>(f.p2, f.p3, i, p2, p3);
+    cnt += epnp_inlier(T, f.Kc, p3, p2, thr2) ? 1 : 0;
   }
   if (cnt == 0) return;
-  out[0] = (double)cnt;
-  for (int k = 0; k < 9; ++k) out[1 + k] = T.R[k];
-  for (int k = 0; k < 3; ++k) out[10 + k] = T.t[k];
+  store_record(out, (double)cnt, T);
 }
 
 // one block per frame: the best hypothesis, its inlier set (the reported mask), EPnP on that set
@@ -989,39 +1034,19 @@ __global__ void __launch_bounds__(kEpnpThreads) epnp_select_refit(const double* 
   __shared__ unsigned long long best_key[kRefineThreads];
   __shared__ EpnpShared sh;
   __shared__ Pose W, T;
-  const int b = blockIdx.x, tid = threadIdx.x;
-  const int o0 = offsets[b], n = offsets[b + 1] - o0;
-  const double* K = Kmat + (size_t)b * 9;
-  const double Kc[4] = {K[0], K[4], K[2], K[5]};
-  const double* f2 = pts2d + (size_t)o0 * 2;
-  const double* f3 = pts3d + (size_t)o0 * 3;
+  const int b = blockIdx.x;
+  const Frame f = frame_view(b, Kmat, pts2d, pts3d, offsets);
   int best_h;
   const int best_cnt = best_hypothesis(hyp, b, H, best_key, &best_h);
-  if (best_cnt >= 4) {
-    if (tid == 0) {
-      const double* src = hyp + ((size_t)b * H + best_h) * kHypStride;
-      for (int k = 0; k < 9; ++k) W.R[k] = src[1 + k];
-      for (int k = 0; k < 3; ++k) W.t[k] = src[10 + k];
-    }
-    __syncthreads();
-    const Pose Wl = W;
-    auto use = [&](int i) {
-      double p2[2], p3[3];
-      load_pair<true>(f2, f3, i, p2, p3);
-      return epnp_inlier(Wl, Kc, p3, p2, thr2);
-    };
-    for (int i = tid; i < n; i += kEpnpThreads) inlier_mask[o0 + i] = use(i) ? 1 : 0;
-    const int m = epnp_block<true>(pts2d + (size_t)o0 * 2, pts3d + (size_t)o0 * 3, n, Kc, use, sh, &T);
-    if (tid == 0) {                                    // a degenerate inlier set keeps the hypothesis's pose
-      write_pose(m >= 4 && pose_finite(T) ? T : W, pose_out + (size_t)b * 12);
-      n_inliers[b] = best_cnt;                         // the mask's count: the same test as the hypothesis's
-    }
+  if (best_cnt < 4) {
+    write_no_model(b, f, pose_out, inlier_mask, n_inliers);
     return;
   }
-  // no model: identity pose, no inliers
-  if (tid < 12) pose_out[(size_t)b * 12 + tid] = (tid == 0 || tid == 5 || tid == 10) ? 1.0 : 0.0;
-  for (int i = tid; i < n; i += kEpnpThreads) inlier_mask[o0 + i] = 0;
-  if (tid == 0) n_inliers[b] = 0;
+  if (threadIdx.x == 0) W = load_record(hyp + ((size_t)b * H + best_h) * kHypStride);
+  __syncthreads();
+  const Pose Wl = W;
+  refit_tail(b, f, W, [&](const double* p3, const double* p2) { return epnp_inlier(Wl, f.Kc, p3, p2, thr2); }, best_cnt, sh, &T, pose_out,
+             inlier_mask, n_inliers);
 }
 
 // ---- EPnP-RANSAC as OpenCV runs it (RANSACPointSetRegistrator::run, calib3d/src/ptsetreg.cpp): OpenCV's sample sequence,
@@ -1036,7 +1061,7 @@ constexpr int kCvModelPoints = 5;
 constexpr int kCvScanThreads = 32;
 
 struct CvState {                                       // per frame, 16 doubles at the end of the workspace
-  double pose[12];                                     // the winning sample's R (9) and t (3)
+  Pose pose;                                           // the winning sample's R (9) and t (3)
   unsigned long long rng;                              // cv::RNG state after the samples drawn so far
   int niters;                                          // the loop's budget (only ever lowered)
   int iter;                                            // the iter at which the loop exited, once done
@@ -1056,11 +1081,8 @@ __device__ __forceinline__ unsigned mwc_next(unsigned long long& s) {   // cv::R
 __device__ __forceinline__ unsigned fast_mod(unsigned x, unsigned long long m, unsigned n) { return (unsigned)__umul64hi(m * x, n); }
 __host__ __device__ __forceinline__ unsigned long long fast_mod_m(unsigned n) { return ~0ull / n + 1; }
 
-// getSubset with the default checkSubset: five indices uniform(0, n), an index repeating an earlier one of the sample redrawn.
-// Five distinct draws in a row (the common case for large n) take one branch-free pass.
-__device__ __forceinline__ void cv_subset(unsigned long long& s, unsigned n, unsigned long long m, int* idx) {
-  unsigned long long t = s;
-  int v[kCvModelPoints];
+// five draws uniform(0, n) from state t (advanced) into v; true when they are distinct
+__device__ __forceinline__ bool draw5(unsigned long long& t, unsigned long long m, unsigned n, int* v) {
 #pragma unroll
   for (int k = 0; k < kCvModelPoints; ++k) v[k] = (int)fast_mod(mwc_next(t), m, n);
   bool distinct = true;
@@ -1068,7 +1090,15 @@ __device__ __forceinline__ void cv_subset(unsigned long long& s, unsigned n, uns
   for (int a = 0; a < kCvModelPoints; ++a)
 #pragma unroll
     for (int c = a + 1; c < kCvModelPoints; ++c) distinct &= v[a] != v[c];
-  if (distinct) {
+  return distinct;
+}
+
+// getSubset with the default checkSubset: five indices uniform(0, n), an index repeating an earlier one of the sample redrawn.
+// Five distinct draws in a row (the common case for large n) take one branch-free pass.
+__device__ __forceinline__ void cv_subset(unsigned long long& s, unsigned n, unsigned long long m, int* idx) {
+  unsigned long long t = s;
+  int v[kCvModelPoints];
+  if (draw5(t, m, n, v)) {
     s = t;
 #pragma unroll
     for (int k = 0; k < kCvModelPoints; ++k) idx[k] = v[k];
@@ -1150,13 +1180,7 @@ __device__ void warp_draw(unsigned long long& s, bool fresh, unsigned n, int cou
     const unsigned long long start = mwc_mulmod(s, jump);
     unsigned long long t = start;
     int v[kCvModelPoints];
-#pragma unroll
-    for (int k = 0; k < kCvModelPoints; ++k) v[k] = (int)fast_mod(mwc_next(t), m, n);
-    bool distinct = true;
-#pragma unroll
-    for (int a = 0; a < kCvModelPoints; ++a)
-#pragma unroll
-      for (int c = a + 1; c < kCvModelPoints; ++c) distinct &= v[a] != v[c];
+    const bool distinct = draw5(t, m, n, v);
     const int avail = min(32, count - h);
     const unsigned bad = __ballot_sync(0xffffffffu, lane < avail && !distinct);
     const int k = bad ? __ffs(bad) - 1 : avail;
@@ -1175,9 +1199,10 @@ __device__ void warp_draw(unsigned long long& s, bool fresh, unsigned n, int cou
   }
 }
 
-// samples first .. first + W - 1 of frame b, those below its budget, into the wave's records (one warp)
-__device__ void draw_wave(CvState& S, double* r, int n, int W, int first, int b, int* trace_samples, int trace_cap) {
-  const int count = min(W, S.niters - first);
+// samples first .. first + W - 1 of frame b, those below its budget niters, into the wave's records (one warp).  Every lane
+// passes its own copy of the budget: lane 0's store to S.niters need not be what the other lanes read back.
+__device__ void draw_wave(CvState& S, double* r, int n, int W, int first, int niters, int b, int* trace_samples, int trace_cap) {
+  const int count = min(W, niters - first);
   unsigned long long s = S.rng;
   if (count > 0)
     warp_draw(s, first == 0, (unsigned)n, count, reinterpret_cast<int*>(r), kHypStride * 2, trace_samples + (trace_samples ? (size_t)b * trace_cap * kCvModelPoints : 0),
@@ -1213,7 +1238,7 @@ __global__ void __launch_bounds__(kCvScanThreads) epnp_cv_scan(const int* __rest
         if (ce > max(best, kCvModelPoints - 1)) {      // strict: the earliest sample wins a tie
           best = ce;
           winner = i;
-          if (lane < 12) S.pose[lane] = r[(size_t)(h0 + e) * kHypStride + 1 + lane];
+          if (lane == 0) S.pose = load_record(r + (size_t)(h0 + e) * kHypStride);
           niters = cv_update_num_iters(confidence, (double)(n - ce) / n, kCvModelPoints, niters);
         }
         if (i + 1 >= niters) { done = 1; iter = i + 1; break; }
@@ -1229,7 +1254,7 @@ __global__ void __launch_bounds__(kCvScanThreads) epnp_cv_scan(const int* __rest
     }
     if (done) return;
     __syncwarp();
-    draw_wave(S, r, n, W, base + W, b, trace_samples, trace_cap);
+    draw_wave(S, r, n, W, base + W, niters, b, trace_samples, trace_cap);
     return;
   }
   if (wave < 0) {
@@ -1247,7 +1272,7 @@ __global__ void __launch_bounds__(kCvScanThreads) epnp_cv_scan(const int* __rest
     }
     if (n <= kCvModelPoints) return;
     __syncwarp();                                      // lane 0's state is visible to the warp
-    draw_wave(S, r, n, W, 0, b, trace_samples, trace_cap);
+    draw_wave(S, r, n, W, 0, H, b, trace_samples, trace_cap);
     return;
   }
   if (lane != 0 || S.done) return;                     // wave >= 0, 4 or 5 pairs: take the one model
@@ -1255,7 +1280,7 @@ __global__ void __launch_bounds__(kCvScanThreads) epnp_cv_scan(const int* __rest
   if (c >= 0) {
     S.winner = 0;
     S.best = n;
-    for (int k = 0; k < 12; ++k) S.pose[k] = r[1 + k];
+    S.pose = load_record(r);
   }
   S.done = 1;
 }
@@ -1271,34 +1296,28 @@ __global__ void __launch_bounds__(kHypThreads) epnp_cv_wave(const double* __rest
   const CvState& S = st[b];
   const int i = wave * W + h;
   if (S.done || i >= S.niters) return;
-  const int o0 = offsets[b], n = offsets[b + 1] - o0;
-  const double* K = Kmat + (size_t)b * 9;
-  const double Kc[4] = {K[0], K[4], K[2], K[5]};
-  const double* f2 = pts2d + (size_t)o0 * 2;
-  const double* f3 = pts3d + (size_t)o0 * 3;
+  const Frame f = frame_view(b, Kmat, pts2d, pts3d, offsets);
   double* out = rec + ((size_t)b * W + h) * kHypStride;
   Pose T;
   bool ok;
-  if (n == 4) {
-    ok = four_pair_model(f2, f3, Kc, T);
+  if (f.n == 4) {
+    ok = four_pair_model(f.p2, f.p3, f.Kc, T);
   } else {
     const int* si = reinterpret_cast<const int*>(out);
     double P[5][3], uv[5][2];
-    for (int k = 0; k < 5; ++k) load_pair<true>(f2, f3, si[k], uv[k], P[k]);
-    ok = epnp_points(P, uv, 5, Kc, T);
+    for (int k = 0; k < 5; ++k) load_pair<true>(f.p2, f.p3, si[k], uv[k], P[k]);
+    ok = epnp_points(P, uv, 5, f.Kc, T);
   }
   int cnt = -1;
   if (ok && pose_finite(T)) {
     cnt = 0;
-    for (int j = 0; j < n; ++j) {
+    for (int j = 0; j < f.n; ++j) {
       double p2[2], p3[3];
-      load_pair<true>(f2, f3, j, p2, p3);
-      cnt += cv_error(T, Kc, p3, p2) <= thr2f ? 1 : 0;
+      load_pair<true>(f.p2, f.p3, j, p2, p3);
+      cnt += cv_error(T, f.Kc, p3, p2) <= thr2f ? 1 : 0;
     }
   }
-  out[0] = (double)cnt;
-  for (int k = 0; k < 9; ++k) out[1 + k] = T.R[k];
-  for (int k = 0; k < 3; ++k) out[10 + k] = T.t[k];
+  store_record(out, (double)cnt, T);
   if (trace_counts && i < trace_cap) trace_counts[(size_t)b * trace_cap + i] = cnt;
 }
 
@@ -1311,45 +1330,28 @@ __global__ void __launch_bounds__(kEpnpThreads) epnp_cv_select_refit(const doubl
   __shared__ EpnpShared sh;
   __shared__ Pose T;
   const int b = blockIdx.x, tid = threadIdx.x;
-  const int o0 = offsets[b], n = offsets[b + 1] - o0;
+  const Frame f = frame_view(b, Kmat, pts2d, pts3d, offsets);
   const CvState& S = st[b];
   const int winner = S.winner;
   if (tid == 0) {
     iterations[b] = S.iter;
     if (trace_winner) trace_winner[b] = winner;
   }
-  if (winner < 0) {                                    // no model: identity pose, no inliers (run() returns false)
-    if (tid < 12) pose_out[(size_t)b * 12 + tid] = (tid == 0 || tid == 5 || tid == 10) ? 1.0 : 0.0;
-    for (int i = tid; i < n; i += kEpnpThreads) inlier_mask[o0 + i] = 0;
-    if (tid == 0) n_inliers[b] = 0;
+  if (winner < 0) {                                    // run() returns false
+    write_no_model(b, f, pose_out, inlier_mask, n_inliers);
     return;
   }
-  const double* K = Kmat + (size_t)b * 9;
-  const double Kc[4] = {K[0], K[4], K[2], K[5]};
-  const double* f2 = pts2d + (size_t)o0 * 2;
-  const double* f3 = pts3d + (size_t)o0 * 3;
-  Pose Wl;
-  for (int k = 0; k < 9; ++k) Wl.R[k] = S.pose[k];
-  for (int k = 0; k < 3; ++k) Wl.t[k] = S.pose[9 + k];
-  if (n <= kCvModelPoints) {
-    for (int i = tid; i < n; i += kEpnpThreads) inlier_mask[o0 + i] = 1;
+  const Pose Wl = S.pose;
+  if (f.n <= kCvModelPoints) {
+    for (int i = tid; i < f.n; i += kEpnpThreads) inlier_mask[f.o0 + i] = 1;
     if (tid == 0) {
       write_pose(Wl, pose_out + (size_t)b * 12);
-      n_inliers[b] = n;
+      n_inliers[b] = f.n;
     }
     return;
   }
-  auto use = [&](int i) {
-    double p2[2], p3[3];
-    load_pair<true>(f2, f3, i, p2, p3);
-    return cv_error(Wl, Kc, p3, p2) <= thr2f;
-  };
-  for (int i = tid; i < n; i += kEpnpThreads) inlier_mask[o0 + i] = use(i) ? 1 : 0;
-  const int m = epnp_block<true>(f2, f3, n, Kc, use, sh, &T);
-  if (tid == 0) {                                      // a degenerate inlier set keeps the winner's pose
-    write_pose(m >= 4 && pose_finite(T) ? T : Wl, pose_out + (size_t)b * 12);
-    n_inliers[b] = S.best;                             // the mask's count: the same test as the winner's
-  }
+  refit_tail(b, f, Wl, [&](const double* p3, const double* p2) { return cv_error(Wl, f.Kc, p3, p2) <= thr2f; }, S.best, sh, &T, pose_out,
+             inlier_mask, n_inliers);
 }
 
 // the first `count` samples of a frame of n pairs, by the generator epnp_cv_scan uses (one warp), in calls of `chunk`
@@ -1377,13 +1379,9 @@ __global__ void __launch_bounds__(kGatherThreads) gather_count(const int64_t* __
   const int64_t* m0 = matches0 + (size_t)b * N;
   int cnt = 0;
   for (int n = tid; n < N; n += kGatherThreads) cnt += is_match(m0[n], M) ? 1 : 0;
-  for (int o = 16; o > 0; o >>= 1) cnt += __shfl_xor_sync(0xffffffffu, cnt, o);
-  if ((tid & 31) == 0) cnt_w[tid >> 5] = cnt;
-  __syncthreads();
+  cnt = block_count<kGatherThreads>(cnt, cnt_w);
   if (tid == 0) {
-    int c = 0;
-    for (int w = 0; w < kGatherThreads / 32; ++w) c += cnt_w[w];
-    offsets[b + 1] = c;
+    offsets[b + 1] = cnt;
     if (b == 0) offsets[0] = 0;
   }
 }
@@ -1502,18 +1500,33 @@ extern "C" int opb_gather_matches_objects(const int64_t* matches0, const float* 
                              stream);
 }
 
+// the arguments every RANSAC entry point takes
+static bool ransac_args_ok(const double* K, const double* pts2d, const double* pts3d, const int32_t* offsets, int32_t B, int32_t hypotheses,
+                           double reproj_error, const double* workspace, const double* pose_out, const int32_t* inlier_mask,
+                           const int32_t* n_inliers) {
+  return K && pts2d && pts3d && offsets && workspace && pose_out && inlier_mask && n_inliers && B > 0 && hypotheses > 0 &&
+         hypotheses <= opb::kMaxHypotheses && reproj_error > 0.0;
+}
+
+// a RANSAC of a fixed number of hypotheses: one thread per hypothesis record, then one block per frame selects
+template <class HypothesesKernel, class SelectKernel>
+static int ransac_fixed(HypothesesKernel hypotheses_kernel, SelectKernel select_kernel, const double* K, const double* pts2d, const double* pts3d,
+                        const int32_t* offsets, int32_t B, int32_t hypotheses, double reproj_error, uint64_t seed, double* workspace,
+                        double* pose_out, int32_t* inlier_mask, int32_t* n_inliers, void* stream) {
+  if (!ransac_args_ok(K, pts2d, pts3d, offsets, B, hypotheses, reproj_error, workspace, pose_out, inlier_mask, n_inliers)) return OPB_E_INVALID;
+  cudaStream_t st = (cudaStream_t)stream;
+  const double thr2 = reproj_error * reproj_error;
+  hypotheses_kernel<<<dim3((unsigned)B, (unsigned)((hypotheses + opb::kHypThreads - 1) / opb::kHypThreads)), opb::kHypThreads, 0, st>>>(
+      K, pts2d, pts3d, offsets, hypotheses, thr2, (unsigned long long)seed, workspace);
+  select_kernel<<<(unsigned)B, opb::kRefineThreads, 0, st>>>(K, pts2d, pts3d, offsets, hypotheses, thr2, workspace, pose_out, inlier_mask, n_inliers);
+  return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_E_CUDA;
+}
+
 extern "C" int opb_ransac_pnp(const double* K, const double* pts2d, const double* pts3d, const int32_t* offsets, int32_t B, int32_t hypotheses,
                               double reproj_error, uint64_t seed, double* workspace, double* pose_out, int32_t* inlier_mask, int32_t* n_inliers,
                               void* stream) {
-  if (!K || !pts2d || !pts3d || !offsets || !workspace || !pose_out || !inlier_mask || !n_inliers || B <= 0 || hypotheses <= 0 ||
-      hypotheses > opb::kMaxHypotheses || !(reproj_error > 0.0))
-    return OPB_E_INVALID;
-  cudaStream_t st = (cudaStream_t)stream;
-  const double thr2 = reproj_error * reproj_error;
-  opb::pnp_hypotheses<<<dim3((unsigned)B, (unsigned)((hypotheses + opb::kHypThreads - 1) / opb::kHypThreads)), opb::kHypThreads, 0, st>>>(
-      K, pts2d, pts3d, offsets, hypotheses, thr2, (unsigned long long)seed, workspace);
-  opb::pnp_select_refine<<<(unsigned)B, opb::kRefineThreads, 0, st>>>(K, pts2d, pts3d, offsets, hypotheses, thr2, workspace, pose_out, inlier_mask, n_inliers);
-  return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_E_CUDA;
+  return ransac_fixed(opb::pnp_hypotheses, opb::pnp_select_refine, K, pts2d, pts3d, offsets, B, hypotheses, reproj_error, seed, workspace, pose_out,
+                      inlier_mask, n_inliers, stream);
 }
 
 extern "C" int opb_epnp(const double* K, const double* pts2d, const double* pts3d, const int32_t* offsets, int32_t B, double* pose_out,
@@ -1526,16 +1539,8 @@ extern "C" int opb_epnp(const double* K, const double* pts2d, const double* pts3
 extern "C" int opb_ransac_epnp(const double* K, const double* pts2d, const double* pts3d, const int32_t* offsets, int32_t B, int32_t hypotheses,
                                double reproj_error, uint64_t seed, double* workspace, double* pose_out, int32_t* inlier_mask, int32_t* n_inliers,
                                void* stream) {
-  if (!K || !pts2d || !pts3d || !offsets || !workspace || !pose_out || !inlier_mask || !n_inliers || B <= 0 || hypotheses <= 0 ||
-      hypotheses > opb::kMaxHypotheses || !(reproj_error > 0.0))
-    return OPB_E_INVALID;
-  cudaStream_t st = (cudaStream_t)stream;
-  const double thr2 = reproj_error * reproj_error;
-  opb::epnp_hypotheses<<<dim3((unsigned)B, (unsigned)((hypotheses + opb::kHypThreads - 1) / opb::kHypThreads)), opb::kHypThreads, 0, st>>>(
-      K, pts2d, pts3d, offsets, hypotheses, thr2, (unsigned long long)seed, workspace);
-  opb::epnp_select_refit<<<(unsigned)B, opb::kEpnpThreads, 0, st>>>(K, pts2d, pts3d, offsets, hypotheses, thr2, workspace, pose_out, inlier_mask,
-                                                                    n_inliers);
-  return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_E_CUDA;
+  return ransac_fixed(opb::epnp_hypotheses, opb::epnp_select_refit, K, pts2d, pts3d, offsets, B, hypotheses, reproj_error, seed, workspace, pose_out,
+                      inlier_mask, n_inliers, stream);
 }
 
 // test hooks of opb_ransac_epnp_cv (host-side settings read at launch; the launch sequence does not change)
@@ -1585,8 +1590,8 @@ static int cv_wave_size(int B, int H) {
 extern "C" int opb_ransac_epnp_cv(const double* K, const double* pts2d, const double* pts3d, const int32_t* offsets, int32_t B, int32_t hypotheses,
                                   double reproj_error, double confidence, double* workspace, double* pose_out, int32_t* inlier_mask,
                                   int32_t* n_inliers, int32_t* iterations, void* stream) {
-  if (!K || !pts2d || !pts3d || !offsets || !workspace || !pose_out || !inlier_mask || !n_inliers || !iterations || B <= 0 || hypotheses <= 0 ||
-      hypotheses > opb::kMaxHypotheses || !(reproj_error > 0.0) || !(confidence >= 0.0 && confidence <= 1.0))
+  if (!ransac_args_ok(K, pts2d, pts3d, offsets, B, hypotheses, reproj_error, workspace, pose_out, inlier_mask, n_inliers) || !iterations ||
+      !(confidence >= 0.0 && confidence <= 1.0))
     return OPB_E_INVALID;
   cudaStream_t st = (cudaStream_t)stream;
   const float thr2f = (float)(reproj_error * reproj_error);   // findInliers: (float)(thresh * thresh)

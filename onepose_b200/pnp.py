@@ -25,6 +25,10 @@ from . import _lib
 DEFAULT_HYPOTHESES = 4096      # minimal samples per frame: P(no all-inlier sample) < 1e-9 down to 15 % inliers
 EPNP_HYPOTHESES = 10000        # the reference's iterationsCount: five-point samples need more draws than three-point ones
 METHODS = ("p3p", "epnp")
+# the workspace layout of include/onepose_b200.h: per frame and hypothesis one record {count, R (9), t (3)}, and for the
+# confidence mode one loop state per frame after all records
+RECORD_DOUBLES = 13
+CV_STATE_DOUBLES = 16
 
 
 def _hypotheses(method, hypotheses, confidence=None):
@@ -40,10 +44,14 @@ def _hypotheses(method, hypotheses, confidence=None):
     return int(hypotheses)
 
 
-def _frames(K, pts2d, pts3d, offsets):
-    dev = pts2d.device
-    if dev.type != "cuda":
+def _cuda_device(t: torch.Tensor) -> torch.device:
+    if t.device.type != "cuda":
         raise RuntimeError("onepose_b200 has no CPU path: tensors must be on a CUDA device")
+    return t.device
+
+
+def _frames(K, pts2d, pts3d, offsets):
+    dev = _cuda_device(pts2d)
     B = int(offsets.numel()) - 1
     K = K.to(device=dev, dtype=torch.float64).reshape(B, 9).contiguous()
     p2 = pts2d.to(torch.float64).contiguous()
@@ -92,7 +100,7 @@ def ransac_pnp_batch(K: torch.Tensor, pts2d: torch.Tensor, pts3d: torch.Tensor, 
             it = torch.empty(B, dtype=torch.int32, device=dev)
         elif it.device != dev or it.dtype != torch.int32 or tuple(it.shape) != (B,) or not it.is_contiguous():
             raise ValueError(f"iterations_out must be a contiguous int32 [{B}] tensor on {dev}")
-        ws = torch.empty(B * (hypotheses * 13 + 16), dtype=torch.float64, device=dev)
+        ws = torch.empty(B * (hypotheses * RECORD_DOUBLES + CV_STATE_DOUBLES), dtype=torch.float64, device=dev)
         with torch.cuda.device(dev):
             _lib.check(lib.opb_ransac_epnp_cv(K.data_ptr(), p2.data_ptr(), p3.data_ptr(), off.data_ptr(), B, int(hypotheses),
                                               float(reproj_error), float(confidence), ws.data_ptr(), pose.data_ptr(), mask.data_ptr(),
@@ -100,7 +108,7 @@ def ransac_pnp_batch(K: torch.Tensor, pts2d: torch.Tensor, pts3d: torch.Tensor, 
         return pose.reshape(B, 3, 4), mask[:total].bool(), cnt
     if iterations_out is not None:
         raise ValueError("iterations_out is filled by the confidence mode only")
-    ws = torch.empty(B * hypotheses * 13, dtype=torch.float64, device=dev)
+    ws = torch.empty(B * hypotheses * RECORD_DOUBLES, dtype=torch.float64, device=dev)
     with torch.cuda.device(dev):
         fn = lib.opb_ransac_pnp if method == "p3p" else lib.opb_ransac_epnp
         _lib.check(fn(K.data_ptr(), p2.data_ptr(), p3.data_ptr(), off.data_ptr(), B, int(hypotheses), float(reproj_error),
@@ -117,19 +125,31 @@ def gather_matches(matches0: torch.Tensor, keypoints2d: torch.Tensor, keypoints3
     offsets int32 [B+1]; frame b owns rows [offsets[b], offsets[b+1]), rows from offsets[B] on are unspecified.  The values are
     exactly the reference's ``kpts2d[valid]``, ``kpts3d[matches[valid]]`` after ``astype(np.float64)``.  No host synchronisation."""
     lib = _lib.load()
-    dev = matches0.device
-    if dev.type != "cuda":
-        raise RuntimeError("onepose_b200 has no CPU path: tensors must be on a CUDA device")
+    dev, B, N = _match_batch(matches0)
+    kp3 = keypoints3d.to(device=dev, dtype=torch.float32).contiguous()
+    if kp3.dim() != 2 or kp3.shape[1] != 3:
+        raise ValueError(f"keypoints3d must be [M, 3], got {tuple(kp3.shape)}")
+    return _gather(matches0, keypoints2d, matching_scores0,
+                   lambda m0, sc, kp2, *outs: lib.opb_gather_matches(m0, sc, kp2, kp3.data_ptr(), B, N, int(kp3.shape[0]), *outs))
+
+
+def _match_batch(matches0):
+    dev = _cuda_device(matches0)
     if matches0.dim() != 2:
         raise ValueError("matches0 must be [B, N]")
     B, N = matches0.shape
+    return dev, B, N
+
+
+def _gather(matches0, keypoints2d, matching_scores0, call):
+    """What both gathers share: the keypoints2d and score checks, the outputs, and ``call(matches0, scores, keypoints2d, pts2d,
+    pts3d, mconf, query_index, offsets, stream)`` on device pointers (None for absent scores and mconf)."""
+    dev = matches0.device
+    B, N = matches0.shape
     m0 = matches0.to(torch.int64).contiguous()
     kp2 = keypoints2d.to(device=dev, dtype=torch.float32).contiguous()
-    kp3 = keypoints3d.to(device=dev, dtype=torch.float32).contiguous()
     if tuple(kp2.shape) != (B, N, 2):
         raise ValueError(f"keypoints2d must be [B, N, 2] = {(B, N, 2)}, got {tuple(kp2.shape)}")
-    if kp3.dim() != 2 or kp3.shape[1] != 3:
-        raise ValueError(f"keypoints3d must be [M, 3], got {tuple(kp3.shape)}")
     sc = None
     if matching_scores0 is not None:
         sc = matching_scores0.to(device=dev, dtype=torch.float32).contiguous()
@@ -140,10 +160,9 @@ def gather_matches(matches0: torch.Tensor, keypoints2d: torch.Tensor, keypoints3
            "query_index": torch.empty(B * N, dtype=torch.int32, device=dev), "offsets": torch.empty(B + 1, dtype=torch.int32, device=dev)}
     st = torch.cuda.current_stream(dev).cuda_stream
     with torch.cuda.device(dev):
-        _lib.check(lib.opb_gather_matches(m0.data_ptr(), sc.data_ptr() if sc is not None else None, kp2.data_ptr(), kp3.data_ptr(),
-                                          B, N, int(kp3.shape[0]), out["pts2d"].data_ptr(), out["pts3d"].data_ptr(),
-                                          out["mconf"].data_ptr() if sc is not None else None, out["query_index"].data_ptr(),
-                                          out["offsets"].data_ptr(), st))
+        _lib.check(call(m0.data_ptr(), sc.data_ptr() if sc is not None else None, kp2.data_ptr(), out["pts2d"].data_ptr(),
+                        out["pts3d"].data_ptr(), out["mconf"].data_ptr() if sc is not None else None, out["query_index"].data_ptr(),
+                        out["offsets"].data_ptr(), st))
     return out
 
 
@@ -154,12 +173,7 @@ def gather_matches_objects(matches0: torch.Tensor, keypoints2d: torch.Tensor, ke
     or a sequence indexed by id), an entry outside [0, M_b) is not a match.  ``object_ids`` is a host sequence (or CPU tensor).
     Same outputs as ``gather_matches``.  The per-frame tables go to the device from pinned memory: no host synchronisation."""
     lib = _lib.load()
-    dev = matches0.device
-    if dev.type != "cuda":
-        raise RuntimeError("onepose_b200 has no CPU path: tensors must be on a CUDA device")
-    if matches0.dim() != 2:
-        raise ValueError("matches0 must be [B, N]")
-    B, N = matches0.shape
+    dev, B, N = _match_batch(matches0)
     ids = [int(i) for i in (object_ids.tolist() if isinstance(object_ids, torch.Tensor) else object_ids)]
     if len(ids) != B:
         raise ValueError(f"object_ids has {len(ids)} entries for {B} frames")
@@ -175,25 +189,9 @@ def gather_matches_objects(matches0: torch.Tensor, keypoints2d: torch.Tensor, ke
     kp3 = torch.cat(parts, 0).contiguous()
     tab = torch.tensor([first[i][0] for i in ids] + [first[i][1] for i in ids], dtype=torch.int32).pin_memory()
     tab = tab.to(dev, non_blocking=True)
-    m0 = matches0.to(torch.int64).contiguous()
-    kp2 = keypoints2d.to(device=dev, dtype=torch.float32).contiguous()
-    if tuple(kp2.shape) != (B, N, 2):
-        raise ValueError(f"keypoints2d must be [B, N, 2] = {(B, N, 2)}, got {tuple(kp2.shape)}")
-    sc = None
-    if matching_scores0 is not None:
-        sc = matching_scores0.to(device=dev, dtype=torch.float32).contiguous()
-        if tuple(sc.shape) != (B, N):
-            raise ValueError("matching_scores0 must be [B, N] like matches0")
-    out = {"pts2d": torch.empty(B * N, 2, dtype=torch.float64, device=dev), "pts3d": torch.empty(B * N, 3, dtype=torch.float64, device=dev),
-           "mconf": torch.empty(B * N, dtype=torch.float32, device=dev) if sc is not None else None,
-           "query_index": torch.empty(B * N, dtype=torch.int32, device=dev), "offsets": torch.empty(B + 1, dtype=torch.int32, device=dev)}
-    st = torch.cuda.current_stream(dev).cuda_stream
-    with torch.cuda.device(dev):
-        _lib.check(lib.opb_gather_matches_objects(m0.data_ptr(), sc.data_ptr() if sc is not None else None, kp2.data_ptr(), kp3.data_ptr(),
-                                                  tab.data_ptr(), tab[B:].data_ptr(), B, N, out["pts2d"].data_ptr(), out["pts3d"].data_ptr(),
-                                                  out["mconf"].data_ptr() if sc is not None else None, out["query_index"].data_ptr(),
-                                                  out["offsets"].data_ptr(), st))
-    return out
+    return _gather(matches0, keypoints2d, matching_scores0,
+                   lambda m0, sc, kp2, *outs: lib.opb_gather_matches_objects(m0, sc, kp2, kp3.data_ptr(), tab.data_ptr(), tab[B:].data_ptr(), B, N,
+                                                                             *outs))
 
 
 def _solve(K, g, B, dev, reproj_error, scale, hypotheses, seed, method, confidence):
