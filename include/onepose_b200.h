@@ -388,9 +388,10 @@ int opb_debug_set_ws_fill(int32_t byte);
 /* Tensor-core passes of the k,v projection: 2 (default: A_hi.(B_hi + B_lo); its output is rounded to one fp16 plane anyway) or
  * 3 (the full split product), for the precision A/B in tests/ and tools/. */
 int opb_debug_set_kv_passes(opb_matcher* m, int32_t passes);
-/* Residual of a layer = identity K-block of its mlp.3 GEMM.  1 (default): k-block j runs as N = 64 MMAs on accumulator columns
- * [64 j, 64 j + 64) against the 64 x 64 diagonal block of I (a quarter of the tensor work); 0: full-width MMAs against I.
- * Bit-identical results (the skipped products are exact zeros); A/B switch for tests/ and tools/. */
+/* Residual of a layer = identity K-block of its mlp.3 GEMM.  0 (default): full-width MMAs against I; 1: k-block j runs as
+ * N = 64 MMAs on accumulator columns [64 j, 64 j + 64) against the 64 x 64 diagonal block of I (a quarter of the tensor work,
+ * but ptxas serialises every MMA of that kernel, and it is slower).  Bit-identical results (the skipped products are exact
+ * zeros); A/B switch for tests/ and tools/. */
 int opb_debug_set_identity_diag(opb_matcher* m, int32_t enable);
 /* C[rows, n_out] (fp32, ld = n_out) = A . B^T with fp16-split operands.  a_hi/a_lo [rows, K], b_hi/b_lo [n_out, K];
  * rows % 256 == 0, K % 64 == 0, n_out % 256 == 0.  backend 0 = the wgmma core, 1 = SIMT fp32 FFMA cross-check

@@ -75,7 +75,7 @@ struct opb_matcher : Handle {
   int ws_frames = 0, ws_N = 0, ws_m_pad = 0;
   DevBuf tab;             // ChunkTable of the chunk in flight (written by assemble_layout)
   bool hoist = true;      // evaluate the frame-invariant layers once per object (object_prologue)
-  int identity_diag = 1;  // residual identity K-block as N = 64 MMAs on the diagonal blocks (opb_debug_set_identity_diag)
+  int identity_diag = 0;  // residual identity K-block at full width (1: N = 64 MMAs on the diagonal blocks; opb_debug_set_identity_diag)
   int kv_two_pass = 1;    // k,v projection as A_hi.(B_hi + B_lo): its output is one fp16 plane, the A_lo term is below that rounding
   PlaneBuf x, qp, pn, g, xq, bd, lin_a, lin_b;
   DevBuf kvt;             // fp16 [rows, 512]

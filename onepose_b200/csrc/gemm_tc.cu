@@ -8,7 +8,7 @@
 // computes in fp32 (GATs_SuperGlue.py:191-193) and the contract is 1e-4 abs on conf.
 //
 // Persistent grid (at most one CTA per SM), static round-robin tile schedule (n-tile fastest so CTAs that share an A row tile
-// run together).  288 threads = 9 warps:
+// run together).  384 threads = 12 warps:
 //   warps 0-7    two consumer warpgroups.  Warpgroup w issues wgmma.m64nBNk16 for rows [64 w, 64 w + 64) of the tile and keeps
 //                that accumulator in registers (BN = 256: 128 registers per thread).  At the end of a tile both warpgroups
 //                park their accumulators in shared memory (over the then idle ring) and the same 8 warps run the fused
@@ -18,9 +18,12 @@
 //                producer starts the next tile's loads once the parked tile has been read (the ring and the parked
 //                accumulator share the shared memory).
 //   warp 8       TMA producer   cp.async.bulk.tensor 2D, SWIZZLE_128B boxes -> a 192 KB shared-memory ring of 2-4 stages
-// (The registers of a block are allocated in whole warpgroups, so 9 warps are budgeted like 12: 168 per thread.)
-// Converter variant (ACV_NORM_RELU): the producer lands the RAW fp32 A tile and each consumer warpgroup rewrites its own 64
-// rows into the (hi, lo) planes in place before it issues the MMAs of that k-block.
+//   warps 9-11   converters (ACV_NORM_RELU only; in every other variant they go straight to the final __syncthreads)
+// (The registers of a block are allocated in whole warpgroups, so the third warpgroup costs no registers: 168 per thread.)
+// Converter variant (ACV_NORM_RELU): the producer lands the RAW fp32 A tile, the converter warps rewrite all 128 rows into the
+// (hi, lo) planes in place and arrive on the stage's conv_bar; the consumers wait on conv_bar instead of full_bar, so their
+// k-blocks are the same branch-free MMA chain as every other variant's and the conversion of stage s + 1 runs under the MMAs
+// of stage s.
 // Every kernel starts with griddepcontrol.wait after its on-chip set-up (programmatic dependent launch: the set-up of launch
 // i+1 overlaps the tail of launch i).
 #include <cuda.h>
@@ -49,8 +52,9 @@ constexpr int kExtraBytes = 1024;                // per-tile scratch of the scor
 constexpr int kMaxStages = 4;
 constexpr int kSmemBytes = kRingBytes + kNumStaging * kStagingBytes + 1024 /*align*/ + 256 /*barriers*/ + kExtraBytes;
 static_assert(kSmemBytes <= 227 * 1024, "exceeds the 227 KB of shared memory an H100 block can have");
-constexpr int kThreads = 288;                    // warpgroups 0, 1: MMA + epilogue; warp 8: TMA producer
+constexpr int kThreads = 384;                    // warpgroups 0, 1: MMA + epilogue; warp 8: TMA producer; warps 9-11: converters
 constexpr int kProducerWarp = 8;
+constexpr int kConvWarps = 3;
 
 // ------------------------------------------------------------------ PTX wrappers (mbarrier / TMA loads: tma.cuh)
 __device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, const void* smem_src, int c_inner, int c_outer) {
@@ -151,7 +155,7 @@ struct Maps {
 };
 
 // A-operand conversion: instead of fp16-split planes prepared by a separate kernel, the TMA producer lands the RAW fp32
-// tile (128 rows x 64 columns = exactly the 32 KB of the stage's A_hi + A_lo planes) and the consumer warpgroups rewrite it
+// tile (128 rows x 64 columns = exactly the 32 KB of the stage's A_hi + A_lo planes) and the converter warps rewrite it
 // IN PLACE as the (hi, lo) planes the MMA descriptors expect -- the pointwise op between two GEMMs runs on data that is
 // already on the SM, and its 4 KB/row HBM round trip disappears:
 //   ACV_NORM_RELU  A  = ReLU((hid - mu_seg) * rstd_seg)          mlp.3 reads mlp.0's fp32 output (GATs_SuperGlue.py:126-127)
@@ -161,12 +165,14 @@ enum { ACV_NONE = 0, ACV_NORM_RELU = 1 };
 // BN_: column-tile width (256 for every matcher GEMM; 64 / 128 for the narrow convolution layers of the extractor: the stage
 // shrinks and the ring deepens to three / four stages).
 // K2B: what the K2 block's B operand is (the residual GEMM's identity: GemmProblem::b2_lo_zero / b2_identity).
-//   K2_LO_ZERO  its lo plane is zero: the A_hi.B_lo pass of those k-blocks is not issued (it would add exact zeros)
+//   K2_LO_ZERO  its lo plane is zero: those k-blocks run a chain of their own without the A_hi.B_lo pass (it would add exact
+//               zeros).  The residual GEMM's default.
 //   K2_DIAG     the identity, run as N = 64 MMAs on the diagonal blocks.  Those MMAs write 32-register slices of the m64n256
-//               accumulator, which makes ptxas serialise every wgmma of the kernel, so the slices live in an instantiation of
-//               their own and the other variants keep back-to-back MMAs.
-// Both are template properties so that the other variants' k-blocks are one branch-free chain of MMAs: a branch between two
-// wgmmas makes ptxas insert a warpgroup.arrive in front of the MMAs that follow it.
+//               accumulator, which makes ptxas serialise every wgmma of the kernel (C7511), so the slices live in an
+//               instantiation of their own and the other variants keep back-to-back MMAs.  A quarter of K2_LO_ZERO's identity
+//               work, but the serialised hidden k-blocks make it the slower form on an H100 (DESIGN.md 5.1).
+// Both are template properties so that every k-block is one branch-free chain of MMAs: a branch between two wgmmas makes ptxas
+// insert a warpgroup.arrive in front of the MMAs that follow it.
 enum { K2_FULL = 0, K2_LO_ZERO = 1, K2_DIAG = 2 };
 
 template <int EPI, int ACV = ACV_NONE, bool HI = false, int BN_ = 256, int K2B = K2_FULL>
@@ -208,6 +214,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + kNumStaging * kStagingBytes);
   uint64_t* empty_bar = full_bar + kMaxStages;
   uint64_t* acc_free_bar = empty_bar + kMaxStages;   // the parked accumulator has been read: the ring may be refilled
+  uint64_t* conv_bar = acc_free_bar + 1;             // ACV: the stage's A tile has been converted (every k-block of the stage arrives)
   float* extra = reinterpret_cast<float*>(staging + kNumStaging * kStagingBytes + 256);   // kExtraBytes of per-tile scratch
   float* acc_smem = reinterpret_cast<float*>(smem);  // parked accumulator [BM][kAccLd]
 
@@ -220,8 +227,8 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
   const int total_units = units_per_batch * p.batch;
 
   if (threadIdx.x == 0) {
-    // full: the TMA transaction arrive; empty: one arrive per consumer warp
-    for (int s = 0; s < kMaxStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); }
+    // full: the TMA transaction arrive; empty: one arrive per consumer warp; conv: one arrive per converter warp
+    for (int s = 0; s < kMaxStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); mbar_init(&conv_bar[s], kConvWarps); }
     mbar_init(acc_free_bar, 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
@@ -303,6 +310,69 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
           }
           tma_load_2d(st + kBOff, mbh, &full_bar[s], kcb, brow);
           tma_load_2d(st + kBOff + kBBytes, mbl, &full_bar[s], kcb, brow);
+        }
+      }
+    }
+  } else if (warp > kProducerWarp) {
+    // ===================== converters: raw fp32 tile -> (hi, lo) planes, in place =====================
+    // Converter warp cw rewrites the 16-row groups cw, cw + 3, cw + 6 of every hidden k-block.  Row r of the raw boxes and row r
+    // of the planes are the same two 128-byte slots, so a lane group reads a row before any lane writes it (__syncwarp between).
+    // Lane = (row 4i + lane/8, 8-column group c = lane%8): every shared-memory instruction touches each bank group once per
+    // wavefront.  Every k-block arrives on conv_bar (the identity k-blocks need no conversion), so conv_bar runs through the
+    // same phases as full_bar.
+    if (ACV != ACV_NONE) {
+      constexpr int kLPR = BK / 8;               // lanes per row = 8-column groups per k-block
+      constexpr int kRPI = 32 / kLPR;            // rows per shared-memory instruction
+      constexpr int kRowIters = 16 / kRPI;
+      const int cw = warp - kProducerWarp - 1;
+      const int c = lane % kLPR, rsub = lane / kLPR;
+      uint32_t it = 0;
+      for (int u = blockIdx.x; u < total_units; u += gridDim.x) {
+        const int m_tile = (u % units_per_batch) / p.n_tiles;
+        const int seg_a = p.L.seg_of_row(m_tile * BM);
+        for (int kb = 0; kb < nkb; ++kb, ++it) {
+          const int s = it % kStages;
+          if (kb < nkb1) {
+            const int kcol = kb * BK + 8 * c;      // first of this lane's 8 source columns
+            float pa[8], pb[8];                    // per-column parameters: (-64 mu rstd, 64 rstd)
+            {
+              const float* base_a = p.mu + (long long)seg_a * 512 + kcol;
+              const float4 a0 = __ldg(reinterpret_cast<const float4*>(base_a)), a1 = __ldg(reinterpret_cast<const float4*>(base_a) + 1);
+              pa[0] = a0.x; pa[1] = a0.y; pa[2] = a0.z; pa[3] = a0.w; pa[4] = a1.x; pa[5] = a1.y; pa[6] = a1.z; pa[7] = a1.w;
+              const float* base_b = p.rstd + (long long)seg_a * 512 + kcol;
+              const float4 b0 = __ldg(reinterpret_cast<const float4*>(base_b)), b1 = __ldg(reinterpret_cast<const float4*>(base_b) + 1);
+              pb[0] = b0.x; pb[1] = b0.y; pb[2] = b0.z; pb[3] = b0.w; pb[4] = b1.x; pb[5] = b1.y; pb[6] = b1.z; pb[7] = b1.w;
+              // 64 * ReLU((h - mu) * rstd) = max(h * (64 rstd) - 64 mu rstd, 0): one FFMA + one FMNMX per element, pre-scale included
+#pragma unroll
+              for (int j = 0; j < 8; ++j) { pb[j] *= kPre; pa[j] = -pa[j] * pb[j]; }
+            }
+            mbar_wait(&full_bar[s], (it / kStages) & 1);
+            const uint32_t stu = smem_u32(smem + s * kStageBytes);
+            const uint32_t rawbox = stu + ((2 * c) >> 3) * (BM * 128);
+            for (int g = cw; g < BM / 16; g += kConvWarps) {
+#pragma unroll
+              for (int i = 0; i < kRowIters; ++i) {
+                const int r = g * 16 + kRPI * i + rsub;
+                const float4 ra = lds128(rawbox + r * 128 + ((((2 * c) & 7) ^ (r & 7)) << 4));
+                const float4 rb = lds128(rawbox + r * 128 + ((((2 * c + 1) & 7) ^ (r & 7)) << 4));
+                __syncwarp();                      // every lane holds its raw values of these rows before any lane overwrites them
+                float v[8] = {ra.x, ra.y, ra.z, ra.w, rb.x, rb.y, rb.z, rb.w};
+#pragma unroll
+                for (int j = 0; j < 8; ++j) v[j] = fmaxf(fmaf(v[j], pb[j], pa[j]), 0.f);     // already x 2^6
+                uint4 oh, ol;
+#pragma unroll
+                for (int j = 0; j < 4; ++j)
+                  split_f32x2(make_float2(v[2 * j], v[2 * j + 1]), reinterpret_cast<__half2*>(&oh)[j], reinterpret_cast<__half2*>(&ol)[j]);
+                sts128(stu + stg_off(r, c), oh);
+                sts128(stu + kABytes + stg_off(r, c), ol);
+              }
+            }
+            fence_async_smem();                    // generic-proxy writes -> visible to the tensor core (async proxy)
+          } else {
+            mbar_wait(&full_bar[s], (it / kStages) & 1);
+          }
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&conv_bar[s]);
         }
       }
     }
@@ -398,60 +468,24 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
           prev_s = s;
         }
       } else {
-        const int seg_a = ACV ? p.L.seg_of_row(m_tile * BM) : 0;
         for (int kb = 0; kb < nkb; ++kb, ++it) {
           const int s = it % kStages;
-          mbar_wait(&full_bar[s], (it / kStages) & 1);
+          mbar_wait(ACV != ACV_NONE ? &conv_bar[s] : &full_bar[s], (it / kStages) & 1);
           uint8_t* st = smem + s * kStageBytes;
-          if (ACV != ACV_NONE && kb < nkb1) {
-            // ---- raw fp32 tile -> (hi, lo) planes, in place, rows [16 cw, 16 cw + 16) per warp (cw = 4 wg + q: the
-            // warpgroup converts exactly the rows its MMAs read).  Row r of the raw boxes and row r of the planes are the same
-            // two 128-byte slots, so a lane group reads a row before any lane writes it (__syncwarp between).  Lane = (row
-            // 4i + lane/8, 8-column group c = lane%8): every shared-memory instruction touches each bank group once per wavefront.
-            constexpr int kLPR = BK / 8;             // lanes per row = 8-column groups per k-block
-            constexpr int kRPI = 32 / kLPR;          // rows per shared-memory instruction
-            constexpr int kRowIters = 16 / kRPI;
-            const int cw = wg * 4 + q;
-            const int c = lane % kLPR, rsub = lane / kLPR;
-            const uint32_t stu = smem_u32(st);
-            const uint32_t rawbox = stu + ((2 * c) >> 3) * (BM * 128);
-            const int kcol = kb * BK + 8 * c;        // first of this lane's 8 source columns
-            float pa[8], pb[8];                      // per-column parameters: (-64 mu rstd, 64 rstd)
-            {
-              const float* base_a = p.mu + (long long)seg_a * 512 + kcol;
-              const float4 a0 = __ldg(reinterpret_cast<const float4*>(base_a)), a1 = __ldg(reinterpret_cast<const float4*>(base_a) + 1);
-              pa[0] = a0.x; pa[1] = a0.y; pa[2] = a0.z; pa[3] = a0.w; pa[4] = a1.x; pa[5] = a1.y; pa[6] = a1.z; pa[7] = a1.w;
-              const float* base_b = p.rstd + (long long)seg_a * 512 + kcol;
-              const float4 b0 = __ldg(reinterpret_cast<const float4*>(base_b)), b1 = __ldg(reinterpret_cast<const float4*>(base_b) + 1);
-              pb[0] = b0.x; pb[1] = b0.y; pb[2] = b0.z; pb[3] = b0.w; pb[4] = b1.x; pb[5] = b1.y; pb[6] = b1.z; pb[7] = b1.w;
-              // 64 * ReLU((h - mu) * rstd) = max(h * (64 rstd) - 64 mu rstd, 0): one FFMA + one FMNMX per element, pre-scale included
-#pragma unroll
-              for (int j = 0; j < 8; ++j) { pb[j] *= kPre; pa[j] = -pa[j] * pb[j]; }
-            }
-#pragma unroll
-            for (int i = 0; i < kRowIters; ++i) {
-              const int r = cw * 16 + kRPI * i + rsub;
-              const float4 ra = lds128(rawbox + r * 128 + ((((2 * c) & 7) ^ (r & 7)) << 4));
-              const float4 rb = lds128(rawbox + r * 128 + ((((2 * c + 1) & 7) ^ (r & 7)) << 4));
-              __syncwarp();                  // every lane holds its raw values of these rows before any lane overwrites them
-              float v[8] = {ra.x, ra.y, ra.z, ra.w, rb.x, rb.y, rb.z, rb.w};
-#pragma unroll
-              for (int j = 0; j < 8; ++j) v[j] = fmaxf(fmaf(v[j], pb[j], pa[j]), 0.f);     // already x 2^6
-              uint4 oh, ol;
-#pragma unroll
-              for (int j = 0; j < 4; ++j)
-                split_f32x2(make_float2(v[2 * j], v[2 * j + 1]), reinterpret_cast<__half2*>(&oh)[j], reinterpret_cast<__half2*>(&ol)[j]);
-              sts128(stu + stg_off(r, c), oh);
-              sts128(stu + kABytes + stg_off(r, c), ol);
-            }
-            fence_async_smem();              // generic-proxy writes -> visible to the tensor core (async proxy)
-            epi_bar();                       // ... from all four warps of the warpgroup
-          }
           const uint32_t sa_h = smem_u32(st) + a_off;
           const uint32_t sa_l = sa_h + kABytes, sb_h = smem_u32(st) + kBOff, sb_l = sb_h + kBBytes;
-          const bool skip_lo = K2B == K2_LO_ZERO && kb >= nkb1;     // B_lo == 0: the A_hi.B_lo pass adds exact zeros
           wgmma_fence();
-          if (DIAG && kb >= nkb1) {
+          if (K2B == K2_LO_ZERO && kb >= nkb1) {
+            // B_lo == 0: the A_hi.B_lo pass would add exact zeros.  A chain of its own, so that no branch sits between MMAs.
+#pragma unroll
+            for (int k = 0; k < BK / MMA_K; ++k) {
+              const uint32_t koff = k * MMA_K * 2;
+              const uint64_t bh = make_desc(sb_h + koff), ah = make_desc(sa_h + koff), al = make_desc(sa_l + koff);
+              mma_k16<BN>(acc, ah, bh);
+              mma_k16<BN>(acc, al, bh);
+            }
+            wgmma_commit();
+          } else if (DIAG && kb >= nkb1) {
             // identity K-block j: only output columns [64 j, 64 j + 64) receive anything -> N = 64 MMAs on that slice of the
             // accumulator (registers [32 j, 32 j + 32) of the fragment; the other 192 columns of a full-width MMA would add zeros)
             const int j = kb - nkb1;
@@ -466,13 +500,14 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
                 default: wgmma_m64n64k16(acc + 96, ah, bh); wgmma_m64n64k16(acc + 96, al, bh); break;
               }
             }
+            wgmma_commit();
           } else {
 #pragma unroll
             for (int k = 0; k < BK / MMA_K; ++k) {
               const uint32_t koff = k * MMA_K * 2;   // bytes inside the swizzle row
               const uint64_t ah = make_desc(sa_h + koff), al = make_desc(sa_l + koff);
               const uint64_t bh = make_desc(sb_h + koff), bl = make_desc(sb_l + koff);
-              if (kSplitAcc) {                                        // narrow tiles: never HI / skip_lo (launch_gemm_tc)
+              if (kSplitAcc) {                                        // narrow tiles: never HI / K2 blocks (launch_gemm_tc)
                 const int dy = (EPI == EPI_CONV && p.taps == 9) ? kb / (3 * p.kb_per_tap) : 0;
                 mma_main(dy % n_main, ah, bh);
                 mma_k16<BN>(acc_c, ah, bl);
@@ -480,12 +515,12 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
                 continue;
               }
               mma_k16<BN>(acc, ah, bh);
-              if (!skip_lo) mma_k16<BN>(acc, ah, bl);
+              mma_k16<BN>(acc, ah, bl);
               if (!HI) mma_k16<BN>(acc, al, bh);
             }
+            wgmma_commit();
           }
-          wgmma_commit();
-          wgmma_wait<1>();                                            // the previous k-block's MMAs are done: free its stage
+          wgmma_wait<1>();                                           // the previous k-block's MMAs are done: free its stage
           if (prev_s >= 0) release(prev_s);
           prev_s = s;
         }

@@ -8,17 +8,24 @@
     line of time against K: the slope is the main loop's cost per k-block, the intercept the per-launch fixed cost (epilogue,
     ring refills, launch).  The slope is reported as executed TFLOP/s (three fp16 passes per product), as the shared-memory
     fill per SM (96 KB land in a CTA's ring per k-block: A hi/lo + B hi/lo) and as that fill summed over the SMs.
-(b) the benchmarked call (match_frames, B = 32, N2D = 1024, N3D = 7000) with the profiling hook on: ms per step and share of
-    the step for every GEMM epilogue and the large helper kernels.
+(b) the mlp.3-shaped GEMM (converter variant: A = ReLU(IN(hid)) formed from raw fp32 in the core, plus the identity K-block)
+    at rows = 262144 (32 frames of 1024 + 7168 rows), n_out = 256 and K1 = 256 / 512 / 768 / 1024, with the identity block as
+    N = 64 diagonal MMAs and at full width.  The same line fit; the slope counts the three passes of the K1 part only, the
+    identity block is in the intercept.  tools/gemm_feed_mlp3.cu is compiled with nvcc into a temporary directory and
+    linked against the library build being measured.
+(c) the benchmarked call (match_frames, B = 32, N2D = 1024, N3D = 7000) with the profiling hook on, with the identity block
+    in both forms: ms per step and share of the step for every GEMM and the large helper kernels.
 
 --lib loads another build of the library (A/B between builds in one process).  Needs a GPU; there is no CPU path.
 """
 from __future__ import annotations
 
 import argparse
+import ctypes
 import os
 import subprocess
 import sys
+import tempfile
 
 import numpy as np
 import torch
@@ -30,8 +37,10 @@ ROWS, N_OUT, KS = 262144, 512, (256, 512, 1024, 2048)
 BM, BN, BK = 128, 256, 64
 STAGE_BYTES = 2 * BM * BK * 2 + 2 * BN * BK * 2          # A hi/lo + B hi/lo of one k-block
 DENSE_FLOP_PER_CLK_SM = 4096                             # fp16 wgmma, dense
+MLP3_FRAMES, MLP3_NPAD, MLP3_MPAD, MLP3_K1S = 32, 1024, 7168, (256, 512, 768, 1024)
 PROFILE_PREFIXES = [("gemm epi9 ", "k,v projection (EPI_QKV)"), ("gemm epi2 ", "q projection (EPI_QSCALE)"),
-                    ("gemm epi10 ", "G fold / mlp.3 / residual (EPI_BIAS_PLANES)"), ("gemm epi1 ", "mlp.0 (EPI_F32_STATS)"),
+                    ("gemm epi10 n256 k256 ", "G fold (EPI_BIAS_PLANES)"), ("gemm epi1 ", "mlp.0 (EPI_F32_STATS)"),
+                    ("gemm epi10 n256 k768 ", "mlp.3 + residual (EPI_BIAS_PLANES, ACV_NORM_RELU)"),
                     ("gemm epi5 ", "final_proj (EPI_L2NORM)"), ("gemm epi6 ", "score pass 1 (EPI_SCORE_SUMS)"),
                     ("gemm epi7 ", "score pass 2 (EPI_SCORE_CONF)"), ("gemm epi0 ", "fp32 out (EPI_F32)"),
                     ("kv_state_h", ""), ("gats_aggregate", ""), ("in_stats_final", ""), ("score_sums_finalize", ""),
@@ -45,6 +54,26 @@ def card():
         return q.stdout.strip().splitlines()[torch.cuda.current_device()]
     except (OSError, subprocess.SubprocessError, IndexError):
         return "nvidia-smi unavailable"
+
+
+def time_launches(launch, window):
+    """(ms per launch, launches) over >= window seconds of back-to-back launches, after a warm-up."""
+    for _ in range(3):
+        launch()
+    torch.cuda.synchronize()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(5):
+        launch()
+    e1.record()
+    torch.cuda.synchronize()
+    n = max(10, int(np.ceil(window / (e0.elapsed_time(e1) * 1e-3 / 5))))
+    e0.record()
+    for _ in range(n):
+        launch()
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / n, n
 
 
 def gemm_slope(lib, window):
@@ -67,23 +96,7 @@ def gemm_slope(lib, window):
             if rc != 0:
                 raise RuntimeError(f"opb_debug_gemm rc={rc}")
 
-        for _ in range(3):
-            launch()
-        torch.cuda.synchronize()
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(5):
-            launch()
-        e1.record()
-        torch.cuda.synchronize()
-        n = max(10, int(np.ceil(window / (e0.elapsed_time(e1) * 1e-3 / 5))))
-        e0.record()
-        for _ in range(n):
-            launch()
-        e1.record()
-        torch.cuda.synchronize()
-        ms = e0.elapsed_time(e1) / n
-        rows.append((K, ms, n))
+        rows.append((K,) + time_launches(launch, window))
         del ak, bk
     Ks = np.array([r[0] for r in rows], float)
     ts = np.array([r[1] for r in rows], float)
@@ -105,8 +118,69 @@ def gemm_slope(lib, window):
             "points": [{"K": K, "ms": ms} for K, ms, _ in rows]}
 
 
-def step_profile(runs=5):
-    from onepose_b200 import GATsSuperGlue, synthetic
+def mlp3_launcher(lib_path):
+    """Build tools/gemm_feed_mlp3.cu against the library at lib_path (already loaded) and return its feed_mlp3."""
+    from onepose_b200 import build
+    tmp = tempfile.mkdtemp(prefix="gemm_feed_")
+    so = os.path.join(tmp, "feed_mlp3.so")
+    cmd = [build._nvcc(), "-std=c++17", "-Xcompiler", "-fPIC", "-shared", "-I", build.CSRC,
+           os.path.join(ROOT, "tools", "gemm_feed_mlp3.cu"), lib_path, "-o", so]
+    res = subprocess.run(cmd, capture_output=True, text=True)
+    if res.returncode != 0:
+        raise RuntimeError("nvcc failed:\n" + " ".join(cmd) + "\n" + res.stdout + res.stderr)
+    fn = ctypes.CDLL(so).feed_mlp3
+    fn.restype = ctypes.c_int
+    P, I = ctypes.c_void_p, ctypes.c_int
+    fn.argtypes = [P, I] + [P] * 11 + [I, I, I, I, P]
+    return fn
+
+
+def mlp3_slope(lib_path, window):
+    feed = mlp3_launcher(lib_path)
+    dev = torch.device("cuda")
+    rows = MLP3_FRAMES * (MLP3_NPAD + MLP3_MPAD)
+    segs = 2 * MLP3_FRAMES
+    g = torch.Generator(device=dev).manual_seed(0)
+    planes = lambda r, c: [torch.randn(r, c, device=dev, generator=g).half() for _ in range(2)]   # noqa: E731
+    x, out = planes(rows, 256), planes(rows, 256)
+    eye = [(64 * torch.eye(256, device=dev)).half(), torch.zeros(256, 256, device=dev).half()]
+    bias = torch.randn(256, device=dev, generator=g)
+    nparam = (segs + max(MLP3_K1S) // 512) * 512
+    mu, rstd = 0.1 * torch.randn(nparam, device=dev, generator=g), 1 + 0.1 * torch.rand(nparam, device=dev, generator=g)
+    res = {}
+    for diag in (1, 0):
+        pts = []
+        for K1 in MLP3_K1S:
+            hid = torch.randn(rows, K1, device=dev, generator=g)
+            w1 = planes(256, K1)
+            args = [hid.data_ptr(), K1, w1[0].data_ptr(), w1[1].data_ptr(), x[0].data_ptr(), x[1].data_ptr(), out[0].data_ptr(),
+                    out[1].data_ptr(), eye[0].data_ptr(), eye[1].data_ptr(), bias.data_ptr(), mu.data_ptr(), rstd.data_ptr(),
+                    MLP3_FRAMES, MLP3_NPAD, MLP3_MPAD, diag, None]
+
+            def launch():
+                rc = feed(*args)
+                if rc != 0:
+                    raise RuntimeError(f"feed_mlp3 rc={rc}")
+
+            pts.append((K1,) + time_launches(launch, window))
+            del hid, w1
+        Ks = np.array([p[0] for p in pts], float)
+        ts = np.array([p[1] for p in pts], float)
+        slope, icept = np.polyfit(Ks, ts, 1)
+        tflops = 3 * 2.0 * rows * 256 / (slope * 1e-3) / 1e12
+        form = "N = 64 diagonal MMAs" if diag else "full width"
+        print(f"(b) mlp.3-shaped GEMM, rows={rows} n_out=256 K2=256 identity block {form}")
+        for K1, ms, n in pts:
+            print(f"    K1={K1:5d}  {ms:8.3f} ms/launch  ({n} launches)")
+        print(f"    main loop  {tflops:6.1f} TFLOP/s executed (K1 part)   intercept {icept:8.3f} ms per launch   "
+              f"fit residual max {np.abs(ts - (slope * Ks + icept)).max():.4f} ms")
+        res["diag" if diag else "full"] = {"slope_tflops_executed": tflops, "intercept_ms": icept,
+                                            "points": [{"K1": K1, "ms": ms} for K1, ms, _ in pts]}
+    return res
+
+
+def step_profile(identity_diag, runs=5):
+    from onepose_b200 import GATsSuperGlue, _lib, synthetic
     dev = torch.device("cuda")
     hp = dict(synthetic.DEFAULT_HPARAMS)
     model = GATsSuperGlue(hp).eval()
@@ -116,6 +190,8 @@ def step_profile(runs=5):
     db, leaves = synthetic.make_object(0, M, 8)
     q = torch.from_numpy(np.stack([synthetic.make_frame(f, db, N)[0] for f in range(B)], 0)).to(dev)
     model.set_object(torch.from_numpy(db).to(dev), torch.from_numpy(leaves).to(dev), reserve=(B, N))
+    model.match_frames(q)                                   # creates the handle
+    _lib.check(_lib.load().opb_debug_set_identity_diag(model._handle, identity_diag), model._handle)
     for _ in range(3):
         model.match_frames(q)
     torch.cuda.synchronize()
@@ -130,7 +206,9 @@ def step_profile(runs=5):
             acc[p][0] += e["ms"]; acc[p][1] += e["flops"]; acc[p][2] = e["launches"]
     model.set_profiling(False)
     total /= runs
-    print(f"(b) match_frames B={B} N2D={N} N3D={M}, profiling on (an event after every launch), mean of {runs} steps: {total:.3f} ms/step")
+    form = "N = 64 diagonal MMAs" if identity_diag else "full width"
+    print(f"(c) match_frames B={B} N2D={N} N3D={M}, identity block {form}, profiling on (an event after every launch), "
+          f"mean of {runs} steps: {total:.3f} ms/step")
     print(f"    {'entry':22s} {'launches':>8s} {'ms/step':>8s} {'share':>6s} {'TFLOP/s alg.':>12s}  what")
     out = {"step_ms": total, "entries": {}}
     for p, what in PROFILE_PREFIXES:
@@ -147,6 +225,7 @@ def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--lib", default=None, help="path of the library build to load (default: the in-tree build)")
     ap.add_argument("--window", type=float, default=0.5, help="seconds of launches per K")
+    ap.add_argument("--no-mlp3", action="store_true", help="skip the fit of the mlp.3-shaped GEMM")
     ap.add_argument("--no-step", action="store_true", help="skip the per-launch profile of the benchmarked call")
     args = ap.parse_args()
     if not torch.cuda.is_available():
@@ -157,8 +236,11 @@ def main():
     lib = _lib.load()
     print("card:", card(), "| library:", _lib.LIB_PATH)
     gemm_slope(lib, args.window)
+    if not args.no_mlp3:
+        mlp3_slope(_lib.LIB_PATH, args.window)
     if not args.no_step:
-        step_profile()
+        for identity_diag in (1, 0):
+            step_profile(identity_diag)
 
 
 if __name__ == "__main__":
