@@ -344,7 +344,8 @@ int opb_sp_get_profile(opb_superpoint* h, int32_t index, char* name, size_t name
 int opb_sp_debug_set_stop(opb_superpoint* h, int32_t layer);
 /* 3x3 convolutions on the 64-wide column tiles: 1 (default) = halo boxes (one (128 + 2)-row A box per kernel row and
  * 64-channel block serves the three horizontal taps through row-offset wgmma descriptors: a third of the L2 -> shared-memory
- * traffic), 0 = nine row-shifted boxes per tile.  Same operand bytes, same products in the same order: bit-identical results.
+ * traffic), 0 = nine row-shifted boxes per tile.  Same operand bytes and products: bit-identical results with 64 input channels;
+ * with more, the halo form visits (kernel row, channel block, dx) instead of (tap, channel block), equal to fp32 rounding.
  * Wider tiles always use the nine boxes (a halo stage of a 128-wide tile leaves no room for a second stage).  A/B switch for
  * tests/ and tools/. */
 int opb_debug_set_conv_halo(int32_t mode);
@@ -393,11 +394,79 @@ int opb_debug_set_kv_passes(opb_matcher* m, int32_t passes);
  * but ptxas serialises every MMA of that kernel, and it is slower).  Bit-identical results (the skipped products are exact
  * zeros); A/B switch for tests/ and tools/. */
 int opb_debug_set_identity_diag(opb_matcher* m, int32_t enable);
-/* C[rows, n_out] (fp32, ld = n_out) = A . B^T with fp16-split operands.  a_hi/a_lo [rows, K], b_hi/b_lo [n_out, K];
- * rows % 256 == 0, K % 64 == 0, n_out % 256 == 0.  backend 0 = the wgmma core, 1 = SIMT fp32 FFMA cross-check
- * (rows, n_out % 128 == 0, K % 16 == 0). */
-int opb_debug_gemm(const void* a_hi, const void* a_lo, const void* b_hi, const void* b_lo,
-                   float* c, int32_t rows, int32_t n_out, int32_t K, int32_t backend, void* stream);
+/* One problem of the GEMM core, field for field the library's own problem description (csrc/gemm_common.cuh GemmProblem):
+ *   C[batch][rows, n_out] = [A1 | A2] . [B1 | B2]^T (+ bias) -> the epilogue `epi`
+ * Operands are fp16-split planes (hi = fp16(64 x), lo = fp16(64 x - hi); opb_debug_split), row-major, each with its own ld in
+ * elements.  Unused pointers are NULL, unused counts 0.  The same rules as the library's own launches apply (rows % 256 == 0,
+ * K1, K2 % 64 == 0, ...); a problem the core does not accept returns OPB_E_INVALID. */
+typedef struct opb_debug_gemm_desc {
+  int32_t epi;              /* 0 fp32 C (+bias), 1 fp32 C + InstanceNorm partials, 2 Q' planes, 5 L2-normalised planes,
+                               6 score sums, 7 score conf + arg-maxes, 9 k,v projection, 10 planes = acc + bias, 11 convolution */
+  int32_t bn;               /* column-tile width: 0 = 256; 128 (epi 0, 11), 64 (epi 11) */
+  int32_t rows;             /* per batch */
+  int32_t n_out;
+  int32_t K1;
+  int32_t K2;               /* 0: no second reduction block */
+  int32_t batch;            /* 0 = 1 */
+  int64_t a_batch_rows;     /* batch z reads A rows from z * a_batch_rows, B rows from z * b_batch_rows */
+  int64_t b_batch_rows;
+  const void* a1_hi;        /* [rows, K1] */
+  const void* a1_lo;
+  int32_t a1_ld;
+  const void* a2_hi;        /* [rows, K2] */
+  const void* a2_lo;
+  int32_t a2_ld;
+  const void* b1_hi;        /* [n_out, K1] */
+  const void* b1_lo;
+  int32_t b1_ld;
+  const void* b2_hi;        /* [n_out, K2], or [segments * n_out, K2] per segment */
+  const void* b2_lo;
+  int32_t b2_ld;
+  int32_t b2_mode;          /* 0 shared, 1 one B2 per segment of the layout, 2 the identity with a zero lo plane, 3 the identity
+                               run on its 64 x 64 diagonal blocks (2, 3: converter problems only) */
+  int32_t a_hi_only;        /* A enters with its hi plane only (epi 9) */
+  const float* a_raw;       /* converter: A1 = ReLU((a_raw - mu[seg]) * rstd[seg]) formed in the core from fp32 [rows, a_raw_ld]; NULL: off */
+  int32_t a_raw_ld;
+  const float* mu;          /* [segments][512] */
+  const float* rstd;
+  int32_t B;                /* activation layout: B frames of n_pad query rows + m_pad 3D rows (B = 0: a plain matrix) */
+  int32_t N;
+  int32_t M;
+  int32_t n_pad;
+  int32_t m_pad;
+  const int32_t* nlen;      /* device [B] valid query rows per frame, or NULL: N */
+  const int32_t* mlen;      /* device [B] valid 3D rows per frame, or NULL: M */
+  const float* bias;        /* [n_out] or NULL */
+  float* c;                 /* epi 0, 1: fp32 [batch * rows, ldc] */
+  int32_t ldc;
+  void* out_hi;             /* planes out [batch * rows, out_ld] (epi 9: out_hi only, 512 columns) */
+  void* out_lo;
+  int32_t out_ld;
+  const float* kmean;       /* epi 2: [segments][256] */
+  int32_t cross;            /* epi 2: source = the other segment of the frame */
+  float* statpart;          /* epi 1: [rows / 32][n_out][2] */
+  float inv_scale;          /* epi 6, 7 */
+  float* rowsum_part;       /* epi 6: [B][2 * n_out / 256][n_pad] */
+  float* colsum_part;       /* epi 6: [B][rows / 32][m_pad] */
+  const float* inv_rowsum;  /* epi 7: [B][n_pad] */
+  const float* inv_colsum;  /* epi 7: [B][m_pad] */
+  float* conf;              /* epi 7: [B][N][conf_ld] or NULL */
+  int32_t conf_ld;          /* 0 = M */
+  uint64_t* rowbest;        /* epi 7: [B][N] packed (conf bits << 32) | ~column */
+  uint64_t* colbest;        /* epi 7: [B][M] */
+  int32_t taps;             /* epi 11: 1 or 9 row-shifted taps of A (0: plain GEMM) */
+  int32_t kb_per_tap;       /* C_in / 64 */
+  int32_t tap_off[9];       /* row shift of each tap */
+  int32_t cv_w2;            /* epi 11 pixel grid: row r is pixel q = r % cv_ppad, y = q / cv_w2, x = q % cv_w2 */
+  int32_t cv_h;
+  int32_t cv_w;
+  int32_t cv_ppad;
+  int32_t relu;
+  int32_t* range_flag;      /* epi 11: set to 1 when an output leaves the split range, or NULL */
+  int32_t max_ctas;         /* grid = min(tiles, SMs, max_ctas); 0: min(tiles, SMs) as the library's own launches */
+  int32_t backend;          /* 0 the wgmma core, 1 the SIMT fp32 FFMA cross-check (epi 0 without converter or identity only) */
+} opb_debug_gemm_desc;
+int opb_debug_gemm(const opb_debug_gemm_desc* desc, void* stream);
 /* The fp16 linear-attention state kernel on a caller-supplied plane kvh [frames*(n_pad+m_pad), 512] (pad rows must be
  * zero); slabs_per_group = 0: the library's own choice; *n_groups = number of partial states; partial [n_groups][4][64*64+64]
  * (NULL: size query only). */

@@ -31,9 +31,46 @@ class OpbSpConfig(C.Structure):
     ]
 
 
-# every symbol include/onepose_b200.h declares: (restype, argtypes)
 _P = C.c_void_p
 _I = C.c_int32
+
+
+class OpbDebugGemmDesc(C.Structure):
+    """opb_debug_gemm_desc: one problem of the GEMM core (see the header).  Pointer fields take device addresses (ints)."""
+    _fields_ = [
+        ("epi", _I), ("bn", _I), ("rows", _I), ("n_out", _I), ("K1", _I), ("K2", _I), ("batch", _I),
+        ("a_batch_rows", C.c_int64), ("b_batch_rows", C.c_int64),
+        ("a1_hi", _P), ("a1_lo", _P), ("a1_ld", _I), ("a2_hi", _P), ("a2_lo", _P), ("a2_ld", _I),
+        ("b1_hi", _P), ("b1_lo", _P), ("b1_ld", _I), ("b2_hi", _P), ("b2_lo", _P), ("b2_ld", _I),
+        ("b2_mode", _I), ("a_hi_only", _I),
+        ("a_raw", _P), ("a_raw_ld", _I), ("mu", _P), ("rstd", _P),
+        ("B", _I), ("N", _I), ("M", _I), ("n_pad", _I), ("m_pad", _I), ("nlen", _P), ("mlen", _P),
+        ("bias", _P), ("c", _P), ("ldc", _I), ("out_hi", _P), ("out_lo", _P), ("out_ld", _I),
+        ("kmean", _P), ("cross", _I), ("statpart", _P),
+        ("inv_scale", C.c_float), ("rowsum_part", _P), ("colsum_part", _P), ("inv_rowsum", _P), ("inv_colsum", _P),
+        ("conf", _P), ("conf_ld", _I), ("rowbest", _P), ("colbest", _P),
+        ("taps", _I), ("kb_per_tap", _I), ("tap_off", _I * 9), ("cv_w2", _I), ("cv_h", _I), ("cv_w", _I), ("cv_ppad", _I),
+        ("relu", _I), ("range_flag", _P),
+        ("max_ctas", _I), ("backend", _I),
+    ]
+
+
+# GemmEpilogue values of opb_debug_gemm_desc.epi
+EPI_F32, EPI_F32_STATS, EPI_QSCALE, EPI_L2NORM, EPI_SCORE_SUMS, EPI_SCORE_CONF, EPI_QKV, EPI_BIAS_PLANES, EPI_CONV = 0, 1, 2, 5, 6, 7, 9, 10, 11
+
+
+def gemm_desc(**fields) -> OpbDebugGemmDesc:
+    """An opb_debug_gemm_desc with the given fields set and every other field zero (torch tensors stand for their data_ptr)."""
+    d = OpbDebugGemmDesc()
+    for k, v in fields.items():
+        if k == "tap_off":
+            d.tap_off[:] = list(v) + [0] * (9 - len(v))
+        else:
+            setattr(d, k, v.data_ptr() if hasattr(v, "data_ptr") else v)
+    return d
+
+
+# every symbol include/onepose_b200.h declares: (restype, argtypes)
 SYMBOLS = {
     "opb_create": (C.c_int, [C.POINTER(OpbConfig), C.POINTER(_P)]),
     "opb_destroy": (None, [_P]),
@@ -71,7 +108,7 @@ SYMBOLS = {
     "opb_debug_set_ws_fill": (C.c_int, [_I]),
     "opb_debug_set_kv_passes": (C.c_int, [_P, _I]),
     "opb_debug_set_identity_diag": (C.c_int, [_P, _I]),
-    "opb_debug_gemm": (C.c_int, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _P]),
+    "opb_debug_gemm": (C.c_int, [C.POINTER(OpbDebugGemmDesc), _P]),
     "opb_debug_kv_state_h": (C.c_int, [_P, _I, _I, _I, _I, _P, C.POINTER(_I), _P]),
     "opb_debug_split": (C.c_int, [_P, _P, _P, C.c_size_t, _P]),
     "opb_debug_set_stop": (C.c_int, [_P, _I, _I]),

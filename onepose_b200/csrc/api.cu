@@ -1045,13 +1045,37 @@ int opb_debug_set_pdl(int32_t enable) {
   return OPB_OK;
 }
 
-int opb_debug_gemm(const void* a_hi, const void* a_lo, const void* b_hi, const void* b_lo, float* c, int32_t rows, int32_t n_out, int32_t K,
-                   int32_t backend, void* stream) {
+int opb_debug_gemm(const opb_debug_gemm_desc* d, void* stream) {
+  if (!d || d->backend < 0 || d->backend > 1 || d->b2_mode < 0 || d->b2_mode > 3) return OPB_E_INVALID;
   GemmProblem p{};
-  p.a1 = CPlanes{(const __half*)a_hi, (const __half*)a_lo, K};
-  p.b1 = CPlanes{(const __half*)b_hi, (const __half*)b_lo, K};
-  p.K1 = K; p.K2 = 0; p.rows = rows; p.n_out = n_out; p.batch = 1; p.c = c; p.ldc = n_out;
-  int rc = backend == 1 ? launch_gemm_simt(p, (cudaStream_t)stream) : launch_gemm_tc(p, (cudaStream_t)stream);
+  p.epi = d->epi; p.bn = d->bn;
+  p.rows = d->rows; p.n_out = d->n_out; p.K1 = d->K1; p.K2 = d->K2;
+  p.batch = d->batch ? d->batch : 1;
+  p.a_batch_rows = d->a_batch_rows; p.b_batch_rows = d->b_batch_rows;
+  p.a1 = CPlanes{(const __half*)d->a1_hi, (const __half*)d->a1_lo, d->a1_ld};
+  p.a2 = CPlanes{(const __half*)d->a2_hi, (const __half*)d->a2_lo, d->a2_ld};
+  p.b1 = CPlanes{(const __half*)d->b1_hi, (const __half*)d->b1_lo, d->b1_ld};
+  p.b2 = CPlanes{(const __half*)d->b2_hi, (const __half*)d->b2_lo, d->b2_ld};
+  p.b2_per_seg = d->b2_mode == 1;
+  p.b2_lo_zero = d->b2_mode >= 2;
+  p.b2_identity = d->b2_mode == 3;
+  p.a_hi_only = d->a_hi_only;
+  p.a_conv = d->a_raw ? 1 : 0; p.a_raw = d->a_raw; p.a_raw_ld = d->a_raw_ld; p.mu = d->mu; p.rstd = d->rstd;
+  p.L.B = d->B; p.L.N = d->N; p.L.M = d->M; p.L.n_pad = d->n_pad; p.L.m_pad = d->m_pad; p.L.R = d->n_pad + d->m_pad;
+  p.L.nlen = d->nlen; p.L.mlen = d->mlen;
+  p.bias = d->bias;
+  p.c = d->c; p.ldc = d->ldc; p.c_batch_elems = (long long)d->rows * d->ldc;
+  p.out = Planes{(__half*)d->out_hi, (__half*)d->out_lo, d->out_ld};
+  p.kmean = d->kmean; p.cross = d->cross; p.statpart = d->statpart;
+  p.inv_scale = d->inv_scale; p.rowsum_part = d->rowsum_part; p.colsum_part = d->colsum_part;
+  p.inv_rowsum = d->inv_rowsum; p.inv_colsum = d->inv_colsum; p.conf = d->conf; p.conf_ld = d->conf_ld;
+  p.rowbest = reinterpret_cast<unsigned long long*>(d->rowbest); p.colbest = reinterpret_cast<unsigned long long*>(d->colbest);
+  p.taps = d->taps; p.kb_per_tap = d->kb_per_tap;
+  for (int t = 0; t < 9; ++t) p.tap_off[t] = d->tap_off[t];
+  p.cv_w2 = d->cv_w2; p.cv_h = d->cv_h; p.cv_w = d->cv_w; p.cv_ppad = d->cv_ppad; p.relu = d->relu; p.range_flag = d->range_flag;
+  p.max_ctas = d->max_ctas;
+  if (d->backend == 1 && (p.epi != EPI_F32 || p.a_conv || p.b2_lo_zero || p.taps || p.a_hi_only)) return OPB_E_INVALID;   // plain product only
+  int rc = d->backend == 1 ? launch_gemm_simt(p, (cudaStream_t)stream) : launch_gemm_tc(p, (cudaStream_t)stream);
   return rc == 0 ? OPB_OK : (rc == -1 ? OPB_E_INVALID : OPB_E_CUDA);
 }
 

@@ -85,6 +85,7 @@ struct GemmProblem {
   int conf_ld;                      // columns of a conf row, >= L.M (0: L.M)
   unsigned long long* rowbest;      // [B][N]
   unsigned long long* colbest;      // [B][M]
+  int max_ctas;                     // test hook (opb_debug_gemm): grid = min(units, SMs, max_ctas); 0 = min(units, SMs)
 };
 
 int launch_gemm_simt(const GemmProblem& p, cudaStream_t stream);

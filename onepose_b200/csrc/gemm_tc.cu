@@ -164,7 +164,8 @@ enum { ACV_NONE = 0, ACV_NORM_RELU = 1 };
 // HI: the A operand enters with its hi plane only (k,v projection, GemmProblem::a_hi_only): two passes, A_hi + B_hi + B_lo per stage.
 // BN_: column-tile width (256 for every matcher GEMM; 64 / 128 for the narrow convolution layers of the extractor: the stage
 // shrinks and the ring deepens to three / four stages).
-// K2B: what the K2 block's B operand is (the residual GEMM's identity: GemmProblem::b2_lo_zero / b2_identity).
+// K2B: what the K2 block's B operand is (the residual GEMM's identity: GemmProblem::b2_lo_zero / b2_identity).  The residual
+// GEMM is mlp.3, so both identity forms exist with the converter only, and the converter only with one of them.
 //   K2_LO_ZERO  its lo plane is zero: those k-blocks run a chain of their own without the A_hi.B_lo pass (it would add exact
 //               zeros).  The residual GEMM's default.
 //   K2_DIAG     the identity, run as N = 64 MMAs on the diagonal blocks.  Those MMAs write 32-register slices of the m64n256
@@ -184,7 +185,8 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
   constexpr int kStageBytes = kBOff + 2 * kBBytes;
   constexpr int kStages = kRingBytes / kStageBytes;      // BN 256: 2, BN 128: 3, BN 64: 4
   constexpr int kDiagBBytes = 64 * BK * 2;         // a 64 x 64 diagonal block of the identity
-  static_assert(K2B == K2_FULL || (BN_ == 256 && EPI == EPI_BIAS_PLANES), "identity K-block: residual GEMMs only");
+  static_assert(K2B == K2_FULL || (BN_ == 256 && EPI == EPI_BIAS_PLANES && ACV == ACV_NORM_RELU), "identity K-block: mlp.3 only");
+  static_assert(ACV == ACV_NONE || K2B != K2_FULL, "the converter comes with the identity K-block");
   static_assert(EPI == EPI_CONV ? BN_ == 64 || BN_ == 128 : EPI == EPI_F32 ? BN_ == 128 || BN_ == 256 : BN_ == 256,
                 "tile widths: EPI_CONV 64 / 128, EPI_F32 128 / 256, every other epilogue 256");
   static_assert(BN_ == 256 || ACV == ACV_NONE && !HI, "narrow tiles: no converter, both A planes");
@@ -1043,9 +1045,10 @@ int launch_gemm_tc(const GemmProblem& p, cudaStream_t stream) {
   TcParams tp{};
   tp.K1 = p.K1; tp.K2 = p.K2; tp.b2_per_seg = p.b2_per_seg; tp.n_out = p.n_out;
   if (p.b2_identity && (!p.b2_lo_zero || p.b2_per_seg || p.K2 != p.n_out || p.n_out != BN || p.K1 <= 0 || bn != BN)) return -1;
-  // the K2 block variants exist for the residual GEMMs: mlp.3 (converted A) with the identity as N = 64 MMAs or as a zero-lo
-  // block, any other EPI_BIAS_PLANES GEMM with the identity as N = 64 MMAs
-  if (p.b2_lo_zero && (p.epi != EPI_BIAS_PLANES || !p.K2 || !(p.a_conv || p.b2_identity))) return -1;
+  // the K2 block variants exist for the residual GEMM mlp.3 (converted A), with the identity as N = 64 MMAs or as a zero-lo
+  // block; the converter always comes with one of them
+  if (p.b2_lo_zero && (p.epi != EPI_BIAS_PLANES || !p.K2 || !p.a_conv)) return -1;
+  if (p.a_conv && !p.b2_lo_zero) return -1;
   const int k2b = p.b2_identity ? K2_DIAG : p.b2_lo_zero ? K2_LO_ZERO : K2_FULL;
   tp.m_tiles = p.rows / BM; tp.n_tiles = p.n_out / bn; tp.batch = p.batch;
   tp.taps = p.taps; tp.kb_per_tap = p.kb_per_tap;
@@ -1060,12 +1063,12 @@ int launch_gemm_tc(const GemmProblem& p, cudaStream_t stream) {
   tp.kmean = p.kmean; tp.cross = p.cross; tp.statpart = p.statpart;
   if ((p.epi == EPI_QSCALE || p.b2_per_seg || p.epi == EPI_QKV || p.epi == EPI_F32_STATS || p.a_conv) && !tp.seg_rows) return -1;
   const int total_units = tp.m_tiles * tp.n_tiles * tp.batch;
-  const int grid = total_units < num_sms() ? total_units : num_sms();
+  int grid = total_units < num_sms() ? total_units : num_sms();
+  if (p.max_ctas > 0 && grid > p.max_ctas) grid = p.max_ctas;      // test hook: the same tiles on fewer CTAs
   cudaError_t le;
   if (p.a_conv) {
-    le = k2b == K2_DIAG      ? launch_variant<EPI_BIAS_PLANES, ACV_NORM_RELU, false, 256, K2_DIAG>(grid, stream, mp, tp)
-         : k2b == K2_LO_ZERO ? launch_variant<EPI_BIAS_PLANES, ACV_NORM_RELU, false, 256, K2_LO_ZERO>(grid, stream, mp, tp)
-                             : launch_variant<EPI_BIAS_PLANES, ACV_NORM_RELU>(grid, stream, mp, tp);
+    le = k2b == K2_DIAG ? launch_variant<EPI_BIAS_PLANES, ACV_NORM_RELU, false, 256, K2_DIAG>(grid, stream, mp, tp)
+                        : launch_variant<EPI_BIAS_PLANES, ACV_NORM_RELU, false, 256, K2_LO_ZERO>(grid, stream, mp, tp);
   } else {
     switch (p.epi) {
       case EPI_F32:
@@ -1080,10 +1083,7 @@ int launch_gemm_tc(const GemmProblem& p, cudaStream_t stream) {
       case EPI_SCORE_SUMS: le = launch_variant<EPI_SCORE_SUMS>(grid, stream, mp, tp); break;
       case EPI_SCORE_CONF: le = launch_variant<EPI_SCORE_CONF>(grid, stream, mp, tp); break;
       case EPI_QKV: le = p.a_hi_only ? launch_variant<EPI_QKV, ACV_NONE, true>(grid, stream, mp, tp) : launch_variant<EPI_QKV>(grid, stream, mp, tp); break;
-      case EPI_BIAS_PLANES:
-        le = k2b == K2_DIAG ? launch_variant<EPI_BIAS_PLANES, ACV_NONE, false, 256, K2_DIAG>(grid, stream, mp, tp)
-                            : launch_variant<EPI_BIAS_PLANES>(grid, stream, mp, tp);
-        break;
+      case EPI_BIAS_PLANES: le = launch_variant<EPI_BIAS_PLANES>(grid, stream, mp, tp); break;
       default: return -1;
     }
   }

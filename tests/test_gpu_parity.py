@@ -301,36 +301,6 @@ def test_full_size_properties():
 
 
 # ----------------------------------------------------------------------------- kernels in isolation
-def test_gemm_cores_agree_and_match_fp64():
-    """wgmma 3-pass fp16-split GEMM vs the SIMT fp32 cross-check vs numpy fp64, same split operands."""
-    lib = _lib.load()
-    rs = np.random.RandomState(0)
-    for rows, n_out, K in [(256, 256, 64), (256, 256, 256), (512, 768, 256), (256, 512, 512), (1024, 7168, 256)]:
-        a = torch.from_numpy((rs.randn(rows, K) * np.exp(rs.randn(rows, 1))).astype(np.float32)).cuda()
-        b = torch.from_numpy((rs.randn(n_out, K) / np.sqrt(K)).astype(np.float32)).cuda()
-        planes = [torch.empty_like(a, dtype=torch.float16) for _ in range(2)] + [torch.empty_like(b, dtype=torch.float16) for _ in range(2)]
-        assert lib.opb_debug_split(a.data_ptr(), planes[0].data_ptr(), planes[1].data_ptr(), a.numel(), None) == 0
-        assert lib.opb_debug_split(b.data_ptr(), planes[2].data_ptr(), planes[3].data_ptr(), b.numel(), None) == 0
-        outs = []
-        for backend in (0, 1):
-            c = torch.zeros(rows, n_out, dtype=torch.float32, device="cuda")
-            rc = lib.opb_debug_gemm(*(p.data_ptr() for p in planes), c.data_ptr(), rows, n_out, K, backend, None)
-            assert rc == 0, (backend, rc)
-            torch.cuda.synchronize()
-            outs.append(c.cpu().double())
-        ah = (planes[0].cpu().double() + planes[1].cpu().double()) / 64.0
-        bh = (planes[2].cpu().double() + planes[3].cpu().double()) / 64.0
-        ref = ah @ bh.T
-        scale = float(ref.abs().max())
-        e_tc = float((outs[0] - ref).abs().max()) / scale
-        e_simt = float((outs[1] - ref).abs().max()) / scale
-        print(f"gemm {rows}x{n_out}x{K}: rel err wgmma {e_tc:.2e}, simt {e_simt:.2e}")
-        # the tensor core truncates (does not round) its fp32 accumulator: ~2^-25 relative per accumulation step
-        assert e_simt < 2e-6 and e_tc < 2e-6 + 1.2e-8 * K
-        # the split itself represents fp32 to ~2^-22
-        assert float((ah.float() - a.cpu()).abs().max() / a.abs().max()) < 2.0 ** -21
-
-
 def test_kv_state_row_groups_are_equivalent():
     """The linear-attention state kernel with 1, 2 and 5 slabs per row group: the per-segment sums agree to fp32 rounding."""
     lib = _lib.load()

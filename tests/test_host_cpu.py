@@ -1,5 +1,6 @@
 """CPU-side checks: the C-ABI library loads and exports every declared symbol, the module is
 state-dict compatible with the reference, host logic that needs no GPU."""
+import ctypes as C
 import json
 import os
 import re
@@ -30,7 +31,7 @@ def test_header_is_plain_c(tmp_path):
     if shutil.which("gcc") is None:
         pytest.skip("no gcc")
     src = tmp_path / "hdr.c"
-    src.write_text('#include "onepose_b200.h"\nint main(void) { opb_config c; (void)c; return 0; }\n')
+    src.write_text('#include "onepose_b200.h"\nint main(void) { opb_config c; opb_debug_gemm_desc d; (void)c; (void)d; return 0; }\n')
     inc = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "include")
     r = subprocess.run(["gcc", "-std=c99", "-Wall", "-Wextra", "-pedantic", "-Werror", "-fsyntax-only", "-I", inc, str(src)], capture_output=True, text=True)
     assert r.returncode == 0, r.stderr
@@ -41,6 +42,31 @@ def test_config_struct_matches_header():
     body = re.search(r"typedef struct opb_config \{(.*?)\} opb_config;", header, re.S).group(1)
     fields = re.findall(r"(?:int32_t|float)\s+(\w+);", body)
     assert fields == [f[0] for f in _lib.OpbConfig._fields_]
+
+
+def test_debug_gemm_desc_matches_header(tmp_path):
+    """opb_debug_gemm_desc: the ctypes Structure has the header's fields in the header's order, and (with gcc) the same size and
+    field offsets as the C compiler gives the struct."""
+    import shutil
+    import subprocess
+    header = open(os.path.join(ROOT, "include", "onepose_b200.h")).read()
+    body = re.search(r"typedef struct opb_debug_gemm_desc \{(.*?)\} opb_debug_gemm_desc;", header, re.S).group(1)
+    body = re.sub(r"/\*.*?\*/", "", body, flags=re.S)
+    fields = re.findall(r"(?:const\s+)?(?:int32_t|int64_t|uint64_t|float|void)\s*\**\s*(\w+)(?:\[\d+\])?;", body)
+    py = [f[0] for f in _lib.OpbDebugGemmDesc._fields_]
+    assert fields == py
+    if shutil.which("gcc") is None:
+        pytest.skip("no gcc")
+    src = tmp_path / "desc.c"
+    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "onepose_b200.h"\nint main(void) {\n'
+                   '  printf("%zu\\n", sizeof(opb_debug_gemm_desc));\n' +
+                   "".join(f'  printf("%zu\\n", offsetof(opb_debug_gemm_desc, {f}));\n' for f in py) + "  return 0;\n}\n")
+    exe = tmp_path / "desc"
+    r = subprocess.run(["gcc", "-std=c99", "-I", os.path.join(ROOT, "include"), str(src), "-o", str(exe)], capture_output=True, text=True)
+    assert r.returncode == 0, r.stderr
+    got = [int(v) for v in subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.split()]
+    D = _lib.OpbDebugGemmDesc
+    assert got == [C.sizeof(D)] + [getattr(D, f).offset for f in py]
 
 
 def test_no_gpu_fails_loudly():

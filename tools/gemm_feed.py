@@ -11,8 +11,7 @@
 (b) the mlp.3-shaped GEMM (converter variant: A = ReLU(IN(hid)) formed from raw fp32 in the core, plus the identity K-block)
     at rows = 262144 (32 frames of 1024 + 7168 rows), n_out = 256 and K1 = 256 / 512 / 768 / 1024, with the identity block as
     N = 64 diagonal MMAs and at full width.  The same line fit; the slope counts the three passes of the K1 part only, the
-    identity block is in the intercept.  tools/gemm_feed_mlp3.cu is compiled with nvcc into a temporary directory and
-    linked against the library build being measured.
+    identity block is in the intercept.  Both (a) and (b) go through opb_debug_gemm's problem descriptor.
 (c) the benchmarked call (match_frames, B = 32, N2D = 1024, N3D = 7000) with the profiling hook on, with the identity block
     in both forms: ms per step and share of the step for every GEMM and the large helper kernels.
 
@@ -21,11 +20,9 @@
 from __future__ import annotations
 
 import argparse
-import ctypes
 import os
 import subprocess
 import sys
-import tempfile
 
 import numpy as np
 import torch
@@ -77,6 +74,7 @@ def time_launches(launch, window):
 
 
 def gemm_slope(lib, window):
+    from onepose_b200 import _lib
     dev = torch.device("cuda")
     sms = torch.cuda.get_device_properties(dev).multi_processor_count
     kmax = max(KS)
@@ -89,10 +87,11 @@ def gemm_slope(lib, window):
         # K-major planes of width K: the first K columns of contiguous copies
         ak = [x[:, :K].contiguous() for x in a]
         bk = [x[:, :K].contiguous() for x in b]
-        args = [t.data_ptr() for t in ak + bk] + [c.data_ptr(), ROWS, N_OUT, K, 0, None]
+        desc = _lib.gemm_desc(epi=_lib.EPI_F32, rows=ROWS, n_out=N_OUT, K1=K, a1_hi=ak[0], a1_lo=ak[1], a1_ld=K,
+                              b1_hi=bk[0], b1_lo=bk[1], b1_ld=K, c=c, ldc=N_OUT)
 
         def launch():
-            rc = lib.opb_debug_gemm(*args)
+            rc = lib.opb_debug_gemm(desc, None)
             if rc != 0:
                 raise RuntimeError(f"opb_debug_gemm rc={rc}")
 
@@ -118,25 +117,8 @@ def gemm_slope(lib, window):
             "points": [{"K": K, "ms": ms} for K, ms, _ in rows]}
 
 
-def mlp3_launcher(lib_path):
-    """Build tools/gemm_feed_mlp3.cu against the library at lib_path (already loaded) and return its feed_mlp3."""
-    from onepose_b200 import build
-    tmp = tempfile.mkdtemp(prefix="gemm_feed_")
-    so = os.path.join(tmp, "feed_mlp3.so")
-    cmd = [build._nvcc(), "-std=c++17", "-Xcompiler", "-fPIC", "-shared", "-I", build.CSRC,
-           os.path.join(ROOT, "tools", "gemm_feed_mlp3.cu"), lib_path, "-o", so]
-    res = subprocess.run(cmd, capture_output=True, text=True)
-    if res.returncode != 0:
-        raise RuntimeError("nvcc failed:\n" + " ".join(cmd) + "\n" + res.stdout + res.stderr)
-    fn = ctypes.CDLL(so).feed_mlp3
-    fn.restype = ctypes.c_int
-    P, I = ctypes.c_void_p, ctypes.c_int
-    fn.argtypes = [P, I] + [P] * 11 + [I, I, I, I, P]
-    return fn
-
-
-def mlp3_slope(lib_path, window):
-    feed = mlp3_launcher(lib_path)
+def mlp3_slope(lib, window):
+    from onepose_b200 import _lib
     dev = torch.device("cuda")
     rows = MLP3_FRAMES * (MLP3_NPAD + MLP3_MPAD)
     segs = 2 * MLP3_FRAMES
@@ -153,14 +135,16 @@ def mlp3_slope(lib_path, window):
         for K1 in MLP3_K1S:
             hid = torch.randn(rows, K1, device=dev, generator=g)
             w1 = planes(256, K1)
-            args = [hid.data_ptr(), K1, w1[0].data_ptr(), w1[1].data_ptr(), x[0].data_ptr(), x[1].data_ptr(), out[0].data_ptr(),
-                    out[1].data_ptr(), eye[0].data_ptr(), eye[1].data_ptr(), bias.data_ptr(), mu.data_ptr(), rstd.data_ptr(),
-                    MLP3_FRAMES, MLP3_NPAD, MLP3_MPAD, diag, None]
+            # every row valid: frames of n_pad + m_pad rows with N = n_pad, M = m_pad
+            desc = _lib.gemm_desc(epi=_lib.EPI_BIAS_PLANES, rows=rows, n_out=256, K1=K1, K2=256, b1_hi=w1[0], b1_lo=w1[1], b1_ld=K1,
+                                  a2_hi=x[0], a2_lo=x[1], a2_ld=256, b2_hi=eye[0], b2_lo=eye[1], b2_ld=256, b2_mode=3 if diag else 2,
+                                  a_raw=hid, a_raw_ld=K1, mu=mu, rstd=rstd, B=MLP3_FRAMES, N=MLP3_NPAD, M=MLP3_MPAD,
+                                  n_pad=MLP3_NPAD, m_pad=MLP3_MPAD, bias=bias, out_hi=out[0], out_lo=out[1], out_ld=256)
 
             def launch():
-                rc = feed(*args)
+                rc = lib.opb_debug_gemm(desc, None)
                 if rc != 0:
-                    raise RuntimeError(f"feed_mlp3 rc={rc}")
+                    raise RuntimeError(f"opb_debug_gemm (mlp.3) rc={rc}")
 
             pts.append((K1,) + time_launches(launch, window))
             del hid, w1
@@ -237,7 +221,7 @@ def main():
     print("card:", card(), "| library:", _lib.LIB_PATH)
     gemm_slope(lib, args.window)
     if not args.no_mlp3:
-        mlp3_slope(_lib.LIB_PATH, args.window)
+        mlp3_slope(lib, args.window)
     if not args.no_step:
         for identity_diag in (1, 0):
             step_profile(identity_diag)
