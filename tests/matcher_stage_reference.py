@@ -494,13 +494,17 @@ def conf_rel_bar(cos, scale):
     return 2 * COS_ERR / scale + 2 * np.log(2.0) * dt + 2 * 2.0 ** -22 + 3 * 2.0 ** -24
 
 
+CONF_ABS = 2.0 ** -148      # below fp32's normal range each of the three products rounds to 2^-150 absolute (factors <= 1)
+
+
 def bar_conf(dev, cos, irs, ics, scale):
-    """One frame's conf [N_b, M_b] (fp32) against (e . irs)(e . ics) entry by entry (conf_rel_bar); inf when an entry is not
-    finite."""
+    """One frame's conf [N_b, M_b] (fp32) against (e . irs)(e . ics) entry by entry (conf_rel_bar, plus CONF_ABS: at scales below
+    ~0.05 the smallest entries fall below 2^-126, where fp32 keeps an absolute, not a relative, precision); inf when an entry is
+    not finite."""
     if not bool(torch.isfinite(dev).all()):
         return float("inf")
     ref = conf_entries(torch.exp((cos - 1.0) / scale), irs, ics)
-    return _ratio((dev.double() - ref).abs(), conf_rel_bar(cos, scale) * ref)
+    return _ratio((dev.double() - ref).abs(), conf_rel_bar(cos, scale) * ref + CONF_ABS)
 
 
 def first_max_mismatches(idx, val, conf, dim):
@@ -525,12 +529,18 @@ def unpack_best(packed):
     return idx, val.double()
 
 
-def argmax_mismatches(dev_idx, conf, dim):
-    """Arg-maxes of conf along `dim` that differ from dev_idx where the fp64 top-1 / top-2 gap exceeds 1e-5 relative."""
+def decided_gap(scale):
+    """Relative top-1 / top-2 gap above which an arg-max is decided: 1e-5 at scale >= 0.07, growing as 0.07 / scale below it
+    (the cos error enters conf amplified by 1 / scale)."""
+    return 1e-5 * max(1.0, 0.07 / scale)
+
+
+def argmax_mismatches(dev_idx, conf, dim, gap=1e-5):
+    """Arg-maxes of conf along `dim` that differ from dev_idx where the fp64 top-1 / top-2 gap exceeds `gap` relative."""
     if conf.shape[dim] < 2:
         decided = torch.ones(conf.shape[1 - dim], dtype=torch.bool, device=conf.device)
     else:
         top2 = conf.topk(2, dim=dim).values
         t0, t1 = (top2[:, 0], top2[:, 1]) if dim == 1 else (top2[0], top2[1])
-        decided = (t0 - t1) > 1e-5 * t0
+        decided = (t0 - t1) > gap * t0
     return int(((dev_idx != conf.argmax(dim)) & decided).sum())

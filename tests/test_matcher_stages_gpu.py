@@ -16,9 +16,10 @@ fp32 semantics):
   X after GATs  1e-5 of the row's max (the rows before W with with_linear_transform likewise); pad rows exactly 0
   pn            unit rows to 1e-6, elements within 1e-5
   inverse sums  1e-5 + 48 x 2^-23 / scale relative (the score GEMM's fp32 accumulation, amplified by 1 / scale)
-  arg-max       equal wherever the fp64 top-1 / top-2 gap exceeds 1e-5 relative
+  arg-max       equal wherever the fp64 top-1 / top-2 gap exceeds 1e-5 relative (x 0.07 / scale below scale 0.07)
   conf          per entry against (e . irs)(e . ics) with the device's own inverse sums: 2 x 48 x 2^-23 / scale + the fp32
-                argument of ex2, ex2.approx and the three products (ref.conf_rel_bar); every entry finite
+                argument of ex2, ex2.approx and the three products (ref.conf_rel_bar), + 2^-148 absolute below fp32's normal
+                range; every entry finite
 Exact checks: the query rows of X as the device first holds them equal the fp16-split value of the caller's queries (zero past
 each frame's length); with hoisting, X entering layer 2 equals the query pass's output and each frame's object prologue output
 bit for bit; the packed arg-maxes are the first maxima of the device's own conf; matches and scores equal `mutual` of the
@@ -213,7 +214,8 @@ class Stages:
             irs_ref[b, :n], ics_ref[b, :mm] = 1.0 / rs, 1.0 / cs
             conf64 = e * e / rs[:, None] / cs[None, :]
             del e
-            bad_argmax += ref.argmax_mismatches(i0[b, :n], conf64, 1) + ref.argmax_mismatches(i1[b, :mm], conf64, 0)
+            gap = ref.decided_gap(scale)
+            bad_argmax += ref.argmax_mismatches(i0[b, :n], conf64, 1, gap) + ref.argmax_mismatches(i1[b, :mm], conf64, 0, gap)
             del conf64
             c = conf[:n, :mm]
             conf_worst = max(conf_worst, ref.bar_conf(c, cos, irs[b, :n], ics[b, :mm], scale))
