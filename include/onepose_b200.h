@@ -277,6 +277,61 @@ int opb_gather_matches_objects(const int64_t* matches0, const float* mscores0, c
                                const int32_t* kp3_first, const int32_t* kp3_count, int32_t B, int32_t N, double* pts2d, double* pts3d,
                                float* mconf, int32_t* query_index, int32_t* offsets, void* stream);
 
+/* ---- between one frame's pose and the next frame's extractor input: the pose-guided crop ----
+ * The reference's live loop (inference_demo.py:193-247) crops every frame after the first around the object's box under the
+ * previous pose: previous_pose_detect (src/local_feature_2D_detector/local_feature_2D_detector.py:232-259), host numpy +
+ * cv2.warpAffine.  The three calls below do it for B frames on the caller's current device and stream: device pointers,
+ * asynchronous, no host synchronisation, no allocation; OPB_E_INVALID for null or non-positive arguments.  B <= 65535.
+ *
+ * Box of the object's 3D bounding-box corners under a pose; replaces reproj (src/utils/vis_utils.py:209-236) and
+ * local_feature_2D_detector.py:246-249 (min / max over the corners, astype(np.int32)).
+ *   K        device f64 [B, 9]             row-major camera matrices
+ *   pose     device f64 [B, 12]            row-major [R | t], the pose_out layout of opb_ransac_*
+ *   corners  device f64 [B, n_corners, 3]  (8 in the reference; any n_corners > 0)
+ *   proj     device f64 [B, n_corners, 2]  out, or NULL: the projections, reproj's result
+ *   box      device int32 [B, 4]           out: [x0, y0, x1, y1]
+ * Per frame, in fp64 with every product and sum rounded on its own and summed in index order: (K @ pose) @ [X; 1], the
+ * division by the third row, min / max, then C truncation towards zero (numpy's cast).  A corner behind the camera projects
+ * as it does in numpy.  A non-finite extreme or one outside int32, where numpy's cast is undefined, gives the empty box
+ * [0, 0, 0, 0], which opb_crop_resize rejects. */
+int opb_boxes_from_poses(const double* K, const double* pose, const double* corners, int32_t B, int32_t n_corners, double* proj,
+                         int32_t* box, void* stream);
+/* crop_img_by_bbox (local_feature_2D_detector.py:160-186) and the `/ 255` of :255-257: the two chained get_image_crop_resize and
+ * get_K_crop_resize calls (src/utils/data_utils.py:233-272), box -> an image of the box's own size -> crop_size x crop_size.
+ *   frames      device uint8 [B, H, W]  full grey camera frames; frame b starts at frames + b * frame_pitch, its row y at
+ *               + y * row_pitch (bytes; row_pitch >= W); H, W <= 32767
+ *   box         device int32 [B, 4]     [x0, y0, x1, y1]
+ *   K           device f64 [B, 9]
+ *   crop_size   S > 0, S % 8 == 0 (the extractor's condition; 512 in the reference)
+ *   image       device fp32 [B, 1, S, S] out: the `images` argument of opb_sp_forward
+ *   K_crop      device f64 [B, 9] out:   T2_homo @ [ (T1_homo @ [K | 0])[:3, :3] | 0 ], fp64, products summed in index order
+ *   trans       device f64 [B, 2, 6] out: T1 and T2, row-major 2x3 (T2 . T1 maps a frame position into the crop)
+ *   status      device int32 [B] out:    1, or 0 for a rejected box
+ * A box is rejected when x1 <= x0 or y1 <= y0 (the reference raises inside cv2 there), when a side exceeds 32767 or a
+ * coordinate 2^20 in magnitude (cv2 addresses source pixels by int16 and positions in 22.10 fixed point): status 0, a zero
+ * image, zero transforms and K_crop = K.  A zero image yields no key points, hence the identity pose and 0 inliers from
+ * opb_ransac_*: the failure reaches the caller through n_inliers, the signal inference_demo.py:206 uses.
+ * Arithmetic (bit-exact against OpenCV 4.13; the model is tests/crop_reference.py):
+ *   transforms  get_affine_transform (data_utils.py:24-57, rot = 0): three float32 point pairs -- the centre, the point half
+ *               the WIDTH above it, get_3rd_point of the two -- then cv2.getAffineTransform's 6x6 system solved in fp64 by LU
+ *               with partial pivoting in OpenCV's elimination order, no fused multiply-add.  Both axes scale by dst_w / src_w:
+ *               the reference's crop is not an anisotropic resize.
+ *   pixels      cv2.warpAffine(INTER_LINEAR, constant border 0) on 8-bit data: the matrix inverted in fp64 as warpAffine does,
+ *               source positions rint((M . (x, y, 1)) * 1024) (round half to even) reduced to 1/32, the pixel index
+ *               saturated to int16, four int16 weights rint(w * 32768) per 1/32 x 1/32 fraction, pixel = (sum + 16384) >> 15.
+ *               Each output pixel evaluates the 4 first-stage pixels it needs (rounded to uint8, zero outside the first-stage
+ *               image) from 16 frame reads; no intermediate image.  The result is the uint8 value / 255 in fp32 (numpy's). */
+int opb_crop_resize(const uint8_t* frames, int64_t frame_pitch, int64_t row_pitch, int32_t B, int32_t H, int32_t W, const int32_t* box,
+                    const double* K, int32_t crop_size, float* image, double* K_crop, double* trans, int32_t* status, void* stream);
+/* One get_image_crop_resize / get_K_crop_resize (data_utils.py:233-272): box -> [out_h, out_w] by one warp -- the pixel and
+ * transform routines opb_crop_resize runs twice.  frames, pitches, box as there; out_h, out_w <= 32767.
+ *   out     device uint8 [B, out_h, out_w] out: cv2.warpAffine's image.  frames and out may both be NULL: transforms only
+ *   trans   device f64 [B, 6] out: trans_crop, row-major 2x3
+ *   K, K_crop  device f64 [B, 9] in / out: trans_crop_homo @ K, or both NULL
+ * A rejected box (as for opb_crop_resize) gives a zero image, a zero transform and K_crop = K. */
+int opb_warp_crop_u8(const uint8_t* frames, int64_t frame_pitch, int64_t row_pitch, int32_t B, int32_t H, int32_t W, const int32_t* box,
+                     const double* K, int32_t out_h, int32_t out_w, uint8_t* out, double* trans, double* K_crop, void* stream);
+
 /* ---- adjacent producer: SuperPoint key-point extractor (SURVEY 8f N4) ----
  * Replaces SuperPoint.forward (reference src/models/extractors/SuperPoint/superpoint.py:140-197): shared VGG-style encoder
  * (:142-152), score head + 65-way softmax + 8x8 pixel shuffle (:155-160), simple_nms (:47-61, :161), threshold / border /
