@@ -332,6 +332,61 @@ int opb_crop_resize(const uint8_t* frames, int64_t frame_pitch, int64_t row_pitc
 int opb_warp_crop_u8(const uint8_t* frames, int64_t frame_pitch, int64_t row_pitch, int32_t B, int32_t H, int32_t W, const int32_t* box,
                      const double* K, int32_t out_h, int32_t out_w, uint8_t* out, double* trans, double* K_crop, void* stream);
 
+/* ---- the first frame, and every frame after a lost pose: detection by 2D-2D matching against reference views ----
+ * LocalFeatureObjectDetector.detect (local_feature_2D_detector.py:76-147, 196-230) between the caller's 2D-2D matcher and the
+ * crop above: each reference view's matches, cv2.estimateAffinePartial2D on the view with the most, the box of its corners.
+ * Caller's current device and stream, device pointers, asynchronous, no host synchronisation, no allocation.
+ *
+ * cv2.estimateAffinePartial2D(from, to, method=RANSAC, threshold, max_iters, confidence, refine_iters) for B independent
+ * problems; problem b is pairs offsets[b] .. offsets[b+1] - 1.
+ *   from, to      device fp32 [sum n, 2]   the point pairs (cv2 converts its input to fp32 too)
+ *   offsets       device int32 [B + 1]
+ *   threshold     ransacReprojThreshold (finite); max_iters >= 0; 0 < confidence < 1; refine_iters >= 0
+ *   affine        device f64 [B, 6] out    row-major 2x3 [a -b tx; b a ty]; zeros where cv2 returns None
+ *   inlier_mask   device uint8 [sum n] out, or NULL: cv2's inlier mask (all zeros where it returns None)
+ *   iterations    device int32 [B] out     iterations of the RANSAC loop (0 for n <= 2)
+ *   status        device int32 [B] out     1: a model, 0: none (cv2's None)
+ * OpenCV's algorithm stage for stage (OpenCV 4.13; the model is tests/affine_ransac_reference.py): n < 2 has no model, n == 2
+ * is the one 2-pair model with both pairs inliers (it may be non-finite, as cv2's is); otherwise the samples of
+ * cv::RNG((uint64)-1) by getSubset (2 distinct indices), each one's closed-form similarity in fp64 from the fp32 points, the
+ * fp32 error ((F0 x + F1 y) + F2 - X)^2 + (...)^2 with the model rounded to fp32, against (float)(threshold^2), every operation
+ * rounded on its own; a sample wins when its count exceeds max(best, 1), and each win lowers the budget to
+ * RANSACUpdateNumIters(confidence, outlier ratio, 2, budget).  The winner's inliers are refined by OpenCV's Levenberg-Marquardt
+ * on (a, b, tx, ty) for at most refine_iters accepted steps (fp64, reductions in a fixed order).  The samples, counts, mask and
+ * the unrefined model are cv2's bit for bit; the refined model agrees to rounding.  Results do not depend on the launch. */
+int opb_estimate_affine_partial(const float* from, const float* to, const int32_t* offsets, int32_t B, double threshold, int32_t max_iters,
+                                double confidence, int32_t refine_iters, double* affine, uint8_t* inlier_mask, int32_t* iterations,
+                                int32_t* status, void* stream);
+/* match_worker + detect_by_matching (local_feature_2D_detector.py:76-147) for B frames against V reference views.
+ *   ref_keypoints    device fp32 [V, cap_ref, 2]  the views' key points (x, y); cap_ref <= 8192
+ *   ref_counts       device int32 [V]             key points of view v (entries past it are ignored)
+ *   ref_sizes        device int32 [V, 2]          the view's image (H, W)
+ *   query_keypoints  device fp32 [B, cap_query, 2], query_counts device int32 [B]
+ *   matches0         device int32 or int64 (matches_int64 = 1) [B, V, cap_ref]: the matcher's matches0 of frame b against
+ *                    view v; entry i is a match iff 0 <= m < query_counts[b]
+ *   query_h, query_w the frames' size.  1 <= V <= 256.
+ *   box              device int32 [B, 4] out     [x0, y0, x1, y1], the input of opb_crop_resize
+ *   view             device int32 [B] out        the chosen view;  n_matches  device int32 [B] out  its match count
+ *   affine           device f64 [B, 6] out       its cv2.estimateAffinePartial2D(ref, query, ransacReprojThreshold=6) model
+ *   status           device int32 [B] out        1: the box of the affine; 2: no view has 6 matches, the box is
+ *                                                [0, 0, query_h, query_w]; 0: the empty box (see below)
+ * Per frame: the views with at least 6 matches compete on their match count, the first view wins a tie (Python's stable sort
+ * on inliers.shape[0], which is the match count); no such view: the first view's [0, 0, size[0], size[1]] box, i.e. x1 = H and
+ * y1 = W as the reference writes it.  The winner's pairs, in ascending reference key-point order, go through the estimator
+ * above with the reference's arguments (threshold 6, 2000 iterations, confidence 0.99, 10 refinement steps); its model maps
+ * the view's corners (0, 0), (W, 0), (0, H), (W, H) in fp64 (products summed in index order), truncated to int32, then min /
+ * max.  The empty box [0, 0, 0, 0], which opb_crop_resize rejects, where the reference fails: the estimator finds no model
+ * (the reference raises a TypeError), or a corner is non-finite or outside int32 (numpy's cast is undefined).  The trace of
+ * opb_debug_set_affine_trace records the winning view's loop. */
+int opb_boxes_from_matches(const float* ref_keypoints, const int32_t* ref_counts, const int32_t* ref_sizes, int32_t V, int32_t cap_ref,
+                           const float* query_keypoints, const int32_t* query_counts, int32_t cap_query, const void* matches0,
+                           int32_t matches_int64, int32_t B, int32_t query_h, int32_t query_w, int32_t* box, int32_t* view,
+                           int32_t* n_matches, double* affine, int32_t* status, void* stream);
+/* Test hook of both calls above: device buffers later calls fill (NULL to stop), per problem b and for every sample i <
+ * capacity the loop evaluates: samples int32 [B][capacity][2], counts int32 [B][capacity], models f64 [B][capacity][6] (the
+ * unrefined 2-pair model, row-major 2x3). */
+int opb_debug_set_affine_trace(int32_t* samples, int32_t* counts, double* models, int32_t capacity);
+
 /* ---- adjacent producer: SuperPoint key-point extractor (SURVEY 8f N4) ----
  * Replaces SuperPoint.forward (reference src/models/extractors/SuperPoint/superpoint.py:140-197): shared VGG-style encoder
  * (:142-152), score head + 65-way softmax + 8x8 pixel shuffle (:155-160), simple_nms (:47-61, :161), threshold / border /

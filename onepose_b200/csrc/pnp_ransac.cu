@@ -19,6 +19,7 @@
 #include <stdint.h>
 
 #include "../../include/onepose_b200.h"
+#include "cv_rng.cuh"
 
 namespace opb {
 namespace {
@@ -1056,7 +1057,6 @@ __global__ void __launch_bounds__(kEpnpThreads) epnp_select_refit(const double* 
 //   cv_scan (wave w)   per frame, in sample order: the loop's bookkeeping, then wave w+1's samples unless the loop ended;
 //   cv_select_refit    the winner's inlier set as the mask, EPnP on it.
 // A frame whose loop ended skips every later launch at its first instruction.
-constexpr unsigned kMwcA = 4164903690u;                // cv::RNG's multiplier (CV_RNG_COEFF)
 constexpr int kCvModelPoints = 5;
 constexpr int kCvScanThreads = 32;
 
@@ -1071,62 +1071,6 @@ struct CvState {                                       // per frame, 16 doubles 
   int pad;
 };
 static_assert(sizeof(CvState) == 16 * sizeof(double), "CvState is 16 doubles");
-
-__device__ __forceinline__ unsigned mwc_next(unsigned long long& s) {   // cv::RNG::next
-  s = (unsigned long long)(unsigned)s * kMwcA + (s >> 32);
-  return (unsigned)s;
-}
-
-// x % n for 32-bit x by a 64-bit reciprocal m = 2^64 / n rounded up (Lemire, Kaser, Kurz 2019): exact for every 32-bit x, n
-__device__ __forceinline__ unsigned fast_mod(unsigned x, unsigned long long m, unsigned n) { return (unsigned)__umul64hi(m * x, n); }
-__host__ __device__ __forceinline__ unsigned long long fast_mod_m(unsigned n) { return ~0ull / n + 1; }
-
-// five draws uniform(0, n) from state t (advanced) into v; true when they are distinct
-__device__ __forceinline__ bool draw5(unsigned long long& t, unsigned long long m, unsigned n, int* v) {
-#pragma unroll
-  for (int k = 0; k < kCvModelPoints; ++k) v[k] = (int)fast_mod(mwc_next(t), m, n);
-  bool distinct = true;
-#pragma unroll
-  for (int a = 0; a < kCvModelPoints; ++a)
-#pragma unroll
-    for (int c = a + 1; c < kCvModelPoints; ++c) distinct &= v[a] != v[c];
-  return distinct;
-}
-
-// getSubset with the default checkSubset: five indices uniform(0, n), an index repeating an earlier one of the sample redrawn.
-// Five distinct draws in a row (the common case for large n) take one branch-free pass.
-__device__ __forceinline__ void cv_subset(unsigned long long& s, unsigned n, unsigned long long m, int* idx) {
-  unsigned long long t = s;
-  int v[kCvModelPoints];
-  if (draw5(t, m, n, v)) {
-    s = t;
-#pragma unroll
-    for (int k = 0; k < kCvModelPoints; ++k) idx[k] = v[k];
-    return;
-  }
-  for (int i = 0; i < kCvModelPoints; ++i) {
-    int u;
-    bool rep;
-    do {
-      u = (int)fast_mod(mwc_next(s), m, n);
-      rep = false;
-      for (int e = 0; e < i; ++e) rep |= idx[e] == u;
-    } while (rep);
-    idx[i] = u;
-  }
-}
-
-// RANSACUpdateNumIters: clamps, DBL_MIN guards and cvRound (round half to even) as OpenCV has them
-__device__ int cv_update_num_iters(double p, double ep, int model_points, int max_iters) {
-  p = fmin(fmax(p, 0.0), 1.0);
-  ep = fmin(fmax(ep, 0.0), 1.0);
-  double num = fmax(1.0 - p, DBL_MIN);
-  double denom = 1.0 - pow(1.0 - ep, (double)model_points);
-  if (denom < DBL_MIN) return 0;
-  num = log(num);
-  denom = log(denom);
-  return denom >= 0.0 || -num >= max_iters * (-denom) ? max_iters : __double2int_rn(num / denom);
-}
 
 // PnPRansacCallback::computeError of one fp32-rounded pair: projectPoints in fp64 (x * (1/z), then * f + c; OpenCV's
 // distortion and tilt terms are exact no-ops for zero coefficients) rounded to fp32, the squared distance in fp32.  Explicit
@@ -1143,69 +1087,13 @@ __device__ __forceinline__ float cv_error(const Pose& T, const double* Kc, const
   return __fadd_rn(__fmul_rn(du, du), __fmul_rn(dv, dv));
 }
 
-constexpr unsigned long long kMwcM = (unsigned long long)kMwcA * 4294967296ull - 1ull;   // the LCG modulus of the MWC
-
-__device__ __forceinline__ unsigned long long mwc_mulmod(unsigned long long x, unsigned long long y) {
-  return (unsigned long long)(((unsigned __int128)x * y) % kMwcM);
-}
-
-// `count` consecutive samples from generator state s (updated), by one warp: every lane calls with the same arguments.
-// The MWC step is state -> state * kMwcA mod kMwcM on residues, so lane l jumps 5 l steps ahead and draws the five indices a
-// sample takes when it needs no redraw; the samples before the first lane that saw a repeat are OpenCV's, and that lane's
-// sample is drawn serially (with its redraws) before the next 32.  fresh: s is the start state 2^64 - 1, which, like the
-// state after it, lies above the modulus (its low word is not its residue's): the first sample is drawn serially.
-// Sample h goes to dst[h * stride .. + 4] (and trace[(trace_first + h) * 5 ..] while below trace_cap).
-__device__ void warp_draw(unsigned long long& s, bool fresh, unsigned n, int count, int* dst, int stride, int* trace, int trace_first,
-                          int trace_cap) {
-  const int lane = threadIdx.x & 31;
-  const unsigned long long m = fast_mod_m(n);
-  auto put = [&](int h, const int* idx) {
-    for (int k = 0; k < kCvModelPoints; ++k) dst[(size_t)h * stride + k] = idx[k];
-    if (trace && trace_first + h < trace_cap)
-      for (int k = 0; k < kCvModelPoints; ++k) trace[(size_t)(trace_first + h) * kCvModelPoints + k] = idx[k];
-  };
-  int h = 0;
-  if (fresh && count > 0) {
-    int idx[kCvModelPoints];
-    cv_subset(s, n, m, idx);
-    if (lane == 0) put(0, idx);
-    h = 1;
-  }
-  unsigned long long jump = 1, sq = kMwcA;             // kMwcA^(5 lane) mod kMwcM
-  for (int e = kCvModelPoints * lane; e; e >>= 1) {
-    if (e & 1) jump = mwc_mulmod(jump, sq);
-    sq = mwc_mulmod(sq, sq);
-  }
-  while (h < count) {
-    const unsigned long long start = mwc_mulmod(s, jump);
-    unsigned long long t = start;
-    int v[kCvModelPoints];
-    const bool distinct = draw5(t, m, n, v);
-    const int avail = min(32, count - h);
-    const unsigned bad = __ballot_sync(0xffffffffu, lane < avail && !distinct);
-    const int k = bad ? __ffs(bad) - 1 : avail;
-    if (lane < k) put(h + lane, v);
-    if (k == avail) {
-      s = __shfl_sync(0xffffffffu, t, k - 1);
-      h += k;
-    } else {
-      unsigned long long u = __shfl_sync(0xffffffffu, start, k);
-      int idx[kCvModelPoints];
-      cv_subset(u, n, m, idx);
-      if (lane == 0) put(h + k, idx);
-      s = u;
-      h += k + 1;
-    }
-  }
-}
-
 // samples first .. first + W - 1 of frame b, those below its budget niters, into the wave's records (one warp).  Every lane
 // passes its own copy of the budget: lane 0's store to S.niters need not be what the other lanes read back.
 __device__ void draw_wave(CvState& S, double* r, int n, int W, int first, int niters, int b, int* trace_samples, int trace_cap) {
   const int count = min(W, niters - first);
   unsigned long long s = S.rng;
   if (count > 0)
-    warp_draw(s, first == 0, (unsigned)n, count, reinterpret_cast<int*>(r), kHypStride * 2, trace_samples + (trace_samples ? (size_t)b * trace_cap * kCvModelPoints : 0),
+    cvrng::warp_draw<kCvModelPoints>(s, first == 0, (unsigned)n, count, reinterpret_cast<int*>(r), kHypStride * 2, trace_samples + (trace_samples ? (size_t)b * trace_cap * kCvModelPoints : 0),
               first, trace_cap);
   if ((threadIdx.x & 31) == 0) S.rng = s;
 }
@@ -1239,7 +1127,7 @@ __global__ void __launch_bounds__(kCvScanThreads) epnp_cv_scan(const int* __rest
           best = ce;
           winner = i;
           if (lane == 0) S.pose = load_record(r + (size_t)(h0 + e) * kHypStride);
-          niters = cv_update_num_iters(confidence, (double)(n - ce) / n, kCvModelPoints, niters);
+          niters = cvrng::update_num_iters(confidence, (double)(n - ce) / n, kCvModelPoints, niters);
         }
         if (i + 1 >= niters) { done = 1; iter = i + 1; break; }
         from = e + 1;
@@ -1358,7 +1246,7 @@ __global__ void __launch_bounds__(kEpnpThreads) epnp_cv_select_refit(const doubl
 __global__ void epnp_cv_subsets(int n, int count, int chunk, int* __restrict__ out) {
   unsigned long long s = ~0ull;
   for (int i = 0; i < count; i += chunk)
-    warp_draw(s, i == 0, (unsigned)n, min(chunk, count - i), out + (size_t)i * kCvModelPoints, kCvModelPoints, nullptr, 0, 0);
+    cvrng::warp_draw<kCvModelPoints>(s, i == 0, (unsigned)n, min(chunk, count - i), out + (size_t)i * kCvModelPoints, kCvModelPoints, nullptr, 0, 0);
 }
 
 // ---- matched pairs -> the ragged correspondence lists above (reference inference.py:147-152: valid = matches > -1;
