@@ -23,7 +23,11 @@
  *     inputs and outputs must live there.  Every handle entry point leaves the
  *     caller's current device as it found it.
  *   - The handle-free entry points (features3d producers, RANSAC-PnP, EPnP,
- *     gather) run on the caller's current device and stream.
+ *     gather, crop, detection, test hooks) run on the caller's current device
+ *     and stream.  A call without a handle that fails -- these and the create
+ *     functions -- leaves its message in a per-thread string that
+ *     opb_last_error(NULL) and opb_sp_last_error(NULL) both return: the
+ *     message of the last failed call on this thread that had no handle.
  *   - Calls on different handles may run concurrently, from different threads;
  *     one handle is used by one thread at a time.
  */
@@ -62,7 +66,7 @@ typedef struct opb_config {
 /* Replaces GATsSuperGlue.__init__ (GATs_SuperGlue.py:145-177). */
 int opb_create(const opb_config* cfg, opb_matcher** out);
 void opb_destroy(opb_matcher* m);
-const char* opb_last_error(const opb_matcher* m); /* m may be NULL: last create error */
+const char* opb_last_error(const opb_matcher* m); /* m may be NULL: last failed call without a handle on this thread */
 
 /* Replaces nn.Module.load_state_dict for the keys of GATs_SuperGlue.py (SURVEY 2.1):
  * `name` is the reference state-dict key ("gnn.layers.1.attn.proj.0.weight", ...),
@@ -411,7 +415,7 @@ typedef struct opb_sp_config {
 
 int opb_sp_create(const opb_sp_config* cfg, opb_superpoint** out);
 void opb_sp_destroy(opb_superpoint* h);
-const char* opb_sp_last_error(const opb_superpoint* h); /* h may be NULL: last create error */
+const char* opb_sp_last_error(const opb_superpoint* h); /* h may be NULL: as opb_last_error(NULL) */
 /* Reference state-dict keys ("conv1a.weight", "conv1a.bias", ... "convDb.bias"; superpoint.py:111-126), HOST fp32 arrays in
  * the reference's own [C_out, C_in, kh, kw] layout.  opb_sp_finalize_weights packs them (tap-major reduction index, the two
  * heads' 3x3 layers side by side, fp16 hi/lo split) and uploads. */

@@ -9,6 +9,8 @@ from __future__ import annotations
 import ctypes as C
 import os
 
+import torch
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(HERE, "libonepose_b200.so")
 
@@ -166,16 +168,26 @@ class OpbError(RuntimeError):
     pass
 
 
-def check_sp(rc: int, handle=None, lib=None):
-    """Status check for the opb_sp_* (extractor) entry points."""
+def check(rc: int, handle=None, kind: str = "matcher"):
+    """Raise OpbError with the library's message unless ``rc`` is OPB_OK.  ``handle`` is the handle the call took -- a
+    matcher's, or an extractor's with ``kind="extractor"`` -- or None for a call without one."""
     if rc == OPB_OK:
         return
-    msg = (lib or load()).opb_sp_last_error(handle)
+    lib = load()
+    msg = (lib.opb_sp_last_error if kind == "extractor" else lib.opb_last_error)(handle)
     raise OpbError(f"{ERRORS.get(rc, rc)}: {msg.decode() if msg else ''}")
 
 
-def check(rc: int, handle=None):
-    if rc == OPB_OK:
-        return
-    msg = load().opb_last_error(handle)
-    raise OpbError(f"{ERRORS.get(rc, rc)}: {msg.decode() if msg else ''}")
+def cuda_device(t: torch.Tensor) -> torch.device:
+    if t.device.type != "cuda":
+        raise RuntimeError("onepose_b200 has no CPU path: tensors must be on a CUDA device")
+    return t.device
+
+
+def call(dev: torch.device, name: str, *args):
+    """Run the handle-free entry point ``name`` on device ``dev`` and its current stream, which is appended to ``args``.
+    Tensors pass as their data_ptr() and None as NULL; a failure raises OpbError with the library's message."""
+    fn = getattr(load(), name)
+    args = [a.data_ptr() if isinstance(a, torch.Tensor) else a for a in args]
+    with torch.cuda.device(dev):
+        check(fn(*args, torch.cuda.current_stream(dev).cuda_stream))

@@ -21,7 +21,6 @@ import numpy as np
 import torch
 
 from . import _lib
-from .pnp import _cuda_device
 
 MAX_SIDE = 32767        # the box sides and |coordinates| opb_crop_resize accepts (include/onepose_b200.h)
 MAX_COORD = 1 << 20
@@ -40,7 +39,7 @@ def _per_frame(t: torch.Tensor, B: int, shape: tuple, name: str, dev) -> torch.T
 
 
 def _project(K, pose, pts, want_proj: bool):
-    dev = _cuda_device(pose)
+    dev = _lib.cuda_device(pose)
     if pose.dim() != 3 or tuple(pose.shape[1:]) not in ((3, 4), (4, 4)) or not pose.dtype.is_floating_point:
         raise ValueError(f"pose must be a floating-point [B, 3, 4] or [B, 4, 4], got {pose.dtype} {list(pose.shape)}")
     B = int(pose.shape[0])
@@ -54,10 +53,7 @@ def _project(K, pose, pts, want_proj: bool):
     pose = pose[:, :3].to(torch.float64).contiguous()
     box = torch.empty(B, 4, dtype=torch.int32, device=dev)
     proj = torch.empty(B, n, 2, dtype=torch.float64, device=dev) if want_proj else None
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        _lib.check(lib.opb_boxes_from_poses(K.data_ptr(), pose.data_ptr(), pts.data_ptr(), B, n, proj.data_ptr() if want_proj else None,
-                                            box.data_ptr(), torch.cuda.current_stream(dev).cuda_stream))
+    _lib.call(dev, "opb_boxes_from_poses", K, pose, pts, B, n, proj, box)
     return box, proj
 
 
@@ -71,7 +67,7 @@ def boxes_from_poses(K: torch.Tensor, pose: torch.Tensor, bbox3d: torch.Tensor) 
 
 
 def _frames_args(frames: torch.Tensor):
-    dev = _cuda_device(frames)
+    dev = _lib.cuda_device(frames)
     if frames.dtype != torch.uint8 or frames.dim() != 3:
         raise ValueError(f"frames must be uint8 [B, H, W], got {frames.dtype} {list(frames.shape)}")
     B, H, W = (int(v) for v in frames.shape)
@@ -104,11 +100,8 @@ def crop_frames(frames: torch.Tensor, boxes: torch.Tensor, K: torch.Tensor, crop
     K = _per_frame(K, B, (3, 3), "K", dev)
     out = {"image": torch.empty(B, 1, S, S, dtype=torch.float32, device=dev), "K_crop": torch.empty(B, 3, 3, dtype=torch.float64, device=dev),
            "trans": torch.empty(B, 2, 2, 3, dtype=torch.float64, device=dev), "status": torch.empty(B, dtype=torch.int32, device=dev)}
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        _lib.check(lib.opb_crop_resize(frames.data_ptr(), frames.stride(0), frames.stride(1), B, H, W, boxes.data_ptr(), K.data_ptr(), S,
-                                       out["image"].data_ptr(), out["K_crop"].data_ptr(), out["trans"].data_ptr(), out["status"].data_ptr(),
-                                       torch.cuda.current_stream(dev).cuda_stream))
+    _lib.call(dev, "opb_crop_resize", frames, frames.stride(0), frames.stride(1), B, H, W, boxes, K, S, out["image"], out["K_crop"], out["trans"],
+              out["status"])
     return out
 
 
@@ -156,7 +149,7 @@ def _warp_crop_np(image, box, K, resize_shape, device):
         frames = torch.from_numpy(np.ascontiguousarray(image))[None].to(dev)
         _, _, H, W = _frames_args(frames)
         out = torch.empty(1, h, w, dtype=torch.uint8, device=dev)
-        fargs = (frames.data_ptr(), frames.stride(0), frames.stride(1), 1, H, W)
+        fargs = (frames, frames.stride(0), frames.stride(1), 1, H, W)
     if K is not None:
         K = np.asarray(K, dtype=np.float64)
         if K.shape != (3, 3):
@@ -165,11 +158,7 @@ def _warp_crop_np(image, box, K, resize_shape, device):
         Kc = torch.empty(3, 3, dtype=torch.float64, device=dev)
     trans = torch.empty(2, 3, dtype=torch.float64, device=dev)
     boxd = torch.from_numpy(box).to(dev)
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        _lib.check(lib.opb_warp_crop_u8(*fargs, boxd.data_ptr(), Kd.data_ptr() if K is not None else None, h, w,
-                                        out.data_ptr() if out is not None else None, trans.data_ptr(),
-                                        Kc.data_ptr() if K is not None else None, torch.cuda.current_stream(dev).cuda_stream))
+    _lib.call(dev, "opb_warp_crop_u8", *fargs, boxd, Kd, h, w, out, trans, Kc)
     return (out[0].cpu().numpy() if out is not None else None, trans.cpu().numpy(), Kc.cpu().numpy() if K is not None else None)
 
 

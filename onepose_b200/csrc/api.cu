@@ -23,7 +23,6 @@ constexpr int kDefaultChunk = 32;   // frames pushed through the GNN together (m
 constexpr int kQPassFrames = 16;    // granularity of the query-side layer-1 pass when the queries stream in from the host
 constexpr double kMinScaleFactor = 2.0 * 1.4426950408889634 / 126.0;   // ~0.0229: smallest scale_factor opb_create accepts
 
-static thread_local std::string g_create_error;
 static bool g_pdl = true;
 static int g_ws_fill = -1;     // >= 0: byte value written into every fresh allocation that the algorithm does not require to be zero
 int ws_fill_byte() { return g_ws_fill; }
@@ -421,8 +420,8 @@ static int chunk_of(const opb_matcher* m, int B) {
 // Not counted here: it also runs outside a forward (opb_set_object / opb_add_object), where it must not touch the profile of
 // the last forward; forward_frames counts it.
 static cudaError_t launch_leaf_logits(const opb_matcher* m, const ObjectState& o, cudaStream_t st) {
-  return launch_k(gats_leaf_logits, dim3(m->num_sms * 4), dim3(256), 0, st, (const float*)o.leaves.as<float>(), (long long)o.M * o.Lf,
-                  (const float*)m->wa2.as<float>(), o.s2.as<float>());
+  return launch_k(pdl_enabled(), gats_leaf_logits, dim3(m->num_sms * 4), dim3(256), 0, st, (const float*)o.leaves.as<float>(),
+                  (long long)o.M * o.Lf, (const float*)m->wa2.as<float>(), o.s2.as<float>());
 }
 
 // Upload an object's constants into `o` (buffers only grow) and compute its leaf logits; its prologue runs on first use.
@@ -437,11 +436,11 @@ static int load_object(opb_matcher* m, ObjectState& o, const float* desc3d_db, c
   CK(m, o.s2.ensure((size_t)4 * n_leaf_rows * sizeof(float)));
   CK(m, o.xo.ensure((size_t)m_pad * kD));
   if (o.leaves.grew || o.db.hi.grew || o.s2.grew || o.xo.hi.grew) CK(m, cudaDeviceSynchronize());   // frees of the old buffers vs work in flight
-  launch_k(transpose_cf_to_rows<1>, dim3((unsigned)((n_leaf_rows + 31) / 32), 1), dim3(32, 8), 0, st, desc2d_db, (int)n_leaf_rows, (int)n_leaf_rows, 0ll,
-           (const int*)nullptr, (int)n_leaf_rows, (__half*)nullptr, (__half*)nullptr, o.leaves.as<float>(), 0ll, 0);
+  launch_k(pdl_enabled(), transpose_cf_to_rows<1>, dim3((unsigned)((n_leaf_rows + 31) / 32), 1), dim3(32, 8), 0, st, desc2d_db, (int)n_leaf_rows,
+           (int)n_leaf_rows, 0ll, (const int*)nullptr, (int)n_leaf_rows, (__half*)nullptr, (__half*)nullptr, o.leaves.as<float>(), 0ll, 0);
   // rows [M, m_pad) of the object planes are written as zero by the transpose (MODE 0 pads to rows_out)
-  launch_k(transpose_cf_to_rows<0>, dim3(m_pad / 32, 1), dim3(32, 8), 0, st, desc3d_db, (int)M, (int)M, 0ll, (const int*)nullptr, m_pad,
-           o.db.hi.as<__half>(), o.db.lo.as<__half>(), (float*)nullptr, 0ll, 0);
+  launch_k(pdl_enabled(), transpose_cf_to_rows<0>, dim3(m_pad / 32, 1), dim3(32, 8), 0, st, desc3d_db, (int)M, (int)M, 0ll, (const int*)nullptr,
+           m_pad, o.db.hi.as<__half>(), o.db.lo.as<__half>(), (float*)nullptr, 0ll, 0);
   CK(m, cudaGetLastError());
   CK(m, launch_leaf_logits(m, o, st));
   o.s2_ready = true;
@@ -505,29 +504,43 @@ static int forward_frames(opb_matcher* m, ObjectState* const* fobj, const float*
   return OPB_OK;
 }
 
+// A segmented mean: the offsets (exclusive scan of seg_len) in a stream-ordered temporary, then `kern`; the temporary is freed
+// behind it whether or not the launches succeed.
+template <typename... KArgs, typename... Tail>
+static int segmented(const char* fn, const char* name, void (*kern)(KArgs...), unsigned grid, unsigned block, const double* values,
+                     const int64_t* seg_len, int32_t M, cudaStream_t st, Tail... tail) {
+  const long long* len = reinterpret_cast<const long long*>(seg_len);
+  long long* offs = nullptr;
+  CK(no_handle_error, cudaMallocAsync(&offs, (size_t)M * sizeof(long long), st));
+  int rc = launched(fn, "exclusive_scan_i64", launch_k(false, exclusive_scan_i64, 1, 1024, 0, st, len, offs, M));
+  if (rc == OPB_OK) rc = launched(fn, name, launch_k(false, kern, grid, block, 0, st, values, len, offs, M, tail...));
+  CK(no_handle_error, cudaFreeAsync(offs, st));
+  return rc;
+}
+
 }  // namespace opb
 
 // =========================================================================================
 extern "C" {
 
 int opb_create(const opb_config* cfg, opb_matcher** out) {
-  if (!cfg || !out) return fail(g_create_error, OPB_E_INVALID, "null argument");
+  if (!cfg || !out) return fail(no_handle_error, OPB_E_INVALID, "null argument");
   if (cfg->descriptor_dim != kD || cfg->num_heads != kHeads)
-    return fail(g_create_error, OPB_E_INVALID, "only descriptor_dim=256, num_heads=4 are supported (got %d, %d)", cfg->descriptor_dim,
+    return fail(no_handle_error, OPB_E_INVALID, "only descriptor_dim=256, num_heads=4 are supported (got %d, %d)", cfg->descriptor_dim,
                 cfg->num_heads);
   // The tail's fixed shift e = exp((cos - 1) / scale) runs on ex2.approx.ftz, which flushes results below 2^-126 to zero: every
   // cosine in [-1, 1] keeps e a normal fp32 value only when 2 log2(e) / scale <= 126.  Below that a query whose cosines are all
   // low would get a zero row sum and a NaN conf row.
   if (!((double)cfg->scale_factor >= kMinScaleFactor))
-    return fail(g_create_error, OPB_E_INVALID, "scale_factor must be >= 2 log2(e) / 126 = %.6f (got %g)", kMinScaleFactor, (double)cfg->scale_factor);
+    return fail(no_handle_error, OPB_E_INVALID, "scale_factor must be >= 2 log2(e) / 126 = %.6f (got %g)", kMinScaleFactor, (double)cfg->scale_factor);
   cudaDeviceProp prop;
-  if (int rc = select_device(cfg->device, prop, g_create_error)) return rc;
+  if (int rc = select_device(cfg->device, prop, no_handle_error)) return rc;
   DeviceGuard dg(cfg->device);
-  if (dg.err) return fail(g_create_error, OPB_E_CUDA, "cudaSetDevice: %s", cudaGetErrorString(dg.err));
+  if (dg.err) return fail(no_handle_error, OPB_E_CUDA, "cudaSetDevice: %s", cudaGetErrorString(dg.err));
   auto* m = new opb_matcher();
   m->cfg = *cfg;
   m->num_sms = prop.multiProcessorCount;
-  if (int rc = create_handle_state(m, cfg->device, &m->range_host, g_create_error)) {
+  if (int rc = create_handle_state(m, cfg->device, &m->range_host, no_handle_error)) {
     delete m;
     return rc;
   }
@@ -542,10 +555,10 @@ void opb_destroy(opb_matcher* m) {
   delete m;
 }
 
-const char* opb_last_error(const opb_matcher* m) { return m ? m->err.c_str() : g_create_error.c_str(); }
+const char* opb_last_error(const opb_matcher* m) { return m ? m->err.c_str() : no_handle_error.c_str(); }
 
 int opb_load_weight(opb_matcher* m, const char* name, const float* data, size_t n) {
-  if (!m || !name || !data) return m ? fail(m, OPB_E_INVALID, "null argument") : fail(g_create_error, OPB_E_INVALID, "null argument");
+  if (!m || !name || !data) return m ? fail(m, OPB_E_INVALID, "null argument") : fail(no_handle_error, OPB_E_INVALID, "null argument");
   m->host_w[name] = std::vector<float>(data, data + n);
   m->weights_ready = false;
   return OPB_OK;
@@ -912,42 +925,29 @@ int opb_poll_range(opb_matcher* m) {
 int opb_last_launch_count(const opb_matcher* m) { return m ? m->last_launches : 0; }
 
 // ---- adjacent producers ------------------------------------------------------------------
-static int scan_offsets(const int64_t* seg_len, int32_t M, long long** offs, cudaStream_t st) {
-  if (cudaMallocAsync(offs, (size_t)M * sizeof(long long), st) != cudaSuccess) return OPB_E_CUDA;
-  exclusive_scan_i64<<<1, 1024, 0, st>>>(reinterpret_cast<const long long*>(seg_len), *offs, M);
-  return OPB_OK;
-}
-
 int opb_segmented_mean_f64(const double* desc, const int64_t* seg_len, int32_t M, int32_t D, double* out, void* stream) {
-  if (!desc || !seg_len || !out || M <= 0 || D <= 0) return OPB_E_INVALID;
-  cudaStream_t st = (cudaStream_t)stream;
-  long long* offs = nullptr;
-  if (int rc = scan_offsets(seg_len, M, &offs, st)) return rc;
-  segmented_mean_f64<<<(unsigned)(((long long)M * 32 + 255) / 256), 256, 0, st>>>(desc, reinterpret_cast<const long long*>(seg_len), offs, M, D, out);
-  cudaFreeAsync(offs, st);
-  return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_E_CUDA;
+  REQUIRE(__func__, desc && seg_len && out && M > 0 && D > 0);
+  return segmented(__func__, "segmented_mean_f64", segmented_mean_f64, (unsigned)(((long long)M * 32 + 255) / 256), 256, desc, seg_len, M,
+                   (cudaStream_t)stream, D, out);
 }
 
 int opb_segmented_mean_scores_f64(const double* scores, const int64_t* seg_len, int32_t M, double* out, void* stream) {
-  if (!scores || !seg_len || !out || M <= 0) return OPB_E_INVALID;
-  cudaStream_t st = (cudaStream_t)stream;
-  long long* offs = nullptr;
-  if (int rc = scan_offsets(seg_len, M, &offs, st)) return rc;
-  segmented_mean_scores_f64<<<(unsigned)((M + 127) / 128), 128, 0, st>>>(scores, reinterpret_cast<const long long*>(seg_len), offs, M, out);
-  cudaFreeAsync(offs, st);
-  return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_E_CUDA;
+  REQUIRE(__func__, scores && seg_len && out && M > 0);
+  return segmented(__func__, "segmented_mean_scores_f64", segmented_mean_scores_f64, (unsigned)((M + 127) / 128), 128, scores, seg_len, M,
+                   (cudaStream_t)stream, out);
 }
 
 int opb_gather_features3d(const float* desc, const float* scores, int32_t dim, int64_t n_src, const int64_t* idx, int64_t n_idx, float* desc_out,
                           float* scores_out, int64_t n_out, void* stream) {
-  if (!desc || !desc_out || dim <= 0 || n_src < 0 || n_out <= 0 || n_idx < 0 || n_idx > n_out) return OPB_E_INVALID;
+  REQUIRE(__func__, desc && desc_out && dim > 0 && n_src >= 0 && n_out > 0 && n_idx >= 0 && n_idx <= n_out);
   cudaStream_t st = (cudaStream_t)stream;
   const unsigned gx = (unsigned)((n_out + 255) / 256);
-  gather_columns_f32<<<dim3(gx, (unsigned)dim), 256, 0, st>>>(desc, dim, (long long)n_src, reinterpret_cast<const long long*>(idx), (long long)n_idx,
-                                                              desc_out, (long long)n_out);
+  LAUNCH_NH(__func__, gather_columns_f32, dim3(gx, (unsigned)dim), 256, 0, st, desc, dim, (long long)n_src, reinterpret_cast<const long long*>(idx),
+            (long long)n_idx, desc_out, (long long)n_out);
   if (scores && scores_out)
-    gather_scores_f32<<<gx, 256, 0, st>>>(scores, (long long)n_src, reinterpret_cast<const long long*>(idx), (long long)n_idx, scores_out, (long long)n_out);
-  return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_E_CUDA;
+    LAUNCH_NH(__func__, gather_scores_f32, gx, 256, 0, st, scores, (long long)n_src, reinterpret_cast<const long long*>(idx), (long long)n_idx,
+              scores_out, (long long)n_out);
+  return OPB_OK;
 }
 
 // ---- test hooks ---------------------------------------------------------------------------
@@ -1046,7 +1046,7 @@ int opb_debug_set_pdl(int32_t enable) {
 }
 
 int opb_debug_gemm(const opb_debug_gemm_desc* d, void* stream) {
-  if (!d || d->backend < 0 || d->backend > 1 || d->b2_mode < 0 || d->b2_mode > 3) return OPB_E_INVALID;
+  REQUIRE(__func__, d && d->backend >= 0 && d->backend <= 1 && d->b2_mode >= 0 && d->b2_mode <= 3);
   GemmProblem p{};
   p.epi = d->epi; p.bn = d->bn;
   p.rows = d->rows; p.n_out = d->n_out; p.K1 = d->K1; p.K2 = d->K2;
@@ -1074,9 +1074,11 @@ int opb_debug_gemm(const opb_debug_gemm_desc* d, void* stream) {
   for (int t = 0; t < 9; ++t) p.tap_off[t] = d->tap_off[t];
   p.cv_w2 = d->cv_w2; p.cv_h = d->cv_h; p.cv_w = d->cv_w; p.cv_ppad = d->cv_ppad; p.relu = d->relu; p.range_flag = d->range_flag;
   p.max_ctas = d->max_ctas;
-  if (d->backend == 1 && (p.epi != EPI_F32 || p.a_conv || p.b2_lo_zero || p.taps || p.a_hi_only)) return OPB_E_INVALID;   // plain product only
-  int rc = d->backend == 1 ? launch_gemm_simt(p, (cudaStream_t)stream) : launch_gemm_tc(p, (cudaStream_t)stream);
-  return rc == 0 ? OPB_OK : (rc == -1 ? OPB_E_INVALID : OPB_E_CUDA);
+  REQUIRE(__func__, d->backend == 0 || (p.epi == EPI_F32 && !p.a_conv && !p.b2_lo_zero && !p.taps && !p.a_hi_only));   // SIMT: plain product only
+  const int rc = d->backend == 1 ? launch_gemm_simt(p, (cudaStream_t)stream) : launch_gemm_tc(p, (cudaStream_t)stream);
+  if (rc == 0) return OPB_OK;
+  return fail(no_handle_error, rc == -1 ? OPB_E_INVALID : OPB_E_CUDA, "%s: GEMM core of backend %d: %s", __func__, d->backend,
+              rc == -1 ? "unsupported problem" : "launch failed");
 }
 
 int opb_debug_kv_state_h(const void* kvh, int32_t frames, int32_t n, int32_t m_pts, int32_t slabs_per_group, float* partial, int32_t* n_groups,
@@ -1085,8 +1087,8 @@ int opb_debug_kv_state_h(const void* kvh, int32_t frames, int32_t n, int32_t m_p
   L.B = frames; L.N = n; L.M = m_pts; L.n_pad = (n + kSegPad - 1) / kSegPad * kSegPad; L.m_pad = (m_pts + kSegPad - 1) / kSegPad * kSegPad;
   L.R = L.n_pad + L.m_pad;
   int dev = 0, sms = 0;
-  cudaGetDevice(&dev);
-  if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) return OPB_E_CUDA;
+  CK(no_handle_error, cudaGetDevice(&dev));
+  CK(no_handle_error, cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   KvGroups G = kv_groups_for(L, sms);
   if (slabs_per_group > 0) {
     G.slabs = slabs_per_group;
@@ -1095,12 +1097,12 @@ int opb_debug_kv_state_h(const void* kvh, int32_t frames, int32_t n, int32_t m_p
   }
   if (n_groups) *n_groups = frames * (G.gq + G.gd);
   if (!partial) return OPB_OK;                    // size query
-  return launch_kv_state_h((const __half*)kvh, L, G, partial, (cudaStream_t)stream) == cudaSuccess ? OPB_OK : OPB_E_CUDA;
+  return launched(__func__, "kv_state_h_kernel", launch_kv_state_h((const __half*)kvh, L, G, partial, (cudaStream_t)stream));
 }
 
 int opb_debug_split(const float* x, void* hi, void* lo, size_t n, void* stream) {
-  split_planes<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(x, (__half*)hi, (__half*)lo, (long long)n);
-  return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_E_CUDA;
+  LAUNCH_NH(__func__, split_planes, (unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream, x, (__half*)hi, (__half*)lo, (long long)n);
+  return OPB_OK;
 }
 
 }  // extern "C"

@@ -18,6 +18,7 @@
 #include <stdint.h>
 
 #include "../../include/onepose_b200.h"
+#include "host_util.cuh"
 
 namespace opb {
 namespace {
@@ -234,21 +235,22 @@ __global__ void boxes_from_poses_kernel(const double* __restrict__ K, const doub
   for (int a = 0; a < 4; ++a) box[(size_t)b * 4 + a] = finite ? (int32_t)e[a] : 0;
 }
 
-int launch_crop(const uint8_t* frames, int64_t frame_pitch, int64_t row_pitch, int32_t B, int32_t H, int32_t W, const int32_t* box, const double* K,
-                int stages, int32_t out_h, int32_t out_w, uint8_t* out_u8, float* out_f32, double* trans, double* K_crop, int32_t* status,
-                void* stream) {
+int launch_crop(const char* fn, const uint8_t* frames, int64_t frame_pitch, int64_t row_pitch, int32_t B, int32_t H, int32_t W, const int32_t* box,
+                const double* K, int stages, int32_t out_h, int32_t out_w, uint8_t* out_u8, float* out_f32, double* trans, double* K_crop,
+                int32_t* status, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
-  crop_transforms_kernel<<<(unsigned)((B + 127) / 128), 128, 0, st>>>(box, K, B, stages, out_h, out_w, trans, K_crop, status);
+  LAUNCH_NH(fn, crop_transforms_kernel, (unsigned)((B + 127) / 128), 128, 0, st, box, K, B, stages, out_h, out_w, trans, K_crop, status);
   if (frames) {
     const long long blocks = ((long long)out_h * out_w + kWarpThreads - 1) / kWarpThreads;
-    crop_warp_kernel<<<dim3((unsigned)blocks, (unsigned)B), kWarpThreads, 0, st>>>(frames, frame_pitch, row_pitch, H, W, box, trans, stages, out_h,
-                                                                                  out_w, out_u8, out_f32);
+    LAUNCH_NH(fn, crop_warp_kernel, dim3((unsigned)blocks, (unsigned)B), kWarpThreads, 0, st, frames, frame_pitch, row_pitch, H, W, box, trans, stages,
+              out_h, out_w, out_u8, out_f32);
   }
-  return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_E_CUDA;
+  return OPB_OK;
 }
 
-bool frames_ok(int64_t frame_pitch, int64_t row_pitch, int32_t B, int32_t H, int32_t W) {
-  return B > 0 && B <= 65535 && H > 0 && H <= kMaxSide && W > 0 && W <= kMaxSide && row_pitch >= W && frame_pitch >= 0;
+int check_frames(const char* fn, int64_t frame_pitch, int64_t row_pitch, int32_t B, int32_t H, int32_t W) {
+  REQUIRE(fn, B > 0 && B <= 65535 && H > 0 && H <= kMaxSide && W > 0 && W <= kMaxSide && row_pitch >= W && frame_pitch >= 0);
+  return OPB_OK;
 }
 
 }  // namespace
@@ -256,23 +258,26 @@ bool frames_ok(int64_t frame_pitch, int64_t row_pitch, int32_t B, int32_t H, int
 
 extern "C" int opb_boxes_from_poses(const double* K, const double* pose, const double* corners, int32_t B, int32_t n_corners, double* proj,
                                     int32_t* box, void* stream) {
-  if (!K || !pose || !corners || !box || B <= 0 || n_corners <= 0) return OPB_E_INVALID;
-  opb::boxes_from_poses_kernel<<<(unsigned)((B + 127) / 128), 128, 0, (cudaStream_t)stream>>>(K, pose, corners, B, n_corners, proj, box);
-  return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_E_CUDA;
+  REQUIRE(__func__, K && pose && corners && box && B > 0 && n_corners > 0);
+  LAUNCH_NH(__func__, opb::boxes_from_poses_kernel, (unsigned)((B + 127) / 128), 128, 0, (cudaStream_t)stream, K, pose, corners, B, n_corners, proj,
+            box);
+  return OPB_OK;
 }
 
 extern "C" int opb_crop_resize(const uint8_t* frames, int64_t frame_pitch, int64_t row_pitch, int32_t B, int32_t H, int32_t W, const int32_t* box,
                                const double* K, int32_t crop_size, float* image, double* K_crop, double* trans, int32_t* status, void* stream) {
-  if (!frames || !box || !K || !image || !K_crop || !trans || !status || !opb::frames_ok(frame_pitch, row_pitch, B, H, W) || crop_size <= 0 ||
-      crop_size % 8 != 0 || crop_size > opb::kMaxSide)
-    return OPB_E_INVALID;
-  return opb::launch_crop(frames, frame_pitch, row_pitch, B, H, W, box, K, 2, crop_size, crop_size, nullptr, image, trans, K_crop, status, stream);
+  REQUIRE(__func__, frames && box && K && image && K_crop && trans && status);
+  if (int rc = opb::check_frames(__func__, frame_pitch, row_pitch, B, H, W)) return rc;
+  REQUIRE(__func__, crop_size > 0 && crop_size % 8 == 0 && crop_size <= opb::kMaxSide);
+  return opb::launch_crop(__func__, frames, frame_pitch, row_pitch, B, H, W, box, K, 2, crop_size, crop_size, nullptr, image, trans, K_crop, status,
+                          stream);
 }
 
 extern "C" int opb_warp_crop_u8(const uint8_t* frames, int64_t frame_pitch, int64_t row_pitch, int32_t B, int32_t H, int32_t W, const int32_t* box,
                                 const double* K, int32_t out_h, int32_t out_w, uint8_t* out, double* trans, double* K_crop, void* stream) {
-  if (!box || !trans || (frames != nullptr) != (out != nullptr) || (K != nullptr) != (K_crop != nullptr) || B <= 0 || B > 65535 || out_h <= 0 ||
-      out_h > opb::kMaxSide || out_w <= 0 || out_w > opb::kMaxSide || (frames && !opb::frames_ok(frame_pitch, row_pitch, B, H, W)))
-    return OPB_E_INVALID;
-  return opb::launch_crop(frames, frame_pitch, row_pitch, B, H, W, box, K, 1, out_h, out_w, out, nullptr, trans, K_crop, nullptr, stream);
+  REQUIRE(__func__, box && trans && (frames != nullptr) == (out != nullptr) && (K != nullptr) == (K_crop != nullptr));
+  REQUIRE(__func__, B > 0 && B <= 65535 && out_h > 0 && out_h <= opb::kMaxSide && out_w > 0 && out_w <= opb::kMaxSide);
+  if (frames)
+    if (int rc = opb::check_frames(__func__, frame_pitch, row_pitch, B, H, W)) return rc;
+  return opb::launch_crop(__func__, frames, frame_pitch, row_pitch, B, H, W, box, K, 1, out_h, out_w, out, nullptr, trans, K_crop, nullptr, stream);
 }

@@ -26,6 +26,7 @@
 
 #include "../../include/onepose_b200.h"
 #include "cv_rng.cuh"
+#include "host_util.cuh"
 
 namespace opb {
 namespace {
@@ -448,8 +449,9 @@ __global__ void __launch_bounds__(kAffThreads) boxes_from_matches_kernel(
   status[b] = ok ? 1 : 0;
 }
 
-bool params_ok(double threshold, int32_t max_iters, double confidence, int32_t refine_iters) {
-  return isfinite(threshold) && max_iters >= 0 && confidence > 0.0 && confidence < 1.0 && refine_iters >= 0;
+int check_params(const char* fn, double threshold, int32_t max_iters, double confidence, int32_t refine_iters) {
+  REQUIRE(fn, isfinite(threshold) && max_iters >= 0 && confidence > 0.0 && confidence < 1.0 && refine_iters >= 0);
+  return OPB_OK;
 }
 
 AffineParams make_params(double threshold, int32_t max_iters, double confidence, int32_t refine_iters) {
@@ -468,7 +470,7 @@ static int g_aff_trace_cap = 0;
 static opb::AffineTrace aff_trace() { return {g_aff_trace_samples, g_aff_trace_counts, g_aff_trace_models, g_aff_trace_cap}; }
 
 extern "C" int opb_debug_set_affine_trace(int32_t* samples, int32_t* counts, double* models, int32_t capacity) {
-  if (capacity < 0 || ((samples || counts || models) && capacity == 0)) return OPB_E_INVALID;
+  REQUIRE(__func__, capacity > 0 || (capacity == 0 && !samples && !counts && !models));
   g_aff_trace_samples = samples;
   g_aff_trace_counts = counts;
   g_aff_trace_models = models;
@@ -479,27 +481,25 @@ extern "C" int opb_debug_set_affine_trace(int32_t* samples, int32_t* counts, dou
 extern "C" int opb_estimate_affine_partial(const float* from, const float* to, const int32_t* offsets, int32_t B, double threshold,
                                            int32_t max_iters, double confidence, int32_t refine_iters, double* affine, uint8_t* inlier_mask,
                                            int32_t* iterations, int32_t* status, void* stream) {
-  if (!from || !to || !offsets || !affine || !iterations || !status || B <= 0 ||
-      !opb::params_ok(threshold, max_iters, confidence, refine_iters))
-    return OPB_E_INVALID;
-  opb::affine_partial_kernel<<<(unsigned)B, opb::kAffThreads, 0, (cudaStream_t)stream>>>(
-      from, to, offsets, opb::make_params(threshold, max_iters, confidence, refine_iters), aff_trace(), affine, inlier_mask, iterations, status);
-  return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_E_CUDA;
+  REQUIRE(__func__, from && to && offsets && affine && iterations && status && B > 0);
+  if (int rc = opb::check_params(__func__, threshold, max_iters, confidence, refine_iters)) return rc;
+  LAUNCH_NH(__func__, opb::affine_partial_kernel, (unsigned)B, opb::kAffThreads, 0, (cudaStream_t)stream, from, to, offsets,
+            opb::make_params(threshold, max_iters, confidence, refine_iters), aff_trace(), affine, inlier_mask, iterations, status);
+  return OPB_OK;
 }
 
 extern "C" int opb_boxes_from_matches(const float* ref_keypoints, const int32_t* ref_counts, const int32_t* ref_sizes, int32_t V, int32_t cap_ref,
                                       const float* query_keypoints, const int32_t* query_counts, int32_t cap_query, const void* matches0,
                                       int32_t matches_int64, int32_t B, int32_t query_h, int32_t query_w, int32_t* box, int32_t* view,
                                       int32_t* n_matches, double* affine, int32_t* status, void* stream) {
-  if (!ref_keypoints || !ref_counts || !ref_sizes || !query_keypoints || !query_counts || !matches0 || !box || !view || !n_matches || !affine ||
-      !status || V <= 0 || V > opb::kMaxViews || cap_ref <= 0 || cap_ref > opb::kMaxRefPoints || cap_query <= 0 || B <= 0 ||
-      (matches_int64 != 0 && matches_int64 != 1) || query_h <= 0 || query_w <= 0)
-    return OPB_E_INVALID;
+  REQUIRE(__func__, ref_keypoints && ref_counts && ref_sizes && query_keypoints && query_counts && matches0 && box && view && n_matches && affine &&
+                        status);
+  REQUIRE(__func__, V > 0 && V <= opb::kMaxViews && cap_ref > 0 && cap_ref <= opb::kMaxRefPoints && cap_query > 0 && B > 0);
+  REQUIRE(__func__, (matches_int64 == 0 || matches_int64 == 1) && query_h > 0 && query_w > 0);
   const size_t smem = (size_t)cap_ref * sizeof(float4);
-  if (cudaFuncSetAttribute(opb::boxes_from_matches_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
-    return OPB_E_CUDA;
-  opb::boxes_from_matches_kernel<<<(unsigned)B, opb::kAffThreads, smem, (cudaStream_t)stream>>>(
-      ref_keypoints, ref_counts, ref_sizes, V, cap_ref, query_keypoints, query_counts, cap_query, matches0, matches_int64, query_h, query_w,
-      opb::make_params(6.0, 2000, 0.99, 10), aff_trace(), box, view, n_matches, affine, status);
-  return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_E_CUDA;
+  CK(opb::no_handle_error, cudaFuncSetAttribute(opb::boxes_from_matches_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  LAUNCH_NH(__func__, opb::boxes_from_matches_kernel, (unsigned)B, opb::kAffThreads, smem, (cudaStream_t)stream, ref_keypoints, ref_counts, ref_sizes,
+            V, cap_ref, query_keypoints, query_counts, cap_query, matches0, matches_int64, query_h, query_w,
+            opb::make_params(6.0, 2000, 0.99, 10), aff_trace(), box, view, n_matches, affine, status);
+  return OPB_OK;
 }

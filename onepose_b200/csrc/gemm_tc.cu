@@ -959,7 +959,7 @@ template <int EPI, int ACV = ACV_NONE, bool HI = false, int BN_ = 256, int K2B =
 cudaError_t launch_variant(int grid, cudaStream_t stream, const Maps& mp, const TcParams& tp) {
   auto* kern = gemm_tc_kernel<EPI, ACV, HI, BN_, K2B>;
   if (cudaError_t e = ensure_smem_limit((const void*)kern, kSmemBytes)) return e;
-  return launch_k(kern, dim3(grid), dim3(kThreads), kSmemBytes, stream, mp, tp);
+  return launch_k(pdl_enabled(), kern, dim3(grid), dim3(kThreads), kSmemBytes, stream, mp, tp);
 }
 
 }  // namespace

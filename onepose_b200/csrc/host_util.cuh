@@ -1,6 +1,6 @@
-// Host-side helpers shared by the translation units of the library (matcher api.cu, extractor superpoint.cu):
-// device buffers that own their memory and only ever grow, fp16-split plane pairs, the PDL-aware kernel launcher, and the
-// runtime every handle shares -- its error message, host weights, launch count and profiling timeline.
+// Host-side helpers shared by the translation units of the library: device buffers that own their memory and only ever grow,
+// fp16-split plane pairs, the kernel launcher, the runtime every handle shares -- its error message, host weights, launch count
+// and profiling timeline -- and the error message and argument checks of the calls without a handle.
 #pragma once
 #include <cstdarg>
 #include <cstdio>
@@ -72,9 +72,10 @@ inline void split_host(const std::vector<double>& w, std::vector<__half>& hi, st
   for (size_t i = 0; i < w.size(); ++i) split_f32((float)w[i], hi[i], lo[i]);
 }
 
-// Every kernel of the library begins with griddep_sync() and is launched with programmatic stream serialization (PDL).
+// `pdl`: launch with programmatic stream serialization (PDL).  Only a kernel that begins with griddep_sync() may take it: the
+// handles' launches pass pdl_enabled(), and a kernel that reads its inputs without that wait is launched without it.
 template <typename... KArgs, typename... Args>
-inline cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
+inline cudaError_t launch_k(bool pdl, void (*kern)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args&&... args) {
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = grid;
   cfg.blockDim = block;
@@ -84,7 +85,7 @@ inline cudaError_t launch_k(void (*kern)(KArgs...), dim3 grid, dim3 block, size_
   attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
   attr[0].val.programmaticStreamSerializationAllowed = 1;
   cfg.attrs = attr;
-  cfg.numAttrs = pdl_enabled() ? 1 : 0;
+  cfg.numAttrs = pdl ? 1 : 0;
   return cudaLaunchKernelEx(&cfg, kern, std::forward<Args>(args)...);
 }
 
@@ -193,8 +194,12 @@ struct Handle {
   }
 };
 
-// Sets the message of a failed call and returns its code: into the handle, or -- for a call that has none, such as create --
-// into the create-error string of the handle kind (what opb_last_error(NULL) / opb_sp_last_error(NULL) return).
+// The message of the last failed call on this thread that had no handle (the create functions and the handle-free entry
+// points): what opb_last_error(NULL) and opb_sp_last_error(NULL) return.  A successful call leaves it as it is.
+inline thread_local std::string no_handle_error;
+
+// Sets the message of a failed call and returns its code: into the handle, or -- for a call that has none -- into
+// no_handle_error.
 inline void set_error(std::string& dst, const char* fmt, va_list ap) {
   char buf[512];
   vsnprintf(buf, sizeof buf, fmt, ap);
@@ -219,7 +224,7 @@ inline int fail(Handle* h, int code, const char* fmt, ...) {
   do {                                                                                                \
     cudaError_t _e = (expr);                                                                          \
     if (_e != cudaSuccess)                                                                            \
-      return fail(h, OPB_E_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); \
+      return opb::fail(h, OPB_E_CUDA, "%s failed: %s (%s:%d)", #expr, cudaGetErrorString(_e), __FILE__, __LINE__); \
   } while (0)
 
 // Runs `enqueue()` -- the part of a call that enqueues work for handle `h` on `st` -- after the handle's previous call, and
@@ -241,10 +246,23 @@ inline int launched(Handle* h, cudaStream_t st, const char* name, cudaError_t e)
   return 0;
 }
 
-#define LAUNCH(h, st, name, ...)                                              \
-  do {                                                                        \
-    if (int _rc = launched(h, st, name, launch_k(__VA_ARGS__))) return _rc;   \
+#define LAUNCH(h, st, name, ...)                                                            \
+  do {                                                                                      \
+    if (int _rc = launched(h, st, name, launch_k(pdl_enabled(), __VA_ARGS__))) return _rc; \
   } while (0)
+
+// Argument check of entry point `fn` without a handle: OPB_E_INVALID unless `cond` holds, with a message that names both.
+#define REQUIRE(fn, cond) \
+  do { if (!(cond)) return opb::fail(opb::no_handle_error, OPB_E_INVALID, "%s: %s", fn, #cond); } while (0)
+
+// Result of the launch of kernel `name` by entry point `fn` without a handle: a failure becomes OPB_E_CUDA and the message.
+inline int launched(const char* fn, const char* name, cudaError_t e) {
+  return e == cudaSuccess ? OPB_OK : fail(no_handle_error, OPB_E_CUDA, "%s: launch of %s failed: %s", fn, name, cudaGetErrorString(e));
+}
+
+// A launch by entry point `fn` without a handle.  Its kernels do not begin with griddep_sync(), so they go without PDL.
+#define LAUNCH_NH(fn, kern, ...) \
+  do { if (int _rc = opb::launched(fn, #kern, opb::launch_k(false, kern, __VA_ARGS__))) return _rc; } while (0)
 
 // One counted launch of the wgmma GEMM core: `flops` = algorithmic FLOPs, `name` = its profile entry, `what` names it in an error.
 inline int run_gemm(Handle* h, const GemmProblem& p, cudaStream_t st, double flops, const char* what, const char* name) {
@@ -289,7 +307,7 @@ inline int upload_f32(Handle* h, DevBuf& dst, const std::vector<double>& w) {
 }
 
 // create: `device` must be an sm_90 device; `prop` receives its properties.  The caller's current device is left as it is (the
-// create functions make `device` current with a DeviceGuard).  Messages go to `err`, the create-error string of the handle kind.
+// create functions make `device` current with a DeviceGuard).  Messages go to `err`.
 inline int select_device(int device, cudaDeviceProp& prop, std::string& err) {
   int n_dev = 0;
   cudaError_t e = cudaGetDeviceCount(&n_dev);

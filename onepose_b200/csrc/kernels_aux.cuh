@@ -1,8 +1,9 @@
 // Bandwidth-bound helper kernels of the GATsSPG matcher (everything that is not a GEMM):
 // layout changes, GATs aggregation, linear-attention state reduction, InstanceNorm statistics,
 // dual-softmax bookkeeping, mutual-NN, and the adjacent producers (segmented means, leaf gathering).
-// sm_90a; plain coalesced warp-per-row / block-per-tile kernels.  Every kernel begins with griddep_sync()
-// (programmatic dependent launch, see common.cuh) and is launched through launch_k().
+// sm_90a; plain coalesced warp-per-row / block-per-tile kernels.  The kernels of the matcher's forward begin with
+// griddep_sync() (programmatic dependent launch, see common.cuh).  split_planes, join_planes and the adjacent producers
+// (exclusive_scan_i64, segmented_mean*, gather_*) do not: they are launched without PDL.
 #pragma once
 #include "common.cuh"
 #include "gemm_tc.cuh"

@@ -179,6 +179,6 @@ cudaError_t launch_kv_state_h(const __half* kvh, const Layout& L, const KvGroups
   if (const cudaError_t e = ensure_smem_limit((const void*)kv_state_h_kernel, kHSmemBytes)) return e;
   CUtensorMap map;
   if (!make_tensor_map_2d(&map, kvh, L.rows(), 512, 512, 64, kHRows, false)) return cudaErrorInvalidValue;
-  return launch_k(kv_state_h_kernel, dim3((unsigned)(L.B * (G.gq + G.gd))), dim3(kHThreads), kHSmemBytes, stream, map, L, G, partial);
+  return launch_k(pdl_enabled(), kv_state_h_kernel, dim3((unsigned)(L.B * (G.gq + G.gd))), dim3(kHThreads), kHSmemBytes, stream, map, L, G, partial);
 }
 }  // namespace opb

@@ -20,6 +20,7 @@
 
 #include "../../include/onepose_b200.h"
 #include "cv_rng.cuh"
+#include "host_util.cuh"
 
 namespace opb {
 namespace {
@@ -1355,80 +1356,82 @@ __global__ void __launch_bounds__(kGatherThreads) gather_compact(const int64_t* 
 }  // namespace opb
 
 // The gather of both entry points: kp3_first / kp3_count == nullptr means one object of M key points for every frame.
-static int gather_matches_impl(const int64_t* matches0, const float* mscores0, const float* keypoints2d, const float* keypoints3d, int32_t B,
-                               int32_t N, int32_t M, const int32_t* kp3_first, const int32_t* kp3_count, double* pts2d, double* pts3d,
+static int gather_matches_impl(const char* fn, const int64_t* matches0, const float* mscores0, const float* keypoints2d, const float* keypoints3d,
+                               int32_t B, int32_t N, int32_t M, const int32_t* kp3_first, const int32_t* kp3_count, double* pts2d, double* pts3d,
                                float* mconf, int32_t* query_index, int32_t* offsets, void* stream) {
-  if (N > 0 && (!matches0 || !keypoints2d || !pts2d || !pts3d)) return OPB_E_INVALID;
-  if (mconf && !mscores0) return OPB_E_INVALID;
+  REQUIRE(fn, N == 0 || (matches0 && keypoints2d && pts2d && pts3d));
+  REQUIRE(fn, !mconf || mscores0);
   cudaStream_t st = (cudaStream_t)stream;
   if (N == 0) {
-    if (cudaMemsetAsync(offsets, 0, sizeof(int32_t) * ((size_t)B + 1), st) != cudaSuccess) return OPB_E_CUDA;
+    CK(opb::no_handle_error, cudaMemsetAsync(offsets, 0, sizeof(int32_t) * ((size_t)B + 1), st));
     return OPB_OK;
   }
-  opb::gather_count<<<(unsigned)B, opb::kGatherThreads, 0, st>>>(matches0, N, M, kp3_count, offsets);
-  opb::gather_scan<<<1, opb::kScanThreads, 0, st>>>(B, offsets);
-  opb::gather_compact<<<(unsigned)B, opb::kGatherThreads, 0, st>>>(matches0, mscores0, keypoints2d, keypoints3d, N, M, kp3_first, kp3_count, offsets,
-                                                                   pts2d, pts3d, mconf, query_index);
-  return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_E_CUDA;
+  LAUNCH_NH(fn, opb::gather_count, (unsigned)B, opb::kGatherThreads, 0, st, matches0, N, M, kp3_count, offsets);
+  LAUNCH_NH(fn, opb::gather_scan, 1, opb::kScanThreads, 0, st, B, offsets);
+  LAUNCH_NH(fn, opb::gather_compact, (unsigned)B, opb::kGatherThreads, 0, st, matches0, mscores0, keypoints2d, keypoints3d, N, M, kp3_first, kp3_count,
+            offsets, pts2d, pts3d, mconf, query_index);
+  return OPB_OK;
 }
 
 extern "C" int opb_gather_matches(const int64_t* matches0, const float* mscores0, const float* keypoints2d, const float* keypoints3d,
                                   int32_t B, int32_t N, int32_t M, double* pts2d, double* pts3d, float* mconf, int32_t* query_index,
                                   int32_t* offsets, void* stream) {
-  if (B <= 0 || N < 0 || M <= 0 || !keypoints3d || !offsets || (int64_t)B * N > (int64_t)INT32_MAX) return OPB_E_INVALID;
-  return gather_matches_impl(matches0, mscores0, keypoints2d, keypoints3d, B, N, M, nullptr, nullptr, pts2d, pts3d, mconf, query_index, offsets,
-                             stream);
+  REQUIRE(__func__, B > 0 && N >= 0 && M > 0 && keypoints3d && offsets && (int64_t)B * N <= (int64_t)INT32_MAX);
+  return gather_matches_impl(__func__, matches0, mscores0, keypoints2d, keypoints3d, B, N, M, nullptr, nullptr, pts2d, pts3d, mconf, query_index,
+                             offsets, stream);
 }
 
 extern "C" int opb_gather_matches_objects(const int64_t* matches0, const float* mscores0, const float* keypoints2d, const float* keypoints3d,
                                           const int32_t* kp3_first, const int32_t* kp3_count, int32_t B, int32_t N, double* pts2d, double* pts3d,
                                           float* mconf, int32_t* query_index, int32_t* offsets, void* stream) {
-  if (B <= 0 || N < 0 || !keypoints3d || !kp3_first || !kp3_count || !offsets || (int64_t)B * N > (int64_t)INT32_MAX) return OPB_E_INVALID;
-  return gather_matches_impl(matches0, mscores0, keypoints2d, keypoints3d, B, N, 0, kp3_first, kp3_count, pts2d, pts3d, mconf, query_index, offsets,
-                             stream);
+  REQUIRE(__func__, B > 0 && N >= 0 && keypoints3d && kp3_first && kp3_count && offsets && (int64_t)B * N <= (int64_t)INT32_MAX);
+  return gather_matches_impl(__func__, matches0, mscores0, keypoints2d, keypoints3d, B, N, 0, kp3_first, kp3_count, pts2d, pts3d, mconf, query_index,
+                             offsets, stream);
 }
 
 // the arguments every RANSAC entry point takes
-static bool ransac_args_ok(const double* K, const double* pts2d, const double* pts3d, const int32_t* offsets, int32_t B, int32_t hypotheses,
-                           double reproj_error, const double* workspace, const double* pose_out, const int32_t* inlier_mask,
-                           const int32_t* n_inliers) {
-  return K && pts2d && pts3d && offsets && workspace && pose_out && inlier_mask && n_inliers && B > 0 && hypotheses > 0 &&
-         hypotheses <= opb::kMaxHypotheses && reproj_error > 0.0;
+static int check_ransac_args(const char* fn, const double* K, const double* pts2d, const double* pts3d, const int32_t* offsets, int32_t B,
+                             int32_t hypotheses, double reproj_error, const double* workspace, const double* pose_out, const int32_t* inlier_mask,
+                             const int32_t* n_inliers) {
+  REQUIRE(fn, K && pts2d && pts3d && offsets && workspace && pose_out && inlier_mask && n_inliers);
+  REQUIRE(fn, B > 0 && hypotheses > 0 && hypotheses <= opb::kMaxHypotheses && reproj_error > 0.0);
+  return OPB_OK;
 }
 
 // a RANSAC of a fixed number of hypotheses: one thread per hypothesis record, then one block per frame selects
 template <class HypothesesKernel, class SelectKernel>
-static int ransac_fixed(HypothesesKernel hypotheses_kernel, SelectKernel select_kernel, const double* K, const double* pts2d, const double* pts3d,
-                        const int32_t* offsets, int32_t B, int32_t hypotheses, double reproj_error, uint64_t seed, double* workspace,
-                        double* pose_out, int32_t* inlier_mask, int32_t* n_inliers, void* stream) {
-  if (!ransac_args_ok(K, pts2d, pts3d, offsets, B, hypotheses, reproj_error, workspace, pose_out, inlier_mask, n_inliers)) return OPB_E_INVALID;
+static int ransac_fixed(const char* fn, HypothesesKernel hypotheses_kernel, SelectKernel select_kernel, const double* K, const double* pts2d,
+                        const double* pts3d, const int32_t* offsets, int32_t B, int32_t hypotheses, double reproj_error, uint64_t seed,
+                        double* workspace, double* pose_out, int32_t* inlier_mask, int32_t* n_inliers, void* stream) {
+  if (int rc = check_ransac_args(fn, K, pts2d, pts3d, offsets, B, hypotheses, reproj_error, workspace, pose_out, inlier_mask, n_inliers)) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   const double thr2 = reproj_error * reproj_error;
-  hypotheses_kernel<<<dim3((unsigned)B, (unsigned)((hypotheses + opb::kHypThreads - 1) / opb::kHypThreads)), opb::kHypThreads, 0, st>>>(
-      K, pts2d, pts3d, offsets, hypotheses, thr2, (unsigned long long)seed, workspace);
-  select_kernel<<<(unsigned)B, opb::kRefineThreads, 0, st>>>(K, pts2d, pts3d, offsets, hypotheses, thr2, workspace, pose_out, inlier_mask, n_inliers);
-  return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_E_CUDA;
+  LAUNCH_NH(fn, hypotheses_kernel, dim3((unsigned)B, (unsigned)((hypotheses + opb::kHypThreads - 1) / opb::kHypThreads)), opb::kHypThreads, 0, st,
+            K, pts2d, pts3d, offsets, hypotheses, thr2, (unsigned long long)seed, workspace);
+  LAUNCH_NH(fn, select_kernel, (unsigned)B, opb::kRefineThreads, 0, st, K, pts2d, pts3d, offsets, hypotheses, thr2, workspace, pose_out, inlier_mask,
+            n_inliers);
+  return OPB_OK;
 }
 
 extern "C" int opb_ransac_pnp(const double* K, const double* pts2d, const double* pts3d, const int32_t* offsets, int32_t B, int32_t hypotheses,
                               double reproj_error, uint64_t seed, double* workspace, double* pose_out, int32_t* inlier_mask, int32_t* n_inliers,
                               void* stream) {
-  return ransac_fixed(opb::pnp_hypotheses, opb::pnp_select_refine, K, pts2d, pts3d, offsets, B, hypotheses, reproj_error, seed, workspace, pose_out,
-                      inlier_mask, n_inliers, stream);
+  return ransac_fixed(__func__, opb::pnp_hypotheses, opb::pnp_select_refine, K, pts2d, pts3d, offsets, B, hypotheses, reproj_error, seed, workspace,
+                      pose_out, inlier_mask, n_inliers, stream);
 }
 
 extern "C" int opb_epnp(const double* K, const double* pts2d, const double* pts3d, const int32_t* offsets, int32_t B, double* pose_out,
                         int32_t* status, void* stream) {
-  if (!K || !pts2d || !pts3d || !offsets || !pose_out || !status || B <= 0) return OPB_E_INVALID;
-  opb::epnp_frames<<<(unsigned)B, opb::kEpnpThreads, 0, (cudaStream_t)stream>>>(K, pts2d, pts3d, offsets, pose_out, status);
-  return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_E_CUDA;
+  REQUIRE(__func__, K && pts2d && pts3d && offsets && pose_out && status && B > 0);
+  LAUNCH_NH(__func__, opb::epnp_frames, (unsigned)B, opb::kEpnpThreads, 0, (cudaStream_t)stream, K, pts2d, pts3d, offsets, pose_out, status);
+  return OPB_OK;
 }
 
 extern "C" int opb_ransac_epnp(const double* K, const double* pts2d, const double* pts3d, const int32_t* offsets, int32_t B, int32_t hypotheses,
                                double reproj_error, uint64_t seed, double* workspace, double* pose_out, int32_t* inlier_mask, int32_t* n_inliers,
                                void* stream) {
-  return ransac_fixed(opb::epnp_hypotheses, opb::epnp_select_refit, K, pts2d, pts3d, offsets, B, hypotheses, reproj_error, seed, workspace, pose_out,
-                      inlier_mask, n_inliers, stream);
+  return ransac_fixed(__func__, opb::epnp_hypotheses, opb::epnp_select_refit, K, pts2d, pts3d, offsets, B, hypotheses, reproj_error, seed, workspace,
+                      pose_out, inlier_mask, n_inliers, stream);
 }
 
 // test hooks of opb_ransac_epnp_cv (host-side settings read at launch; the launch sequence does not change)
@@ -1439,13 +1442,13 @@ static int32_t* g_cv_trace_winner = nullptr;
 static int g_cv_trace_cap = 0;
 
 extern "C" int opb_debug_set_cv_wave(int32_t wave) {
-  if (wave < 0) return OPB_E_INVALID;
+  REQUIRE(__func__, wave >= 0);
   g_cv_wave = wave;
   return OPB_OK;
 }
 
 extern "C" int opb_debug_set_cv_trace(int32_t* samples, int32_t* counts, int32_t* winner, int32_t capacity) {
-  if (capacity < 0 || ((samples || counts) && capacity == 0)) return OPB_E_INVALID;
+  REQUIRE(__func__, capacity > 0 || (capacity == 0 && !samples && !counts));
   g_cv_trace_samples = samples;
   g_cv_trace_counts = counts;
   g_cv_trace_winner = winner;
@@ -1454,20 +1457,21 @@ extern "C" int opb_debug_set_cv_trace(int32_t* samples, int32_t* counts, int32_t
 }
 
 extern "C" int opb_debug_cv_subsets(int32_t n, int32_t count, int32_t chunk, int32_t* out, void* stream) {
-  if (n < 5 || count <= 0 || chunk <= 0 || !out) return OPB_E_INVALID;
-  opb::epnp_cv_subsets<<<1, 32, 0, (cudaStream_t)stream>>>(n, count, chunk, out);
-  return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_E_CUDA;
+  REQUIRE(__func__, n >= 5 && count > 0 && chunk > 0 && out);
+  LAUNCH_NH(__func__, opb::epnp_cv_subsets, 1, 32, 0, (cudaStream_t)stream, n, count, chunk, out);
+  return OPB_OK;
 }
 
 // samples per frame and wave: B x W about one 128-thread block per SM.  A wave's time is one thread's EPnP latency (about
 // 2.5 ms on an H100) up to roughly that many threads, and grows with the thread count beyond it (tools/epnp_cv_bench.py,
 // DESIGN 5.4): smaller waves add waves without saving time, larger ones evaluate samples the loop may never need.  Whole
-// blocks, at most the budget.
+// blocks, at most the budget.  OPB_E_CUDA if the device query fails.
 static int cv_wave_size(int B, int H) {
   int w = g_cv_wave;
   if (w == 0) {
-    int dev = 0, sms = 132;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) sms = 132;
+    int dev = 0, sms = 0;
+    CK(opb::no_handle_error, cudaGetDevice(&dev));
+    CK(opb::no_handle_error, cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
     const int target = sms * opb::kHypThreads;
     w = (target / B + opb::kHypThreads - 1) / opb::kHypThreads * opb::kHypThreads;
     w = w < opb::kHypThreads ? opb::kHypThreads : w;
@@ -1478,24 +1482,25 @@ static int cv_wave_size(int B, int H) {
 extern "C" int opb_ransac_epnp_cv(const double* K, const double* pts2d, const double* pts3d, const int32_t* offsets, int32_t B, int32_t hypotheses,
                                   double reproj_error, double confidence, double* workspace, double* pose_out, int32_t* inlier_mask,
                                   int32_t* n_inliers, int32_t* iterations, void* stream) {
-  if (!ransac_args_ok(K, pts2d, pts3d, offsets, B, hypotheses, reproj_error, workspace, pose_out, inlier_mask, n_inliers) || !iterations ||
-      !(confidence >= 0.0 && confidence <= 1.0))
-    return OPB_E_INVALID;
+  if (int rc = check_ransac_args(__func__, K, pts2d, pts3d, offsets, B, hypotheses, reproj_error, workspace, pose_out, inlier_mask, n_inliers))
+    return rc;
+  REQUIRE(__func__, iterations && confidence >= 0.0 && confidence <= 1.0);
   cudaStream_t st = (cudaStream_t)stream;
   const float thr2f = (float)(reproj_error * reproj_error);   // findInliers: (float)(thresh * thresh)
   const int W = cv_wave_size(B, hypotheses);
+  if (W < 0) return W;
   const int waves = (hypotheses + W - 1) / W;
   opb::CvState* state = reinterpret_cast<opb::CvState*>(workspace + (size_t)B * hypotheses * opb::kHypStride);
   int* ts = g_cv_trace_samples;
   int* tc = g_cv_trace_counts;
   const int cap = g_cv_trace_cap;
-  opb::epnp_cv_scan<<<(unsigned)B, opb::kCvScanThreads, 0, st>>>(offsets, hypotheses, W, -1, confidence, state, workspace, ts, cap);
+  LAUNCH_NH(__func__, opb::epnp_cv_scan, (unsigned)B, opb::kCvScanThreads, 0, st, offsets, hypotheses, W, -1, confidence, state, workspace, ts, cap);
   for (int w = 0; w < waves; ++w) {
-    opb::epnp_cv_wave<<<dim3((unsigned)B, (unsigned)((W + opb::kHypThreads - 1) / opb::kHypThreads)), opb::kHypThreads, 0, st>>>(
-        K, pts2d, pts3d, offsets, W, w, thr2f, state, workspace, tc, cap);
-    opb::epnp_cv_scan<<<(unsigned)B, opb::kCvScanThreads, 0, st>>>(offsets, hypotheses, W, w, confidence, state, workspace, ts, cap);
+    LAUNCH_NH(__func__, opb::epnp_cv_wave, dim3((unsigned)B, (unsigned)((W + opb::kHypThreads - 1) / opb::kHypThreads)), opb::kHypThreads, 0, st,
+              K, pts2d, pts3d, offsets, W, w, thr2f, state, workspace, tc, cap);
+    LAUNCH_NH(__func__, opb::epnp_cv_scan, (unsigned)B, opb::kCvScanThreads, 0, st, offsets, hypotheses, W, w, confidence, state, workspace, ts, cap);
   }
-  opb::epnp_cv_select_refit<<<(unsigned)B, opb::kEpnpThreads, 0, st>>>(K, pts2d, pts3d, offsets, thr2f, state, pose_out, inlier_mask, n_inliers,
-                                                                       iterations, g_cv_trace_winner);
-  return cudaGetLastError() == cudaSuccess ? OPB_OK : OPB_E_CUDA;
+  LAUNCH_NH(__func__, opb::epnp_cv_select_refit, (unsigned)B, opb::kEpnpThreads, 0, st, K, pts2d, pts3d, offsets, thr2f, state, pose_out, inlier_mask,
+            n_inliers, iterations, g_cv_trace_winner);
+  return OPB_OK;
 }

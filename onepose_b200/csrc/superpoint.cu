@@ -481,8 +481,6 @@ struct opb_superpoint : Handle {
 
 namespace {
 
-thread_local std::string g_sp_create_error;
-
 // The range guard's premise (split_out_of_range): finite weights and biases, and weights that split (|64 w| < 65 520)
 template <typename V>
 int sp_check_weights(opb_superpoint* h, const std::string& name, const V& w, const V& b, bool split) {
@@ -590,19 +588,19 @@ int sp_run_conv(opb_superpoint* h, const SpConv& L, const PlaneBuf& in, int in_l
 extern "C" {
 
 int opb_sp_create(const opb_sp_config* cfg, opb_superpoint** out) {
-  if (!cfg || !out) return fail(g_sp_create_error, OPB_E_INVALID, "null argument");
-  if (cfg->descriptor_dim != 256) return fail(g_sp_create_error, OPB_E_INVALID, "descriptor_dim %d: only 256 is supported", cfg->descriptor_dim);
+  if (!cfg || !out) return fail(no_handle_error, OPB_E_INVALID, "null argument");
+  if (cfg->descriptor_dim != 256) return fail(no_handle_error, OPB_E_INVALID, "descriptor_dim %d: only 256 is supported", cfg->descriptor_dim);
   if (cfg->max_keypoints == 0 || cfg->max_keypoints < -1)
-    return fail(g_sp_create_error, OPB_E_INVALID, "\"max_keypoints\" must be positive or \"-1\"");
+    return fail(no_handle_error, OPB_E_INVALID, "\"max_keypoints\" must be positive or \"-1\"");
   if (cfg->nms_radius < 0 || cfg->nms_radius > 6)
-    return fail(g_sp_create_error, OPB_E_NOT_IMPLEMENTED, "nms_radius %d: the tiled NMS supports 0..6", cfg->nms_radius);
+    return fail(no_handle_error, OPB_E_NOT_IMPLEMENTED, "nms_radius %d: the tiled NMS supports 0..6", cfg->nms_radius);
   cudaDeviceProp prop;
-  if (int rc = select_device(cfg->device, prop, g_sp_create_error)) return rc;
+  if (int rc = select_device(cfg->device, prop, no_handle_error)) return rc;
   DeviceGuard dg(cfg->device);
-  if (dg.err) return fail(g_sp_create_error, OPB_E_CUDA, "cudaSetDevice: %s", cudaGetErrorString(dg.err));
+  if (dg.err) return fail(no_handle_error, OPB_E_CUDA, "cudaSetDevice: %s", cudaGetErrorString(dg.err));
   auto* h = new opb_superpoint();
   h->cfg = *cfg;
-  if (int rc = create_handle_state(h, cfg->device, &h->range_host, g_sp_create_error)) {
+  if (int rc = create_handle_state(h, cfg->device, &h->range_host, no_handle_error)) {
     delete h;
     return rc;
   }
@@ -617,7 +615,7 @@ void opb_sp_destroy(opb_superpoint* h) {
   delete h;
 }
 
-const char* opb_sp_last_error(const opb_superpoint* h) { return h ? h->err.c_str() : g_sp_create_error.c_str(); }
+const char* opb_sp_last_error(const opb_superpoint* h) { return h ? h->err.c_str() : no_handle_error.c_str(); }
 
 int opb_sp_load_weight(opb_superpoint* h, const char* name, const float* data, size_t n_elems) {
   if (!h || !name || !data) return OPB_E_INVALID;
@@ -819,7 +817,7 @@ int opb_sp_get_profile(opb_superpoint* h, int32_t index, char* name, size_t name
 }
 
 int opb_debug_set_conv_halo(int32_t mode) {
-  if (mode < 0 || mode > 1) return OPB_E_INVALID;
+  REQUIRE(__func__, mode >= 0 && mode <= 1);
   set_conv_halo_mode(mode);
   return OPB_OK;
 }

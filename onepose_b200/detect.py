@@ -18,15 +18,10 @@ import numpy as np
 import torch
 
 from . import _lib, crop
-from .pnp import _cuda_device
 
 MAX_VIEWS = 256         # opb_boxes_from_matches' bounds (include/onepose_b200.h)
 MAX_REF_POINTS = 8192
 MIN_MATCHES = 6         # match_worker: fewer matches give the [0, 0, H, W] box
-
-
-def _stream(dev):
-    return torch.cuda.current_stream(dev).cuda_stream
 
 
 def _check_params(threshold, max_iters, confidence, refine_iters):
@@ -45,7 +40,7 @@ def affine_partial_batch(from_pts: torch.Tensor, to_pts: torch.Tensor, offsets: 
     offsets[b+1] - 1).  Returns device tensors: affine f64 [B, 2, 3] (zeros where cv2 returns None), inliers uint8 [sum n]
     (cv2's mask), iterations int32 [B] (the RANSAC loop's) and status int32 [B] (1: a model, 0: None).  No host
     synchronisation."""
-    dev = _cuda_device(from_pts)
+    dev = _lib.cuda_device(from_pts)
     _check_params(threshold, max_iters, confidence, refine_iters)
     if from_pts.dim() != 2 or from_pts.shape[1] != 2 or tuple(to_pts.shape) != tuple(from_pts.shape):
         raise ValueError(f"from_pts and to_pts must both be [n, 2], got {list(from_pts.shape)} and {list(to_pts.shape)}")
@@ -57,11 +52,8 @@ def affine_partial_batch(from_pts: torch.Tensor, to_pts: torch.Tensor, offsets: 
     o = offsets.contiguous()
     out = {"affine": torch.empty(B, 2, 3, dtype=torch.float64, device=dev), "inliers": torch.empty(f.shape[0], dtype=torch.uint8, device=dev),
            "iterations": torch.empty(B, dtype=torch.int32, device=dev), "status": torch.empty(B, dtype=torch.int32, device=dev)}
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        _lib.check(lib.opb_estimate_affine_partial(f.data_ptr(), t.data_ptr(), o.data_ptr(), B, float(threshold), int(max_iters), float(confidence),
-                                                   int(refine_iters), out["affine"].data_ptr(), out["inliers"].data_ptr() if f.shape[0] else None,
-                                                   out["iterations"].data_ptr(), out["status"].data_ptr(), _stream(dev)))
+    _lib.call(dev, "opb_estimate_affine_partial", f, t, o, B, float(threshold), int(max_iters), float(confidence), int(refine_iters), out["affine"],
+              out["inliers"] if f.shape[0] else None, out["iterations"], out["status"])
     return out
 
 
@@ -100,7 +92,7 @@ def boxes_from_matches(ref: dict, query: dict, matches0: torch.Tensor, query_siz
     [B, 4] (the input of ``crop.crop_frames``), view int32 [B], n_matches int32 [B], affine f64 [B, 2, 3] and status int32 [B]:
     1 for the box of the affine, 2 where no view has 6 matches and the box is the reference's [0, 0, H, W], 0 for the empty box
     where the reference fails (the chosen view has no affine) or a corner leaves int32.  No host synchronisation."""
-    dev = _cuda_device(matches0)
+    dev = _lib.cuda_device(matches0)
     rk, rc, rs = _ref_args(ref, dev)
     V, cap_ref = int(rk.shape[0]), int(rk.shape[1])
     qk, qc = query["keypoints"], query["counts"]
@@ -118,11 +110,8 @@ def boxes_from_matches(ref: dict, query: dict, matches0: torch.Tensor, query_siz
     out = {"box": torch.empty(B, 4, dtype=torch.int32, device=dev), "view": torch.empty(B, dtype=torch.int32, device=dev),
            "n_matches": torch.empty(B, dtype=torch.int32, device=dev), "affine": torch.empty(B, 2, 3, dtype=torch.float64, device=dev),
            "status": torch.empty(B, dtype=torch.int32, device=dev)}
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        _lib.check(lib.opb_boxes_from_matches(rk.data_ptr(), rc.data_ptr(), rs.data_ptr(), V, cap_ref, qk.data_ptr(), qc.data_ptr(), int(qk.shape[1]),
-                                              m.data_ptr(), int(m.dtype == torch.int64), B, H, W, out["box"].data_ptr(), out["view"].data_ptr(),
-                                              out["n_matches"].data_ptr(), out["affine"].data_ptr(), out["status"].data_ptr(), _stream(dev)))
+    _lib.call(dev, "opb_boxes_from_matches", rk, rc, rs, V, cap_ref, qk, qc, int(qk.shape[1]), m, int(m.dtype == torch.int64), B, H, W, out["box"],
+              out["view"], out["n_matches"], out["affine"], out["status"])
     return out
 
 

@@ -76,7 +76,7 @@ class SuperPoint(nn.Module):
         cfg = _lib.OpbSpConfig(int(c["descriptor_dim"]), int(c["nms_radius"]), float(c["keypoint_threshold"]), int(c["max_keypoints"]),
                                int(c["remove_borders"]), int(self.align_corners), device.index or 0)
         h = C.c_void_p()
-        _lib.check_sp(self._lib.opb_sp_create(C.byref(cfg), C.byref(h)), None, self._lib)
+        _lib.check(self._lib.opb_sp_create(C.byref(cfg), C.byref(h)))
         self._handle, self._handle_device, self._weights_key = h, device, None
 
     def _sync_weights(self):
@@ -85,8 +85,8 @@ class SuperPoint(nn.Module):
             return
         for name, p in self.named_parameters():
             w = p.detach().to("cpu", torch.float32).contiguous()
-            _lib.check_sp(self._lib.opb_sp_load_weight(self._handle, name.encode(), w.data_ptr(), w.numel()), self._handle, self._lib)
-        _lib.check_sp(self._lib.opb_sp_finalize_weights(self._handle), self._handle, self._lib)
+            _lib.check(self._lib.opb_sp_load_weight(self._handle, name.encode(), w.data_ptr(), w.numel()), self._handle, "extractor")
+        _lib.check(self._lib.opb_sp_finalize_weights(self._handle), self._handle, "extractor")
         self._weights_key = key
 
     def _prepare(self, inp: torch.Tensor):
@@ -117,8 +117,8 @@ class SuperPoint(nn.Module):
         sc = torch.empty(B, cap, dtype=torch.float32, device=dev)
         de = torch.empty(B, 256, cap, dtype=torch.float32, device=dev) if descriptors else None
         cnt = torch.empty(B, dtype=torch.int32, device=dev)
-        _lib.check_sp(self._lib.opb_sp_forward(self._handle, img.data_ptr(), B, H, W, kp.data_ptr(), sc.data_ptr(),
-                                               de.data_ptr() if de is not None else None, cnt.data_ptr(), cap, st), self._handle, self._lib)
+        _lib.check(self._lib.opb_sp_forward(self._handle, img.data_ptr(), B, H, W, kp.data_ptr(), sc.data_ptr(),
+                                            de.data_ptr() if de is not None else None, cnt.data_ptr(), cap, st), self._handle, "extractor")
         return {"keypoints": kp, "scores": sc, "descriptors": de, "counts": cnt}
 
     # ------------------------------------------------------------------ reference contract
@@ -130,15 +130,15 @@ class SuperPoint(nn.Module):
         B, _, H, W = img.shape
         dev = img.device
         cnt = torch.empty(B, dtype=torch.int32, device=dev)
-        _lib.check_sp(self._lib.opb_sp_detect(self._handle, img.data_ptr(), B, H, W, cnt.data_ptr(), st), self._handle, self._lib)
+        _lib.check(self._lib.opb_sp_detect(self._handle, img.data_ptr(), B, H, W, cnt.data_ptr(), st), self._handle, "extractor")
         n = [int(v) for v in cnt.cpu()]
         self.check_range()                 # the read of the counts has synchronised: an out-of-range call raises here
         cap = max(max(n), 1)
         kp = torch.empty(B, cap, 2, dtype=torch.float32, device=dev)
         sc = torch.empty(B, cap, dtype=torch.float32, device=dev)
         de = torch.empty(B, 256, cap, dtype=torch.float32, device=dev)
-        _lib.check_sp(self._lib.opb_sp_describe(self._handle, kp.data_ptr(), sc.data_ptr(), de.data_ptr(), cnt.data_ptr(), cap, st),
-                      self._handle, self._lib)
+        _lib.check(self._lib.opb_sp_describe(self._handle, kp.data_ptr(), sc.data_ptr(), de.data_ptr(), cnt.data_ptr(), cap, st),
+                   self._handle, "extractor")
         return {
             "keypoints": [kp[b, :n[b]] for b in range(B)],
             "scores": [sc[b, :n[b]] for b in range(B)],
@@ -149,14 +149,14 @@ class SuperPoint(nn.Module):
         """Wait for the last call and raise OpbError(OPB_E_RANGE) if an activation left the fp16-split operand range
         (|x| >= 1023) or became NaN; that call reported no key points.  Reporting clears the error."""
         if self._handle is not None:
-            _lib.check_sp(self._lib.opb_sp_check_range(self._handle, None), self._handle, self._lib)
+            _lib.check(self._lib.opb_sp_check_range(self._handle, None), self._handle, "extractor")
 
     # ------------------------------------------------------------------ measurement / test hooks
     def launch_count(self) -> int:
         return int(self._lib.opb_sp_last_launch_count(self._handle)) if self._handle is not None else 0
 
     def set_profiling(self, enable: bool):
-        _lib.check_sp(self._lib.opb_sp_set_profiling(self._handle, int(enable)), self._handle, self._lib)
+        _lib.check(self._lib.opb_sp_set_profiling(self._handle, int(enable)), self._handle, "extractor")
 
     def get_profile(self):
         """[(name, ms, algorithmic flops)] of the launches of the last call (profiling on)."""
@@ -170,11 +170,11 @@ class SuperPoint(nn.Module):
         return out
 
     def debug_stop_after(self, layer: int):
-        _lib.check_sp(self._lib.opb_sp_debug_set_stop(self._handle, int(layer)), self._handle, self._lib)
+        _lib.check(self._lib.opb_sp_debug_set_stop(self._handle, int(layer)), self._handle, "extractor")
 
     def debug_read(self, which: int, capacity: int):
         out = torch.empty(capacity, dtype=torch.float32, device=self._handle_device)
         n = C.c_int64()
         st = torch.cuda.current_stream(self._handle_device).cuda_stream
-        _lib.check_sp(self._lib.opb_sp_debug_read(self._handle, which, out.data_ptr(), capacity, C.byref(n), st), self._handle, self._lib)
+        _lib.check(self._lib.opb_sp_debug_read(self._handle, which, out.data_ptr(), capacity, C.byref(n), st), self._handle, "extractor")
         return out[:n.value]

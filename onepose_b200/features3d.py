@@ -38,16 +38,11 @@ def _as_f32(x, device):
 
 
 def _gather(desc, scores, idx, n_out, device):
-    lib = _lib.load()
     dim, n_src = desc.shape
     out_d = torch.empty(dim, n_out, dtype=torch.float32, device=device)
     out_s = torch.empty(n_out, 1, dtype=torch.float32, device=device)
     n_idx = min(int(idx.numel()) if idx is not None else n_src, n_out)
-    st = torch.cuda.current_stream(device).cuda_stream
-    with torch.cuda.device(device):
-        _lib.check(lib.opb_gather_features3d(desc.data_ptr(), scores.data_ptr(), dim, n_src,
-                                             idx.data_ptr() if idx is not None else None, n_idx,
-                                             out_d.data_ptr(), out_s.data_ptr(), n_out, st))
+    _lib.call(device, "opb_gather_features3d", desc, scores, dim, n_src, idx, n_idx, out_d, out_s, n_out)
     return out_d, out_s
 
 
@@ -87,20 +82,15 @@ def build_features3d_leaves(descriptors, scores, idxs, n_target_shape, num_leaf,
     return _gather(d, s, sel_dev, int(num_leaf) * int(n_target_shape), device)
 
 
-def _segmented(fn_name, values, idxs, D, device):
-    lib = _lib.load()
+def _segmented(name, values, idxs, D, device, *dims):
+    """Entry point ``name`` over the segments of ``values`` -> f64 [n_points, D]; ``dims`` are its arguments after M."""
     device = _dev(device)
     v = torch.as_tensor(np.ascontiguousarray(np.asarray(values, dtype=np.float64)) if not isinstance(values, torch.Tensor) else values)
     v = v.to(device=device, dtype=torch.float64).contiguous()
     lens = torch.as_tensor(np.asarray(idxs, dtype=np.int64)).to(device)
     M = int(lens.numel())
     out = torch.empty(M, D, dtype=torch.float64, device=device)
-    st = torch.cuda.current_stream(device).cuda_stream
-    with torch.cuda.device(device):
-        if fn_name == "desc":
-            _lib.check(lib.opb_segmented_mean_f64(v.data_ptr(), lens.data_ptr(), M, D, out.data_ptr(), st))
-        else:
-            _lib.check(lib.opb_segmented_mean_scores_f64(v.data_ptr(), lens.data_ptr(), M, out.data_ptr(), st))
+    _lib.call(device, name, v, lens, M, *dims, out)
     return out
 
 
@@ -108,10 +98,10 @@ def mean_descriptors(descriptors, idxs, device=None):
     """Average the leaf descriptors of every 3D point: descriptors [sum(idxs), D] fp64 -> [n_points, D] fp64
     (np.mean over each track's rows).  Reference feature_process.py:297-305."""
     D = int(descriptors.shape[1])
-    return _segmented("desc", descriptors, idxs, D, device)
+    return _segmented("opb_segmented_mean_f64", descriptors, idxs, D, device, D)
 
 
 def mean_scores(scores, idxs, device=None):
     """Average the leaf scores of every 3D point: scores [sum(idxs), 1] fp64 -> [n_points, 1] fp64.
     Reference feature_process.py:308-317."""
-    return _segmented("score", scores, idxs, 1, device)
+    return _segmented("opb_segmented_mean_scores_f64", scores, idxs, 1, device)

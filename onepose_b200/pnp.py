@@ -44,14 +44,8 @@ def _hypotheses(method, hypotheses, confidence=None):
     return int(hypotheses)
 
 
-def _cuda_device(t: torch.Tensor) -> torch.device:
-    if t.device.type != "cuda":
-        raise RuntimeError("onepose_b200 has no CPU path: tensors must be on a CUDA device")
-    return t.device
-
-
 def _frames(K, pts2d, pts3d, offsets):
-    dev = _cuda_device(pts2d)
+    dev = _lib.cuda_device(pts2d)
     B = int(offsets.numel()) - 1
     K = K.to(device=dev, dtype=torch.float64).reshape(B, 9).contiguous()
     p2 = pts2d.to(torch.float64).contiguous()
@@ -64,13 +58,10 @@ def epnp_batch(K: torch.Tensor, pts2d: torch.Tensor, pts3d: torch.Tensor, offset
     """EPnP on every correspondence of each frame -- ``cv2.solvePnP(..., flags=SOLVEPNP_EPNP)`` for B frames in one launch.
     Arguments as in ``ransac_pnp_batch``.  Returns (pose [B,3,4] f64, status [B] int32) on the device: status 1 for a pose,
     0 (and the identity pose) for a frame with fewer than 4 pairs or a degenerate point set.  No host synchronisation."""
-    lib = _lib.load()
     dev, B, K, p2, p3, off = _frames(K, pts2d, pts3d, offsets)
     pose = torch.empty(B, 12, dtype=torch.float64, device=dev)
     status = torch.empty(B, dtype=torch.int32, device=dev)
-    st = torch.cuda.current_stream(dev).cuda_stream
-    with torch.cuda.device(dev):
-        _lib.check(lib.opb_epnp(K.data_ptr(), p2.data_ptr(), p3.data_ptr(), off.data_ptr(), B, pose.data_ptr(), status.data_ptr(), st))
+    _lib.call(dev, "opb_epnp", K, p2, p3, off, B, pose, status)
     return pose.reshape(B, 3, 4), status
 
 
@@ -87,13 +78,11 @@ def ransac_pnp_batch(K: torch.Tensor, pts2d: torch.Tensor, pts3d: torch.Tensor, 
     its fp32 inlier count, and a frame stops when OpenCV's would.  ``iterations_out``, an int32 [B] device tensor, then receives
     the number of samples each frame's loop ran (0 for frames of fewer than 6 pairs)."""
     hypotheses = _hypotheses(method, hypotheses, confidence)
-    lib = _lib.load()
     dev, B, K, p2, p3, off = _frames(K, pts2d, pts3d, offsets)
     total = int(p2.shape[0])
     pose = torch.empty(B, 12, dtype=torch.float64, device=dev)
     mask = torch.zeros(max(total, 1), dtype=torch.int32, device=dev)
     cnt = torch.empty(B, dtype=torch.int32, device=dev)
-    st = torch.cuda.current_stream(dev).cuda_stream
     if confidence is not None:
         it = iterations_out
         if it is None:
@@ -101,18 +90,13 @@ def ransac_pnp_batch(K: torch.Tensor, pts2d: torch.Tensor, pts3d: torch.Tensor, 
         elif it.device != dev or it.dtype != torch.int32 or tuple(it.shape) != (B,) or not it.is_contiguous():
             raise ValueError(f"iterations_out must be a contiguous int32 [{B}] tensor on {dev}")
         ws = torch.empty(B * (hypotheses * RECORD_DOUBLES + CV_STATE_DOUBLES), dtype=torch.float64, device=dev)
-        with torch.cuda.device(dev):
-            _lib.check(lib.opb_ransac_epnp_cv(K.data_ptr(), p2.data_ptr(), p3.data_ptr(), off.data_ptr(), B, int(hypotheses),
-                                              float(reproj_error), float(confidence), ws.data_ptr(), pose.data_ptr(), mask.data_ptr(),
-                                              cnt.data_ptr(), it.data_ptr(), st))
+        _lib.call(dev, "opb_ransac_epnp_cv", K, p2, p3, off, B, int(hypotheses), float(reproj_error), float(confidence), ws, pose, mask, cnt, it)
         return pose.reshape(B, 3, 4), mask[:total].bool(), cnt
     if iterations_out is not None:
         raise ValueError("iterations_out is filled by the confidence mode only")
     ws = torch.empty(B * hypotheses * RECORD_DOUBLES, dtype=torch.float64, device=dev)
-    with torch.cuda.device(dev):
-        fn = lib.opb_ransac_pnp if method == "p3p" else lib.opb_ransac_epnp
-        _lib.check(fn(K.data_ptr(), p2.data_ptr(), p3.data_ptr(), off.data_ptr(), B, int(hypotheses), float(reproj_error),
-                      int(seed) & 0xFFFFFFFFFFFFFFFF, ws.data_ptr(), pose.data_ptr(), mask.data_ptr(), cnt.data_ptr(), st))
+    _lib.call(dev, "opb_ransac_pnp" if method == "p3p" else "opb_ransac_epnp", K, p2, p3, off, B, int(hypotheses), float(reproj_error),
+              int(seed) & 0xFFFFFFFFFFFFFFFF, ws, pose, mask, cnt)
     return pose.reshape(B, 3, 4), mask[:total].bool(), cnt
 
 
@@ -124,26 +108,24 @@ def gather_matches(matches0: torch.Tensor, keypoints2d: torch.Tensor, keypoints3
     capacity B*N: pts2d f64 [B*N,2], pts3d f64 [B*N,3], mconf fp32 [B*N] (None without scores), query_index int32 [B*N] and
     offsets int32 [B+1]; frame b owns rows [offsets[b], offsets[b+1]), rows from offsets[B] on are unspecified.  The values are
     exactly the reference's ``kpts2d[valid]``, ``kpts3d[matches[valid]]`` after ``astype(np.float64)``.  No host synchronisation."""
-    lib = _lib.load()
     dev, B, N = _match_batch(matches0)
     kp3 = keypoints3d.to(device=dev, dtype=torch.float32).contiguous()
     if kp3.dim() != 2 or kp3.shape[1] != 3:
         raise ValueError(f"keypoints3d must be [M, 3], got {tuple(kp3.shape)}")
-    return _gather(matches0, keypoints2d, matching_scores0,
-                   lambda m0, sc, kp2, *outs: lib.opb_gather_matches(m0, sc, kp2, kp3.data_ptr(), B, N, int(kp3.shape[0]), *outs))
+    return _gather(matches0, keypoints2d, matching_scores0, "opb_gather_matches", kp3, B, N, int(kp3.shape[0]))
 
 
 def _match_batch(matches0):
-    dev = _cuda_device(matches0)
+    dev = _lib.cuda_device(matches0)
     if matches0.dim() != 2:
         raise ValueError("matches0 must be [B, N]")
     B, N = matches0.shape
     return dev, B, N
 
 
-def _gather(matches0, keypoints2d, matching_scores0, call):
-    """What both gathers share: the keypoints2d and score checks, the outputs, and ``call(matches0, scores, keypoints2d, pts2d,
-    pts3d, mconf, query_index, offsets, stream)`` on device pointers (None for absent scores and mconf)."""
+def _gather(matches0, keypoints2d, matching_scores0, name, *args):
+    """What both gathers share: the keypoints2d and score checks, the outputs, and the call of entry point ``name``, whose
+    arguments between keypoints2d and the outputs are ``args``."""
     dev = matches0.device
     B, N = matches0.shape
     m0 = matches0.to(torch.int64).contiguous()
@@ -158,11 +140,7 @@ def _gather(matches0, keypoints2d, matching_scores0, call):
     out = {"pts2d": torch.empty(B * N, 2, dtype=torch.float64, device=dev), "pts3d": torch.empty(B * N, 3, dtype=torch.float64, device=dev),
            "mconf": torch.empty(B * N, dtype=torch.float32, device=dev) if sc is not None else None,
            "query_index": torch.empty(B * N, dtype=torch.int32, device=dev), "offsets": torch.empty(B + 1, dtype=torch.int32, device=dev)}
-    st = torch.cuda.current_stream(dev).cuda_stream
-    with torch.cuda.device(dev):
-        _lib.check(call(m0.data_ptr(), sc.data_ptr() if sc is not None else None, kp2.data_ptr(), out["pts2d"].data_ptr(),
-                        out["pts3d"].data_ptr(), out["mconf"].data_ptr() if sc is not None else None, out["query_index"].data_ptr(),
-                        out["offsets"].data_ptr(), st))
+    _lib.call(dev, name, m0, sc, kp2, *args, out["pts2d"], out["pts3d"], out["mconf"], out["query_index"], out["offsets"])
     return out
 
 
@@ -172,7 +150,6 @@ def gather_matches_objects(matches0: torch.Tensor, keypoints2d: torch.Tensor, ke
     3D key points ``keypoints3d[object_ids[b]]`` (fp32 [M_b, 3] CUDA tensors; ``keypoints3d`` maps object id -> tensor, a dict
     or a sequence indexed by id), an entry outside [0, M_b) is not a match.  ``object_ids`` is a host sequence (or CPU tensor).
     Same outputs as ``gather_matches``.  The per-frame tables go to the device from pinned memory: no host synchronisation."""
-    lib = _lib.load()
     dev, B, N = _match_batch(matches0)
     ids = [int(i) for i in (object_ids.tolist() if isinstance(object_ids, torch.Tensor) else object_ids)]
     if len(ids) != B:
@@ -189,9 +166,7 @@ def gather_matches_objects(matches0: torch.Tensor, keypoints2d: torch.Tensor, ke
     kp3 = torch.cat(parts, 0).contiguous()
     tab = torch.tensor([first[i][0] for i in ids] + [first[i][1] for i in ids], dtype=torch.int32).pin_memory()
     tab = tab.to(dev, non_blocking=True)
-    return _gather(matches0, keypoints2d, matching_scores0,
-                   lambda m0, sc, kp2, *outs: lib.opb_gather_matches_objects(m0, sc, kp2, kp3.data_ptr(), tab.data_ptr(), tab[B:].data_ptr(), B, N,
-                                                                             *outs))
+    return _gather(matches0, keypoints2d, matching_scores0, "opb_gather_matches_objects", kp3, tab, tab[B:], B, N)
 
 
 def _solve(K, g, B, dev, reproj_error, scale, hypotheses, seed, method, confidence):

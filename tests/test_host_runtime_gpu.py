@@ -1,5 +1,5 @@
 """Host runtime shared by the matcher and extractor handles (csrc/host_util.cuh): launch accounting and the profiling timeline,
-the error codes of weight loading and of create, the separate create-error strings of the two handle kinds, and the return
+the error codes of weight loading and of create, the create-error message both handle kinds report, and the return
 of every device buffer when a handle is destroyed.  Launch counts and FLOPs are pinned to the values the handles have always
 reported: a change to the host code must not move them."""
 import ctypes as C
@@ -142,19 +142,20 @@ def test_weight_errors():
             lib.opb_sp_destroy(s)
 
 
-def test_create_errors_stay_with_their_handle_kind():
+def test_each_failed_create_leaves_its_message_for_both_handle_kinds():
+    """Calls without a handle share one message per thread: opb_last_error(NULL) and opb_sp_last_error(NULL) both give the
+    message of the last failed create, whichever kind it was."""
     lib = _lib.load()
     h = C.c_void_p()
-    cfg = _lib.OpbConfig(256, 4, 0.0, 0.2, 1, 1, 0, 0)                   # scale_factor 0
-    assert lib.opb_create(C.byref(cfg), C.byref(h)) == OPB_E_INVALID
-    scfg = _lib.OpbSpConfig(128, 4, 0.005, -1, 4, 1, 0)                  # descriptor_dim 128
-    assert lib.opb_sp_create(C.byref(scfg), C.byref(h)) == OPB_E_INVALID
-    assert b"scale_factor" in lib.opb_last_error(None) and b"descriptor_dim" in lib.opb_sp_last_error(None)
-    cfg = _lib.OpbConfig(128, 4, 1.0, 0.2, 1, 1, 0, 0)                   # descriptor_dim 128
-    assert lib.opb_create(C.byref(cfg), C.byref(h)) == OPB_E_INVALID
-    scfg = _lib.OpbSpConfig(256, 4, 0.005, 0, 4, 1, 0)                   # max_keypoints 0
-    assert lib.opb_sp_create(C.byref(scfg), C.byref(h)) == OPB_E_INVALID
-    assert b"descriptor_dim" in lib.opb_last_error(None) and b"max_keypoints" in lib.opb_sp_last_error(None)
+
+    def refused(create, cfg, text):
+        assert create(C.byref(cfg), C.byref(h)) == OPB_E_INVALID
+        assert text in lib.opb_last_error(None) and text in lib.opb_sp_last_error(None)
+
+    refused(lib.opb_create, _lib.OpbConfig(256, 4, 0.0, 0.2, 1, 1, 0, 0), b"scale_factor")
+    refused(lib.opb_sp_create, _lib.OpbSpConfig(128, 4, 0.005, -1, 4, 1, 0), b"descriptor_dim")
+    refused(lib.opb_create, _lib.OpbConfig(128, 4, 1.0, 0.2, 1, 1, 0, 0), b"descriptor_dim")
+    refused(lib.opb_sp_create, _lib.OpbSpConfig(256, 4, 0.005, 0, 4, 1, 0), b"max_keypoints")
 
 
 # ----------------------------------------------------------------------------- memory is returned
