@@ -159,17 +159,23 @@ int opb_set_hoist(opb_matcher* m, int32_t enable);
 int opb_set_chunk_frames(opb_matcher* m, int32_t frames);
 
 /* ---- adjacent producers: the per-object feature files the path consumes (SURVEY 8f N2) ---- */
-/* mean_descriptors (reference src/sfm/postprocess/feature_process.py:297-305, fp64):
- * desc device f64 [sum(seg_len), D], seg_len device int64 [M] -> out device f64 [M, D]. */
+/* mean_descriptors (reference src/sfm/postprocess/feature_process.py:297-305, fp64): seg_len device int64 [M] track lengths,
+ * out device f64 [M, D] = np.mean of each track's rows, bit-identical, in the summation order numpy uses for the layout given
+ * (its reduction loop runs along the axis with the smaller stride).  Both sums start from +0.0; a zero-length track gives NaN.
+ * opb_segmented_mean_f64: desc device f64 [sum(seg_len), D] row-major (numpy on C-ordered input, D > 1): the rows are added
+ * in order, one running sum per channel. */
 int opb_segmented_mean_f64(const double* desc, const int64_t* seg_len, int32_t M, int32_t D,
                            double* out, void* stream);
-/* mean_scores (feature_process.py:308-317, fp64): scores device f64 [sum(seg_len)] -> out device f64 [M]
- * (numpy's pairwise summation order reproduced, bit-identical). */
+/* opb_segmented_mean_channels_f64: desc device f64 [D, sum(seg_len)], each channel's observations contiguous (numpy on
+ * F-ordered input such as the transpose of channel-first features, or D = 1): each channel's track is summed pairwise. */
+int opb_segmented_mean_channels_f64(const double* desc, const int64_t* seg_len, int32_t M, int32_t D, double* out, void* stream);
+/* mean_scores (feature_process.py:308-317, fp64): scores device f64 [sum(seg_len)] -> out device f64 [M]; the D = 1 case of
+ * opb_segmented_mean_channels_f64 (pairwise, as numpy sums a contiguous run). */
 int opb_segmented_mean_scores_f64(const double* scores, const int64_t* seg_len, int32_t M, double* out, void* stream);
 /* Column gather of pad_features3d_random / build_features3d_leaves (reference src/utils/data_utils.py:143-205):
  * desc device fp32 [dim, n_src] (channel-first), scores device fp32 [n_src] (may be NULL), idx device int64 [n_idx] = source
  * column of each output column (n_src = the all-ones / zero-score dustbin; NULL = identity) -> desc_out [dim, n_out],
- * scores_out [n_out]; output columns >= n_idx are all-ones / zero padding. */
+ * scores_out [n_out]; output columns >= n_idx are all-ones / zero padding.  dim <= 65535; n_out = 0 writes nothing. */
 int opb_gather_features3d(const float* desc, const float* scores, int32_t dim, int64_t n_src, const int64_t* idx, int64_t n_idx,
                           float* desc_out, float* scores_out, int64_t n_out, void* stream);
 

@@ -95,6 +95,7 @@ SYMBOLS = {
     "opb_get_profile_entry": (C.c_int, [_P, C.c_char_p, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(_I)]),
     "opb_get_profile": (C.c_int, [_P, C.POINTER(C.c_double), C.POINTER(C.c_double), C.POINTER(_I), C.POINTER(C.c_double)]),
     "opb_segmented_mean_f64": (C.c_int, [_P, _P, _I, _I, _P, _P]),
+    "opb_segmented_mean_channels_f64": (C.c_int, [_P, _P, _I, _I, _P, _P]),
     "opb_segmented_mean_scores_f64": (C.c_int, [_P, _P, _I, _P, _P]),
     "opb_gather_features3d": (C.c_int, [_P, _P, _I, C.c_int64, _P, C.c_int64, _P, _P, C.c_int64, _P]),
     "opb_ransac_pnp": (C.c_int, [_P, _P, _P, _P, _I, _I, C.c_double, C.c_uint64, _P, _P, _P, _P, _P]),

@@ -504,16 +504,17 @@ static int forward_frames(opb_matcher* m, ObjectState* const* fobj, const float*
   return OPB_OK;
 }
 
-// A segmented mean: the offsets (exclusive scan of seg_len) in a stream-ordered temporary, then `kern`; the temporary is freed
-// behind it whether or not the launches succeed.
-template <typename... KArgs, typename... Tail>
-static int segmented(const char* fn, const char* name, void (*kern)(KArgs...), unsigned grid, unsigned block, const double* values,
-                     const int64_t* seg_len, int32_t M, cudaStream_t st, Tail... tail) {
+// A segmented mean: the offsets (exclusive scan of seg_len) in a stream-ordered temporary, then segmented_mean_f64; the
+// temporary is freed behind it whether or not the launches succeed.
+static int segmented(const char* fn, const double* x, const int64_t* seg_len, int32_t M, int32_t D, int channel_major, double* out,
+                     cudaStream_t st) {
   const long long* len = reinterpret_cast<const long long*>(seg_len);
   long long* offs = nullptr;
   CK(no_handle_error, cudaMallocAsync(&offs, (size_t)M * sizeof(long long), st));
+  const unsigned grid = (unsigned)std::min<long long>(((long long)M * D + 255) / 256, 1 << 20);   // grid-stride past 2^28 entries
   int rc = launched(fn, "exclusive_scan_i64", launch_k(false, exclusive_scan_i64, 1, 1024, 0, st, len, offs, M));
-  if (rc == OPB_OK) rc = launched(fn, name, launch_k(false, kern, grid, block, 0, st, values, len, offs, M, tail...));
+  if (rc == OPB_OK)
+    rc = launched(fn, "segmented_mean_f64", launch_k(false, segmented_mean_f64, grid, 256, 0, st, x, len, offs, M, D, channel_major, out));
   CK(no_handle_error, cudaFreeAsync(offs, st));
   return rc;
 }
@@ -927,24 +928,29 @@ int opb_last_launch_count(const opb_matcher* m) { return m ? m->last_launches : 
 // ---- adjacent producers ------------------------------------------------------------------
 int opb_segmented_mean_f64(const double* desc, const int64_t* seg_len, int32_t M, int32_t D, double* out, void* stream) {
   REQUIRE(__func__, desc && seg_len && out && M > 0 && D > 0);
-  return segmented(__func__, "segmented_mean_f64", segmented_mean_f64, (unsigned)(((long long)M * 32 + 255) / 256), 256, desc, seg_len, M,
-                   (cudaStream_t)stream, D, out);
+  return segmented(__func__, desc, seg_len, M, D, 0, out, (cudaStream_t)stream);
+}
+
+int opb_segmented_mean_channels_f64(const double* desc, const int64_t* seg_len, int32_t M, int32_t D, double* out, void* stream) {
+  REQUIRE(__func__, desc && seg_len && out && M > 0 && D > 0);
+  return segmented(__func__, desc, seg_len, M, D, 1, out, (cudaStream_t)stream);
 }
 
 int opb_segmented_mean_scores_f64(const double* scores, const int64_t* seg_len, int32_t M, double* out, void* stream) {
   REQUIRE(__func__, scores && seg_len && out && M > 0);
-  return segmented(__func__, "segmented_mean_scores_f64", segmented_mean_scores_f64, (unsigned)((M + 127) / 128), 128, scores, seg_len, M,
-                   (cudaStream_t)stream, out);
+  return segmented(__func__, scores, seg_len, M, 1, 1, out, (cudaStream_t)stream);
 }
 
 int opb_gather_features3d(const float* desc, const float* scores, int32_t dim, int64_t n_src, const int64_t* idx, int64_t n_idx, float* desc_out,
                           float* scores_out, int64_t n_out, void* stream) {
-  REQUIRE(__func__, desc && desc_out && dim > 0 && n_src >= 0 && n_out > 0 && n_idx >= 0 && n_idx <= n_out);
+  REQUIRE(__func__, (desc || n_src == 0) && (desc_out || n_out == 0) && dim > 0 && dim <= 65535 && n_src >= 0 && n_out >= 0 && n_idx >= 0 &&
+                        n_idx <= n_out);   // dim is gridDim.y
+  if (n_out == 0) return OPB_OK;                           // n_target_shape = 0: empty outputs, as the reference gives
   cudaStream_t st = (cudaStream_t)stream;
   const unsigned gx = (unsigned)((n_out + 255) / 256);
   LAUNCH_NH(__func__, gather_columns_f32, dim3(gx, (unsigned)dim), 256, 0, st, desc, dim, (long long)n_src, reinterpret_cast<const long long*>(idx),
             (long long)n_idx, desc_out, (long long)n_out);
-  if (scores && scores_out)
+  if (scores_out && (scores || n_src == 0))                // no source scores: every output score is dustbin or padding
     LAUNCH_NH(__func__, gather_scores_f32, gx, 256, 0, st, scores, (long long)n_src, reinterpret_cast<const long long*>(idx), (long long)n_idx,
               scores_out, (long long)n_out);
   return OPB_OK;

@@ -606,26 +606,9 @@ __global__ void __launch_bounds__(1024) exclusive_scan_i64(const long long* __re
   for (int i = lo; i < hi; ++i) { out[i] = run; run += in[i]; }
 }
 
-// mean_descriptors (feature_process.py:297-305): np.mean(descriptors[start:end], axis=0) for a C-contiguous [len, D] fp64
-// block reduces over the OUTER axis: one running sum per channel, rows added in order, one division.
-// Warp per segment, lanes stride the D channels.
-__global__ void segmented_mean_f64(const double* __restrict__ desc, const long long* __restrict__ seg_len,
-                                   const long long* __restrict__ offsets, int M, int D, double* __restrict__ out) {
-  const int lane = threadIdx.x & 31;
-  const long long seg = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  if (seg >= M) return;
-  const long long start = offsets[seg], len = seg_len[seg];
-  for (int c = lane; c < D; c += 32) {
-    double acc = 0.0;
-    for (long long r = 0; r < len; ++r) acc += desc[(start + r) * D + c];
-    out[seg * D + c] = acc / (double)len;
-  }
-}
-
-// mean_scores (feature_process.py:308-317): np.mean(scores[start:end], axis=0) on a [len, 1] block is a CONTIGUOUS 1-D
-// reduction, which numpy evaluates with its pairwise scheme (numpy/core/src/umath/loops_utils.h: < 8 elements sequential;
-// up to 128: eight interleaved accumulators combined as ((r0+r1)+(r2+r3))+((r4+r5)+(r6+r7)) then the remainder; above: halves
-// rounded down to a multiple of 8, recursively).  Restated here so that the GPU result is bit-identical.  Thread per segment.
+// numpy's pairwise sum of a contiguous run (numpy/core/src/umath/loops_utils.h: < 8 elements sequential; up to 128: eight
+// interleaved accumulators combined as ((r0+r1)+(r2+r3))+((r4+r5)+(r6+r7)) then the remainder; above: halves rounded down to
+// a multiple of 8, recursively).  Restated here so that the GPU result is bit-identical.
 __device__ inline double np_pairwise_sum(const double* a, long long n) {
   if (n < 8) {
     double res = 0.0;
@@ -649,12 +632,28 @@ __device__ inline double np_pairwise_sum(const double* a, long long n) {
   n2 -= n2 % 8;
   return np_pairwise_sum(a, n2) + np_pairwise_sum(a + n2, n - n2);
 }
-__global__ void segmented_mean_scores_f64(const double* __restrict__ scores, const long long* __restrict__ seg_len,
-                                          const long long* __restrict__ offsets, int M, double* __restrict__ out) {
-  const long long seg = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (seg >= M) return;
-  const long long len = seg_len[seg];
-  out[seg] = np_pairwise_sum(scores + offsets[seg], len) / (double)len;
+
+// mean_descriptors / mean_scores (feature_process.py:297-317): np.mean(x[start:end], axis=0) of each track's [len, D] fp64
+// block, in numpy's summation order, which follows the caller's layout (numpy's reduction loop runs along the axis with the
+// smaller stride):
+//   channel_major == 0: x is [sum(len), D] row-major; numpy adds the rows in order, one running sum per channel;
+//   channel_major != 0: x is [D, sum(len)], each channel's track contiguous; numpy sums it pairwise (D = 1 is this case).
+// Both sums start from numpy's identity +0.0 (an all -0.0 track gives +0.0), then one division.  Thread per (track, channel).
+__global__ void segmented_mean_f64(const double* __restrict__ x, const long long* __restrict__ seg_len, const long long* __restrict__ offsets,
+                                   int M, int D, int channel_major, double* __restrict__ out) {
+  const long long n_rows = offsets[M - 1] + seg_len[M - 1];
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < (long long)M * D; i += (long long)gridDim.x * blockDim.x) {
+    const long long seg = i / D;
+    const int c = (int)(i % D);
+    const long long start = offsets[seg], len = seg_len[seg];
+    double acc = 0.0;
+    if (channel_major) {
+      acc += np_pairwise_sum(x + c * n_rows + start, len);
+    } else {
+      for (long long r = 0; r < len; ++r) acc += x[(start + r) * D + c];
+    }
+    out[i] = acc / (double)len;
+  }
 }
 
 // build_features3d_leaves / pad_features3d_random (data_utils.py:143-205): column gather from the channel-first descriptor

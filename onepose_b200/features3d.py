@@ -10,8 +10,8 @@ Mirrors the reference functions (same names, arguments, results):
 The leaf selection of ``build_features3d_leaves`` is defined by numpy's global RNG (one ``np.random.permutation`` per 3D
 point, reference ``:182-192``); the index list is drawn on the host with exactly those calls -- so that the same
 ``np.random.seed`` gives byte-identical tensors -- and the column gather / dustbin / padding run in one CUDA kernel
-(``opb_gather_features3d``).  The segmented means run in fp64 on the device and reproduce numpy's summation order
-(sequential over rows for the [len, 256] descriptors, pairwise for the [len, 1] scores), bit for bit.
+(``opb_gather_features3d``).  The segmented means run in fp64 on the device and reproduce numpy's result bit for bit,
+summation order included; ``_mean`` states the rule.
 
 There is no CPU path: results are CUDA tensors (``inference.py``'s later ``.cuda()`` calls are no-ops on them).
 """
@@ -82,26 +82,45 @@ def build_features3d_leaves(descriptors, scores, idxs, n_target_shape, num_leaf,
     return _gather(d, s, sel_dev, int(num_leaf) * int(n_target_shape), device)
 
 
-def _segmented(name, values, idxs, D, device, *dims):
-    """Entry point ``name`` over the segments of ``values`` -> f64 [n_points, D]; ``dims`` are its arguments after M."""
+def _mean(name, values, idxs, device):
+    """np.mean(values[s:e], axis=0) of every track [s, e) of ``idxs``, bit for bit -> f64 [n_points, D] on the device.
+
+    numpy's reduction loop runs along the axis of ``values`` with the smaller stride, and that sets the summation order:
+      * rows contiguous (a C-ordered [sum(idxs), D] array, or a row-strided or column-sliced view of one), D > 1: numpy adds the
+        rows in order, one running sum per channel;
+      * the reduced axis contiguous (an F-ordered array such as ``obs.T`` of channel-first [D, sum(idxs)] features, a strided
+        view of one, or D = 1): numpy sums each channel's track pairwise.
+    Both sums start from numpy's identity +0.0, so an all -0.0 track gives +0.0; a zero-length track gives NaN.  The layout is
+    read here, before anything is made contiguous, and the device gets the rows (first case) or the channels (second) in
+    order.  Only fp64 is accepted: the reference's producer builds these arrays in fp64 (``np.empty`` / ``np.append``,
+    feature_process.py:143-188), and np.mean of fp32 input accumulates in fp32, which this port does not reproduce."""
     device = _dev(device)
-    v = torch.as_tensor(np.ascontiguousarray(np.asarray(values, dtype=np.float64)) if not isinstance(values, torch.Tensor) else values)
-    v = v.to(device=device, dtype=torch.float64).contiguous()
+    x = values if isinstance(values, torch.Tensor) else np.asarray(values)
+    if x.dtype != (torch.float64 if isinstance(x, torch.Tensor) else np.float64):
+        raise ValueError(f"{name}: values must be fp64 (the reference's feature files hold fp64 arrays), got {x.dtype}")
+    if x.ndim == 1:
+        x = x[:, None]
+    D = int(x.shape[1])
+    s0, s1 = x.stride() if isinstance(x, torch.Tensor) else x.strides
+    pairwise = D == 1 or abs(s0) < abs(s1)
+    if isinstance(x, torch.Tensor):
+        v = (x.T if pairwise else x).to(device).contiguous()
+    else:
+        v = torch.from_numpy(np.ascontiguousarray(x.T if pairwise else x)).to(device)
     lens = torch.as_tensor(np.asarray(idxs, dtype=np.int64)).to(device)
     M = int(lens.numel())
     out = torch.empty(M, D, dtype=torch.float64, device=device)
-    _lib.call(device, name, v, lens, M, *dims, out)
+    _lib.call(device, "opb_segmented_mean_channels_f64" if pairwise else "opb_segmented_mean_f64", v, lens, M, D, out)
     return out
 
 
 def mean_descriptors(descriptors, idxs, device=None):
     """Average the leaf descriptors of every 3D point: descriptors [sum(idxs), D] fp64 -> [n_points, D] fp64
-    (np.mean over each track's rows).  Reference feature_process.py:297-305."""
-    D = int(descriptors.shape[1])
-    return _segmented("opb_segmented_mean_f64", descriptors, idxs, D, device, D)
+    (np.mean over each track's rows, in numpy's summation order for the layout given).  Reference feature_process.py:297-305."""
+    return _mean("mean_descriptors", descriptors, idxs, device)
 
 
 def mean_scores(scores, idxs, device=None):
     """Average the leaf scores of every 3D point: scores [sum(idxs), 1] fp64 -> [n_points, 1] fp64.
     Reference feature_process.py:308-317."""
-    return _segmented("opb_segmented_mean_scores_f64", scores, idxs, 1, device)
+    return _mean("mean_scores", scores, idxs, device)

@@ -25,6 +25,7 @@ def _desc(**fields):
 CASES = [
     # null pointers
     ("opb_segmented_mean_f64", (None, P, 4, 8, P), "desc && seg_len && out"),
+    ("opb_segmented_mean_channels_f64", (P, None, 4, 8, P), "desc && seg_len && out"),
     ("opb_gather_matches", (None, None, P, P, 2, 4, 10, P, P, None, None, P), "N == 0 || (matches0 && keypoints2d && pts2d && pts3d)"),
     ("opb_gather_matches", (P, None, P, P, 2, 4, 10, P, P, P, None, P), "!mconf || mscores0"),
     ("opb_gather_matches_objects", (P, None, P, P, None, P, 2, 4, P, P, None, None, P), "kp3_first && kp3_count"),
@@ -36,6 +37,7 @@ CASES = [
     ("opb_debug_gemm", (None,), "d && d->backend >= 0"),
     # counts <= 0
     ("opb_segmented_mean_f64", (P, P, 4, 0, P), "D > 0"),
+    ("opb_segmented_mean_channels_f64", (P, P, 4, 0, P), "D > 0"),
     ("opb_segmented_mean_scores_f64", (P, P, -1, P), "M > 0"),
     ("opb_gather_features3d", (P, None, 0, 10, None, 10, P, None, 10), "dim > 0"),
     ("opb_gather_matches", (P, None, P, P, 2, -1, 10, P, P, None, None, P), "N >= 0"),
@@ -46,6 +48,7 @@ CASES = [
     ("opb_debug_cv_subsets", (4, 1, 1, P), "n >= 5"),
     # other bounds
     ("opb_gather_features3d", (P, None, 8, 10, None, 11, P, None, 10), "n_idx <= n_out"),
+    ("opb_gather_features3d", (P, None, 65536, 10, None, 10, P, None, 10), "dim <= 65535"),
     ("opb_gather_matches", (P, None, P, P, 65536, 65536, 10, P, P, None, None, P), "(int64_t)B * N <= (int64_t)INT32_MAX"),
     ("opb_crop_resize", (P, 100, 10, 65536, 10, 10, P, P, 16, P, P, P, P), "B <= 65535"),
     ("opb_warp_crop_u8", (P, 100, 10, 65536, 10, 10, P, None, 8, 8, P, P, None), "B <= 65535"),
@@ -103,12 +106,13 @@ def test_a_refused_test_hook_names_itself_and_its_condition(name, args, cond):
 def test_every_handle_free_entry_point_that_can_refuse_is_covered():
     covered = {c[0] for c in CASES + HOOK_CASES}
     assert covered == {
-        "opb_segmented_mean_f64", "opb_segmented_mean_scores_f64", "opb_gather_features3d", "opb_debug_gemm", "opb_debug_set_conv_halo",
+        "opb_segmented_mean_f64", "opb_segmented_mean_channels_f64", "opb_segmented_mean_scores_f64", "opb_gather_features3d",
+        "opb_debug_gemm", "opb_debug_set_conv_halo",
         "opb_gather_matches", "opb_gather_matches_objects", "opb_ransac_pnp", "opb_epnp", "opb_ransac_epnp", "opb_ransac_epnp_cv",
         "opb_debug_set_cv_wave", "opb_debug_set_cv_trace", "opb_debug_cv_subsets", "opb_boxes_from_poses", "opb_crop_resize",
         "opb_warp_crop_u8", "opb_estimate_affine_partial", "opb_boxes_from_matches", "opb_debug_set_affine_trace",
     }
-    assert len(covered | NO_REFUSAL) == 24 and covered | NO_REFUSAL <= set(_lib.SYMBOLS)
+    assert len(covered | NO_REFUSAL) == 25 and covered | NO_REFUSAL <= set(_lib.SYMBOLS)
 
 
 def test_a_later_refusal_replaces_the_message():
