@@ -223,13 +223,12 @@ def test_quirks_and_the_no_model_departure(golden):
     assert not image[0].any() and image[1].any() and torch.equal(K_crop[0], torch.from_numpy(sc["K"]).to(DEV))
 
 
-def _random_case(rng, V, B, cap=300):
+def _random_case(rng, V, B, cap=300, qcap=400):
     sizes = rng.integers(100, 700, (V, 2))
     counts = rng.integers(1, cap + 1, V)
     kp = np.zeros((V, cap, 2), np.float32)
     for v in range(V):
         kp[v, :counts[v]] = np.stack([rng.integers(0, sizes[v, 1], counts[v]), rng.integers(0, sizes[v, 0], counts[v])], 1)
-    qcap = 400
     qc = rng.integers(1, qcap + 1, B)
     qkp = rng.uniform(0, 800, (B, qcap, 2)).astype(np.float32)
     m0 = np.full((B, V, cap), -1, np.int64)
@@ -263,10 +262,30 @@ def _host_boxes(sizes, counts, kp, qc, qkp, m0, hw):
     return out
 
 
-@pytest.mark.parametrize("V,B", [(1, 1), (1, 64), (7, 13), (15, 8), (32, 1), (32, 64)])
-def test_views_and_frames(V, B):
+VIEWS_AND_FRAMES = [(1, 1, 300), (1, 64, 300), (7, 13, 300), (15, 8, 300), (32, 1, 300), (32, 64, 300),
+                    (256, 4, 8192)]        # the most views and reference key points opb_boxes_from_matches takes
+
+
+def _full_view(rng, sizes, counts, kp, qc, qkp, m0, b, v):
+    """View v of frame b with all its cap reference key points matched, half of them to a planted similarity: the winner's pairs
+    fill the kernel's dynamic shared memory (cap * 16 bytes) exactly."""
+    cap = kp.shape[1]
+    counts[v] = cap
+    kp[v] = np.stack([rng.integers(0, sizes[v, 1], cap), rng.integers(0, sizes[v, 0], cap)], 1)
+    qc[b] = max(qc[b], cap)
+    m0[b, v] = rng.choice(qc[b], cap, replace=False)
+    S = np.array([[0.9, 0.2, 30.0], [-0.2, 0.9, 12.0]])
+    qkp[b, m0[b, v, :cap // 2]] = np.round(kp[v, :cap // 2] @ S[:, :2].T + S[:, 2])
+
+
+@pytest.mark.parametrize("V,B,cap", VIEWS_AND_FRAMES, ids=[f"{V}-{B}" if cap == 300 else f"{V}-{B}-{cap}" for V, B, cap in VIEWS_AND_FRAMES])
+def test_views_and_frames(V, B, cap):
+    """Random views and frames against _host_boxes.  At cap = 8192 the query holds 16384 key points, and frame 0's winning view
+    has all 8192 of its key points matched."""
     rng = np.random.default_rng(V * 100 + B)
-    sizes, counts, kp, qc, qkp, m0 = _random_case(rng, V, B)
+    sizes, counts, kp, qc, qkp, m0 = _random_case(rng, V, B, cap, 400 if cap == 300 else 2 * cap)
+    if cap == 8192:
+        _full_view(rng, sizes, counts, kp, qc, qkp, m0, 0, V - 1)
     ref = {"keypoints": torch.from_numpy(kp).to(DEV), "counts": torch.from_numpy(counts).to(DEV), "sizes": torch.from_numpy(sizes).to(DEV)}
     query = {"keypoints": torch.from_numpy(qkp).to(DEV), "counts": torch.from_numpy(qc).to(DEV)}
     out = detect.boxes_from_matches(ref, query, torch.from_numpy(m0).to(DEV), (720, 960))
@@ -277,7 +296,9 @@ def test_views_and_frames(V, B):
             near += 1
             continue
         assert out["box"][b].tolist() == box, (b, out["box"][b], box)
-    print(f"V={V} B={B}: {near} frames with a corner within 1e-9 of an integer")
+    print(f"V={V} B={B} cap={cap}: {near} frames with a corner within 1e-9 of an integer")
+    if cap == 8192:
+        assert int(out["view"][0]) == V - 1 and int(out["n_matches"][0]) == cap and int(out["status"][0]) == 1
     one = detect.boxes_from_matches(ref, {k: v[B - 1:] for k, v in query.items()}, torch.from_numpy(m0[B - 1:]).to(DEV), (720, 960))
     for k in out:
         assert torch.equal(one[k][0], out[k][B - 1]), k
