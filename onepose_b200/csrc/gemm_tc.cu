@@ -11,12 +11,12 @@
 // run together).  384 threads = 12 warps:
 //   warps 0-7    two consumer warpgroups.  Warpgroup w issues wgmma.m64nBNk16 for rows [64 w, 64 w + 64) of the tile and keeps
 //                that accumulator in registers (BN = 256: 128 registers per thread).  At the end of a tile both warpgroups
-//                park their accumulators in shared memory (over the then idle ring) and the same 8 warps run the fused
-//                epilogue as two groups of 4 warps: thread = tile row, group g = half g of the tile's columns,
-//                smem -> registers -> fused op -> swizzled smem staging -> TMA store.  Every epilogue that writes fp16-split
-//                planes goes through one store path (store_planes32: 32 columns, the group's two SWIZZLE_64B buffers).  The
-//                producer starts the next tile's loads once the parked tile has been read (the ring and the parked
-//                accumulator share the shared memory).
+//                park their accumulators in shared memory and the same 8 warps run the fused epilogue as two groups of 4
+//                warps: thread = tile row, group g = half g of the tile's columns, smem -> registers -> fused op -> swizzled
+//                smem staging -> TMA store.  Every epilogue that writes fp16-split planes goes through one store path
+//                (store_planes32: 32 columns, two SWIZZLE_64B buffers).  BN 256 parks in the last k-block's ring stage and
+//                the staging buffers and stages every chunk in place (kStagePark), so the next tile's first k-block loads
+//                into the other stage during the epilogue; narrow tiles park over the ring and load the next tile after it.
 //   warp 8       TMA producer   cp.async.bulk.tensor 2D, SWIZZLE_128B boxes -> a 192 KB shared-memory ring of 2-4 stages
 //   warps 9-11   converters (ACV_NORM_RELU only; in every other variant they go straight to the final __syncthreads)
 // (The registers of a block are allocated in whole warpgroups, so the third warpgroup costs no registers: 168 per thread.)
@@ -48,6 +48,7 @@ constexpr int kABytes = BM * BK * 2;             // one plane of the A tile (16 
 constexpr int kRingBytes = 192 * 1024;           // load ring; also holds the parked fp32 accumulator tile between main loops
 constexpr int kStagingBytes = 16384;             // one 128-row x 128-B swizzled epilogue buffer
 constexpr int kNumStaging = 2;
+constexpr int kParkBoxBytes = 128 * 128;         // BN 256: one 128-row x 32-column fp32 box of the parked accumulator
 constexpr int kExtraBytes = 1024;                // per-tile scratch of the score epilogue (inverse column sums of the tile)
 constexpr int kMaxStages = 4;
 constexpr int kSmemBytes = kRingBytes + kNumStaging * kStagingBytes + 1024 /*align*/ + 256 /*barriers*/ + kExtraBytes;
@@ -212,6 +213,15 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
   constexpr int kHaloStagesDiv = kHaloStages ? kHaloStages : 1;  // (modulus of the halo ring; never used when there is none)
   constexpr int kAccLd = BN + 4;                                 // row stride (floats) of the parked accumulator: conflict-free row reads
   static_assert(BM * kAccLd * 4 <= kRingBytes, "parked accumulator exceeds the ring");
+  // BN 256: the accumulator is parked as eight 128-row x 32-column fp32 SWIZZLE_128B boxes (box b = tile columns [32 b, +32)),
+  // the first kStageBoxes in the ring stage of the tile's last k-block, the rest behind the ring (the staging buffers).  The
+  // other stage stays free, so the next tile's first k-block loads under this tile's epilogue.  The epilogue stages each
+  // chunk's stores in place, in the box it was read from.
+  constexpr bool kStagePark = BN_ == 256;
+  constexpr int kStageBoxes = kStageBytes / kParkBoxBytes;
+  static_assert(!kStagePark || (kStageBytes % kParkBoxBytes == 0 &&
+                                (8 - kStageBoxes) * kParkBoxBytes <= kRingBytes + kNumStaging * kStagingBytes - kStages * kStageBytes),
+                "the parked tile fits one stage and the bytes behind the ring");
   uint8_t* staging = smem + kRingBytes;
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(staging + kNumStaging * kStagingBytes);
   uint64_t* empty_bar = full_bar + kMaxStages;
@@ -249,7 +259,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
     if (lane == 0) {
       uint32_t it = 0, tc = 0;   // k-block counter across all tiles of this CTA, tile counter
       for (int u = blockIdx.x; u < total_units; u += gridDim.x, ++tc) {
-        if (tc) mbar_wait(acc_free_bar, (tc - 1) & 1);            // the previous tile's parked accumulator has been read
+        if (!kStagePark && tc) mbar_wait(acc_free_bar, (tc - 1) & 1);   // the previous tile's parked accumulator has been read
         const int z = u / units_per_batch, rem = u - z * units_per_batch;
         const int m_tile = rem / p.n_tiles, n_tile = rem % p.n_tiles;
         const int row0 = m_tile * BM;
@@ -279,6 +289,10 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
         }
         for (int kb = 0; kb < nkb; ++kb, ++it) {
           const int s = it % kStages;
+          // kStagePark: k-block 0 goes to the stage the previous tile did not park in; k-block 1 refills the parked stage once
+          // the parked tile has been read.  (One k-block per tile: wait before k-block 0, so that the tile's epilogue cannot
+          // complete a second acc_free phase before this wait.)
+          if (kStagePark && tc && kb == (nkb > 1 ? 1 : 0)) mbar_wait(acc_free_bar, (tc - 1) & 1);
           mbar_wait(&empty_bar[s], ((it / kStages) & 1) ^ 1);
           uint8_t* st = smem + s * kStageBytes;
           const bool first = kb < nkb1;
@@ -405,16 +419,24 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
     // one staging buffer per group (the other group's chain overlaps); before the group rewrites it, the store that last
     // read it must be done with it.  Staging rows are written with st.shared on 32-bit addresses (sts128): through generic
     // pointers, ptxas keeps the tile-invariant 64-bit row addresses live across the main loop and spills them there.
-    auto stage_wait = [leader]() {
-      if (leader) tma_store_wait_read<0>();
+    auto stage_wait = [leader]() {                  // (kStagePark: no buffer is reused within a tile)
+      if (!kStagePark && leader) tma_store_wait_read<0>();
     };
-    // fp16-split planes out, one 32-column chunk at (col, row): pair(j) returns the pre-scaled (x 2^6) values of the chunk's
-    // columns 2 j, 2 j + 1 for this thread's row; it runs after the staging buffers are free, in column order
-    auto store_planes32 = [&](int col, int row, auto&& pair) {
-      uint8_t* sh = staging + grp * 8192;           // this group's 8 KB halves of the two staging buffers
-      uint8_t* sl = staging + kStagingBytes + grp * 8192;
+    // kStagePark: box b of the parked tile (the first kStageBoxes in the parked stage, the rest behind the ring)
+    uint8_t* park_stage = smem;
+    auto park_box = [&](int b) {
+      return b < kStageBoxes ? park_stage + b * kParkBoxBytes : smem + kStages * kStageBytes + (b - kStageBoxes) * kParkBoxBytes;
+    };
+    // staging buffer of the chunk at tile column ct: the group's buffer, or (kStagePark) the chunk's own box
+    auto chunk_buf = [&](int ct) { return kStagePark ? park_box(ct >> 5) : staging + grp * kStagingBytes; };
+    // fp16-split planes out, one 32-column chunk at (col, row), tile column ct: pair(j) returns the pre-scaled (x 2^6) values
+    // of the chunk's columns 2 j, 2 j + 1 for this thread's row; it runs after the staging buffers are free, in column order
+    auto store_planes32 = [&](int ct, int col, int row, auto&& pair) {
+      // this group's 8 KB halves of the two staging buffers, or the two halves of the chunk's box
+      uint8_t* sh = kStagePark ? park_box(ct >> 5) : staging + grp * 8192;
+      uint8_t* sl = kStagePark ? sh + 8192 : staging + kStagingBytes + grp * 8192;
       stage_wait();                                 // the store that last read these buffers is done with them
-      epi_bar();
+      epi_bar();                                    // (kStagePark: the group's threads have read every row of the box)
 #pragma unroll
       for (int j8 = 0; j8 < 4; ++j8) {
         uint4 oh, ol;
@@ -532,9 +554,19 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
       if (kSplitAcc) fence_regs<kRegs>(acc_c);
       if (kMainAcc > 1) { fence_regs<kRegs>(acc_m1); fence_regs<kRegs>(acc_m2); }
       if (prev_s >= 0) release(prev_s);
-      // ---- park the accumulator: fragment -> acc_smem [BM][kAccLd] (split accumulators summed with round-to-nearest)
+      // ---- park the accumulator: fragment -> the eight boxes (BN 256), or acc_smem [BM][kAccLd] (narrow tiles: split
+      // accumulators summed with round-to-nearest)
       consumers_bar();                                                // both warpgroups' MMAs have finished reading the ring
-      {
+      if (kStagePark) {
+        park_stage = smem + prev_s * kStageBytes;                     // the last k-block's stage
+        const int r = 64 * wg + 16 * q + (lane >> 2), cq = 2 * (lane & 3);
+#pragma unroll
+        for (int g = 0; g < BN / 8; ++g) {                            // columns 8 g + cq, + 1 of rows r, r + 8
+          float* p0 = reinterpret_cast<float*>(park_box(g >> 2) + stg_off(r, 2 * (g & 3) + (cq >> 2))) + (cq & 3);
+          *reinterpret_cast<float2*>(p0) = make_float2(acc[4 * g], acc[4 * g + 1]);
+          *reinterpret_cast<float2*>(p0 + 8 * 32) = make_float2(acc[4 * g + 2], acc[4 * g + 3]);   // stg_off(r + 8, j) = + 1024 B
+        }
+      } else {
         const int r = 64 * wg + 16 * q + (lane >> 2), cq = 2 * (lane & 3);
 #pragma unroll
         for (int g = 0; g < BN / 8; ++g) {
@@ -550,8 +582,17 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
         }
       }
       consumers_bar();
-      // 32 accumulator columns of this thread's row starting at column c
+      // 32 accumulator columns of this thread's row starting at column c (a multiple of 32)
       auto ld32 = [&](int c, uint32_t (&v)[32]) {
+        if (kStagePark) {
+          const uint32_t box = smem_u32(park_box(c >> 5));
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const float4 f = lds128(box + stg_off(r_in_tile, j));
+            v[4 * j] = __float_as_uint(f.x); v[4 * j + 1] = __float_as_uint(f.y); v[4 * j + 2] = __float_as_uint(f.z); v[4 * j + 3] = __float_as_uint(f.w);
+          }
+          return;
+        }
         const float* src = acc_smem + r_in_tile * kAccLd + c;
 #pragma unroll
         for (int j = 0; j < 8; ++j) {
@@ -574,7 +615,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
           uint32_t v[32];
           ld32(c0, v);
           const int col0 = n_tile * BN + c0;
-          uint8_t* sb = staging + grp * kStagingBytes;
+          uint8_t* sb = chunk_buf(c0);
           stage_wait();                             // the store that last read this buffer is done with it
           epi_bar();
 #pragma unroll
@@ -625,7 +666,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
           ld32(c0, v0);
           ld32(c0 + 32, v1);
           const int col0 = n_tile * BN + c0;
-          uint8_t* sb = staging + grp * kStagingBytes;
+          uint8_t* sb = chunk_buf(c0);
           stage_wait();
           epi_bar();
 #pragma unroll
@@ -714,7 +755,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
           uint32_t v[32];
           ld32(c0, v);
           const int col0 = n_tile * BN + c0;
-          uint8_t* sb = staging + grp * kStagingBytes;
+          uint8_t* sb = chunk_buf(c0);
           float o[32];
 #pragma unroll
           for (int j4 = 0; j4 < 8; ++j4) {
@@ -730,7 +771,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
               if (c > rbest_v) { rbest_v = c; rbest_c = col0 + j; }
             }
           }
-          if (p.conf_tma && leader) tma_store_wait_read<0>();       // the store that last read this group's buffer is done with it
+          if (!kStagePark && p.conf_tma && leader) tma_store_wait_read<0>();   // the store that last read this group's buffer is done with it
           epi_bar();                                                // ... and every thread has finished scanning the previous chunk
 #pragma unroll
           for (int j = 0; j < 8; ++j)
@@ -789,7 +830,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
           uint32_t v[32];
           ld32(c0, v);
           const int col0 = n_tile * BN + c0;
-          store_planes32(col0, out_row0, [&](int j) {
+          store_planes32(c0, col0, out_row0, [&](int j) {
             const float2 bb = p.bias ? __ldg(reinterpret_cast<const float2*>(p.bias + col0) + j) : make_float2(0.f, 0.f);
             float2 sc = make_float2(fmaf(__uint_as_float(v[2 * j]), kPreInv, bb.x * kPre), fmaf(__uint_as_float(v[2 * j + 1]), kPreInv, bb.y * kPre));
             if (relu) sc = make_float2(fmaxf(sc.x, 0.f), fmaxf(sc.y, 0.f));
@@ -819,6 +860,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
             }
           }
           inv_norm = 1.f / fmaxf(sqrtf((ssp[0] + ssp[1]) + (ssp[2] + ssp[3])), 1e-12f);
+          if (kStagePark) consumers_bar();          // both groups have read the whole row before either stages in place
         }
         int src = 0;
         float eps_m = 0.f;
@@ -873,10 +915,12 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
           // two 32-column sub-chunks
 #pragma unroll
           for (int sc = 0; sc < 2; ++sc)
-            store_planes32(col0 + sc * 32, out_row0, [&](int j) { return make_float2(x[sc * 32 + 2 * j] * kPre, x[sc * 32 + 2 * j + 1] * kPre); });
+            store_planes32(c0 + sc * 32, col0 + sc * 32, out_row0, [&](int j) { return make_float2(x[sc * 32 + 2 * j] * kPre, x[sc * 32 + 2 * j + 1] * kPre); });
         }
       }
-      // the next tile's loads refill the ring: order this thread's reads of the parked tile before them
+      // the next tile's loads refill the ring: order this thread's reads of the parked tile before them (kStagePark: and the
+      // stores staged in the boxes have read them)
+      if (kStagePark && leader) tma_store_wait_read<0>();
       fence_async_smem();
       consumers_bar();
       if (threadIdx.x == 0) mbar_arrive(acc_free_bar);
