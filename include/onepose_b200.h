@@ -333,6 +333,15 @@ int opb_boxes_from_poses(const double* K, const double* pose, const double* corn
  *               image) from 16 frame reads; no intermediate image.  The result is the uint8 value / 255 in fp32 (numpy's). */
 int opb_crop_resize(const uint8_t* frames, int64_t frame_pitch, int64_t row_pitch, int32_t B, int32_t H, int32_t W, const int32_t* box,
                     const double* K, int32_t crop_size, float* image, double* K_crop, double* trans, int32_t* status, void* stream);
+/* opb_crop_resize for B crops of n_frames frames (several boxes per frame): crop b reads frame frame_index[b].
+ *   frames        device uint8 [n_frames, H, W] with the pitches of opb_crop_resize
+ *   frame_index   device int32 [B]
+ *   B <= 65535; box, K, crop_size, image, K_crop, trans, status as in opb_crop_resize, per crop.
+ * Crop b equals, bit for bit, opb_crop_resize's crop b of the gathered frames frames[frame_index[b]].  An index outside
+ * [0, n_frames) is rejected as a rejected box is: status 0, a zero image, zero transforms and K_crop = K. */
+int opb_crop_resize_indexed(const uint8_t* frames, int64_t frame_pitch, int64_t row_pitch, int32_t n_frames, int32_t H, int32_t W,
+                            const int32_t* frame_index, int32_t B, const int32_t* box, const double* K, int32_t crop_size, float* image,
+                            double* K_crop, double* trans, int32_t* status, void* stream);
 /* One get_image_crop_resize / get_K_crop_resize (data_utils.py:233-272): box -> [out_h, out_w] by one warp -- the pixel and
  * transform routines opb_crop_resize runs twice.  frames, pitches, box as there; out_h, out_w <= 32767.
  *   out     device uint8 [B, out_h, out_w] out: cv2.warpAffine's image.  frames and out may both be NULL: transforms only
@@ -392,7 +401,27 @@ int opb_boxes_from_matches(const float* ref_keypoints, const int32_t* ref_counts
                            const float* query_keypoints, const int32_t* query_counts, int32_t cap_query, const void* matches0,
                            int32_t matches_int64, int32_t B, int32_t query_h, int32_t query_w, int32_t* box, int32_t* view,
                            int32_t* n_matches, double* affine, int32_t* status, void* stream);
-/* Test hook of both calls above: device buffers later calls fill (NULL to stop), per problem b and for every sample i <
+/* opb_boxes_from_matches for B (frame, object) pairs in one launch, each object against its own reference views.
+ *   ref_keypoints, ref_counts, ref_sizes   the views of every object in one table: [n_views, cap_ref, 2], [n_views], [n_views, 2]
+ *   view_first, view_count   device int32 [B]: pair b's object is views view_first[b] .. view_first[b] + view_count[b] - 1
+ *   V_max                    the matches0 row stride, 1 <= V_max <= 256; view_count[b] <= V_max
+ *   query_keypoints          device fp32 [n_query, cap_query, 2], query_counts device int32 [n_query]: one row per frame
+ *   query_index              device int32 [B]: the query row of pair b, so a frame shared by several pairs is extracted once
+ *   matches0                 device int32 or int64 [B, V_max, cap_ref]: row [b, v] is the matcher's matches0 of pair b's frame
+ *                            against its object's view v (entries past view_count[b] are never read)
+ *   query_h, query_w, box, view, n_matches, affine, status   as in opb_boxes_from_matches; view is the index among pair b's
+ *                            object's views.
+ * Pair b's results equal, bit for bit, those of opb_boxes_from_matches on its object's views alone and its frame's row, and
+ * the trace of opb_debug_set_affine_trace records them as problem b.  A pair whose view range leaves [0, n_views) or whose
+ * view_count is outside [1, V_max] or whose query_index is outside [0, n_query) gets status 0, the empty box, view 0,
+ * n_matches 0 and a zero affine. */
+int opb_boxes_from_matches_objects(const float* ref_keypoints, const int32_t* ref_counts, const int32_t* ref_sizes, int32_t n_views,
+                                   int32_t cap_ref, const int32_t* view_first, const int32_t* view_count, int32_t V_max,
+                                   const float* query_keypoints, const int32_t* query_counts, int32_t n_query, int32_t cap_query,
+                                   const int32_t* query_index, const void* matches0, int32_t matches_int64, int32_t B, int32_t query_h,
+                                   int32_t query_w, int32_t* box, int32_t* view, int32_t* n_matches, double* affine, int32_t* status,
+                                   void* stream);
+/* Test hook of the three calls above: device buffers later calls fill (NULL to stop), per problem b and for every sample i <
  * capacity the loop evaluates: samples int32 [B][capacity][2], counts int32 [B][capacity], models f64 [B][capacity][6] (the
  * unrefined 2-pair model, row-major 2x3). */
 int opb_debug_set_affine_trace(int32_t* samples, int32_t* counts, double* models, int32_t capacity);

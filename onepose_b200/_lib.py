@@ -109,9 +109,12 @@ SYMBOLS = {
     "opb_gather_matches_objects": (C.c_int, [_P, _P, _P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P]),
     "opb_boxes_from_poses": (C.c_int, [_P, _P, _P, _I, _I, _P, _P, _P]),
     "opb_crop_resize": (C.c_int, [_P, C.c_int64, C.c_int64, _I, _I, _I, _P, _P, _I, _P, _P, _P, _P, _P]),
+    "opb_crop_resize_indexed": (C.c_int, [_P, C.c_int64, C.c_int64, _I, _I, _I, _P, _I, _P, _P, _I, _P, _P, _P, _P, _P]),
     "opb_warp_crop_u8": (C.c_int, [_P, C.c_int64, C.c_int64, _I, _I, _I, _P, _P, _I, _I, _P, _P, _P, _P]),
     "opb_estimate_affine_partial": (C.c_int, [_P, _P, _P, _I, C.c_double, _I, C.c_double, _I, _P, _P, _P, _P, _P]),
     "opb_boxes_from_matches": (C.c_int, [_P, _P, _P, _I, _I, _P, _P, _I, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P]),
+    "opb_boxes_from_matches_objects": (C.c_int, [_P, _P, _P, _I, _I, _P, _P, _I, _P, _P, _I, _I, _P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P,
+                                                 _P]),
     "opb_debug_set_affine_trace": (C.c_int, [_P, _P, _P, _I]),
     "opb_debug_set_pdl": (C.c_int, [_I]),
     "opb_debug_set_ws_fill": (C.c_int, [_I]),

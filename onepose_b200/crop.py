@@ -84,34 +84,66 @@ def _boxes(boxes: torch.Tensor, B: int, dev) -> torch.Tensor:
     return boxes.to(dev).contiguous()
 
 
-def crop_frames(frames: torch.Tensor, boxes: torch.Tensor, K: torch.Tensor, crop_size: int = 512) -> dict:
+def _indices(index, n: int, bound: int, name: str, dev) -> torch.Tensor:
+    """An integer [n] sequence or tensor -> contiguous int32 [n] on ``dev``.  Other integer dtypes are clamped to [-1, bound]
+    first, so that no entry wraps into the range the kernels accept (which lies inside [0, bound)); the kernels reject what
+    is out of range.  No host synchronisation for a device tensor."""
+    t = torch.as_tensor(index)
+    if t.dtype.is_floating_point or t.dtype == torch.bool or t.is_complex() or tuple(t.shape) != (n,):
+        raise ValueError(f"{name} must be an integer [{n}] sequence or tensor, got {t.dtype} {list(t.shape)}")
+    t = t.to(dev)
+    if t.dtype != torch.int32:
+        t = t.clamp(-1, bound).to(torch.int32)
+    return t.contiguous()
+
+
+def crop_frames(frames: torch.Tensor, boxes: torch.Tensor, K: torch.Tensor, crop_size: int = 512, frame_index=None) -> dict:
     """``crop_img_by_bbox`` (local_feature_2D_detector.py:160-186) and the ``/ 255`` after it, for B frames: frames uint8 [B,H,W]
     CUDA (full grey camera frames; any row and frame stride, unit pixel stride), boxes int32 [B,4] = [x0, y0, x1, y1], K [3,3] or
     [B,3,3], crop_size S (S % 8 == 0).  Returns device tensors: image fp32 [B,1,S,S] (the extractor's input; the pixels are
     ``cv2.warpAffine``'s), K_crop f64 [B,3,3], trans f64 [B,2,2,3] (T1 and T2: ``T2 @ T1`` in homogeneous form maps a frame
     position into the crop) and status int32 [B]: 0, with a zero image and K_crop = K, for a box with x1 <= x0 or y1 <= y0, a
     side over 32767 or a coordinate beyond 2^20.  A zero image gives no key points, so the failure shows as 0 inliers in the
-    pose of that frame.  No host synchronisation."""
+    pose of that frame.  No host synchronisation.
+
+    With ``frame_index`` (integer [B], on the device for no host synchronisation), frames is [F,H,W] and crop b reads frame
+    frame_index[b]: several boxes per frame, each crop equal to the one ``crop_frames(frames[frame_index], ...)`` makes without
+    the copy.  boxes and K are then per crop; an index outside [0, F) gives status 0 as a rejected box does."""
     dev, B, H, W = _frames_args(frames)
     S = int(crop_size)
     if S <= 0 or S % 8 or S > MAX_SIDE:
         raise ValueError(f"crop_size must be a positive multiple of 8 up to {MAX_SIDE}, got {crop_size!r}")
+    F = B
+    if frame_index is not None:
+        frame_index = torch.as_tensor(frame_index)
+        B = int(frame_index.shape[0]) if frame_index.dim() == 1 else 0
+        if not 0 < B <= MAX_FRAMES:
+            raise ValueError(f"frame_index must be an integer [B] sequence or tensor with 1 <= B <= {MAX_FRAMES}")
+        frame_index = _indices(frame_index, B, F, "frame_index", dev)
     boxes = _boxes(boxes, B, dev)
     K = _per_frame(K, B, (3, 3), "K", dev)
     out = {"image": torch.empty(B, 1, S, S, dtype=torch.float32, device=dev), "K_crop": torch.empty(B, 3, 3, dtype=torch.float64, device=dev),
            "trans": torch.empty(B, 2, 2, 3, dtype=torch.float64, device=dev), "status": torch.empty(B, dtype=torch.int32, device=dev)}
-    _lib.call(dev, "opb_crop_resize", frames, frames.stride(0), frames.stride(1), B, H, W, boxes, K, S, out["image"], out["K_crop"], out["trans"],
-              out["status"])
+    if frame_index is None:
+        _lib.call(dev, "opb_crop_resize", frames, frames.stride(0), frames.stride(1), B, H, W, boxes, K, S, out["image"], out["K_crop"],
+                  out["trans"], out["status"])
+    else:
+        _lib.call(dev, "opb_crop_resize_indexed", frames, frames.stride(0), frames.stride(1), F, H, W, frame_index, B, boxes, K, S, out["image"],
+                  out["K_crop"], out["trans"], out["status"])
     return out
 
 
-def previous_pose_detect(frames: torch.Tensor, K: torch.Tensor, pre_pose: torch.Tensor, bbox3d: torch.Tensor, crop_size: int = 512):
+def previous_pose_detect(frames: torch.Tensor, K: torch.Tensor, pre_pose: torch.Tensor, bbox3d: torch.Tensor, crop_size: int = 512,
+                         frame_index=None):
     """The reference method of this name (local_feature_2D_detector.py:232-259) for B frames on the device: frames uint8 [B,H,W]
     in place of the image path, K, pre_pose and bbox3d as in ``boxes_from_poses``.  Returns its triple (bbox int32 [B,4],
-    image_crop fp32 [B,1,S,S], K_crop f64 [B,3,3]).  No host synchronisation."""
+    image_crop fp32 [B,1,S,S], K_crop f64 [B,3,3]).  No host synchronisation.
+
+    With ``frame_index`` (as in ``crop_frames``), frames is [F,H,W] and B = len(frame_index) objects are cropped from them: K,
+    pre_pose and bbox3d are per object (or shared), and object b's box is cut from frame frame_index[b]."""
     _frames_args(frames)
     bbox = boxes_from_poses(K, pre_pose, bbox3d)
-    out = crop_frames(frames, bbox, K, crop_size)
+    out = crop_frames(frames, bbox, K, crop_size, frame_index)
     return bbox, out["image"], out["K_crop"]
 
 

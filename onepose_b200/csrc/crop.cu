@@ -2,6 +2,7 @@
 // loop (inference_demo.py:193-247).  Replaces, for B frames and without leaving the device,
 //   previous_pose_detect   local_feature_2D_detector.py:232-259   reproj -> min / max -> astype(int32)        opb_boxes_from_poses
 //   crop_img_by_bbox       :160-186   get_K_crop_resize x 2, get_image_crop_resize x 2, then / 255           opb_crop_resize
+//                          the same where crop b reads frame frame_index[b] (several boxes per frame)   opb_crop_resize_indexed
 //   get_image_crop_resize / get_K_crop_resize   data_utils.py:233-272   one cv2.warpAffine, T @ K             opb_warp_crop_u8
 //
 // The pixels are OpenCV's, bit for bit.  cv2.warpAffine(INTER_LINEAR) on 8-bit data with a constant border is integer
@@ -106,16 +107,13 @@ __device__ void apply_to_K(const double* T, const double* K, double* out) {
   for (int c = 0; c < 3; ++c) out[6 + c] = K[6 + c];
 }
 
-// One thread per frame: the transform(s) of the box, K_crop and status.  stages = 2 is crop_img_by_bbox (box -> its own size
-// -> [out_h, out_w]), stages = 1 is one get_image_crop_resize (box -> [out_h, out_w]).  trans [B][stages][6].  A rejected box
-// gives zero transforms, K_crop = K and status 0.  K / K_crop / status may be null.
-__global__ void crop_transforms_kernel(const int32_t* __restrict__ box, const double* __restrict__ K, int B, int stages, int out_h, int out_w,
-                                       double* __restrict__ trans, double* __restrict__ K_crop, int32_t* __restrict__ status) {
-  const int b = blockIdx.x * blockDim.x + threadIdx.x;
-  if (b >= B) return;
+// Crop b of crop_transforms_kernel below; frame_ok false rejects it as a rejected box does.
+__device__ __forceinline__ void crop_transforms(int b, bool frame_ok, const int32_t* __restrict__ box, const double* __restrict__ K, int stages,
+                                                int out_h, int out_w, double* __restrict__ trans, double* __restrict__ K_crop,
+                                                int32_t* __restrict__ status) {
   const int32_t* bx = box + (size_t)b * 4;
   double* T = trans + (size_t)b * stages * 6;
-  const bool ok = box_ok(bx);
+  const bool ok = frame_ok && box_ok(bx);
   if (status) status[b] = ok ? 1 : 0;
   double Kc[9];
   if (K)
@@ -137,6 +135,32 @@ __global__ void crop_transforms_kernel(const int32_t* __restrict__ box, const do
   }
   if (K)
     for (int i = 0; i < 9; ++i) K_crop[(size_t)b * 9 + i] = Kc[i];
+}
+
+// One thread per frame: the transform(s) of the box, K_crop and status.  stages = 2 is crop_img_by_bbox (box -> its own size
+// -> [out_h, out_w]), stages = 1 is one get_image_crop_resize (box -> [out_h, out_w]).  trans [B][stages][6].  A rejected box
+// gives zero transforms, K_crop = K and status 0.  K / K_crop / status may be null.
+__global__ void crop_transforms_kernel(const int32_t* __restrict__ box, const double* __restrict__ K, int B, int stages, int out_h, int out_w,
+                                       double* __restrict__ trans, double* __restrict__ K_crop, int32_t* __restrict__ status) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  crop_transforms(b, true, box, K, stages, out_h, out_w, trans, K_crop, status);
+}
+
+// frame_index[b] names the frame of crop b among n_frames
+__device__ __forceinline__ bool frame_in_range(const int32_t* __restrict__ frame_index, int b, int n_frames) {
+  const int32_t f = frame_index[b];
+  return f >= 0 && f < n_frames;
+}
+
+// crop_transforms_kernel for crop_img_by_bbox (stages = 2) where crop b reads frame frame_index[b]: an index outside
+// [0, n_frames) is rejected as a rejected box is.
+__global__ void crop_transforms_indexed_kernel(const int32_t* __restrict__ box, const int32_t* __restrict__ frame_index, int n_frames,
+                                               const double* __restrict__ K, int B, int out_size, double* __restrict__ trans,
+                                               double* __restrict__ K_crop, int32_t* __restrict__ status) {
+  const int b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= B) return;
+  crop_transforms(b, frame_in_range(frame_index, b, n_frames), box, K, 2, out_size, out_size, trans, K_crop, status);
 }
 
 // warpAffine's inversion of the forward matrix T (imgproc/src/imgwarp.cpp): m maps an output pixel to its source position
@@ -174,22 +198,21 @@ __device__ __forceinline__ int warp_pixel(const double* m, int x, int y, int sw,
   return (acc * 32 + (1 << 14)) >> 15;
 }
 
-// One thread per output pixel of frame blockIdx.y.  stages as in crop_transforms_kernel, whose trans this reads.  The result
-// goes to out_u8 as it is, or to out_f32 as numpy's float32 `/ 255`; a rejected box gives zeros.
-__global__ void __launch_bounds__(kWarpThreads) crop_warp_kernel(const uint8_t* __restrict__ frames, long long frame_pitch, long long row_pitch, int H,
-                                                                 int W, const int32_t* __restrict__ box, const double* __restrict__ trans, int stages,
-                                                                 int out_h, int out_w, uint8_t* __restrict__ out_u8, float* __restrict__ out_f32) {
+// Output pixels of crop b = blockIdx.y from frame f (read only when frame_ok); see crop_warp_kernel below.
+__device__ __forceinline__ void crop_warp(int f, bool frame_ok, const uint8_t* __restrict__ frames, long long frame_pitch, long long row_pitch,
+                                          int H, int W, const int32_t* __restrict__ box, const double* __restrict__ trans, int stages, int out_h,
+                                          int out_w, uint8_t* __restrict__ out_u8, float* __restrict__ out_f32) {
   __shared__ double m[2][6];
   __shared__ int ok;
   const int b = blockIdx.y;
   const int32_t* bx = box + (size_t)b * 4;
-  if (threadIdx.x == 0) ok = box_ok(bx);
+  if (threadIdx.x == 0) ok = frame_ok && box_ok(bx);
   if ((int)threadIdx.x < stages) invert_transform(trans + ((size_t)b * stages + threadIdx.x) * 6, m[threadIdx.x]);
   __syncthreads();
   const long long idx = (long long)blockIdx.x * kWarpThreads + threadIdx.x;
   if (idx >= (long long)out_h * out_w) return;
   const int x = (int)(idx % out_w), y = (int)(idx / out_w);
-  const uint8_t* frame = frames + (size_t)b * frame_pitch;
+  const uint8_t* frame = frames + (size_t)f * frame_pitch;
   auto pixel = [&](int u, int v) { return (int)__ldg(frame + (size_t)v * row_pitch + u); };
   int val = 0;
   if (ok) {
@@ -203,6 +226,25 @@ __global__ void __launch_bounds__(kWarpThreads) crop_warp_kernel(const uint8_t* 
   const size_t o = (size_t)b * out_h * out_w + (size_t)idx;
   if (out_u8) out_u8[o] = (uint8_t)val;
   else out_f32[o] = __fdiv_rn((float)val, 255.f);
+}
+
+// One thread per output pixel of frame blockIdx.y.  stages as in crop_transforms_kernel, whose trans this reads.  The result
+// goes to out_u8 as it is, or to out_f32 as numpy's float32 `/ 255`; a rejected box gives zeros.
+__global__ void __launch_bounds__(kWarpThreads) crop_warp_kernel(const uint8_t* __restrict__ frames, long long frame_pitch, long long row_pitch, int H,
+                                                                 int W, const int32_t* __restrict__ box, const double* __restrict__ trans, int stages,
+                                                                 int out_h, int out_w, uint8_t* __restrict__ out_u8, float* __restrict__ out_f32) {
+  crop_warp(blockIdx.y, true, frames, frame_pitch, row_pitch, H, W, box, trans, stages, out_h, out_w, out_u8, out_f32);
+}
+
+// crop_warp_kernel for crop_img_by_bbox into fp32 where crop blockIdx.y reads frame frame_index[blockIdx.y] of n_frames; an
+// index outside that range gives zeros.
+__global__ void __launch_bounds__(kWarpThreads) crop_warp_indexed_kernel(const uint8_t* __restrict__ frames, long long frame_pitch,
+                                                                         long long row_pitch, int n_frames, int H, int W,
+                                                                         const int32_t* __restrict__ frame_index, const int32_t* __restrict__ box,
+                                                                         const double* __restrict__ trans, int out_size, float* __restrict__ out) {
+  const int b = blockIdx.y;
+  const bool in = frame_in_range(frame_index, b, n_frames);
+  crop_warp(in ? frame_index[b] : 0, in, frames, frame_pitch, row_pitch, H, W, box, trans, 2, out_size, out_size, nullptr, out);
 }
 
 // One thread per frame: vis_utils.reproj (:209-236) of n points, (K_homo @ pose_homo) @ X then the division by the third row, and
@@ -271,6 +313,21 @@ extern "C" int opb_crop_resize(const uint8_t* frames, int64_t frame_pitch, int64
   REQUIRE(__func__, crop_size > 0 && crop_size % 8 == 0 && crop_size <= opb::kMaxSide);
   return opb::launch_crop(__func__, frames, frame_pitch, row_pitch, B, H, W, box, K, 2, crop_size, crop_size, nullptr, image, trans, K_crop, status,
                           stream);
+}
+
+extern "C" int opb_crop_resize_indexed(const uint8_t* frames, int64_t frame_pitch, int64_t row_pitch, int32_t n_frames, int32_t H, int32_t W,
+                                       const int32_t* frame_index, int32_t B, const int32_t* box, const double* K, int32_t crop_size, float* image,
+                                       double* K_crop, double* trans, int32_t* status, void* stream) {
+  REQUIRE(__func__, frames && frame_index && box && K && image && K_crop && trans && status);
+  if (int rc = opb::check_frames(__func__, frame_pitch, row_pitch, B, H, W)) return rc;
+  REQUIRE(__func__, n_frames > 0 && crop_size > 0 && crop_size % 8 == 0 && crop_size <= opb::kMaxSide);
+  cudaStream_t st = (cudaStream_t)stream;
+  LAUNCH_NH(__func__, opb::crop_transforms_indexed_kernel, (unsigned)((B + 127) / 128), 128, 0, st, box, frame_index, n_frames, K, B, crop_size,
+            trans, K_crop, status);
+  const long long blocks = ((long long)crop_size * crop_size + opb::kWarpThreads - 1) / opb::kWarpThreads;
+  LAUNCH_NH(__func__, opb::crop_warp_indexed_kernel, dim3((unsigned)blocks, (unsigned)B), opb::kWarpThreads, 0, st, frames, frame_pitch, row_pitch,
+            n_frames, H, W, frame_index, box, trans, crop_size, image);
+  return OPB_OK;
 }
 
 extern "C" int opb_warp_crop_u8(const uint8_t* frames, int64_t frame_pitch, int64_t row_pitch, int32_t B, int32_t H, int32_t W, const int32_t* box,

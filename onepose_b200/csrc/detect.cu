@@ -3,6 +3,8 @@
 //   cv2.estimateAffinePartial2D(from, to, RANSAC, ...)         calib3d/src/ptsetreg.cpp                 opb_estimate_affine_partial
 //   match_worker + detect_by_matching: per-view match count,   local_feature_2D_detector.py:76-147      opb_boxes_from_matches
 //   the view with the most matches, its affine and box
+//   the same for (frame, object) pairs, each object's views       DESIGN 5.8                               opb_boxes_from_matches_objects
+//   a range of one table of every object's views
 //
 // The estimator is OpenCV's, stage for stage (the model is tests/affine_ransac_reference.py):
 //   samples   cv::RNG((uint64)-1) and getSubset with 2 model points (cv_rng.cuh, the generator of the EPnP loop);
@@ -354,21 +356,24 @@ __global__ void __launch_bounds__(kAffThreads) affine_partial_kernel(const float
   }
 }
 
-// One block per frame b: match_worker's per-view match counts, detect_by_matching's choice, the winner's pairs compacted in
-// ascending reference key-point order (numpy's mask order), the estimator on them, and the box of the view's corners.
-__global__ void __launch_bounds__(kAffThreads) boxes_from_matches_kernel(
-    const float* __restrict__ ref_kp, const int* __restrict__ ref_count, const int* __restrict__ ref_size, int V, int cap_ref,
-    const float* __restrict__ q_kp, const int* __restrict__ q_count, int cap_q, const void* __restrict__ matches0, int matches_int64,
-    int qH, int qW, AffineParams prm, AffineTrace tr, int32_t* __restrict__ box, int32_t* __restrict__ view, int32_t* __restrict__ n_matches,
-    double* __restrict__ affine, int32_t* __restrict__ status) {
+// One block per problem b: match_worker's per-view match counts, detect_by_matching's choice, the winner's pairs compacted in
+// ascending reference key-point order (numpy's mask order), the estimator on them, and the box of the view's corners.  The
+// problem's V views are ref_kp / ref_count / ref_size (already offset to its first view), its matches rows b * v_stride + v of
+// matches0, its query key points row q of q_kp / q_count.  Outputs go to row b.
+__device__ __forceinline__ void boxes_block(int b, const float* __restrict__ ref_kp, const int* __restrict__ ref_count,
+                                            const int* __restrict__ ref_size, int V, int v_stride, int cap_ref, const float* __restrict__ q_kp,
+                                            const int* __restrict__ q_count, int q, int cap_q, const void* __restrict__ matches0,
+                                            int matches_int64, int qH, int qW, const AffineParams& prm, const AffineTrace& tr,
+                                            int32_t* __restrict__ box, int32_t* __restrict__ view, int32_t* __restrict__ n_matches,
+                                            double* __restrict__ affine, int32_t* __restrict__ status) {
   extern __shared__ float4 pairs[];
   __shared__ AffShared sh;
   __shared__ int cnt[kMaxViews];
   __shared__ int warp_n[kAffWarps];
-  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  const long long nq = min(max(q_count[b], 0), cap_q);
+  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const long long nq = min(max(q_count[q], 0), cap_q);
   auto match = [&](int v, int i) -> long long {
-    const size_t o = ((size_t)b * V + v) * cap_ref + i;
+    const size_t o = ((size_t)b * v_stride + v) * cap_ref + i;
     return matches_int64 ? static_cast<const long long*>(matches0)[o] : (long long)static_cast<const int*>(matches0)[o];
   };
   auto n_ref = [&](int v) { return min(max(ref_count[v], 0), cap_ref); };
@@ -421,8 +426,8 @@ __global__ void __launch_bounds__(kAffThreads) boxes_from_matches_kernel(
     }
     if (f) {
       const float* r = ref_kp + ((size_t)win * cap_ref + i) * 2;
-      const float* q = q_kp + ((size_t)b * cap_q + m) * 2;
-      pairs[off + __popc(bal & ((1u << lane) - 1u))] = make_float4(r[0], r[1], q[0], q[1]);
+      const float* p = q_kp + ((size_t)q * cap_q + m) * 2;
+      pairs[off + __popc(bal & ((1u << lane) - 1u))] = make_float4(r[0], r[1], p[0], p[1]);
     }
     n += total;
     __syncthreads();
@@ -449,6 +454,42 @@ __global__ void __launch_bounds__(kAffThreads) boxes_from_matches_kernel(
   status[b] = ok ? 1 : 0;
 }
 
+// One block per frame b against all V views.
+__global__ void __launch_bounds__(kAffThreads) boxes_from_matches_kernel(
+    const float* __restrict__ ref_kp, const int* __restrict__ ref_count, const int* __restrict__ ref_size, int V, int cap_ref,
+    const float* __restrict__ q_kp, const int* __restrict__ q_count, int cap_q, const void* __restrict__ matches0, int matches_int64,
+    int qH, int qW, AffineParams prm, AffineTrace tr, int32_t* __restrict__ box, int32_t* __restrict__ view, int32_t* __restrict__ n_matches,
+    double* __restrict__ affine, int32_t* __restrict__ status) {
+  const int b = blockIdx.x;
+  boxes_block(b, ref_kp, ref_count, ref_size, V, V, cap_ref, q_kp, q_count, b, cap_q, matches0, matches_int64, qH, qW, prm, tr, box, view,
+              n_matches, affine, status);
+}
+
+// One block per (frame, object) pair b: views view_first[b] .. + view_count[b] - 1 of the table of n_views, query row
+// query_index[b] of n_query, matches rows [b, 0 .. view_count[b]) of [B, v_stride, cap_ref].  A pair whose view range or query
+// row is out of bounds gets status 0, the empty box, view 0, n_matches 0 and a zero affine.
+__global__ void __launch_bounds__(kAffThreads) boxes_from_matches_objects_kernel(
+    const float* __restrict__ ref_kp, const int* __restrict__ ref_count, const int* __restrict__ ref_size, int n_views, int cap_ref,
+    const int* __restrict__ view_first, const int* __restrict__ view_count, int v_stride, const float* __restrict__ q_kp,
+    const int* __restrict__ q_count, int n_query, int cap_q, const int* __restrict__ query_index, const void* __restrict__ matches0,
+    int matches_int64, int qH, int qW, AffineParams prm, AffineTrace tr, int32_t* __restrict__ box, int32_t* __restrict__ view,
+    int32_t* __restrict__ n_matches, double* __restrict__ affine, int32_t* __restrict__ status) {
+  const int b = blockIdx.x;
+  const int v0 = view_first[b], V = view_count[b], q = query_index[b];
+  if (v0 < 0 || V < 1 || V > v_stride || v0 > n_views - V || q < 0 || q >= n_query) {
+    if (threadIdx.x == 0) {
+      for (int k = 0; k < 4; ++k) box[(size_t)b * 4 + k] = 0;
+      for (int k = 0; k < 6; ++k) affine[(size_t)b * 6 + k] = 0.0;
+      view[b] = 0;
+      n_matches[b] = 0;
+      status[b] = 0;
+    }
+    return;
+  }
+  boxes_block(b, ref_kp + (size_t)v0 * cap_ref * 2, ref_count + v0, ref_size + (size_t)v0 * 2, V, v_stride, cap_ref, q_kp, q_count, q, cap_q,
+              matches0, matches_int64, qH, qW, prm, tr, box, view, n_matches, affine, status);
+}
+
 int check_params(const char* fn, double threshold, int32_t max_iters, double confidence, int32_t refine_iters) {
   REQUIRE(fn, isfinite(threshold) && max_iters >= 0 && confidence > 0.0 && confidence < 1.0 && refine_iters >= 0);
   return OPB_OK;
@@ -461,7 +502,7 @@ AffineParams make_params(double threshold, int32_t max_iters, double confidence,
 }  // namespace
 }  // namespace opb
 
-// test hook: device buffers later calls of both entry points fill (NULL to stop); see the header
+// test hook: device buffers later calls of the three entry points fill (NULL to stop); see the header
 static int32_t* g_aff_trace_samples = nullptr;
 static int32_t* g_aff_trace_counts = nullptr;
 static double* g_aff_trace_models = nullptr;
@@ -501,5 +542,24 @@ extern "C" int opb_boxes_from_matches(const float* ref_keypoints, const int32_t*
   LAUNCH_NH(__func__, opb::boxes_from_matches_kernel, (unsigned)B, opb::kAffThreads, smem, (cudaStream_t)stream, ref_keypoints, ref_counts, ref_sizes,
             V, cap_ref, query_keypoints, query_counts, cap_query, matches0, matches_int64, query_h, query_w,
             opb::make_params(6.0, 2000, 0.99, 10), aff_trace(), box, view, n_matches, affine, status);
+  return OPB_OK;
+}
+
+extern "C" int opb_boxes_from_matches_objects(const float* ref_keypoints, const int32_t* ref_counts, const int32_t* ref_sizes, int32_t n_views,
+                                              int32_t cap_ref, const int32_t* view_first, const int32_t* view_count, int32_t V_max,
+                                              const float* query_keypoints, const int32_t* query_counts, int32_t n_query, int32_t cap_query,
+                                              const int32_t* query_index, const void* matches0, int32_t matches_int64, int32_t B, int32_t query_h,
+                                              int32_t query_w, int32_t* box, int32_t* view, int32_t* n_matches, double* affine, int32_t* status,
+                                              void* stream) {
+  REQUIRE(__func__, ref_keypoints && ref_counts && ref_sizes && view_first && view_count && query_keypoints && query_counts && query_index &&
+                        matches0 && box && view && n_matches && affine && status);
+  REQUIRE(__func__, n_views > 0 && cap_ref > 0 && cap_ref <= opb::kMaxRefPoints && V_max > 0 && V_max <= opb::kMaxViews);
+  REQUIRE(__func__, n_query > 0 && cap_query > 0 && B > 0);
+  REQUIRE(__func__, (matches_int64 == 0 || matches_int64 == 1) && query_h > 0 && query_w > 0);
+  const size_t smem = (size_t)cap_ref * sizeof(float4);
+  CK(opb::no_handle_error, cudaFuncSetAttribute(opb::boxes_from_matches_objects_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  LAUNCH_NH(__func__, opb::boxes_from_matches_objects_kernel, (unsigned)B, opb::kAffThreads, smem, (cudaStream_t)stream, ref_keypoints, ref_counts,
+            ref_sizes, n_views, cap_ref, view_first, view_count, V_max, query_keypoints, query_counts, n_query, cap_query, query_index, matches0,
+            matches_int64, query_h, query_w, opb::make_params(6.0, 2000, 0.99, 10), aff_trace(), box, view, n_matches, affine, status);
   return OPB_OK;
 }
