@@ -426,6 +426,55 @@ int opb_boxes_from_matches_objects(const float* ref_keypoints, const int32_t* re
  * unrefined 2-pair model, row-major 2x3). */
 int opb_debug_set_affine_trace(int32_t* samples, int32_t* counts, double* models, int32_t capacity);
 
+/* ---- the tracker's flow step: an object's keyframe points followed into the next crop (ba_tracker.py:113-126, 295-356) ----
+ * Caller's current device and stream, device pointers, asynchronous, no host synchronisation, no allocation.
+ *
+ * cv2.calcOpticalFlowPyrLK(prev[b], next[b], pts, None, winSize=(win_w, win_h), maxLevel=max_level,
+ * criteria=(criteria_type, max_count, epsilon), flags=0, minEigThreshold=min_eig_threshold) for B image pairs:
+ *   prev, next    device uint8 [B, H, W] grey images with the given frame and row pitches in bytes (row pitch >= W)
+ *   sizes         device int32 [B, 2] = (h_b, w_b) <= (H, W): pair b's images are the top-left h_b x w_b of its slots (an entry
+ *                 outside [1, H] x [1, W] is clamped into it); NULL: every pair is H x W.  H, W <= 32767, B <= 65535
+ *   pts, offsets  device fp32 [total, 2] (x, y), int32 [B + 1]: pair b owns rows offsets[b] .. offsets[b + 1] - 1, offsets[0] =
+ *                 0 and offsets[B] = total
+ *   win_w, win_h  odd, 3 .. 31;  max_level 0 .. 4 (fewer levels where cv2 builds fewer: see the pyramid below)
+ *   criteria_type 1 (COUNT), 2 (EPS) or 3; max_count 1 .. 100 with COUNT (30 without), epsilon >= 0 with EPS (0.01 without;
+ *                 clamped to 10); flags must be 0 (OPTFLOW_USE_INITIAL_FLOW and OPTFLOW_LK_GET_MIN_EIGENVALS are refused)
+ *   workspace     device, at least opb_optical_flow_workspace_bytes(B, H, W, max_level) bytes; after the call it holds the
+ *                 pyramids: per pair a slot of pair_bytes = that size / B, and in it per level l = 0 .. max_level of an
+ *                 H x W pyramid (h_l = ceil(h_{l-1} / 2), likewise w_l) the Scharr derivatives of prev int16 [h_l, w_l, 2],
+ *                 then for l >= 1 prev and next uint8 [h_l, w_l], each starting at a multiple of 16 bytes.  A smaller pair
+ *                 fills the top-left corner of each level (row pitch w_l); levels past its last are not written.
+ *   next_pts, status, err   device fp32 [total, 2], uint8 [total], fp32 [total] out
+ * The results are cv2's, bit for bit for status, points and err (OpenCV 4.13; the model is tests/lk_reference.py):
+ *   pyramid      level l+1 = cv2.pyrDown(level l), BORDER_REFLECT_101; a pair stops after level l when level l+1 would have a
+ *                side <= the window's (cv2.buildOpticalFlowPyramid's return value)
+ *   derivatives  cv2.Scharr dx / dy of each prev level as int16, BORDER_REFLECT_101; windows read images through
+ *                BORDER_REFLECT_101 and derivatives through a zero border
+ *   per point    from the coarsest level: 14-bit bilinear weights, the structure tensor and mismatch vector summed in fp32 in
+ *                OpenCV's SIMD order, the minimum-eigenvalue test, up to max_count Newton steps (stop at |d|^2 <= eps^2, or
+ *                half a step back when two steps cancel to < 0.01), the guess doubled level to level
+ *   status       0 for a point that starts or ends outside the level-0 image or fails the eigenvalue test at level 0
+ *   err          mean |next - prev| over the window in grey levels; 0 where status is 0 (cv2 leaves it unset there) */
+int opb_optical_flow_workspace_bytes(int32_t B, int32_t H, int32_t W, int32_t max_level, int64_t* bytes);
+int opb_calc_optical_flow_pyr_lk(const uint8_t* prev, int64_t prev_frame_pitch, int64_t prev_row_pitch, const uint8_t* next,
+                                 int64_t next_frame_pitch, int64_t next_row_pitch, int32_t B, int32_t H, int32_t W, const int32_t* sizes,
+                                 const float* pts, const int32_t* offsets, int32_t total, int32_t win_w, int32_t win_h, int32_t max_level,
+                                 int32_t criteria_type, int32_t max_count, double epsilon, double min_eig_threshold, int32_t flags,
+                                 void* workspace, int64_t workspace_bytes, float* next_pts, uint8_t* status, float* err, void* stream);
+/* np.where(status == 1) of B tracks, kpt_flow_track's valid ids (ba_tracker.py:122-124) applied to both point lists:
+ *   status, pts2d, pts3d   device uint8 [B, cap], fp32 [B, cap, 2], fp32 [B, cap, 3]; track b's rows are 0 .. counts[b] - 1
+ *   counts                 device int32 [B] (clamped to [0, cap])
+ *   out2d, out3d           device f64 [B * cap, 2], [B * cap, 3] out: the kept rows, track-major, in row order
+ *   offsets, n_tracked     device int32 [B + 1], [B] out: track b's kept rows are offsets[b] .. offsets[b + 1] - 1
+ *   pad2d, pad3d           device fp32 [B, cap, 2], [B, cap, 3] out: track b's kept rows first, then zeros */
+int opb_flow_compact(const uint8_t* status, const float* pts2d, const float* pts3d, const int32_t* counts, int32_t B, int32_t cap,
+                     double* out2d, double* out3d, int32_t* offsets, int32_t* n_tracked, float* pad2d, float* pad3d, void* stream);
+/* flow_track's kpt_dist (ba_tracker.py:326-327): per track b, the fp64 mean over rows offsets[b] .. offsets[b + 1] - 1 of
+ * |project(pts3d, K[b], pose[b]) - pts2d| (tracking_utils.project: X R^T + t, then K, then x / z); NaN for a track without
+ * rows.  K f64 [B, 9], pose f64 [B, 12] (row-major 3x4), pts2d f64 [n, 2], pts3d f64 [n, 3], dist f64 [B] out. */
+int opb_flow_reprojection(const double* K, const double* pose, const double* pts2d, const double* pts3d, const int32_t* offsets, int32_t B,
+                          double* dist, void* stream);
+
 /* ---- adjacent producer: SuperPoint key-point extractor (SURVEY 8f N4) ----
  * Replaces SuperPoint.forward (reference src/models/extractors/SuperPoint/superpoint.py:140-197): shared VGG-style encoder
  * (:142-152), score head + 65-way softmax + 8x8 pixel shuffle (:155-160), simple_nms (:47-61, :161), threshold / border /

@@ -116,6 +116,11 @@ SYMBOLS = {
     "opb_boxes_from_matches_objects": (C.c_int, [_P, _P, _P, _I, _I, _P, _P, _I, _P, _P, _I, _I, _P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P,
                                                  _P]),
     "opb_debug_set_affine_trace": (C.c_int, [_P, _P, _P, _I]),
+    "opb_optical_flow_workspace_bytes": (C.c_int, [_I, _I, _I, _I, C.POINTER(C.c_int64)]),
+    "opb_calc_optical_flow_pyr_lk": (C.c_int, [_P, C.c_int64, C.c_int64, _P, C.c_int64, C.c_int64, _I, _I, _I, _P, _P, _P, _I, _I, _I, _I, _I, _I,
+                                               C.c_double, C.c_double, _I, _P, C.c_int64, _P, _P, _P, _P]),
+    "opb_flow_compact": (C.c_int, [_P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P, _P]),
+    "opb_flow_reprojection": (C.c_int, [_P, _P, _P, _P, _P, _I, _P, _P]),
     "opb_debug_set_pdl": (C.c_int, [_I]),
     "opb_debug_set_ws_fill": (C.c_int, [_I]),
     "opb_debug_set_kv_passes": (C.c_int, [_P, _I]),

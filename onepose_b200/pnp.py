@@ -181,7 +181,7 @@ def _solve(K, g, B, dev, reproj_error, scale, hypotheses, seed, method, confiden
     pose_homo[:, :3] = pose
     pose_homo[:, 3, 3] = 1.0
     out = {"pose": pose, "pose_homo": pose_homo, "n_inliers": cnt, "inlier_mask": mask, "query_index": g["query_index"],
-           "mconf": g["mconf"], "offsets": g["offsets"]}
+           "mconf": g["mconf"], "offsets": g["offsets"], "pts2d": g["pts2d"], "pts3d": g["pts3d"]}
     if its is not None:
         out["iterations"] = its
     return out
@@ -205,8 +205,8 @@ def poses_from_matches(K: torch.Tensor, keypoints2d: torch.Tensor, keypoints3d: 
     ``gather_matches``.  ``scale`` multiplies the 3D points before the solve and divides the translation after it, as
     ``ransac_PnP(..., scale=1000)`` does in the reference.  A frame with fewer than 4 pairs, or no model, gets the identity pose
     and 0 inliers.  ``method`` / ``hypotheses`` / ``confidence`` as in ``ransac_pnp_batch``.  Returns a dict: pose [B,3,4] and
-    pose_homo [B,4,4] f64, n_inliers int32 [B], inlier_mask bool [B*N], query_index, mconf and offsets (rows indexed as in
-    ``gather_matches``), and with ``confidence`` also iterations int32 [B] (the samples each frame's loop ran)."""
+    pose_homo [B,4,4] f64, n_inliers int32 [B], inlier_mask bool [B*N], query_index, mconf, offsets and the gathered pairs
+    pts2d / pts3d (rows indexed as in ``gather_matches``; pts3d unscaled), and with ``confidence`` also iterations int32 [B] (the samples each frame's loop ran)."""
     hypotheses = _hypotheses(method, hypotheses, confidence)
     g = gather_matches(matches0, keypoints2d, keypoints3d, matching_scores0)
     return _solve(K, g, int(matches0.shape[0]), matches0.device, reproj_error, scale, hypotheses, seed, method, confidence)
