@@ -8,8 +8,18 @@
 // computes in fp32 (GATs_SuperGlue.py:191-193) and the contract is 1e-4 abs on conf.
 //
 // Persistent grid (at most one CTA per SM), static round-robin tile schedule (n-tile fastest so CTAs that share an A row tile
-// run together).  384 threads = 12 warps:
-//   warps 0-7    two consumer warpgroups.  Warpgroup w issues wgmma.m64nBNk16 for rows [64 w, 64 w + 64) of the tile and keeps
+// run together).  Two consumer schedules:
+//   ping-pong (PP: EPI_F32 / EPI_F32_STATS / EPI_SCORE_SUMS)  128 x 128 tiles; warpgroup w owns the
+//                CTA's units w, w + 2, ... whole (two m64n128 accumulators: rows [0, 64) and [64, 128), 128 registers per
+//                thread).  An order barrier (two mbarriers) hands the tensor pipe to the other warpgroup once a warpgroup has
+//                issued its tile's last MMAs, so one warpgroup's epilogue runs under the other's main loop.  The epilogue
+//                walks the tile in 32-column chunks through the warpgroup's own 16 KB staging box: fragment -> box ->
+//                thread = row -> fused op -> staged in place -> TMA store.  Ring: 3 stages of 64 KB.
+//   cooperative  every other variant.  EPI_L2NORM needs a row's 256 columns; the epilogues of EPI_QKV, EPI_QSCALE and
+//                EPI_SCORE_CONF need more registers than a live 128-register accumulator leaves (they spill as PP).  The
+//                converter (mlp.3), EPI_BIAS_PLANES and the extractor's narrow EPI_CONV / EPI_F32 tiles were not measured as PP.
+// 384 threads = 12 warps:
+//   warps 0-7    two consumer warpgroups.  Cooperative: warpgroup w issues wgmma.m64nBNk16 for rows [64 w, 64 w + 64) of the tile and keeps
 //                that accumulator in registers (BN = 256: 128 registers per thread).  At the end of a tile both warpgroups
 //                park their accumulators in shared memory and the same 8 warps run the fused epilogue as two groups of 4
 //                warps: thread = tile row, group g = half g of the tile's columns, smem -> registers -> fused op -> swizzled
@@ -177,10 +187,13 @@ enum { ACV_NONE = 0, ACV_NORM_RELU = 1 };
 // insert a warpgroup.arrive in front of the MMAs that follow it.
 enum { K2_FULL = 0, K2_LO_ZERO = 1, K2_DIAG = 2 };
 
-template <int EPI, int ACV = ACV_NONE, bool HI = false, int BN_ = 256, int K2B = K2_FULL>
+// PP: the ping-pong schedule (BN_ 128; see the top of the file).
+template <int EPI, int ACV = ACV_NONE, bool HI = false, int BN_ = 256, int K2B = K2_FULL, bool PP = false>
 __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_constant__ Maps maps, TcParams p) {
   constexpr int BN = BN_;
   constexpr bool DIAG = K2B == K2_DIAG;
+  static_assert(!PP || (BN_ == 128 && ACV == ACV_NONE && !HI && K2B == K2_FULL && (EPI == EPI_F32 || EPI == EPI_F32_STATS || EPI == EPI_SCORE_SUMS)),
+                "ping-pong: 128-column tiles of the variants that move");
   constexpr int kBBytes = BN * BK * 2;             // one plane of the B tile
   constexpr int kBOff = HI ? kABytes : 2 * kABytes;      // offset of the B planes inside a stage
   constexpr int kStageBytes = kBOff + 2 * kBBytes;
@@ -188,8 +201,8 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
   constexpr int kDiagBBytes = 64 * BK * 2;         // a 64 x 64 diagonal block of the identity
   static_assert(K2B == K2_FULL || (BN_ == 256 && EPI == EPI_BIAS_PLANES && ACV == ACV_NORM_RELU), "identity K-block: mlp.3 only");
   static_assert(ACV == ACV_NONE || K2B != K2_FULL, "the converter comes with the identity K-block");
-  static_assert(EPI == EPI_CONV ? BN_ == 64 || BN_ == 128 : EPI == EPI_F32 ? BN_ == 128 || BN_ == 256 : BN_ == 256,
-                "tile widths: EPI_CONV 64 / 128, EPI_F32 128 / 256, every other epilogue 256");
+  static_assert(PP || (EPI == EPI_CONV ? BN_ == 64 || BN_ == 128 : EPI == EPI_F32 ? BN_ == 128 || BN_ == 256 : BN_ == 256),
+                "tile widths: EPI_CONV 64 / 128, EPI_F32 128 / 256, every other cooperative epilogue 256");
   static_assert(BN_ == 256 || ACV == ACV_NONE && !HI, "narrow tiles: no converter, both A planes");
   static_assert(!HI || ACV == ACV_NONE, "converters need the full stage");
   static_assert(kStages >= 2 && kStages <= kMaxStages, "ring depth");
@@ -207,7 +220,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
   // Split accumulators (narrow tiles only).  The two correction passes (A_hi.B_lo, A_lo.B_hi: 2^-11 of the main term) get an
   // accumulator of their own, and with 64-wide tiles the main term is further split by kernel row; the partial sums are added
   // with round-to-nearest when the tile is parked -- fewer accumulate steps at full magnitude per fp32 accumulator.
-  constexpr bool kSplitAcc = BN_ != 256;
+  constexpr bool kSplitAcc = BN_ != 256 && !PP;
   constexpr int kMainAcc = BN_ == 64 ? 3 : 1;                    // accumulators of the A_hi.B_hi term (3: one per kernel row of a 3x3 convolution)
   const int n_main = (kMainAcc > 1 && EPI == EPI_CONV && p.taps == 9) ? kMainAcc : 1;
   constexpr int kHaloStagesDiv = kHaloStages ? kHaloStages : 1;  // (modulus of the halo ring; never used when there is none)
@@ -227,11 +240,11 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
   uint64_t* empty_bar = full_bar + kMaxStages;
   uint64_t* acc_free_bar = empty_bar + kMaxStages;   // the parked accumulator has been read: the ring may be refilled
   uint64_t* conv_bar = acc_free_bar + 1;             // ACV: the stage's A tile has been converted (every k-block of the stage arrives)
+  uint64_t* order_bar = conv_bar + kMaxStages;       // PP: order_bar[w] = the other warpgroup has issued its tile's last MMAs
   float* extra = reinterpret_cast<float*>(staging + kNumStaging * kStagingBytes + 256);   // kExtraBytes of per-tile scratch
   float* acc_smem = reinterpret_cast<float*>(smem);  // parked accumulator [BM][kAccLd]
 
-  constexpr int kEpiGroups = 2;
-  constexpr int kColsPerGroup = BN / kEpiGroups;
+  constexpr int kColsPerGroup = PP ? BN : BN / 2;    // columns of a tile that one epilogue group (warpgroup) writes
   // warp index through a shuffle: provably warp-uniform, so the wgmma issue paths below are not treated as divergent
   const int warp = __shfl_sync(0xffffffffu, threadIdx.x >> 5, 0), lane = threadIdx.x & 31;
   const int nkb1 = p.K1 / BK, nkb = (p.K1 + p.K2) / BK;
@@ -239,9 +252,12 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
   const int total_units = units_per_batch * p.batch;
 
   if (threadIdx.x == 0) {
-    // full: the TMA transaction arrive; empty: one arrive per consumer warp; conv: one arrive per converter warp
-    for (int s = 0; s < kMaxStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], 8); mbar_init(&conv_bar[s], kConvWarps); }
+    // full: the TMA transaction arrive; empty: one arrive per consumer warp that reads the stage; conv: one arrive per
+    // converter warp; order: one arrive per warp of the other warpgroup
+    for (int s = 0; s < kMaxStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], PP ? 4 : 8); mbar_init(&conv_bar[s], kConvWarps); }
     mbar_init(acc_free_bar, 1);
+    mbar_init(&order_bar[0], 4);
+    mbar_init(&order_bar[1], 4);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
   if (warp == kProducerWarp && lane == 0) {
@@ -259,7 +275,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
     if (lane == 0) {
       uint32_t it = 0, tc = 0;   // k-block counter across all tiles of this CTA, tile counter
       for (int u = blockIdx.x; u < total_units; u += gridDim.x, ++tc) {
-        if (!kStagePark && tc) mbar_wait(acc_free_bar, (tc - 1) & 1);   // the previous tile's parked accumulator has been read
+        if (!kStagePark && !PP && tc) mbar_wait(acc_free_bar, (tc - 1) & 1);   // the previous tile's parked accumulator has been read
         const int z = u / units_per_batch, rem = u - z * units_per_batch;
         const int m_tile = rem / p.n_tiles, n_tile = rem % p.n_tiles;
         const int row0 = m_tile * BM;
@@ -394,10 +410,13 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
     }
   } else {
     // ===================== consumers: MMA main loop, then the epilogue =====================
-    const int wg = warp >> 2;                 // consumer warpgroup = rows [64 wg, +64) of the MMA, columns half wg of the epilogue
+    // cooperative: warpgroup wg = rows [64 wg, +64) of the MMA, columns half wg of the epilogue; PP: every row and column of
+    // its own tiles
+    const int wg = warp >> 2;
     const int q = warp & 3;                   // warp within the warpgroup
-    const uint32_t a_off = (uint32_t)wg * 64 * 128; // this warpgroup's rows inside an A box (8-row groups of 1024 B)
-    constexpr int kRegs = BN / 2;                   // accumulator registers per thread of one m64nBN accumulator
+    const uint32_t a_off = PP ? 0u : (uint32_t)wg * 64 * 128; // this warpgroup's rows inside an A box (8-row groups of 1024 B)
+    constexpr uint32_t kHalfOff = 64 * 128;         // PP: rows [64, 128) of an A box
+    constexpr int kRegs = PP ? BN : BN / 2;         // accumulator registers per thread (PP: two m64n128 accumulators)
     float acc[kRegs];                               // main term (BN 64, 3x3 convolution: kernel row 0)
     float acc_c[kSplitAcc ? kRegs : 1];             // split accumulators: correction passes
     float acc_m1[kMainAcc > 1 ? kRegs : 1], acc_m2[kMainAcc > 1 ? kRegs : 1];   // BN 64: kernel rows 1, 2
@@ -414,7 +433,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
     const int r_in_tile = q * 32 + lane;
     const int t_in_grp = threadIdx.x - grp * 128;
     const bool leader = t_in_grp == 0;
-    const int c_begin = grp * kColsPerGroup, c_end = c_begin + kColsPerGroup;
+    const int c_begin = PP ? 0 : grp * kColsPerGroup, c_end = c_begin + kColsPerGroup;
     auto epi_bar = [grp]() { epi_bar_id(1 + grp); };
     // one staging buffer per group (the other group's chain overlaps); before the group rewrites it, the store that last
     // read it must be done with it.  Staging rows are written with st.shared on 32-bit addresses (sts128): through generic
@@ -422,13 +441,15 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
     auto stage_wait = [leader]() {                  // (kStagePark: no buffer is reused within a tile)
       if (!kStagePark && leader) tma_store_wait_read<0>();
     };
-    // kStagePark: box b of the parked tile (the first kStageBoxes in the parked stage, the rest behind the ring)
+    // kStagePark: box b of the parked tile (the first kStageBoxes in the parked stage, the rest behind the ring).  PP: every
+    // chunk goes through the warpgroup's own staging box (PP epilogues write no planes: store_planes32 never sees it).
     uint8_t* park_stage = smem;
     auto park_box = [&](int b) {
+      if (PP) return staging + grp * kStagingBytes;
       return b < kStageBoxes ? park_stage + b * kParkBoxBytes : smem + kStages * kStageBytes + (b - kStageBoxes) * kParkBoxBytes;
     };
-    // staging buffer of the chunk at tile column ct: the group's buffer, or (kStagePark) the chunk's own box
-    auto chunk_buf = [&](int ct) { return kStagePark ? park_box(ct >> 5) : staging + grp * kStagingBytes; };
+    // staging buffer of the chunk at tile column ct: the group's buffer, or (kStagePark, PP) the chunk's own box
+    auto chunk_buf = [&](int ct) { return kStagePark || PP ? park_box(ct >> 5) : staging + grp * kStagingBytes; };
     // fp16-split planes out, one 32-column chunk at (col, row), tile column ct: pair(j) returns the pre-scaled (x 2^6) values
     // of the chunk's columns 2 j, 2 j + 1 for this thread's row; it runs after the staging buffers are free, in column order
     auto store_planes32 = [&](int ct, int col, int row, auto&& pair) {
@@ -453,10 +474,15 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
         tma_store_commit();
       }
     };
-    uint32_t it = 0;
-    for (int u = blockIdx.x; u < total_units; u += gridDim.x) {
+    // PP: warpgroup wg runs the CTA's units tl = wg, wg + 2, ...; k-block kb of unit tl is ring position tl * nkb + kb
+    const int unit_step = PP ? 2 * gridDim.x : gridDim.x;
+    uint32_t it = PP ? wg * nkb : 0;
+    for (int u = blockIdx.x + (PP ? wg * gridDim.x : 0), tl = PP ? wg : 0; u < total_units; u += unit_step, tl += PP ? 2 : 1) {
       const int z = u / units_per_batch, rem = u - z * units_per_batch;
       const int m_tile = rem / p.n_tiles, n_tile = rem % p.n_tiles;
+      // PP: the other warpgroup has issued the MMAs of unit tl - 1 (its ((tl - 1) >> 1)-th arrival on order_bar[wg]).  Only
+      // then are the full barriers of this unit's k-blocks at most one phase behind the one awaited.
+      if (PP && tl > 0) mbar_wait(&order_bar[wg], ((tl - 1) >> 1) & 1);
 #pragma unroll
       for (int i = 0; i < kRegs; ++i) {
         acc[i] = 0.f;
@@ -541,6 +567,13 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
               mma_k16<BN>(acc, ah, bh);
               mma_k16<BN>(acc, ah, bl);
               if (!HI) mma_k16<BN>(acc, al, bh);
+              if (PP) {                                               // rows [64, 128) of the tile: the second accumulator
+                const uint64_t ah1 = make_desc(sa_h + kHalfOff + koff), al1 = make_desc(sa_l + kHalfOff + koff);
+                float* acc1 = acc + (PP ? 64 : 0);
+                mma_k16<BN>(acc1, ah1, bh);
+                mma_k16<BN>(acc1, ah1, bl);
+                mma_k16<BN>(acc1, al1, bh);
+              }
             }
             wgmma_commit();
           }
@@ -549,14 +582,19 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
           prev_s = s;
         }
       }
+      if (PP) {                                                       // hand the tensor pipe to the other warpgroup
+        it += nkb;                                                    // (skip the other warpgroup's unit tl + 1)
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&order_bar[wg ^ 1]);
+      }
       wgmma_wait<0>();
       fence_regs<kRegs>(acc);
       if (kSplitAcc) fence_regs<kRegs>(acc_c);
       if (kMainAcc > 1) { fence_regs<kRegs>(acc_m1); fence_regs<kRegs>(acc_m2); }
       if (prev_s >= 0) release(prev_s);
       // ---- park the accumulator: fragment -> the eight boxes (BN 256), or acc_smem [BM][kAccLd] (narrow tiles: split
-      // accumulators summed with round-to-nearest)
-      consumers_bar();                                                // both warpgroups' MMAs have finished reading the ring
+      // accumulators summed with round-to-nearest); PP parks chunk by chunk in ld32
+      if (!PP) consumers_bar();                                       // both warpgroups' MMAs have finished reading the ring
       if (kStagePark) {
         park_stage = smem + prev_s * kStageBytes;                     // the last k-block's stage
         const int r = 64 * wg + 16 * q + (lane >> 2), cq = 2 * (lane & 3);
@@ -566,7 +604,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
           *reinterpret_cast<float2*>(p0) = make_float2(acc[4 * g], acc[4 * g + 1]);
           *reinterpret_cast<float2*>(p0 + 8 * 32) = make_float2(acc[4 * g + 2], acc[4 * g + 3]);   // stg_off(r + 8, j) = + 1024 B
         }
-      } else {
+      } else if (!PP) {
         const int r = 64 * wg + 16 * q + (lane >> 2), cq = 2 * (lane & 3);
 #pragma unroll
         for (int g = 0; g < BN / 8; ++g) {
@@ -581,9 +619,36 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
           *reinterpret_cast<float2*>(acc_smem + (r + 8) * kAccLd + 8 * g + cq) = make_float2(v[2], v[3]);
         }
       }
-      consumers_bar();
+      if (!PP) consumers_bar();
       // 32 accumulator columns of this thread's row starting at column c (a multiple of 32)
       auto ld32 = [&](int c, uint32_t (&v)[32]) {
+        if (PP) {
+          // fragment columns [c, c + 32) of both accumulators -> the group's box, once the store that last read the box is
+          // done with it and every thread has finished with its previous contents
+          const uint32_t box = smem_u32(park_box(0));
+          if (leader) tma_store_wait_read<0>();
+          epi_bar();
+          const int cq = 2 * (lane & 3);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            const int r = 64 * h + 16 * q + (lane >> 2);
+#pragma unroll
+            for (int g = 0; g < BN / 8; ++g) {                          // columns 8 g + cq, + 1 of rows r, r + 8
+              if ((g >> 2) != (c >> 5)) continue;
+              const float* a = acc + 64 * h + 4 * g;
+              const uint32_t p0 = box + stg_off(r, 2 * (g & 3) + (cq >> 2)) + (cq & 3) * 4;
+              asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(p0), "f"(a[0]), "f"(a[1]) : "memory");
+              asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(p0 + 1024), "f"(a[2]), "f"(a[3]) : "memory");   // row r + 8
+            }
+          }
+          epi_bar();
+#pragma unroll
+          for (int j = 0; j < 8; ++j) {
+            const float4 f = lds128(box + stg_off(r_in_tile, j));
+            v[4 * j] = __float_as_uint(f.x); v[4 * j + 1] = __float_as_uint(f.y); v[4 * j + 2] = __float_as_uint(f.z); v[4 * j + 3] = __float_as_uint(f.w);
+          }
+          return;
+        }
         if (kStagePark) {
           const uint32_t box = smem_u32(park_box(c >> 5));
 #pragma unroll
@@ -600,6 +665,9 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
           v[4 * j] = __float_as_uint(f.x); v[4 * j + 1] = __float_as_uint(f.y); v[4 * j + 2] = __float_as_uint(f.z); v[4 * j + 3] = __float_as_uint(f.w);
         }
       };
+      // PP: the chunk loops are unrolled, so that the fragment registers of a chunk are free once it has been parked (the
+      // whole accumulator would otherwise stay live through the epilogue and spill)
+      constexpr int kChunkUnroll = PP ? 4 : 1;
       const int out_row0 = z * p.c_batch_rows + m_tile * BM;
       const int row0 = m_tile * BM;                               // within the batch
       int n_valid = BM;                                           // valid rows of this tile (segment-aware launches)
@@ -610,7 +678,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
       }
       if (EPI == EPI_F32 || EPI == EPI_F32_STATS) {
         // ---- fp32 tile out through swizzled staging + TMA store, 32 columns per chunk
-#pragma unroll 1
+#pragma unroll kChunkUnroll
         for (int c0 = c_begin; c0 < c_end; c0 += 32) {
           uint32_t v[32];
           ld32(c0, v);
@@ -643,7 +711,12 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
             // cancels catastrophically when a channel's mean is large against its spread)
             const int t = t_in_grp, qq = t >> 5, cc = t & 31;
             const int r_end = min(32, n_valid - qq * 32);
-            auto staged = [&](int i) { return *reinterpret_cast<const float*>(sb + stg_off(qq * 32 + i, cc >> 2) + (cc & 3) * 4); };
+            const uint32_t sbu = smem_u32(sb) + (cc & 3) * 4;
+            auto staged = [&](int i) {
+              float x;
+              asm volatile("ld.shared.f32 %0, [%1];" : "=f"(x) : "r"(sbu + stg_off(qq * 32 + i, cc >> 2)));
+              return x;
+            };
             float sum = 0.f, m2 = 0.f;
             for (int i = 0; i < r_end; ++i) sum += staged(i);
             const float mq = r_end > 0 ? sum / (float)r_end : 0.f;
@@ -660,7 +733,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
         // elu+1 on K (GATs_SuperGlue.py:71-72); pad rows are zeroed so the state kernel needs no row masks.
         const bool is_k = n_tile == 0;
         const bool row_ok = r_in_tile < n_valid;
-#pragma unroll 1
+#pragma unroll kChunkUnroll
         for (int c0 = c_begin; c0 < c_end; c0 += 64) {
           uint32_t v0[32], v1[32];
           ld32(c0, v0);
@@ -704,7 +777,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
         const bool row_ok = row < Nz;
         const float ea = kProdInv * p.inv_scale * 1.4426950408889634f, eb = -p.inv_scale * 1.4426950408889634f;
         float rs = 0.f;
-#pragma unroll 1
+#pragma unroll kChunkUnroll
         for (int c0 = c_begin; c0 < c_end; c0 += 32) {
           uint32_t v[32];
           ld32(c0, v);
@@ -729,7 +802,9 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
           }
           p.colsum_part[((long long)z * (p.m_tiles * 4) + m_tile * 4 + q) * p.L.m_pad + col0 + lane] = e[0];
         }
-        p.rowsum_part[((long long)z * (p.n_tiles * 2) + n_tile * 2 + grp) * p.L.n_pad + row] = rs;
+        // one row sum per 128-column half of the score matrix: a PP tile, or half grp of a cooperative one
+        const int halves = PP ? p.n_tiles : p.n_tiles * 2, half = PP ? n_tile : n_tile * 2 + grp;
+        p.rowsum_part[((long long)z * halves + half) * p.L.n_pad + row] = rs;
       } else if (EPI == EPI_SCORE_CONF) {
         // ---- dual-softmax tail, pass 2: conf = (e / rowsum) * (e / colsum) recomputed from the accumulator (the cos matrix is
         // never materialised), optional conf store, packed row / column arg-max (reference :218-220).  The 32-column chunk is
@@ -750,7 +825,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
         float rbest_v = 0.f;
         int rbest_c = -1;
         const bool store_plain = p.conf != nullptr && !p.conf_tma;
-#pragma unroll 1
+#pragma unroll kChunkUnroll
         for (int c0 = c_begin; c0 < c_end; c0 += 32) {
           uint32_t v[32];
           ld32(c0, v);
@@ -825,7 +900,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
         }
         const bool relu = EPI == EPI_CONV && p.relu;
         float peak = 0.f;              // EPI_CONV range guard: the largest |output| of this thread's row (see split_out_of_range)
-#pragma unroll 1
+#pragma unroll kChunkUnroll
         for (int c0 = c_begin; c0 < c_end; c0 += 32) {
           uint32_t v[32];
           ld32(c0, v);
@@ -868,7 +943,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
           src = p.L.src_seg(seg, p.cross);
           eps_m = 1e-6f / (float)max(p.L.seg_valid(src), 1);
         }
-#pragma unroll 1
+#pragma unroll kChunkUnroll
         for (int c0 = c_begin; c0 < c_end; c0 += 64) {
           uint32_t v0[32], v1[32];
           ld32(c0, v0);
@@ -920,10 +995,12 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
       }
       // the next tile's loads refill the ring: order this thread's reads of the parked tile before them (kStagePark: and the
       // stores staged in the boxes have read them)
-      if (kStagePark && leader) tma_store_wait_read<0>();
-      fence_async_smem();
-      consumers_bar();
-      if (threadIdx.x == 0) mbar_arrive(acc_free_bar);
+      if (!PP) {                                // (PP: the next tile's epilogue waits on its own box in ld32)
+        if (kStagePark && leader) tma_store_wait_read<0>();
+        fence_async_smem();
+        consumers_bar();
+        if (threadIdx.x == 0) mbar_arrive(acc_free_bar);
+      }
     }
     if (leader) tma_store_wait_all();
   }
@@ -999,9 +1076,9 @@ int num_sms() {
   return n;
 }
 
-template <int EPI, int ACV = ACV_NONE, bool HI = false, int BN_ = 256, int K2B = K2_FULL>
+template <int EPI, int ACV = ACV_NONE, bool HI = false, int BN_ = 256, int K2B = K2_FULL, bool PP = false>
 cudaError_t launch_variant(int grid, cudaStream_t stream, const Maps& mp, const TcParams& tp) {
-  auto* kern = gemm_tc_kernel<EPI, ACV, HI, BN_, K2B>;
+  auto* kern = gemm_tc_kernel<EPI, ACV, HI, BN_, K2B, PP>;
   if (cudaError_t e = ensure_smem_limit((const void*)kern, kSmemBytes)) return e;
   return launch_k(pdl_enabled(), kern, dim3(grid), dim3(kThreads), kSmemBytes, stream, mp, tp);
 }
@@ -1038,6 +1115,9 @@ int launch_gemm_tc(const GemmProblem& p, cudaStream_t stream) {
   if (p.a_hi_only && (p.a_conv || p.K2 || p.epi != EPI_QKV)) return -1;
   if (p.a_conv && (p.a_conv != ACV_NORM_RELU || p.batch != 1 || !p.a_raw || p.epi != EPI_BIAS_PLANES || p.b2_per_seg || !p.mu || !p.rstd)) return -1;
   const bool f32_out = p.epi == EPI_F32 || p.epi == EPI_F32_STATS;
+  // the ping-pong schedule runs every 256-column problem of these epilogues as 128-column tiles (DESIGN.md 5.1)
+  const bool pp = bn == BN && (f32_out || p.epi == EPI_SCORE_SUMS);
+  const int tile_n = pp ? 128 : bn;                // column width of a tile
   // halo convolution: 3x3 taps in row-major order with unit horizontal steps, 64-column tiles (wider tiles have no room for two
   // halo stages in the ring)
   int halo = (p.epi == EPI_CONV && p.taps == 9 && bn == 64) ? conv_halo_mode() : 0;
@@ -1054,7 +1134,7 @@ int launch_gemm_tc(const GemmProblem& p, cudaStream_t stream) {
   const long long b1_rows = (long long)(p.batch - 1) * p.b_batch_rows + p.n_out;
   const long long b2_rows = p.b2_per_seg ? (long long)p.L.segs() * p.n_out : p.n_out;
   Maps mp;
-  bool ok = make_map(&mp.b1h, p.b1.hi, b1_rows, p.K1, p.b1.ld, BK, bn, false) && make_map(&mp.b1l, p.b1.lo, b1_rows, p.K1, p.b1.ld, BK, bn, false);
+  bool ok = make_map(&mp.b1h, p.b1.hi, b1_rows, p.K1, p.b1.ld, BK, tile_n, false) && make_map(&mp.b1l, p.b1.lo, b1_rows, p.K1, p.b1.ld, BK, tile_n, false);
   if (p.a_conv) { mp.a1h = mp.b1h; mp.a1l = mp.b1l; }     // every A1 tile comes in raw: the plane maps are never used
   else {
     const long long a_cols = p.taps ? (long long)p.kb_per_tap * BK : p.K1;      // convolution: A has C_in columns, the taps shift its rows
@@ -1064,7 +1144,7 @@ int launch_gemm_tc(const GemmProblem& p, cudaStream_t stream) {
   if (ok && p.a_conv) ok = make_map(&mp.a_raw, p.a_raw, a_rows, p.K1, p.a_raw_ld, 32, BM, true);
   else mp.a_raw = mp.b1h;
   if (ok && p.K2) {
-    ok = make_map(&mp.b2h, p.b2.hi, b2_rows, p.K2, p.b2.ld, BK, p.b2_identity ? 64 : BN, false) && make_map(&mp.b2l, p.b2.lo, b2_rows, p.K2, p.b2.ld, BK, BN, false) &&
+    ok = make_map(&mp.b2h, p.b2.hi, b2_rows, p.K2, p.b2.ld, BK, p.b2_identity ? 64 : tile_n, false) && make_map(&mp.b2l, p.b2.lo, b2_rows, p.K2, p.b2.ld, BK, tile_n, false) &&
          make_map(&mp.a2h, p.a2.hi, a_rows, p.K2, p.a2.ld, BK, BM, false) && make_map(&mp.a2l, p.a2.lo, a_rows, p.K2, p.a2.ld, BK, BM, false);
   } else if (ok) {
     mp.a2h = mp.a1h; mp.a2l = mp.a1l; mp.b2h = mp.b1h; mp.b2l = mp.b1l;
@@ -1094,7 +1174,7 @@ int launch_gemm_tc(const GemmProblem& p, cudaStream_t stream) {
   if (p.b2_lo_zero && (p.epi != EPI_BIAS_PLANES || !p.K2 || !p.a_conv)) return -1;
   if (p.a_conv && !p.b2_lo_zero) return -1;
   const int k2b = p.b2_identity ? K2_DIAG : p.b2_lo_zero ? K2_LO_ZERO : K2_FULL;
-  tp.m_tiles = p.rows / BM; tp.n_tiles = p.n_out / bn; tp.batch = p.batch;
+  tp.m_tiles = p.rows / BM; tp.n_tiles = p.n_out / tile_n; tp.batch = p.batch;
   tp.taps = p.taps; tp.kb_per_tap = p.kb_per_tap;
   for (int t = 0; t < 9; ++t) tp.tap_off[t] = p.tap_off[t];
   tp.cv_w2 = p.cv_w2; tp.cv_h = p.cv_h; tp.cv_w = p.cv_w; tp.cv_ppad = p.cv_ppad; tp.relu = p.relu; tp.range_flag = p.range_flag; tp.halo = halo;
@@ -1116,15 +1196,16 @@ int launch_gemm_tc(const GemmProblem& p, cudaStream_t stream) {
   } else {
     switch (p.epi) {
       case EPI_F32:
-        le = bn == 128 ? launch_variant<EPI_F32, ACV_NONE, false, 128>(grid, stream, mp, tp) : launch_variant<EPI_F32>(grid, stream, mp, tp);
+        le = bn == 128 ? launch_variant<EPI_F32, ACV_NONE, false, 128>(grid, stream, mp, tp)
+                       : launch_variant<EPI_F32, ACV_NONE, false, 128, K2_FULL, true>(grid, stream, mp, tp);
         break;
       case EPI_CONV:
         le = bn == 64 ? launch_variant<EPI_CONV, ACV_NONE, false, 64>(grid, stream, mp, tp) : launch_variant<EPI_CONV, ACV_NONE, false, 128>(grid, stream, mp, tp);
         break;
-      case EPI_F32_STATS: le = launch_variant<EPI_F32_STATS>(grid, stream, mp, tp); break;
+      case EPI_F32_STATS: le = launch_variant<EPI_F32_STATS, ACV_NONE, false, 128, K2_FULL, true>(grid, stream, mp, tp); break;
       case EPI_QSCALE: le = launch_variant<EPI_QSCALE>(grid, stream, mp, tp); break;
       case EPI_L2NORM: le = launch_variant<EPI_L2NORM>(grid, stream, mp, tp); break;
-      case EPI_SCORE_SUMS: le = launch_variant<EPI_SCORE_SUMS>(grid, stream, mp, tp); break;
+      case EPI_SCORE_SUMS: le = launch_variant<EPI_SCORE_SUMS, ACV_NONE, false, 128, K2_FULL, true>(grid, stream, mp, tp); break;
       case EPI_SCORE_CONF: le = launch_variant<EPI_SCORE_CONF>(grid, stream, mp, tp); break;
       case EPI_QKV: le = p.a_hi_only ? launch_variant<EPI_QKV, ACV_NONE, true>(grid, stream, mp, tp) : launch_variant<EPI_QKV>(grid, stream, mp, tp); break;
       case EPI_BIAS_PLANES: le = launch_variant<EPI_BIAS_PLANES>(grid, stream, mp, tp); break;
