@@ -439,7 +439,8 @@ int opb_debug_set_affine_trace(int32_t* samples, int32_t* counts, double* models
  *   win_w, win_h  odd, 3 .. 31;  max_level 0 .. 4 (fewer levels where cv2 builds fewer: see the pyramid below)
  *   criteria_type 1 (COUNT), 2 (EPS) or 3; max_count 1 .. 100 with COUNT (30 without), epsilon >= 0 with EPS (0.01 without;
  *                 clamped to 10); flags must be 0 (OPTFLOW_USE_INITIAL_FLOW and OPTFLOW_LK_GET_MIN_EIGENVALS are refused)
- *   workspace     device, at least opb_optical_flow_workspace_bytes(B, H, W, max_level) bytes; after the call it holds the
+ *   workspace     device, 16-byte aligned, at least opb_optical_flow_workspace_bytes(B, H, W, max_level) bytes (a misaligned
+ *                 workspace is refused); after the call it holds the
  *                 pyramids: per pair a slot of pair_bytes = that size / B, and in it per level l = 0 .. max_level of an
  *                 H x W pyramid (h_l = ceil(h_{l-1} / 2), likewise w_l) the Scharr derivatives of prev int16 [h_l, w_l, 2],
  *                 then for l >= 1 prev and next uint8 [h_l, w_l], each starting at a multiple of 16 bytes.  A smaller pair

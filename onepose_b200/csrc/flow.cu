@@ -453,6 +453,7 @@ extern "C" int opb_calc_optical_flow_pyr_lk(const uint8_t* prev, int64_t prev_fr
                                             void* workspace, int64_t workspace_bytes, float* next_pts, uint8_t* status, float* err, void* stream) {
   using namespace opb;
   REQUIRE(__func__, prev && next && offsets && workspace && (total == 0 || (pts && next_pts && status && err)));
+  REQUIRE(__func__, ((uintptr_t)workspace & 15) == 0);   // the derivative planes are read and written as short2
   REQUIRE(__func__, B > 0 && B <= 65535 && H > 0 && H <= kMaxSideLk && W > 0 && W <= kMaxSideLk && total >= 0);
   REQUIRE(__func__, prev_row_pitch >= W && next_row_pitch >= W && prev_frame_pitch >= 0 && next_frame_pitch >= 0);
   REQUIRE(__func__, win_w >= 3 && win_w <= kMaxWin && win_w % 2 == 1 && win_h >= 3 && win_h <= kMaxWin && win_h % 2 == 1);

@@ -122,8 +122,9 @@ def lk_batch(prev_u8: torch.Tensor, next_u8: torch.Tensor, pts: torch.Tensor, of
     offsets[0] = 0, offsets[B] = total), ``sizes`` an optional int32 [B,2] device tensor of per-pair (h, w) <= (H, W) (the
     pair's images are the top-left corners of its slots).  win_size odd 3..31, max_level 0..4, criteria (type, count, eps) as
     cv2's.  Returns (next_pts fp32 [total,2], status uint8 [total], err fp32 [total]), cv2's bit for bit (err is 0 where
-    status is 0).  ``workspace``: a uint8 CUDA tensor of at least ``workspace_bytes(B, H, W, max_level)`` to use (the
-    pyramids are left in it, see ``pyramid_views``).  No host synchronisation."""
+    status is 0).  ``workspace``: a contiguous uint8 CUDA tensor of at least ``workspace_bytes(B, H, W, max_level)`` bytes
+    whose data starts at a multiple of 16 bytes (a misaligned one is refused with OpbError), to use (the pyramids are left in
+    it, see ``pyramid_views``).  No host synchronisation."""
     dev = _lib.cuda_device(prev_u8)
     ww, wh, max_level, ty, count, eps, min_eig = _params(win_size, max_level, criteria, min_eig_threshold)
     B, H, W = _images(prev_u8, "prev_u8")

@@ -219,6 +219,8 @@ def _track_level(I, dI, J, win, level, top, prev_pts, next_pts, status, err, cou
         status[k[out]] = 0
         m = ~out
         k, q, iq = k[m], q[m], iq[m]
+        if k.size == 0:
+            return
         ab = (q - iq).astype(F32)
         Jw = _window(Jpad, off, iq[:, 1], iq[:, 0], wh, ww, _weights(ab[:, 0], ab[:, 1]), W_BITS - 5)
         rows = np.searchsorted(idx, k)

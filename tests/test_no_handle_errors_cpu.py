@@ -15,6 +15,17 @@ from onepose_b200 import _lib, pnp
 OPB_E_INVALID = -1
 P = 64                      # a non-null address; never dereferenced (the call is refused first)
 MAX_HYPOTHESES = 65535 * 128
+LK_WS = 1 << 30             # a workspace size every refused LK call below would accept
+
+
+def _lk(**kw):
+    """The arguments of opb_calc_optical_flow_pyr_lk without the stream: one 64 x 64 pair, 4 points, the tracker's parameters,
+    with the given ones replaced."""
+    a = dict(prev=P, prev_frame_pitch=4096, prev_row_pitch=64, next=P, next_frame_pitch=4096, next_row_pitch=64, B=1, H=64, W=64,
+             sizes=None, pts=P, offsets=P, total=4, win_w=15, win_h=15, max_level=2, criteria_type=3, max_count=10, epsilon=0.03,
+             min_eig_threshold=1e-4, flags=0, workspace=P, workspace_bytes=LK_WS, next_pts=P, status=P, err=P)
+    a.update(kw)
+    return tuple(a.values())
 
 
 def _desc(**fields):
@@ -35,6 +46,13 @@ CASES = [
     ("opb_warp_crop_u8", (P, 100, 10, 1, 10, 10, P, None, 8, 8, None, P, None), "(frames != nullptr) == (out != nullptr)"),
     ("opb_warp_crop_u8", (None, 0, 0, 1, 0, 0, P, P, 8, 8, None, P, None), "(K != nullptr) == (K_crop != nullptr)"),
     ("opb_debug_gemm", (None,), "d && d->backend >= 0"),
+    ("opb_calc_optical_flow_pyr_lk", _lk(workspace=None), "prev && next && offsets && workspace"),
+    ("opb_calc_optical_flow_pyr_lk", _lk(err=None), "total == 0 || (pts && next_pts && status && err)"),
+    ("opb_flow_compact", (P, P, P, None, 1, 10, P, P, P, P, P, P), "counts && offsets && n_tracked"),
+    ("opb_flow_compact", (P, None, P, P, 1, 10, P, P, P, P, P, P), "cap == 0 || (status && pts2d && pts3d"),
+    ("opb_flow_reprojection", (P, None, P, P, P, 1, P), "K && pose && offsets && dist"),
+    # a workspace that does not start at a multiple of 16 bytes: the derivative planes are read and written as short2
+    ("opb_calc_optical_flow_pyr_lk", _lk(workspace=P + 1), "((uintptr_t)workspace & 15) == 0"),
     # counts <= 0
     ("opb_segmented_mean_f64", (P, P, 4, 0, P), "D > 0"),
     ("opb_segmented_mean_channels_f64", (P, P, 4, 0, P), "D > 0"),
@@ -46,6 +64,10 @@ CASES = [
     ("opb_estimate_affine_partial", (P, P, P, 0, 3.0, 2000, 0.99, 10, P, None, P, P), "B > 0"),
     ("opb_boxes_from_matches", (P, P, P, 1, 16, P, P, 0, P, 1, 1, 480, 640, P, P, P, P, P), "cap_query > 0"),
     ("opb_debug_cv_subsets", (4, 1, 1, P), "n >= 5"),
+    ("opb_calc_optical_flow_pyr_lk", _lk(B=0), "B > 0"),
+    ("opb_flow_compact", (P, P, P, P, 0, 10, P, P, P, P, P, P), "B > 0"),
+    ("opb_flow_compact", (P, P, P, P, 1, -1, P, P, P, P, P, P), "cap >= 0"),
+    ("opb_flow_reprojection", (P, P, P, P, P, 0, P), "B > 0"),
     # other bounds
     ("opb_gather_features3d", (P, None, 8, 10, None, 11, P, None, 10), "n_idx <= n_out"),
     ("opb_gather_features3d", (P, None, 65536, 10, None, 10, P, None, 10), "dim <= 65535"),
@@ -59,6 +81,20 @@ CASES = [
     ("opb_ransac_epnp", (P, P, P, P, 1, 100, 0.0, 0, P, P, P, P), "reproj_error > 0.0"),
     ("opb_crop_resize", (P, 100, 10, 1, 10, 10, P, P, 12, P, P, P, P), "crop_size % 8 == 0"),
     ("opb_boxes_from_matches", (P, P, P, 1, 16, P, P, 16, P, 2, 1, 480, 640, P, P, P, P, P), "(matches_int64 == 0 || matches_int64 == 1)"),
+    ("opb_calc_optical_flow_pyr_lk", _lk(B=65536), "B <= 65535"),
+    ("opb_calc_optical_flow_pyr_lk", _lk(W=32768, prev_row_pitch=32768, next_row_pitch=32768), "W <= kMaxSideLk"),
+    ("opb_calc_optical_flow_pyr_lk", _lk(next_row_pitch=63), "next_row_pitch >= W"),
+    ("opb_calc_optical_flow_pyr_lk", _lk(prev_frame_pitch=-1), "prev_frame_pitch >= 0"),
+    ("opb_calc_optical_flow_pyr_lk", _lk(win_h=14), "win_h % 2 == 1"),
+    ("opb_calc_optical_flow_pyr_lk", _lk(win_w=33), "win_w <= kMaxWin"),
+    ("opb_calc_optical_flow_pyr_lk", _lk(max_level=5), "max_level <= kMaxLevel"),
+    ("opb_calc_optical_flow_pyr_lk", _lk(criteria_type=4), "(criteria_type & ~3) == 0"),
+    ("opb_calc_optical_flow_pyr_lk", _lk(max_count=101), "max_count <= 100"),
+    ("opb_calc_optical_flow_pyr_lk", _lk(epsilon=math.nan), "epsilon >= 0.0"),
+    ("opb_calc_optical_flow_pyr_lk", _lk(min_eig_threshold=-1e-9), "min_eig_threshold >= 0.0"),
+    ("opb_calc_optical_flow_pyr_lk", _lk(flags=4), "flags == 0"),
+    ("opb_calc_optical_flow_pyr_lk", _lk(workspace_bytes=1000), "workspace_bytes >= (int64_t)B * (int64_t)L.pair_bytes"),
+    ("opb_flow_compact", (P, P, P, P, 65536, 32768, P, P, P, P, P, P), "(int64_t)B * cap <= (int64_t)INT32_MAX"),
     ("opb_debug_gemm", (_desc(backend=2),), "d->backend <= 1"),
     ("opb_debug_gemm", (_desc(backend=1, epi=_lib.EPI_QSCALE),), "p.epi == EPI_F32"),
     # confidence
@@ -75,6 +111,13 @@ HOOK_CASES = [
     ("opb_debug_set_cv_trace", (P, None, None, 0), "capacity > 0 || (capacity == 0 && !samples && !counts)"),
     ("opb_debug_set_cv_trace", (None, None, None, -1), "capacity > 0 || (capacity == 0 && !samples && !counts)"),
     ("opb_debug_set_affine_trace", (None, None, P, 0), "capacity > 0 || (capacity == 0 && !samples && !counts && !models)"),
+]
+
+# calls that take no stream; (entry point, arguments, text of the refused condition)
+NO_STREAM_CASES = [
+    ("opb_optical_flow_workspace_bytes", (1, 64, 64, 2, None), "bytes && B > 0"),
+    ("opb_optical_flow_workspace_bytes", (1, 64, 32768, 2, C.byref(C.c_int64())), "W <= opb::kMaxSideLk"),
+    ("opb_optical_flow_workspace_bytes", (1, 64, 64, 5, C.byref(C.c_int64())), "max_level <= opb::kMaxLevel"),
 ]
 
 NO_REFUSAL = {"opb_debug_set_pdl", "opb_debug_set_ws_fill", "opb_debug_split", "opb_debug_kv_state_h"}
@@ -103,16 +146,22 @@ def test_a_refused_test_hook_names_itself_and_its_condition(name, args, cond):
     _refused(name, args, cond)
 
 
+@pytest.mark.parametrize("name,args,cond", NO_STREAM_CASES, ids=[f"{c[0]}:{c[2]}" for c in NO_STREAM_CASES])
+def test_a_refused_call_without_a_stream_names_its_entry_point_and_condition(name, args, cond):
+    _refused(name, args, cond)
+
+
 def test_every_handle_free_entry_point_that_can_refuse_is_covered():
-    covered = {c[0] for c in CASES + HOOK_CASES}
+    covered = {c[0] for c in CASES + HOOK_CASES + NO_STREAM_CASES}
     assert covered == {
         "opb_segmented_mean_f64", "opb_segmented_mean_channels_f64", "opb_segmented_mean_scores_f64", "opb_gather_features3d",
         "opb_debug_gemm", "opb_debug_set_conv_halo",
         "opb_gather_matches", "opb_gather_matches_objects", "opb_ransac_pnp", "opb_epnp", "opb_ransac_epnp", "opb_ransac_epnp_cv",
         "opb_debug_set_cv_wave", "opb_debug_set_cv_trace", "opb_debug_cv_subsets", "opb_boxes_from_poses", "opb_crop_resize",
         "opb_warp_crop_u8", "opb_estimate_affine_partial", "opb_boxes_from_matches", "opb_debug_set_affine_trace",
+        "opb_optical_flow_workspace_bytes", "opb_calc_optical_flow_pyr_lk", "opb_flow_compact", "opb_flow_reprojection",
     }
-    assert len(covered | NO_REFUSAL) == 25 and covered | NO_REFUSAL <= set(_lib.SYMBOLS)
+    assert len(covered | NO_REFUSAL) == 29 and covered | NO_REFUSAL <= set(_lib.SYMBOLS)
 
 
 def test_a_later_refusal_replaces_the_message():

@@ -15,9 +15,11 @@ import numpy as np
 import pytest
 import torch
 
-from onepose_b200 import GATsSuperGlue, SuperPoint, _lib, features3d, pnp, synthetic
+from onepose_b200 import GATsSuperGlue, SuperPoint, _lib, features3d, flow, pnp, synthetic
 from oracle import gats_spg_oracle as oracle
 from oracle import superpoint_oracle as sp_oracle
+from tests import flow_scenes as FS
+from tests import lk_reference as lk_model
 
 pytestmark = pytest.mark.gpu
 
@@ -28,6 +30,8 @@ IMG_B, IMG_H, IMG_W, CAP = 2, 96, 128, 256
 SP_CONF = {"nms_radius": 3, "max_keypoints": CAP}
 N_PNP = 200
 CONF_TOL = 1e-4
+LK_S, LK_COUNTS, LK_CAP = 128, [200, 90], 60
+K_LK = np.array([[300.0, 0, 64.0], [0, 300.0, 64.0], [0, 0, 1]])
 
 
 # ----------------------------------------------------------------------------- modules and inputs
@@ -136,6 +140,52 @@ def _leaves(inp):
 TRACKS = np.random.RandomState(11).randint(1, 12, size=50)
 
 
+def _lk_pairs(seed):
+    return [FS.warp_scene(70 + 10 * seed + b, LK_S, LK_S) for b in range(IMG_B)]
+
+
+def _lk_inputs(seed, dev):
+    pairs = _lk_pairs(seed)
+    return {"prev": _t(np.stack([a for a, _ in pairs]), dev), "next": _t(np.stack([n for _, n in pairs]), dev),
+            "pts": _t(np.concatenate([FS.scene_points(seed + b, LK_S, LK_S, n) for b, n in enumerate(LK_COUNTS)]), dev),
+            "off": _t(np.array([0, LK_COUNTS[0], sum(LK_COUNTS)], np.int32), dev)}
+
+
+def _keyframe_inputs(seed, dev):
+    """A keyframe state of IMG_B tracks (3D points seen at the 2D ones from [I | 0]), the next crops, and reference poses."""
+    rs = np.random.RandomState(500 + seed)
+    pairs = _lk_pairs(seed)
+    p2 = np.stack([FS.scene_points(seed + b, LK_S, LK_S, LK_CAP, margin=-20.0) for b in range(IMG_B)])
+    ray = np.concatenate([p2, np.ones((IMG_B, LK_CAP, 1))], 2) @ np.linalg.inv(K_LK).T
+    return {"image": _t(np.stack([a for a, _ in pairs]), dev), "query": _t(np.stack([n for _, n in pairs]), dev), "pts2d": _t(p2, dev),
+            "pts3d": _t((ray * rs.uniform(0.4, 0.6, (IMG_B, LK_CAP, 1))).astype(np.float32), dev),
+            "counts": _t(np.array([LK_CAP, LK_CAP - 7], np.int32), dev), "K": _t(K_LK, dev), "ref": _t(np.tile(np.eye(4), (IMG_B, 1, 1)), dev)}
+
+
+def _flow_track(i):
+    return flow.flow_track({k: i[k] for k in ("image", "pts2d", "pts3d", "counts")}, i["query"], i["K"], i["ref"])
+
+
+def _tracked(o):
+    return [o[k] for k in ("pose_init_homo", "kpt_dist", "trans_dist", "rot_dist", "n_tracked", "n_inliers", "accept")] + \
+        [o["kf"][k] for k in ("image", "pts2d", "pts3d", "counts")]
+
+
+def _pose_result(seed, dev):
+    """A poses_from_matches-style result of IMG_B frames of 50 pairs each (ragged: 50 and 31 used) and its crops."""
+    rs = np.random.RandomState(600 + seed)
+    n = 50
+    return {"offsets": _t(np.array([0, 50, 81], np.int32), dev), "inlier_mask": _t(rs.rand(IMG_B * n) < 0.6, dev),
+            "pts2d": _t(rs.rand(IMG_B * n, 2).astype(np.float32).astype(np.float64) * LK_S, dev),
+            "pts3d": _t(rs.rand(IMG_B * n, 3).astype(np.float32).astype(np.float64), dev),
+            "crops": _t(np.stack([a for a, _ in _lk_pairs(seed)]), dev)}
+
+
+def _keyframes(i):
+    kf = flow.keyframes_from_poses({k: i[k] for k in ("offsets", "inlier_mask", "pts2d", "pts3d")}, i["crops"])
+    return [kf[k] for k in ("image", "pts2d", "pts3d", "counts")]
+
+
 def _sfm(seed, dev):
     rs = np.random.RandomState(400 + seed)
     S = int(TRACKS.sum())
@@ -184,6 +234,9 @@ CASES = {
     "build_features3d_leaves": (lambda c, s: _sfm(s, c.dev), lambda c, i: _leaves(i), False),
     "mean_descriptors": (lambda c, s: _sfm(s, c.dev), lambda c, i: [features3d.mean_descriptors(i["tr"], TRACKS, device=c.dev)], False),
     "mean_scores": (lambda c, s: _sfm(s, c.dev), lambda c, i: [features3d.mean_scores(i["tr_s"], TRACKS, device=c.dev)], False),
+    "lk_batch": (lambda c, s: _lk_inputs(s, c.dev), lambda c, i: list(flow.lk_batch(i["prev"], i["next"], i["pts"], i["off"])), True),
+    "flow_track": (lambda c, s: _keyframe_inputs(s, c.dev), lambda c, i: _flow_track(i), True, _tracked),
+    "keyframes_from_poses": (lambda c, s: _pose_result(s, c.dev), lambda c, i: _keyframes(i), True),
 }
 
 
@@ -285,6 +338,13 @@ def test_a_results_against_the_oracles(ctx0, refs0):
     ends = np.cumsum(TRACKS)
     mean = np.stack([tr[e - n:e].mean(axis=0) for e, n in zip(ends, TRACKS)])
     np.testing.assert_allclose(refs0["mean_descriptors"][0].numpy(), mean, rtol=1e-13, atol=1e-15)
+    pts = np.concatenate([FS.scene_points(b, LK_S, LK_S, n) for b, n in enumerate(LK_COUNTS)])
+    got = [x.numpy() for x in refs0["lk_batch"]]
+    for b, (a, n) in enumerate(_lk_pairs(0)):
+        rows = slice(sum(LK_COUNTS[:b]), sum(LK_COUNTS[:b + 1]))
+        want = lk_model.calc_optical_flow_pyr_lk(a, n, pts[rows], flow.TRACK_WIN, flow.TRACK_LEVELS, flow.TRACK_CRITERIA)
+        for g, w in zip(got, want):
+            np.testing.assert_array_equal(g[rows], w)
 
 
 # ----------------------------------------------------------------------------- B: one handle, two streams
