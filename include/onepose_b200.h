@@ -184,8 +184,10 @@ int opb_gather_features3d(const float* desc, const float* scores, int32_t dim, i
  * ransac_PnP (reference src/utils/eval_utils.py:18-42) for B frames in one call, on the device:
  *   K          device f64 [B, 9]   row-major camera matrices
  *   pts2d      device f64 [total, 2], pts3d device f64 [total, 3]  matched key points of all frames, concatenated
- *   offsets    device int32 [B+1]  frame b owns correspondences [offsets[b], offsets[b+1])
- *   hypotheses minimal samples per frame (P3P), 1 .. 65535 * 128; reproj_error in pixels, > 0; seed of the sample generator
+ *   offsets    device int32 [B+1]  frame b owns correspondences [offsets[b], offsets[b+1]); offsets[0] may be above 0, and
+ *              inlier_mask rows outside every frame are never written
+ *   hypotheses minimal samples per frame (P3P), 1 .. 65535 * 128; reproj_error in pixels, > 0 (inf allowed; 0, negative and
+ *              NaN are refused, where OpenCV squares a negative threshold); seed of the sample generator
  *              (results are a deterministic function of it)
  *   workspace  device f64 [B * hypotheses * 13]: one record of 13 doubles per frame and hypothesis, frame-major
  *              (record b * hypotheses + h): the inlier count of the hypothesis's best P3P pose, then that pose's R (9,
@@ -194,7 +196,12 @@ int opb_gather_features3d(const float* desc, const float* scores, int32_t dim, i
  *              splitmix64(seed ^ (b << 40) ^ h) and its successors.
  * Outputs (device): pose f64 [B, 12] = row-major [R | t] (world -> camera), inlier_mask int32 [total], n_inliers int32 [B].
  * A frame with fewer than 4 correspondences or no model gets the identity pose and no inliers (the reference's cv2.error
- * branch).  Parity with the reference is on the pose (cm / degree), not on bits: OpenCV draws its own samples. */
+ * branch).  Inlier: in front of the camera and squared reprojection error < reproj_error^2, in fp64; a pair with a NaN or an
+ * infinity is never one, and a sample holding one has no model.  A refinement that ends with fewer than 4 inliers (a
+ * threshold that admits gross outliers can drag the pose off the object) gives way to the winning hypothesis's pose.  K:
+ * only fx = K[0], fy = K[4], cx = K[2], cy = K[5] are read (skew and the last row are ignored, as OpenCV's EPnP and
+ * projectPoints ignore them).  Parity with the reference is on the pose (cm / degree), not on bits: OpenCV draws its own
+ * samples. */
 int opb_ransac_pnp(const double* K, const double* pts2d, const double* pts3d, const int32_t* offsets, int32_t B, int32_t hypotheses,
                    double reproj_error, uint64_t seed, double* workspace, double* pose_out, int32_t* inlier_mask, int32_t* n_inliers,
                    void* stream);
@@ -220,7 +227,8 @@ int opb_epnp(const double* K, const double* pts2d, const double* pts3d, const in
  *               P3P on correspondences 0-2 and keeps the solution that reprojects 3 best: OpenCV also fits a 4-point model
  *               there (it returns a pose with 4 inliers where no 5-point sample exists: tests/golden/make_epnp.py);
  *   count       inliers over all n by OpenCV's rule: squared reprojection error <= reproj_error^2, in fp64, with no depth
- *               test (points behind the camera that project close enough count); a non-finite pose counts 0;
+ *               test (points behind the camera that project close enough count); a non-finite pose counts 0, and a
+ *               non-finite error (a pair with a NaN or an infinity) is never an inlier, not even at reproj_error = inf;
  *   selection   most inliers, lowest index on ties (the arg-max of opb_ransac_pnp);
  *   refit       EPnP (the block routine of opb_epnp) on the winning sample's inlier set, which is the reported inlier_mask.
  * Fewer than 4 correspondences, or a best count below 4, gives the identity pose and no inliers.  OpenCV raises or returns
@@ -232,6 +240,7 @@ int opb_ransac_epnp(const double* K, const double* pts2d, const double* pts3d, c
 /* EPnP-RANSAC as OpenCV runs it: cv2.solvePnPRansac(..., iterationsCount=hypotheses, confidence, flags=SOLVEPNP_EPNP) for B
  * frames, with OpenCV's sample sequence and stopping rule; no host synchronisation.  Arguments as opb_ransac_epnp without the
  * seed (OpenCV's generator starts from the same state on every call), plus:
+ *   hypotheses  1 .. 65535 * 128 (OpenCV runs iterationsCount = 0 as one iteration; 0 is refused here)
  *   confidence  0 .. 1 (OpenCV's run() asserts 0 < confidence < 1; 0 and 1 follow RANSACUpdateNumIters' clamped formula:
  *               0 stops after the first winning sample; 1 lowers the budget to at most
  *               cvRound(log(DBL_MIN) / log(1 - (1 - outlier ratio)^5)), e.g. about 8700 at 40 % outliers)
@@ -242,7 +251,11 @@ int opb_ransac_epnp(const double* K, const double* pts2d, const double* pts3d, c
  *               five per sample, an index equal to an earlier one of the same sample drawn again; sample i of a frame is the
  *               i-th subset OpenCV draws for its n;
  *   model       EPnP on the five fp32-rounded pairs (the routine of opb_ransac_epnp); no finite pose = no model;
- *   count       OpenCV's fp32 error: the projection in fp64 rounded to fp32, the squared distance in fp32, <= (float)thr^2;
+ *   count       OpenCV's fp32 error: the projection in fp64 rounded to fp32, the squared distance in fp32, <= the bound
+ *               fp32(fp32(reproj_error)^2): solvePnPRansac takes a float threshold and findInliers squares it in double
+ *               and rounds to float.  This is not (float)(reproj_error^2), which is one ulp off for about half of all
+ *               thresholds (5.3, 0.7, ...).  A non-finite error is never an inlier (OpenCV counts an infinite one at
+ *               reproj_error = inf);
  *   loop        sample i wins when its count > max(best, 4) (the earliest wins a tie); each win lowers the budget to
  *               RANSACUpdateNumIters(confidence, outlier ratio, 5, budget); the loop exits at iter >= budget;
  *   result      the winner's inlier set is inlier_mask (n_inliers its count), the pose EPnP on it.  No winner: the identity

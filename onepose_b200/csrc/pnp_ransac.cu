@@ -488,14 +488,22 @@ __global__ void __launch_bounds__(kRefineThreads) pnp_select_refine(const double
     const double step = fabs(delta[0]) + fabs(delta[1]) + fabs(delta[2]) + fabs(delta[3]) + fabs(delta[4]) + fabs(delta[5]);
     if (step < 1e-12) break;
   }
-  // ---- outputs
+  // ---- outputs.  A threshold that admits gross outliers lets the refinement leave the model (on 40 % outliers at 1000 px it
+  // ends with the object behind the camera): a refined pose with fewer than 4 inliers gives way to the hypothesis it started from.
   int cnt = 0;
-  for (int i = tid; i < f.n; i += kRefineThreads) {
-    const int in = reproj_inlier(T, f.Kc, f.p3 + (size_t)i * 3, f.p2 + (size_t)i * 2, thr2) ? 1 : 0;
-    inlier_mask[f.o0 + i] = in;
-    cnt += in;
+  for (int pass = 0; pass < 2; ++pass) {
+    cnt = 0;
+    for (int i = tid; i < f.n; i += kRefineThreads) {
+      const int in = reproj_inlier(T, f.Kc, f.p3 + (size_t)i * 3, f.p2 + (size_t)i * 2, thr2) ? 1 : 0;
+      inlier_mask[f.o0 + i] = in;
+      cnt += in;
+    }
+    cnt = block_count<kRefineThreads>(cnt, cnt_w);
+    if (cnt >= 4) break;
+    __syncthreads();                                 // every thread has read T and cnt_w
+    if (tid == 0) T = load_record(hyp + ((size_t)b * H + best_h) * kHypStride);
+    __syncthreads();
   }
-  cnt = block_count<kRefineThreads>(cnt, cnt_w);
   if (tid == 0) {
     n_inliers[b] = cnt;
     write_pose(T, pose_out + (size_t)b * 12);
@@ -820,9 +828,11 @@ __device__ __forceinline__ bool pose_finite(const Pose& T) {
   return f;
 }
 
-// OpenCV's RANSAC inlier rule: squared reprojection error <= thr^2, no depth test
+// OpenCV's RANSAC inlier rule: squared reprojection error <= thr^2, no depth test.  A non-finite error (a pair with a NaN or
+// an infinity) is never an inlier, not even at thr = inf.
 __device__ __forceinline__ bool epnp_inlier(const Pose& T, const double* Kc, const double* p3, const double* p2, double thr2) {
-  return reproj_err2(T, Kc, p3, p2) <= thr2;
+  const double e = reproj_err2(T, Kc, p3, p2);
+  return e <= thr2 && e < INFINITY;
 }
 
 // correspondence i of a frame, rounded to fp32 first when kRound (as OpenCV's solvePnPRansac converts its inputs)
@@ -1088,6 +1098,9 @@ __device__ __forceinline__ float cv_error(const Pose& T, const double* Kc, const
   return __fadd_rn(__fmul_rn(du, du), __fmul_rn(dv, dv));
 }
 
+// OpenCV's fp32 inlier rule on cv_error; a non-finite error is never an inlier (OpenCV counts an infinite one at thr = inf)
+__device__ __forceinline__ bool cv_inlier(float e, float thr2f) { return e <= thr2f && e < INFINITY; }
+
 // samples first .. first + W - 1 of frame b, those below its budget niters, into the wave's records (one warp).  Every lane
 // passes its own copy of the budget: lane 0's store to S.niters need not be what the other lanes read back.
 __device__ void draw_wave(CvState& S, double* r, int n, int W, int first, int niters, int b, int* trace_samples, int trace_cap) {
@@ -1203,7 +1216,7 @@ __global__ void __launch_bounds__(kHypThreads) epnp_cv_wave(const double* __rest
     for (int j = 0; j < f.n; ++j) {
       double p2[2], p3[3];
       load_pair<true>(f.p2, f.p3, j, p2, p3);
-      cnt += cv_error(T, f.Kc, p3, p2) <= thr2f ? 1 : 0;
+      cnt += cv_inlier(cv_error(T, f.Kc, p3, p2), thr2f) ? 1 : 0;
     }
   }
   store_record(out, (double)cnt, T);
@@ -1239,7 +1252,7 @@ __global__ void __launch_bounds__(kEpnpThreads) epnp_cv_select_refit(const doubl
     }
     return;
   }
-  refit_tail(b, f, Wl, [&](const double* p3, const double* p2) { return cv_error(Wl, f.Kc, p3, p2) <= thr2f; }, S.best, sh, &T, pose_out,
+  refit_tail(b, f, Wl, [&](const double* p3, const double* p2) { return cv_inlier(cv_error(Wl, f.Kc, p3, p2), thr2f); }, S.best, sh, &T, pose_out,
              inlier_mask, n_inliers);
 }
 
@@ -1486,7 +1499,10 @@ extern "C" int opb_ransac_epnp_cv(const double* K, const double* pts2d, const do
     return rc;
   REQUIRE(__func__, iterations && confidence >= 0.0 && confidence <= 1.0);
   cudaStream_t st = (cudaStream_t)stream;
-  const float thr2f = (float)(reproj_error * reproj_error);   // findInliers: (float)(thresh * thresh)
+  // solvePnPRansac takes a float reprojectionError; findInliers squares it in double (exact) and rounds to float: the fp32
+  // square of the fp32 threshold, which differs from (float)(reproj_error^2) by an ulp for about half of all thresholds
+  const float thr_f = (float)reproj_error;
+  const float thr2f = thr_f * thr_f;
   const int W = cv_wave_size(B, hypotheses);
   if (W < 0) return W;
   const int waves = (hypotheses + W - 1) / W;

@@ -9,7 +9,7 @@ OpenCV's loop (``RANSACPointSetRegistrator::run`` and ``getSubset`` in calib3d/s
 - ``scan``              the loop's bookkeeping on given per-sample counts: a sample wins when its count is strictly greater
                         than max(best, modelPoints - 1), the budget is updated after each win, the loop stops at iter >= niters;
 - ``solve_pnp_ransac``  everything: inputs rounded to fp32, each minimal model from ``cv2.solvePnP(EPNP)``, OpenCV's fp32
-                        error (``projectPoints`` to fp32, squared norm in fp32, against (float)(thr * thr)), the winner's
+                        error (``projectPoints`` to fp32, squared norm in fp32, against ``fp32_threshold2``), the winner's
                         mask, and the EPnP refit on it.  Frames of 4 or 5 pairs (``model_points == npoints``) are solved
                         directly and every pair is an inlier, as there.
 Only ``solve_pnp_ransac`` and ``fp32_errors`` need cv2; the generator and the scan do not, so GPU tests use them without it.
@@ -83,6 +83,60 @@ def scan(counts, n: int, confidence: float, max_iters: int):
     return winner, best, it
 
 
+def fp32_threshold2(thr: float) -> np.float32:
+    """findInliers' squared threshold: solvePnPRansac's ``float reprojectionError`` (the threshold rounded to fp32 first),
+    squared in double (exact) and rounded to fp32 -- the fp32 product of the fp32 threshold."""
+    t = np.float32(thr)
+    return t * t
+
+
+# the boundary scene: integer world points at depths 2 .. 16 seen from the identity pose through K = diag(1000, 1000, 1); every
+# normalised coordinate x / z is dyadic, so it survives OpenCV's fp32 undistortPoints, EPnP on any five of them returns the
+# identity pose to ~1e-15 and every pixel reprojects to its fp32 value (error below 1e-20).  Row 0 is the probe, a point on the
+# optical axis: it projects to (0, 0) and its fp32 error is that of its observation (du, dv) alone.  Sample 0 of 13 pairs is
+# (9, 11, 4, 12, 7): with iterationsCount = 1 the mask is that exact pose's, probe included.
+BOUNDARY_POINTS = ((0, 0, 7), (1, 0, 16), (-1, -3, 4), (-3, -2, 2), (1, 3, 16), (1, 3, 8), (1, 0, 8), (3, -2, 8), (1, -3, 16),
+                   (3, 0, 4), (2, 2, 2), (-2, -3, 16), (-3, 0, 16))
+
+
+def _round32(q):
+    """The rational q rounded to fp32, to nearest with ties to even, exactly."""
+    from fractions import Fraction
+    a = np.float32(float(q))
+    best = None
+    for c in (np.nextafter(a, np.float32(-np.inf)), a, np.nextafter(a, np.float32(np.inf))):
+        d = abs(Fraction(float(c)) - q)
+        if best is None or d < best[0] or (d == best[0] and int(np.float32(c).view(np.uint32)) & 1 == 0):
+            best = (d, c)
+    return np.float32(best[1])
+
+
+def probe_offset(err):
+    """fp32 (du, dv) whose squared norm is exactly the fp32 value err in fp32 with and without FMA contraction (either
+    product fused), so that the probe's error does not depend on how computeError's sum is compiled."""
+    from fractions import Fraction
+    err = np.float32(err)
+    dv0 = np.float32(0.5 if err > 1 else 0.05)
+    dvs = (dv0 + np.arange(-4000, 4000, dtype=np.float32) * np.spacing(dv0)).astype(np.float32)
+    du0 = np.float32(math.sqrt(float(err) - float(dv0) ** 2))
+    for k in range(-20, 21):
+        du = np.float32(du0 + np.float32(k) * np.spacing(du0))
+        for j in np.nonzero(du * du + dvs * dvs == err)[0]:
+            a, b = Fraction(float(du)) ** 2, Fraction(float(dvs[j])) ** 2
+            ra, rb = Fraction(float(_round32(a))), Fraction(float(_round32(b)))
+            if _round32(ra + rb) == _round32(a + rb) == _round32(ra + b) == err:
+                return du, dvs[j]
+    raise ValueError(f"no probe offset for {err!r}")
+
+
+def boundary_scene(err):
+    """(K, uv, P) of 13 pairs: the boundary scene with the probe (row 0) observed at fp32 squared error err."""
+    P = np.array(BOUNDARY_POINTS, np.float64)
+    uv = 1000 * P[:, :2] / P[:, 2:]
+    uv[0] = probe_offset(err)
+    return np.diag([1000.0, 1000.0, 1.0]), uv, P
+
+
 def fp32_errors(P32, uv32, K, dist, rvec, tvec):
     """``PnPRansacCallback::computeError``: projectPoints of the fp32 points (fp32 output), squared distance in fp32."""
     import cv2
@@ -111,7 +165,7 @@ def solve_pnp_ransac(P, uv, K, dist=None, thr=5.0, iterations_count=10000, confi
         return bool(ok), rv, tv, np.arange(n) if ok else np.zeros(0, np.int64), info
     if not 0 < confidence < 1:
         raise ValueError("OpenCV's run() asserts 0 < confidence < 1")
-    thr2 = np.float32(thr * thr)
+    thr2 = fp32_threshold2(thr)
     rng = CvRNG()
     niters = max(iterations_count, 1)
     best, best_mask, it = 0, None, 0

@@ -29,6 +29,7 @@ def test_entry_point_rejects_bad_arguments():
 
     for kw in (dict(K=None), dict(p2=None), dict(p3=None), dict(off=None), dict(ws=None), dict(pose=None), dict(mask=None),
                dict(cnt=None), dict(its=None), dict(B=0), dict(H=0), dict(H=65535 * 128 + 1), dict(thr=0.0), dict(thr=float("nan")),
+               dict(thr=-5.0), dict(thr=-float("inf")),
                dict(conf=-0.01), dict(conf=1.01), dict(conf=float("nan"))):
         assert call(**kw) == -1, kw
     assert lib.opb_debug_set_cv_wave(-1) == -1

@@ -141,7 +141,8 @@ def test_epnp_entry_points_reject_bad_arguments():
         return lib.opb_ransac_epnp(K, p2, p3, off, B, H, thr, 0, ws, pose, mask, cnt, None)
 
     for kw in (dict(K=None), dict(p2=None), dict(p3=None), dict(off=None), dict(ws=None), dict(pose=None), dict(mask=None),
-               dict(cnt=None), dict(B=0), dict(H=0), dict(H=65535 * 128 + 1), dict(thr=0.0), dict(thr=float("nan"))):
+               dict(cnt=None), dict(B=0), dict(H=0), dict(H=65535 * 128 + 1), dict(thr=0.0), dict(thr=float("nan")), dict(thr=-1.0),
+               dict(thr=-float("inf"))):
         assert ransac(**kw) == -1, kw
 
 

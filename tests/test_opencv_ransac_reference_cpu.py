@@ -103,3 +103,108 @@ def test_update_num_iters_edges():
     assert O.scan([4, 3, 6, 6, 7] + [0] * 100, 10, 0.0, 100) == (2, 6, 3)
     assert O.scan([6, 6, 6] + [0] * 100, 10, 0.99, 100)[0] == 0
     assert O.scan([-1] * 10, 10, 0.99, 10) == (-1, 0, 10)
+
+
+def _pin(P, uv, K, thr, iters, conf):
+    """The restatement equals cv2.solvePnPRansac(EPNP) on one scene: success, inlier list, pose bits, and the loop's own
+    bookkeeping (samples, scan).  Returns (inliers, info)."""
+    cv2 = pytest.importorskip("cv2")
+    ok, rv, tv, inl, info = O.solve_pnp_ransac(P, uv, K, None, thr, iters, conf)
+    ok_cv, rv_cv, tv_cv, inl_cv = cv2.solvePnPRansac(P, uv, K, np.zeros((8, 1)), reprojectionError=thr, iterationsCount=iters,
+                                                     confidence=conf, flags=cv2.SOLVEPNP_EPNP)
+    inl_cv = np.zeros(0, np.int64) if inl_cv is None else inl_cv.reshape(-1)
+    assert ok == ok_cv
+    assert inl.tolist() == inl_cv.tolist()
+    if ok:
+        assert rv.tobytes() == rv_cv.tobytes() and tv.tobytes() == tv_cv.tobytes()
+    n = len(uv)
+    if n > 5:
+        assert info["iterations"] == len(info["samples"]) <= max(iters, 1)
+        assert info["samples"] == O.subsets(n, info["iterations"])
+        assert O.scan(info["counts"], n, conf, iters) == (info["winner"], len(inl) if ok else 0, info["iterations"])
+    return inl, info
+
+
+@pytest.mark.parametrize("thr", [0.1, 0.7, 3.3, 5.3, 5.7])
+def test_threshold_is_rounded_to_fp32_before_it_is_squared(thr):
+    """solvePnPRansac declares ``float reprojectionError``: the inlier bound is fp32(fp32(thr)^2), not fp32(thr^2).  At these
+    thresholds the two differ by one ulp.  The boundary scene puts one pair at an exactly known fp32 error: one ulp below the
+    lower bound and at it (inlier under both), at the upper bound (the rule decides), one ulp above it (outlier under both).
+    The controls pass only if the probe's error is what the scene says it is."""
+    cv2 = pytest.importorskip("cv2")
+    t_first, t_late = O.fp32_threshold2(thr), np.float32(thr * thr)
+    assert t_first != t_late
+    lo, hi = min(t_first, t_late), max(t_first, t_late)
+    probes = ((np.nextafter(lo, np.float32(0)), True), (lo, True), (hi, hi == t_first), (np.nextafter(hi, np.float32(np.inf)), False))
+    for err, inlier in probes:
+        K, uv, P = O.boundary_scene(err)
+        P32, uv32 = P.astype(np.float32), uv.astype(np.float32)
+        ok, rv, tv = cv2.solvePnP(P32[[9, 11, 4, 12, 7]], uv32[[9, 11, 4, 12, 7]], K, np.zeros((8, 1)), flags=cv2.SOLVEPNP_EPNP)
+        e = O.fp32_errors(P32, uv32, K, np.zeros((8, 1)), rv, tv)
+        assert e[0] == err and np.all(e[1:] < 1e-20), (err, e[0])      # the error model of the probe itself
+        inl, info = _pin(P, uv, K, thr, 1, 0.99)
+        assert info["samples"] == [(9, 11, 4, 12, 7)]
+        assert (0 in inl.tolist()) == inlier and inl.tolist()[-12:] == list(range(1, 13)), (thr, err, inlier)
+
+
+@pytest.mark.parametrize("thr", [0.05, 0.7, 1.0, 3.0, 5.3, 5.7, 8.0, 1e6, float("inf")])
+def test_restatement_equals_cv2_at_thresholds(thr):
+    for k, (n, frac, noise) in enumerate(((100, 0.4, 1.0), (60, 0.6, 0.5), (200, 0.3, 2.0))):
+        K, uv, P, _ = synthetic.make_pnp_scene(1200 + k, n, outlier_frac=frac, noise_px=noise)
+        inl, info = _pin(P * 1000, uv, K, thr, 2000 if thr < 1 else 10000, 0.99)
+        if thr == float("inf"):
+            assert len(inl) == n and info["iterations"] == 1          # every pair, and the first sample ends the loop
+        print(f"thr={thr} n={n}: {info['iterations']} iterations, winner {info['winner']}, {len(inl)} inliers")
+
+
+@pytest.mark.parametrize("iters", [0, 1, 2, 3])
+def test_restatement_equals_cv2_at_tiny_budgets(iters):
+    """iterationsCount = 0 runs one iteration in OpenCV (niters = max(iterationsCount, 1))."""
+    for k, frac in enumerate((0.0, 0.5, 0.9)):
+        K, uv, P, _ = synthetic.make_pnp_scene(1300 + k, 40, outlier_frac=frac, noise_px=1.0)
+        inl, info = _pin(P * 1000, uv, K, 5.0, iters, 0.99)
+        assert 1 <= info["iterations"] <= max(iters, 1)
+
+
+@pytest.mark.parametrize("conf", [1e-300, 0.5, 1 - 2 ** -53])
+def test_restatement_equals_cv2_at_confidence_edges(conf):
+    for k, frac in enumerate((0.2, 0.6)):
+        K, uv, P, _ = synthetic.make_pnp_scene(1400 + k, 80, outlier_frac=frac, noise_px=1.0)
+        inl, info = _pin(P * 1000, uv, K, 5.0, 3000, conf)
+        if conf == 1e-300:
+            assert info["iterations"] == info["winner"] + 1                  # the first improvement ends the loop
+
+
+@pytest.mark.parametrize("n", [5, 6, 7])
+def test_restatement_equals_cv2_on_small_frames(n):
+    for k, (frac, noise) in enumerate(((0.0, 0.0), (0.0, 1.0), (0.2, 1.0))):
+        K, uv, P, _ = synthetic.make_pnp_scene(1500 + 10 * n + k, n, outlier_frac=frac, noise_px=noise)
+        for thr in (1.0, 5.0):
+            _pin(P * 1000, uv, K, thr, 100, 0.99)
+
+
+def test_cv2_departures_the_device_refuses():
+    """What cv2 accepts and the device entry points refuse or define otherwise: a negative threshold is squared (it acts as
+    its absolute value), and iterationsCount = 0 runs one iteration."""
+    cv2 = pytest.importorskip("cv2")
+    K, uv, P, _ = synthetic.make_pnp_scene(1600, 60, outlier_frac=0.3, noise_px=1.0)
+    P = P * 1000
+    a = cv2.solvePnPRansac(P, uv, K, np.zeros((8, 1)), reprojectionError=-5, iterationsCount=500, confidence=0.99, flags=cv2.SOLVEPNP_EPNP)
+    b = cv2.solvePnPRansac(P, uv, K, np.zeros((8, 1)), reprojectionError=5, iterationsCount=500, confidence=0.99, flags=cv2.SOLVEPNP_EPNP)
+    assert a[0] and a[3].tolist() == b[3].tolist() and a[1].tobytes() == b[1].tobytes()
+
+
+def test_cv2_reads_only_fx_fy_cx_cy():
+    """EPnP and projectPoints ignore K's skew, its [1][0] entry and its last row, as the device's frame view does."""
+    cv2 = pytest.importorskip("cv2")
+    K, uv, P, _ = synthetic.make_pnp_scene(1650, 50, outlier_frac=0.0, noise_px=1.0)
+    P = P * 1000
+    K2 = K.copy()
+    K2[0, 1], K2[1, 0], K2[2] = 3.5, -0.7, (0.3, -0.2, 7.0)
+    a = cv2.solvePnP(P, uv, K, None, flags=cv2.SOLVEPNP_EPNP)
+    b = cv2.solvePnP(P, uv, K2, None, flags=cv2.SOLVEPNP_EPNP)
+    assert a[1].tobytes() == b[1].tobytes() and a[2].tobytes() == b[2].tobytes()
+    assert cv2.projectPoints(P, a[1], a[2], K, None)[0].tobytes() == cv2.projectPoints(P, a[1], a[2], K2, None)[0].tobytes()
+    r = cv2.solvePnPRansac(P, uv, K, None, reprojectionError=2, iterationsCount=200, flags=cv2.SOLVEPNP_EPNP)
+    r2 = cv2.solvePnPRansac(P, uv, K2, None, reprojectionError=2, iterationsCount=200, flags=cv2.SOLVEPNP_EPNP)
+    assert r[3].tolist() == r2[3].tolist() and r[1].tobytes() == r2[1].tobytes()
