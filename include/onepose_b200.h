@@ -383,9 +383,13 @@ int opb_warp_crop_u8(const uint8_t* frames, int64_t frame_pitch, int64_t row_pit
  * cv::RNG((uint64)-1) by getSubset (2 distinct indices), each one's closed-form similarity in fp64 from the fp32 points, the
  * fp32 error ((F0 x + F1 y) + F2 - X)^2 + (...)^2 with the model rounded to fp32, against (float)(threshold^2), every operation
  * rounded on its own; a sample wins when its count exceeds max(best, 1), and each win lowers the budget to
- * RANSACUpdateNumIters(confidence, outlier ratio, 2, budget).  The winner's inliers are refined by OpenCV's Levenberg-Marquardt
- * on (a, b, tx, ty) for at most refine_iters accepted steps (fp64, reductions in a fixed order).  The samples, counts, mask and
- * the unrefined model are cv2's bit for bit; the refined model agrees to rounding.  Results do not depend on the launch. */
+ * RANSACUpdateNumIters(confidence, outlier ratio, 2, budget).  The winner's inliers are refined by OpenCV's LMSolver on
+ * (a, b, tx, ty) for at most refine_iters iterations, kept steps or not: its damping schedule (lambda from 1, halved to 0 on
+ * good steps, raised by nu on poor ones), its stop once every residual of the kept model is below FLT_EPSILON, and its
+ * eigen-decomposition solve that drops eigenvalues below 2 DBL_EPSILON * trace (fp64, reductions in a fixed order).  The
+ * samples, counts, mask and the unrefined model are cv2's bit for bit; the refined
+ * model was measured within 1.7e-13 relative of cv2 4.13's at every refine_iters from 1 to 1000, with coordinates up to 1e6
+ * and thresholds up to 1e200 (DESIGN 5.8).  Results do not depend on the launch. */
 int opb_estimate_affine_partial(const float* from, const float* to, const int32_t* offsets, int32_t B, double threshold, int32_t max_iters,
                                 double confidence, int32_t refine_iters, double* affine, uint8_t* inlier_mask, int32_t* iterations,
                                 int32_t* status, void* stream);

@@ -13,7 +13,8 @@
 //             <= (float)(thr * thr);
 //   loop      a win is a count strictly above max(best, 1), then RANSACUpdateNumIters(confidence, outlier ratio, 2, budget);
 //             the loop exits at iter >= budget;
-//   refine    the winner's inliers, OpenCV's LMSolver on (a, b, tx, ty) (AffinePartial2DRefineCallback) in fp64.
+//   refine    the winner's inliers, OpenCV's LMSolver on (a, b, tx, ty) (AffinePartial2DRefineCallback) in fp64, its
+//             damping schedule and its eigen-decomposition solve (lm_refine).
 // Every product and sum of the model and the count is rounded on its own (__dmul_rn, __fadd_rn, ...), so nothing is contracted
 // into a fused multiply-add: the samples' models are cv2's bit for bit and the counts exact.  The refinement's reductions run in
 // a fixed order (not OpenCV's), so the refined model agrees with cv2's to rounding (DESIGN 5.8).
@@ -111,32 +112,36 @@ __device__ __forceinline__ void to_f32(const double* M, float* F) {
   for (int k = 0; k < 6; ++k) F[k] = __double2float_rn(M[k]);
 }
 
-constexpr int kSums = 9;
+constexpr int kSums = 9;                   // the first reduction's sums; one max (the largest residual) follows them
 
 struct AffShared {
   int samples[kAffWave * kModelPoints];
   int counts[kAffWave];
   int first, niters, best, win0, win1, done, iter, go;
-  double red[kAffWarps][kSums];
+  double red[kAffWarps][kSums + 1];
   double xd[4];
   double H[6];                             // the result: the model (zeros for none)
   int status;                              // 1: a model, 0: none
 };
 
-// sums[k] over the block in a fixed order (lanes by shuffle, then warps in index order); thread 0 gets the totals
+// v[0 .. N) summed and v[N] maximised (fmax: a NaN is passed over) over the block in a fixed order (lanes by shuffle, then
+// warps in index order); thread 0 gets the totals
 template <int N>
-__device__ void block_sum(double* v, AffShared& sh) {
+__device__ void block_reduce(double* v, AffShared& sh) {
   const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
 #pragma unroll
-  for (int k = 0; k < N; ++k)
-    for (int o = 16; o; o >>= 1) v[k] += __shfl_down_sync(0xffffffffu, v[k], o);
+  for (int k = 0; k <= N; ++k)
+    for (int o = 16; o; o >>= 1) {
+      const double u = __shfl_down_sync(0xffffffffu, v[k], o);
+      v[k] = k < N ? v[k] + u : fmax(v[k], u);
+    }
   if (lane == 0)
-    for (int k = 0; k < N; ++k) sh.red[warp][k] = v[k];
+    for (int k = 0; k <= N; ++k) sh.red[warp][k] = v[k];
   __syncthreads();
   if (threadIdx.x == 0)
-    for (int k = 0; k < N; ++k) {
+    for (int k = 0; k <= N; ++k) {
       double s = sh.red[0][k];
-      for (int w = 1; w < kAffWarps; ++w) s += sh.red[w][k];
+      for (int w = 1; w < kAffWarps; ++w) s = k < N ? s + sh.red[w][k] : fmax(s, sh.red[w][k]);
       v[k] = s;
     }
 }
@@ -148,40 +153,117 @@ __device__ __forceinline__ void residual(const double* h, const Pair& p, double&
   r1 = sub(add(add(mul(h[1], Mx), mul(h[0], My)), h[3]), (double)p.Y);
 }
 
-// Ap d = v for the 4x4 system by Gaussian elimination with partial pivoting
-__device__ void solve4(double (*a)[4], double* v, double* d) {
-  for (int i = 0; i < 4; ++i) {
-    int k = i;
-    for (int j = i + 1; j < 4; ++j)
-      if (fabs(a[j][i]) > fabs(a[k][i])) k = j;
-    if (k != i) {
-      for (int c = 0; c < 4; ++c) { const double t = a[i][c]; a[i][c] = a[k][c]; a[k][c] = t; }
-      const double t = v[i]; v[i] = v[k]; v[k] = t;
-    }
-    for (int j = i + 1; j < 4; ++j) {
-      const double f = a[j][i] / a[i][i];
-      for (int c = i; c < 4; ++c) a[j][c] -= f * a[i][c];
-      v[j] -= f * v[i];
+// cv::eigen of the symmetric 4x4 matrix a as OpenCV's JacobiImpl_ runs it: rotations at the largest off-diagonal |a_kl| (found
+// through per-row and per-column maxima) until it is <= DBL_EPSILON or after 30 n^2 rotations, then the eigenvalues w in
+// descending order with the eigenvectors as the rows of V.  a is overwritten.
+__device__ void jacobi4(double (*a)[4], double* w, double (*V)[4]) {
+  constexpr int n = 4;
+  int ind_r[n], ind_c[n];
+  auto row_max = [&](int k) {
+    int m = k + 1;
+    for (int i = k + 2; i < n; ++i) m = fabs(a[k][m]) < fabs(a[k][i]) ? i : m;
+    return m;
+  };
+  auto col_max = [&](int k) {
+    int m = 0;
+    for (int i = 1; i < k; ++i) m = fabs(a[m][k]) < fabs(a[i][k]) ? i : m;
+    return m;
+  };
+  for (int k = 0; k < n; ++k) {
+    w[k] = a[k][k];
+    for (int c = 0; c < n; ++c) V[k][c] = k == c ? 1.0 : 0.0;
+    ind_r[k] = k < n - 1 ? row_max(k) : 0;
+    ind_c[k] = k > 0 ? col_max(k) : 0;
+  }
+  for (int iter = 0; iter < 30 * n * n; ++iter) {
+    int k = 0, l = ind_r[0];
+    double mv = fabs(a[0][ind_r[0]]);
+    for (int i = 1; i < n - 1; ++i)
+      if (mv < fabs(a[i][ind_r[i]])) { mv = fabs(a[i][ind_r[i]]); k = i; l = ind_r[i]; }
+    for (int i = 1; i < n; ++i)
+      if (mv < fabs(a[ind_c[i]][i])) { mv = fabs(a[ind_c[i]][i]); k = ind_c[i]; l = i; }
+    const double p = a[k][l];
+    if (fabs(p) <= DBL_EPSILON) break;
+    const double y = mul(sub(w[l], w[k]), 0.5);
+    double t = add(fabs(y), hypot(p, y));
+    double s = hypot(p, t);
+    const double c = __ddiv_rn(t, s);
+    s = __ddiv_rn(p, s);
+    t = mul(__ddiv_rn(p, t), p);
+    if (y < 0) { s = -s; t = -t; }
+    a[k][l] = 0.0;
+    w[k] = sub(w[k], t);
+    w[l] = add(w[l], t);
+    auto rot = [&](double& v0, double& v1) {
+      const double a0 = v0, b0 = v1;
+      v0 = sub(mul(a0, c), mul(b0, s));
+      v1 = add(mul(a0, s), mul(b0, c));
+    };
+    for (int i = 0; i < k; ++i) rot(a[i][k], a[i][l]);
+    for (int i = k + 1; i < l; ++i) rot(a[k][i], a[i][l]);
+    for (int i = l + 1; i < n; ++i) rot(a[k][i], a[l][i]);
+    for (int i = 0; i < n; ++i) rot(V[k][i], V[l][i]);
+    for (int idx : {k, l}) {
+      if (idx < n - 1) ind_r[idx] = row_max(idx);
+      if (idx > 0) ind_c[idx] = col_max(idx);
     }
   }
-  for (int i = 3; i >= 0; --i) {
-    double s = v[i];
-    for (int c = i + 1; c < 4; ++c) s -= a[i][c] * d[c];
-    d[i] = s / a[i][i];
+  for (int k = 0; k < n - 1; ++k) {
+    int m = k;
+    for (int i = k + 1; i < n; ++i) m = w[m] < w[i] ? i : m;
+    if (m != k) {
+      const double t = w[k]; w[k] = w[m]; w[m] = t;
+      for (int i = 0; i < n; ++i) { const double u = V[k][i]; V[k][i] = V[m][i]; V[m][i] = u; }
+    }
   }
 }
 
+// SVBkSb's rule: eigenvalue i counts when |w_i| > 2 DBL_EPSILON * sum(w); the others are dropped (a pseudo-inverse)
+__device__ __forceinline__ double kept_bound(const double* w) { return mul(add(add(add(w[0], w[1]), w[2]), w[3]), 2.0 * DBL_EPSILON); }
+
+// cv::solve(a, v, d, DECOMP_EIG): d = sum over the kept eigenpairs of V_i (V_i . v) / w_i, in eigenvalue order.  a is overwritten.
+__device__ void eig_solve4(double (*a)[4], const double* v, double* d) {
+  double w[4], V[4][4];
+  jacobi4(a, w, V);
+  const double bound = kept_bound(w);
+  for (int j = 0; j < 4; ++j) d[j] = 0.0;
+  for (int i = 0; i < 4; ++i) {
+    if (fabs(w[i]) <= bound) continue;
+    double s = 0.0;
+    for (int j = 0; j < 4; ++j) s = add(s, mul(V[i][j], v[j]));
+    s = mul(s, __ddiv_rn(1.0, w[i]));
+    for (int j = 0; j < 4; ++j) d[j] = add(d[j], mul(s, V[i][j]));
+  }
+}
+
+// max |diag(cv::invert(a, DECOMP_EIG))|, the pseudo-inverse over the kept eigenpairs.  a is overwritten.
+__device__ double eig_inverse_diag_max(double (*a)[4]) {
+  double w[4], V[4][4], diag[4] = {0.0, 0.0, 0.0, 0.0};
+  jacobi4(a, w, V);
+  const double bound = kept_bound(w);
+  for (int i = 0; i < 4; ++i) {
+    if (fabs(w[i]) <= bound) continue;
+    const double r = __ddiv_rn(1.0, w[i]);
+    for (int j = 0; j < 4; ++j) diag[j] = add(diag[j], mul(V[i][j], mul(r, V[i][j])));
+  }
+  return fmax(fmax(fabs(diag[0]), fabs(diag[1])), fmax(fabs(diag[2]), fabs(diag[3])));
+}
+
 // OpenCV's LMSolver (calib3d/src/levmarq.cpp, eps = FLT_EPSILON) on h = (a, b, tx, ty) over the pairs `inlier` accepts.
-// J^T J does not depend on h: rows (x, -y, 1, 0) and (y, x, 0, 1).  Each step solves (J^T J with its diagonal times
-// 1 + 10^lg) d = J^T r, tries h - d, and keeps it when the squared error falls (lg - 1) or not (lg + 1, clamped to +-16).
-// Stops after max_iters accepted steps, or when |d|_inf < eps or the error < eps^2.  h: the same in every thread on entry,
-// the result in thread 0 on exit.
+// J^T J does not depend on h: rows (x, -y, 1, 0) and (y, x, 0, 1); D is its diagonal.  From lambda = 1 and lc = 0.75, each
+// iteration solves (J^T J + lambda D) d = J^T r by eigen decomposition (eig_solve4) and tries h - d.  With the predicted
+// decrease dS = d . (2 J^T r - J^T J d) and R = (S - Sd) / dS (dS taken as 1 where |dS| <= DBL_EPSILON): R > 0.75 halves
+// lambda, to 0 once it drops below lc; R < 0.25 multiplies it by nu = clamp((Sd - S) / (d . J^T r) + 2, 2, 10), and from
+// lambda = 0 first sets lambda = lc = 1 / max |diag((J^T J)^+)| and halves nu.  The step is kept when Sd < S.  Every iteration
+// counts; the loop stops after max_iters, or when |d|_inf < eps or when every residual |r_i| of the kept model is below eps
+// (not S < eps^2, which takes more steps on sub-pixel fits; tests/affine_ransac_reference.py's lm_refine, the schedule cv2
+// 4.13 runs).  h: the same in every thread on entry, the result in thread 0 on exit.
 template <class Pairs, class Inlier>
 __device__ void lm_refine(const Pairs& P, int n, Inlier inlier, int max_iters, double* h, AffShared& sh) {
   const int tid = threadIdx.x;
-  double s[kSums];
-  for (int k = 0; k < kSums; ++k) s[k] = 0.0;
-  for (int j = tid; j < n; j += kAffThreads) {        // sums of 1, x, y, x^2 + y^2; then the error and J^T r at h
+  double s[kSums + 1];
+  for (int k = 0; k <= kSums; ++k) s[k] = 0.0;
+  for (int j = tid; j < n; j += kAffThreads) {        // sums of 1, x, y, x^2 + y^2; then the error and J^T r at h; max |r_i|
     const Pair p = P(j);
     if (!inlier(p)) continue;
     const double Mx = p.x, My = p.y;
@@ -190,28 +272,28 @@ __device__ void lm_refine(const Pairs& P, int n, Inlier inlier, int max_iters, d
     s[0] += 1.0; s[1] += Mx; s[2] += My; s[3] += Mx * Mx + My * My;
     s[4] += r0 * r0 + r1 * r1;
     s[5] += Mx * r0 + My * r1; s[6] += Mx * r1 - My * r0; s[7] += r0; s[8] += r1;
+    s[9] = fmax(s[9], fmax(fabs(r0), fabs(r1)));
   }
-  block_sum<kSums>(s, sh);
-  double A[4][4], v[4], S = 0.0;
-  int lg = -3, it = 0;
+  block_reduce<kSums>(s, sh);
+  double A[4][4], v[4], S = 0.0, rmax = 0.0, lambda = 1.0, lc = 0.75;
+  int it = 0;
   if (tid == 0) {
     const double A0[4][4] = {{s[3], 0.0, s[1], s[2]}, {0.0, s[3], -s[2], s[1]}, {s[1], -s[2], s[0], 0.0}, {s[2], s[1], 0.0, s[0]}};
     for (int r = 0; r < 4; ++r)
       for (int c = 0; c < 4; ++c) A[r][c] = A0[r][c];
     S = s[4];
+    rmax = s[9];
     for (int k = 0; k < 4; ++k) v[k] = s[5 + k];
   }
   while (true) {
-    double dmax = 0.0;
+    double d[4], dmax = 0.0;
     if (tid == 0) {
-      double Ap[4][4], vp[4], d[4];
-      const double lambda = exp(lg * log(10.0));
+      double Ap[4][4];
       for (int r = 0; r < 4; ++r) {
         for (int c = 0; c < 4; ++c) Ap[r][c] = A[r][c];
-        Ap[r][r] *= 1.0 + lambda;
-        vp[r] = v[r];
+        Ap[r][r] = add(Ap[r][r], mul(lambda, A[r][r]));
       }
-      solve4(Ap, vp, d);
+      eig_solve4(Ap, v, d);
       for (int k = 0; k < 4; ++k) {
         sh.xd[k] = h[k] - d[k];
         dmax = fmax(dmax, fabs(d[k]));
@@ -220,7 +302,7 @@ __device__ void lm_refine(const Pairs& P, int n, Inlier inlier, int max_iters, d
     }
     __syncthreads();
     const double xd[4] = {sh.xd[0], sh.xd[1], sh.xd[2], sh.xd[3]};
-    double t[5] = {0.0, 0.0, 0.0, 0.0, 0.0};
+    double t[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
     for (int j = tid; j < n; j += kAffThreads) {
       const Pair p = P(j);
       if (!inlier(p)) continue;
@@ -229,19 +311,40 @@ __device__ void lm_refine(const Pairs& P, int n, Inlier inlier, int max_iters, d
       residual(xd, p, r0, r1);
       t[0] += r0 * r0 + r1 * r1;
       t[1] += Mx * r0 + My * r1; t[2] += Mx * r1 - My * r0; t[3] += r0; t[4] += r1;
+      t[5] = fmax(t[5], fmax(fabs(r0), fabs(r1)));
     }
-    block_sum<5>(t, sh);
+    block_reduce<5>(t, sh);
     if (tid == 0) {
-      if (t[0] < S) {
-        S = t[0];
-        for (int k = 0; k < 4; ++k) { h[k] = xd[k]; v[k] = t[1 + k]; }
-        lg = max(lg - 1, -16);
-        ++it;
-      } else {
-        it += lg == 16;
-        lg = min(lg + 1, 16);
+      const double Sd = t[0];
+      double dS = 0.0, dv = 0.0;
+      for (int r = 0; r < 4; ++r) {
+        double Ad = 0.0;
+        for (int c = 0; c < 4; ++c) Ad = add(Ad, mul(A[r][c], d[c]));
+        dS = add(dS, mul(d[r], sub(mul(2.0, v[r]), Ad)));
+        dv = add(dv, mul(d[r], v[r]));
       }
-      sh.go = it < max_iters && dmax >= (double)kFltEps && S >= (double)kFltEps * (double)kFltEps;
+      const double R = __ddiv_rn(sub(S, Sd), fabs(dS) > DBL_EPSILON ? dS : 1.0);
+      if (R > 0.75) {
+        lambda *= 0.5;
+        if (lambda < lc) lambda = 0.0;
+      } else if (R < 0.25) {
+        double nu = fmin(fmax(add(__ddiv_rn(sub(Sd, S), fabs(dv) > DBL_EPSILON ? dv : 1.0), 2.0), 2.0), 10.0);
+        if (lambda == 0.0) {
+          double Ai[4][4];
+          for (int r = 0; r < 4; ++r)
+            for (int c = 0; c < 4; ++c) Ai[r][c] = A[r][c];
+          lambda = lc = __ddiv_rn(1.0, fmax(DBL_EPSILON, eig_inverse_diag_max(Ai)));
+          nu *= 0.5;
+        }
+        lambda = mul(lambda, nu);
+      }
+      if (Sd < S) {
+        S = Sd;
+        rmax = t[5];
+        for (int k = 0; k < 4; ++k) { h[k] = xd[k]; v[k] = t[1 + k]; }
+      }
+      ++it;
+      sh.go = it < max_iters && dmax >= (double)kFltEps && rmax >= (double)kFltEps;
     }
     __syncthreads();
     if (!sh.go) break;

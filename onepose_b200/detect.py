@@ -25,6 +25,7 @@ MAX_VIEWS = 256         # opb_boxes_from_matches' bounds (include/onepose_b200.h
 MAX_REF_POINTS = 8192
 MIN_MATCHES = 6         # match_worker: fewer matches give the [0, 0, H, W] box
 MAX_TABLE_VIEWS = 2**31 - 1     # the views of all objects in one opb_boxes_from_matches_objects table
+INT32_MAX = 2**31 - 1           # maxIters and refineIters reach the library as int32; larger values are refused, not wrapped
 
 
 def _check_params(threshold, max_iters, confidence, refine_iters):
@@ -32,8 +33,8 @@ def _check_params(threshold, max_iters, confidence, refine_iters):
         raise ValueError(f"ransacReprojThreshold must be finite, got {threshold!r}")
     if not 0 < confidence < 1:
         raise ValueError(f"confidence must lie in (0, 1) (OpenCV asserts it), got {confidence!r}")
-    if int(max_iters) < 0 or int(refine_iters) < 0:
-        raise ValueError(f"maxIters and refineIters must be >= 0, got {max_iters!r}, {refine_iters!r}")
+    if not 0 <= int(max_iters) <= INT32_MAX or not 0 <= int(refine_iters) <= INT32_MAX:
+        raise ValueError(f"maxIters and refineIters must lie in [0, 2**31 - 1], got {max_iters!r}, {refine_iters!r}")
 
 
 def affine_partial_batch(from_pts: torch.Tensor, to_pts: torch.Tensor, offsets: torch.Tensor, threshold: float = 3.0,
@@ -63,7 +64,9 @@ def affine_partial_batch(from_pts: torch.Tensor, to_pts: torch.Tensor, offsets: 
 def estimate_affine_partial_2d(from_pts, to_pts, *, ransacReprojThreshold=3, maxIters=2000, confidence=0.99, refineIters=10, device=None):
     """Drop-in for ``cv2.estimateAffinePartial2D(from_pts, to_pts, ransacReprojThreshold=..., ...)`` (method RANSAC): numpy
     [n, 2] (or [n, 1, 2]) in, ``(affine f64 [2, 3] or None, inliers uint8 [n, 1])`` out, computed on the device.  The samples,
-    the mask and the unrefined model are OpenCV 4.13's bit for bit; the refined model agrees to rounding (DESIGN 5.8)."""
+    the mask and the unrefined model are OpenCV 4.13's bit for bit; the refined model follows its LMSolver step for step and
+    was measured within 1.7e-13 relative of cv2's (refineIters 1 to 1000, coordinates up to 1e6; DESIGN 5.8).  maxIters and
+    refineIters above 2**31 - 1 are refused, where cv2 casts them to int."""
     dev = torch.device(device if device is not None else "cuda")
     f = np.asarray(from_pts, dtype=np.float64).reshape(-1, 2).astype(np.float32)
     t = np.asarray(to_pts, dtype=np.float64).reshape(-1, 2).astype(np.float32)

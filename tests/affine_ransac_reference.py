@@ -10,8 +10,11 @@ calib3d/src/levmarq.cpp: ``LMSolver``), stage by stage:
   fp32 error against ``(float)(thr * thr)``, a win when the count is strictly above ``max(best, 1)``, then
   ``RANSACUpdateNumIters(confidence, outlier ratio, 2, budget)``; the loop exits at ``iter >= budget``;
 - no winner: ``(None, zero mask)``;
-- the refinement: the winner's inliers compressed in order, OpenCV's Levenberg-Marquardt on ``(a, b, tx, ty)`` for at most
-  ``refineIters`` iterations (accepted steps), each step ``(J^T J) diag * (1 + 10^k)`` solved against ``J^T r``.
+- the refinement: the winner's inliers compressed in order, OpenCV's ``LMSolver`` on ``(a, b, tx, ty)`` for at most
+  ``refineIters`` iterations (kept or not), each step ``J^T J + lambda diag(J^T J)_0`` solved against ``J^T r`` by eigen
+  decomposition (``lm_refine``; the schedule was worked out from cv2 4.13's results and reproduces them to 1e-13 relative,
+  bit for bit at most points, also at coordinates shifted by 1e6, where ``cv::solve``'s dropped eigenvalues stop the
+  translation from moving).
 ``minimal="cv2"`` takes each minimal model from ``cv2.estimateAffinePartial2D`` on exactly the two sampled pairs (OpenCV's own
 ``runKernel`` result); ``minimal="closed"`` evaluates ``run_kernel`` below, the closed form restated in numpy fp64.  The
 generator and the 2-point scan need no cv2, so GPU tests use them without it.
@@ -24,6 +27,7 @@ from tests.opencv_ransac_reference import CvRNG, draw_subset, update_num_iters
 
 MODEL_POINTS = 2
 FLT_EPSILON = float(np.finfo(np.float32).eps)
+DBL_EPSILON = float(np.finfo(np.float64).eps)
 
 
 def subsets(n: int, count: int):
@@ -93,28 +97,146 @@ def _normal(h, src, dst):
     return J.T @ J, J.T @ r, r
 
 
+def jacobi(M):
+    """``cv::eigen`` of a symmetric fp64 matrix as OpenCV's ``JacobiImpl_`` runs it: cyclic-by-largest Jacobi rotations (the
+    largest off-diagonal |a_kl| found through per-row and per-column maxima), stopping when it is <= DBL_EPSILON (absolute) or
+    after 30 n^2 rotations, then eigenvalues sorted in descending order.  Returns (w [n], V [n, n], row i the eigenvector of w[i])."""
+    A = np.array(M, np.float64)
+    n = len(A)
+    V, W = np.eye(n), np.diag(A).copy()
+    ind_r, ind_c = [0] * n, [0] * n
+
+    def row_max(k):
+        m = k + 1
+        for i in range(k + 2, n):
+            m = i if abs(A[k, m]) < abs(A[k, i]) else m
+        return m
+
+    def col_max(k):
+        m = 0
+        for i in range(1, k):
+            m = i if abs(A[m, k]) < abs(A[i, k]) else m
+        return m
+
+    for k in range(n):
+        ind_r[k] = row_max(k) if k < n - 1 else 0
+        ind_c[k] = col_max(k) if k > 0 else 0
+    for _ in range(30 * n * n if n > 1 else 0):
+        k, mv = 0, abs(A[0, ind_r[0]])
+        for i in range(1, n - 1):
+            if mv < abs(A[i, ind_r[i]]):
+                mv, k = abs(A[i, ind_r[i]]), i
+        l = ind_r[k]
+        for i in range(1, n):
+            if mv < abs(A[ind_c[i], i]):
+                mv, k, l = abs(A[ind_c[i], i]), ind_c[i], i
+        p = A[k, l]
+        if abs(p) <= DBL_EPSILON:
+            break
+        y = (W[l] - W[k]) * 0.5
+        t = abs(y) + np.hypot(p, y)
+        s = np.hypot(p, t)
+        c = t / s
+        s, t = p / s, (p / t) * p
+        if y < 0:
+            s, t = -s, -t
+        A[k, l] = 0.0
+        W[k] -= t
+        W[l] += t
+
+        def rot(a0, b0):
+            return a0 * c - b0 * s, a0 * s + b0 * c
+        for i in range(k):
+            A[i, k], A[i, l] = rot(A[i, k], A[i, l])
+        for i in range(k + 1, l):
+            A[k, i], A[i, l] = rot(A[k, i], A[i, l])
+        for i in range(l + 1, n):
+            A[k, i], A[l, i] = rot(A[k, i], A[l, i])
+        for i in range(n):
+            V[k, i], V[l, i] = rot(V[k, i], V[l, i])
+        for idx in (k, l):
+            if idx < n - 1:
+                ind_r[idx] = row_max(idx)
+            if idx > 0:
+                ind_c[idx] = col_max(idx)
+    for k in range(n - 1):
+        m = k
+        for i in range(k + 1, n):
+            m = i if W[m] < W[i] else m
+        if m != k:
+            W[[k, m]], V[[k, m]] = W[[m, k]], V[[m, k]]
+    return W, V
+
+
+def _kept(w):
+    """``SVBkSb``'s rule: an eigenvalue counts when |w_i| > 2 DBL_EPSILON * sum(w); the others are dropped (a pseudo-inverse)."""
+    thr = 0.0
+    for wi in w:
+        thr += wi
+    return [i for i in range(len(w)) if abs(w[i]) > thr * (2 * DBL_EPSILON)]
+
+
+def eig_solve(M, b):
+    """``cv::solve(M, b, d, DECOMP_EIG)``: sum over the kept eigenpairs of v_i (v_i . b) / w_i, in eigenvalue order."""
+    w, V = jacobi(M)
+    x = np.zeros(len(w))
+    for i in _kept(w):
+        s = 0.0
+        for j in range(len(w)):
+            s += V[i, j] * b[j]
+        x = x + (s * (1.0 / w[i])) * V[i]
+    return x
+
+
+def eig_inverse_diagonal(M):
+    """The diagonal of ``cv::invert(M, DECOMP_EIG)``, the pseudo-inverse over the kept eigenpairs."""
+    w, V = jacobi(M)
+    out = np.zeros(len(w))
+    for i in _kept(w):
+        out = out + V[i] * ((1.0 / w[i]) * V[i])
+    return out
+
+
 def lm_refine(H, src, dst, max_iters: int, eps: float = FLT_EPSILON):
-    """OpenCV's LMSolver (eps = FLT_EPSILON) on (a, b, tx, ty) = (H00, H10, H02, H12).  Returns (H refined, accepted steps)."""
+    """OpenCV's ``LMSolver`` (eps = FLT_EPSILON) on (a, b, tx, ty) = (H00, H10, H02, H12).  D = diag(J^T J) at the start,
+    lambda = 1, lc = 0.75.  Each iteration solves (J^T J + lambda D) d = J^T r by ``eig_solve`` and tries x - d.  With the
+    predicted decrease dS = d . (2 J^T r - J^T J d) and R = (S - Sd) / dS (dS taken as 1 where |dS| <= DBL_EPSILON):
+    R > 0.75 halves lambda, to 0 (Gauss-Newton) once it drops below lc; R < 0.25 multiplies it by
+    nu = clamp((Sd - S) / (d . J^T r) + 2, 2, 10), and from lambda = 0 first sets lambda = lc = 1 / max |diag((J^T J)^+)| and
+    halves nu.  The step is kept when Sd < S.  Every iteration counts, kept or not; the loop stops after max_iters of them, or
+    when |d|_inf < eps or when the largest residual |r_i| of the kept model is < eps (not S < eps^2: on sub-pixel fits every
+    |r_i| can be below eps while S is still above eps^2, and cv2 stops there).  A NaN residual is passed over, as a running
+    std::max from 0 does.  Returns (H refined, iterations)."""
     x = np.array([H[0, 0], H[1, 0], H[0, 2], H[1, 2]], np.float64)
     A, v, r = _normal(x, src, dst)
     S = float(r @ r)
-    lg, it = -3, 0
+    D = np.diag(A).copy()
+    lam, lc, it = 1.0, 0.75, 0
     while True:
         Ap = A.copy()
-        lam = np.exp(lg * np.log(10.0))
-        Ap[np.diag_indices(4)] *= 1 + lam
-        d = np.linalg.solve(Ap, v)
+        Ap[np.diag_indices(4)] += lam * D
+        d = eig_solve(Ap, v)
         xd = x - d
         rd = _residuals(xd, src, dst)
         Sd = float(rd @ rd)
+        dS = float(d @ (2 * v - A @ d))
+        R = (S - Sd) / (dS if abs(dS) > DBL_EPSILON else 1.0)
+        if R > 0.75:
+            lam *= 0.5
+            if lam < lc:
+                lam = 0.0
+        elif R < 0.25:
+            t = float(d @ v)
+            nu = min(max((Sd - S) / (t if abs(t) > DBL_EPSILON else 1.0) + 2, 2.0), 10.0)
+            if lam == 0:
+                lam = lc = 1.0 / max(DBL_EPSILON, float(np.abs(eig_inverse_diagonal(A)).max()))
+                nu *= 0.5
+            lam *= nu
         if Sd < S:
-            S, x, it = Sd, xd, it + 1
-            lg = max(lg - 1, -16)
+            S, x = Sd, xd
             A, v, r = _normal(x, src, dst)
-        else:
-            it += lg == 16
-            lg = min(lg + 1, 16)
-        if not (it < max_iters and np.abs(d).max() >= eps and S >= eps * eps):
+        it += 1
+        if not (it < max_iters and np.abs(d).max() >= eps and np.fmax.reduce(np.abs(r)) >= eps):
             break
     out = np.array([[x[0], -x[1], x[2]], [x[1], x[0], x[3]]], np.float64)
     return out, it

@@ -120,7 +120,8 @@ def test_numpy_drop_in_and_degenerate_inputs():
     H, m = detect.estimate_affine_partial_2d(fp.astype(np.float64), tp.astype(np.float64), ransacReprojThreshold=6)
     Hr, mr, _ = A.estimate_affine_partial_2d(fp, tp, 6.0, minimal=MINIMAL)
     assert np.array_equal(m.ravel(), mr) and np.abs(H - Hr).max() <= REFINE_RTOL * np.abs(Hr).max()
-    for bad in (dict(confidence=1.0), dict(confidence=0.0), dict(maxIters=-1), dict(refineIters=-2), dict(ransacReprojThreshold=np.inf)):
+    for bad in (dict(confidence=1.0), dict(confidence=0.0), dict(maxIters=-1), dict(refineIters=-2), dict(ransacReprojThreshold=np.inf),
+                dict(maxIters=2**31), dict(maxIters=2**32 + 5), dict(refineIters=2**31), dict(refineIters=2**32 + 1)):
         with pytest.raises(ValueError):
             detect.estimate_affine_partial_2d(fp, tp, **bad)
     with pytest.raises(ValueError):

@@ -129,6 +129,19 @@ def test_checks_before_the_library_call(recorder):
     assert not recorder
 
 
+def test_affine_budgets_reach_the_library_as_int32_or_are_refused(recorder):
+    """maxIters and refineIters cross into the library as int32: 2**31 - 1 passes unchanged, anything above is refused rather than
+    wrapped (2**32 + 5 would otherwise run 5 iterations, and 2**31 arrive negative)."""
+    f, offs = torch.zeros(4, 2), torch.tensor([0, 4], dtype=torch.int32)
+    detect.affine_partial_batch(f, f, offs, max_iters=2**31 - 1, refine_iters=2**31 - 1)
+    name, args = recorder.pop()
+    assert name == "opb_estimate_affine_partial" and args[5] == args[7] == 2**31 - 1
+    for kw in (dict(max_iters=2**31), dict(max_iters=2**32 + 5), dict(refine_iters=2**31), dict(refine_iters=2**32 + 1), dict(max_iters=-1)):
+        with pytest.raises(ValueError, match="2\\*\\*31 - 1"):
+            detect.affine_partial_batch(f, f, offs, **kw)
+    assert not recorder
+
+
 def test_crop_and_detect_checks_before_the_library_call(recorder):
     frames = torch.zeros(2, 48, 64, dtype=torch.uint8)
     K = torch.eye(3, dtype=torch.float64)
