@@ -605,11 +605,6 @@ int opb_debug_set_ws_fill(int32_t byte);
 /* Tensor-core passes of the k,v projection: 2 (default: A_hi.(B_hi + B_lo); its output is rounded to one fp16 plane anyway) or
  * 3 (the full split product), for the precision A/B in tests/ and tools/. */
 int opb_debug_set_kv_passes(opb_matcher* m, int32_t passes);
-/* Residual of a layer = identity K-block of its mlp.3 GEMM.  0 (default): full-width MMAs against I; 1: k-block j runs as
- * N = 64 MMAs on accumulator columns [64 j, 64 j + 64) against the 64 x 64 diagonal block of I (a quarter of the tensor work,
- * but ptxas serialises every MMA of that kernel, and it is slower).  Bit-identical results (the skipped products are exact
- * zeros); A/B switch for tests/ and tools/. */
-int opb_debug_set_identity_diag(opb_matcher* m, int32_t enable);
 /* One problem of the GEMM core, field for field the library's own problem description (csrc/gemm_common.cuh GemmProblem):
  *   C[batch][rows, n_out] = [A1 | A2] . [B1 | B2]^T (+ bias) -> the epilogue `epi`
  * Operands are fp16-split planes (hi = fp16(64 x), lo = fp16(64 x - hi); opb_debug_split), row-major, each with its own ld in
@@ -638,8 +633,8 @@ typedef struct opb_debug_gemm_desc {
   const void* b2_hi;        /* [n_out, K2], or [segments * n_out, K2] per segment */
   const void* b2_lo;
   int32_t b2_ld;
-  int32_t b2_mode;          /* 0 shared, 1 one B2 per segment of the layout, 2 the identity with a zero lo plane, 3 the identity
-                               run on its 64 x 64 diagonal blocks (2, 3: converter problems only) */
+  int32_t b2_mode;          /* 0 shared, 1 one B2 per segment of the layout, 2 the identity with a zero lo plane
+                               (converter problems only) */
   int32_t a_hi_only;        /* A enters with its hi plane only (epi 9) */
   const float* a_raw;       /* converter: A1 = ReLU((a_raw - mu[seg]) * rstd[seg]) formed in the core from fp32 [rows, a_raw_ld]; NULL: off */
   int32_t a_raw_ld;

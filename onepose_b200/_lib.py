@@ -124,7 +124,6 @@ SYMBOLS = {
     "opb_debug_set_pdl": (C.c_int, [_I]),
     "opb_debug_set_ws_fill": (C.c_int, [_I]),
     "opb_debug_set_kv_passes": (C.c_int, [_P, _I]),
-    "opb_debug_set_identity_diag": (C.c_int, [_P, _I]),
     "opb_debug_gemm": (C.c_int, [C.POINTER(OpbDebugGemmDesc), _P]),
     "opb_debug_kv_state_h": (C.c_int, [_P, _I, _I, _I, _I, _P, C.POINTER(_I), _P]),
     "opb_debug_split": (C.c_int, [_P, _P, _P, C.c_size_t, _P]),

@@ -74,7 +74,6 @@ struct opb_matcher : Handle {
   int ws_frames = 0, ws_N = 0, ws_m_pad = 0;
   DevBuf tab;             // ChunkTable of the chunk in flight (written by assemble_layout)
   bool hoist = true;      // evaluate the frame-invariant layers once per object (object_prologue)
-  int identity_diag = 0;  // residual identity K-block at full width (1: N = 64 MMAs on the diagonal blocks; opb_debug_set_identity_diag)
   int kv_two_pass = 1;    // k,v projection as A_hi.(B_hi + B_lo): its output is one fp16 plane, the A_lo term is below that rounding
   PlaneBuf x, qp, pn, g, xq, bd, lin_a, lin_b;
   DevBuf kvt;             // fp16 [rows, 512]
@@ -286,7 +285,7 @@ static int run_attn_layer(opb_matcher* m, const Layout& L, XView x, int layer, A
   p3.L = L; p3.batch = 1; p3.rows = rows;
   p3.K1 = 512; p3.b1 = W.w1.c(512); p3.n_out = 256; p3.bias = W.b1.as<float>();
   p3.epi = EPI_BIAS_PLANES; p3.out = x.m(kD);
-  p3.a2 = x.c(kD); p3.K2 = kD; p3.b2 = m->eye.c(kD); p3.b2_lo_zero = 1; p3.b2_identity = m->identity_diag;
+  p3.a2 = x.c(kD); p3.K2 = kD; p3.b2 = m->eye.c(kD); p3.b2_lo_zero = 1;
   p3.a_conv = 1; p3.a_raw = m->hid.as<float>(); p3.a_raw_ld = 512; p3.mu = m->mu.as<float>(); p3.rstd = m->rstd.as<float>();
   if (int rc = gemm(m, p3, st, 2.0 * valid_rows * 256 * 512, "mlp3")) return rc;
   return stop_here(m, layer, 7, L, x) ? kStopped : 0;
@@ -964,13 +963,6 @@ int opb_debug_set_kv_passes(opb_matcher* m, int32_t passes) {
   return OPB_OK;
 }
 
-int opb_debug_set_identity_diag(opb_matcher* m, int32_t enable) {
-  if (!m) return OPB_E_INVALID;
-  m->identity_diag = enable ? 1 : 0;
-  invalidate_prologues(m);
-  return OPB_OK;
-}
-
 int opb_debug_set_stop(opb_matcher* m, int32_t layer, int32_t step) {
   if (!m || layer < -1 || step < 0) return OPB_E_INVALID;
   m->dbg_layer = layer;
@@ -1052,7 +1044,7 @@ int opb_debug_set_pdl(int32_t enable) {
 }
 
 int opb_debug_gemm(const opb_debug_gemm_desc* d, void* stream) {
-  REQUIRE(__func__, d && d->backend >= 0 && d->backend <= 1 && d->b2_mode >= 0 && d->b2_mode <= 3);
+  REQUIRE(__func__, d && d->backend >= 0 && d->backend <= 1 && d->b2_mode >= 0 && d->b2_mode <= 2);
   GemmProblem p{};
   p.epi = d->epi; p.bn = d->bn;
   p.rows = d->rows; p.n_out = d->n_out; p.K1 = d->K1; p.K2 = d->K2;
@@ -1063,8 +1055,7 @@ int opb_debug_gemm(const opb_debug_gemm_desc* d, void* stream) {
   p.b1 = CPlanes{(const __half*)d->b1_hi, (const __half*)d->b1_lo, d->b1_ld};
   p.b2 = CPlanes{(const __half*)d->b2_hi, (const __half*)d->b2_lo, d->b2_ld};
   p.b2_per_seg = d->b2_mode == 1;
-  p.b2_lo_zero = d->b2_mode >= 2;
-  p.b2_identity = d->b2_mode == 3;
+  p.b2_lo_zero = d->b2_mode == 2;
   p.a_hi_only = d->a_hi_only;
   p.a_conv = d->a_raw ? 1 : 0; p.a_raw = d->a_raw; p.a_raw_ld = d->a_raw_ld; p.mu = d->mu; p.rstd = d->rstd;
   p.L.B = d->B; p.L.N = d->N; p.L.M = d->M; p.L.n_pad = d->n_pad; p.L.m_pad = d->m_pad; p.L.R = d->n_pad + d->m_pad;

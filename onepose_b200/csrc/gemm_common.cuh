@@ -38,9 +38,6 @@ struct GemmProblem {
   int K1, K2;
   int b2_per_seg;
   int b2_lo_zero;        // the lo plane of b2 is identically zero (identity K-block): its A_hi.B_lo pass is skipped (bit-identical)
-  int b2_identity;       // b2 is the [n_out, n_out] identity (n_out = K2 = 256, fp16-split: hi = 64 I, lo = 0; implies b2_lo_zero): k-block j
-                         // of the K2 range touches output columns [64 j, 64 j + 64) only, so it runs as N = 64 MMAs on that column slice of
-                         // the accumulator against the 64 x 64 diagonal block -- a quarter of the tensor work of a full-width pass, same sums
   int a_hi_only;         // use only the hi plane of A (A_lo neither loaded nor multiplied): for a product whose OUTPUT is rounded to one
                          // fp16 plane anyway (k,v projection: the dropped term is below the output rounding, zero-mean per row, and the
                          // consumer averages over the segment's rows)

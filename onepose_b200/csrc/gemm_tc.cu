@@ -175,32 +175,25 @@ enum { ACV_NONE = 0, ACV_NORM_RELU = 1 };
 // HI: the A operand enters with its hi plane only (k,v projection, GemmProblem::a_hi_only): two passes, A_hi + B_hi + B_lo per stage.
 // BN_: column-tile width (256 for every matcher GEMM; 64 / 128 for the narrow convolution layers of the extractor: the stage
 // shrinks and the ring deepens to three / four stages).
-// K2B: what the K2 block's B operand is (the residual GEMM's identity: GemmProblem::b2_lo_zero / b2_identity).  The residual
-// GEMM is mlp.3, so both identity forms exist with the converter only, and the converter only with one of them.
-//   K2_LO_ZERO  its lo plane is zero: those k-blocks run a chain of their own without the A_hi.B_lo pass (it would add exact
-//               zeros).  The residual GEMM's default.
-//   K2_DIAG     the identity, run as N = 64 MMAs on the diagonal blocks.  Those MMAs write 32-register slices of the m64n256
-//               accumulator, which makes ptxas serialise every wgmma of the kernel (C7511), so the slices live in an
-//               instantiation of their own and the other variants keep back-to-back MMAs.  A quarter of K2_LO_ZERO's identity
-//               work, but the serialised hidden k-blocks make it the slower form on an H100 (DESIGN.md 5.1).
-// Both are template properties so that every k-block is one branch-free chain of MMAs: a branch between two wgmmas makes ptxas
-// insert a warpgroup.arrive in front of the MMAs that follow it.
-enum { K2_FULL = 0, K2_LO_ZERO = 1, K2_DIAG = 2 };
+// ACV and the K2 block: the converter exists for mlp.3 only, whose K2 block is its residual as an identity K-block
+// (GemmProblem::b2_lo_zero; launch_gemm_tc requires it with the converter and refuses it without).  The identity's lo plane is
+// zero, so with ACV the K2 k-blocks run a chain of their own without the A_hi.B_lo pass (it would add exact zeros).  The
+// template, not a branch inside the chain, selects it: a branch between two wgmmas makes ptxas insert a warpgroup.arrive in
+// front of the MMAs that follow it.  The identity runs at full width: N = 64 MMAs on its diagonal blocks are slower on an
+// H100 (DESIGN.md 5.1).
 
 // PP: the ping-pong schedule (BN_ 128; see the top of the file).
-template <int EPI, int ACV = ACV_NONE, bool HI = false, int BN_ = 256, int K2B = K2_FULL, bool PP = false>
+template <int EPI, int ACV = ACV_NONE, bool HI = false, int BN_ = 256, bool PP = false>
 __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_constant__ Maps maps, TcParams p) {
   constexpr int BN = BN_;
-  constexpr bool DIAG = K2B == K2_DIAG;
-  static_assert(!PP || (BN_ == 128 && ACV == ACV_NONE && !HI && K2B == K2_FULL && (EPI == EPI_F32 || EPI == EPI_F32_STATS || EPI == EPI_SCORE_SUMS)),
+  static_assert(!PP || (BN_ == 128 && ACV == ACV_NONE && !HI && (EPI == EPI_F32 || EPI == EPI_F32_STATS || EPI == EPI_SCORE_SUMS)),
                 "ping-pong: 128-column tiles of the variants that move");
   constexpr int kBBytes = BN * BK * 2;             // one plane of the B tile
   constexpr int kBOff = HI ? kABytes : 2 * kABytes;      // offset of the B planes inside a stage
   constexpr int kStageBytes = kBOff + 2 * kBBytes;
   constexpr int kStages = kRingBytes / kStageBytes;      // BN 256: 2, BN 128: 3, BN 64: 4
-  constexpr int kDiagBBytes = 64 * BK * 2;         // a 64 x 64 diagonal block of the identity
-  static_assert(K2B == K2_FULL || (BN_ == 256 && EPI == EPI_BIAS_PLANES && ACV == ACV_NORM_RELU), "identity K-block: mlp.3 only");
-  static_assert(ACV == ACV_NONE || K2B != K2_FULL, "the converter comes with the identity K-block");
+  static_assert(ACV == ACV_NONE || (BN_ == 256 && EPI == EPI_BIAS_PLANES), "the converter: mlp.3 only");
+  static_assert(EPI != EPI_SCORE_SUMS || PP, "score sums: one row sum per 128-column ping-pong tile");
   static_assert(PP || (EPI == EPI_CONV ? BN_ == 64 || BN_ == 128 : EPI == EPI_F32 ? BN_ == 128 || BN_ == 256 : BN_ == 256),
                 "tile widths: EPI_CONV 64 / 128, EPI_F32 128 / 256, every other cooperative epilogue 256");
   static_assert(BN_ == 256 || ACV == ACV_NONE && !HI, "narrow tiles: no converter, both A planes");
@@ -313,8 +306,7 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
           uint8_t* st = smem + s * kStageBytes;
           const bool first = kb < nkb1;
           const bool conv = ACV == ACV_NORM_RELU && first;           // this k-block's A tile comes in raw
-          const bool diag = DIAG && !first;                                // identity K-block: B = one 64 x 64 diagonal block, hi plane only
-          mbar_expect_tx(&full_bar[s], diag ? 2 * kABytes + kDiagBBytes : kStageBytes);
+          mbar_expect_tx(&full_bar[s], kStageBytes);
           int kc = (first ? kb * BK : (kb - nkb1) * BK);
           int arow = a_row, kcb = kc;                                   // A rows / B columns of this k-block
           if (EPI == EPI_CONV && p.taps) {                              // implicit-GEMM convolution: tap t = row-shifted A, B columns follow kb
@@ -335,10 +327,6 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
           } else {
             tma_load_2d(st, mah, &full_bar[s], kc, arow);
             if (!HI) tma_load_2d(st + kABytes, mal, &full_bar[s], kc, arow);
-          }
-          if (diag) {                                                   // rows [kc, kc + 64) x columns [kc, kc + 64) of I
-            tma_load_2d(st + kBOff, mbh, &full_bar[s], kc, kc);
-            continue;
           }
           tma_load_2d(st + kBOff, mbh, &full_bar[s], kcb, brow);
           tma_load_2d(st + kBOff + kBBytes, mbl, &full_bar[s], kcb, brow);
@@ -525,30 +513,15 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
           const uint32_t sa_h = smem_u32(st) + a_off;
           const uint32_t sa_l = sa_h + kABytes, sb_h = smem_u32(st) + kBOff, sb_l = sb_h + kBBytes;
           wgmma_fence();
-          if (K2B == K2_LO_ZERO && kb >= nkb1) {
-            // B_lo == 0: the A_hi.B_lo pass would add exact zeros.  A chain of its own, so that no branch sits between MMAs.
+          if (ACV != ACV_NONE && kb >= nkb1) {
+            // the identity K-block, B_lo == 0: the A_hi.B_lo pass would add exact zeros.  A chain of its own, so that no branch
+            // sits between MMAs.
 #pragma unroll
             for (int k = 0; k < BK / MMA_K; ++k) {
               const uint32_t koff = k * MMA_K * 2;
               const uint64_t bh = make_desc(sb_h + koff), ah = make_desc(sa_h + koff), al = make_desc(sa_l + koff);
               mma_k16<BN>(acc, ah, bh);
               mma_k16<BN>(acc, al, bh);
-            }
-            wgmma_commit();
-          } else if (DIAG && kb >= nkb1) {
-            // identity K-block j: only output columns [64 j, 64 j + 64) receive anything -> N = 64 MMAs on that slice of the
-            // accumulator (registers [32 j, 32 j + 32) of the fragment; the other 192 columns of a full-width MMA would add zeros)
-            const int j = kb - nkb1;
-#pragma unroll
-            for (int k = 0; k < BK / MMA_K; ++k) {
-              const uint32_t koff = k * MMA_K * 2;
-              const uint64_t bh = make_desc(sb_h + koff), ah = make_desc(sa_h + koff), al = make_desc(sa_l + koff);
-              switch (j) {
-                case 0: wgmma_m64n64k16(acc + 0, ah, bh); wgmma_m64n64k16(acc + 0, al, bh); break;
-                case 1: wgmma_m64n64k16(acc + 32, ah, bh); wgmma_m64n64k16(acc + 32, al, bh); break;
-                case 2: wgmma_m64n64k16(acc + 64, ah, bh); wgmma_m64n64k16(acc + 64, al, bh); break;
-                default: wgmma_m64n64k16(acc + 96, ah, bh); wgmma_m64n64k16(acc + 96, al, bh); break;
-              }
             }
             wgmma_commit();
           } else {
@@ -802,9 +775,8 @@ __global__ void __launch_bounds__(kThreads, 1) gemm_tc_kernel(const __grid_const
           }
           p.colsum_part[((long long)z * (p.m_tiles * 4) + m_tile * 4 + q) * p.L.m_pad + col0 + lane] = e[0];
         }
-        // one row sum per 128-column half of the score matrix: a PP tile, or half grp of a cooperative one
-        const int halves = PP ? p.n_tiles : p.n_tiles * 2, half = PP ? n_tile : n_tile * 2 + grp;
-        p.rowsum_part[((long long)z * halves + half) * p.L.n_pad + row] = rs;
+        // one row sum per 128-column tile of the score matrix
+        p.rowsum_part[((long long)z * p.n_tiles + n_tile) * p.L.n_pad + row] = rs;
       } else if (EPI == EPI_SCORE_CONF) {
         // ---- dual-softmax tail, pass 2: conf = (e / rowsum) * (e / colsum) recomputed from the accumulator (the cos matrix is
         // never materialised), optional conf store, packed row / column arg-max (reference :218-220).  The 32-column chunk is
@@ -1076,9 +1048,9 @@ int num_sms() {
   return n;
 }
 
-template <int EPI, int ACV = ACV_NONE, bool HI = false, int BN_ = 256, int K2B = K2_FULL, bool PP = false>
+template <int EPI, int ACV = ACV_NONE, bool HI = false, int BN_ = 256, bool PP = false>
 cudaError_t launch_variant(int grid, cudaStream_t stream, const Maps& mp, const TcParams& tp) {
-  auto* kern = gemm_tc_kernel<EPI, ACV, HI, BN_, K2B, PP>;
+  auto* kern = gemm_tc_kernel<EPI, ACV, HI, BN_, PP>;
   if (cudaError_t e = ensure_smem_limit((const void*)kern, kSmemBytes)) return e;
   return launch_k(pdl_enabled(), kern, dim3(grid), dim3(kThreads), kSmemBytes, stream, mp, tp);
 }
@@ -1144,7 +1116,7 @@ int launch_gemm_tc(const GemmProblem& p, cudaStream_t stream) {
   if (ok && p.a_conv) ok = make_map(&mp.a_raw, p.a_raw, a_rows, p.K1, p.a_raw_ld, 32, BM, true);
   else mp.a_raw = mp.b1h;
   if (ok && p.K2) {
-    ok = make_map(&mp.b2h, p.b2.hi, b2_rows, p.K2, p.b2.ld, BK, p.b2_identity ? 64 : tile_n, false) && make_map(&mp.b2l, p.b2.lo, b2_rows, p.K2, p.b2.ld, BK, tile_n, false) &&
+    ok = make_map(&mp.b2h, p.b2.hi, b2_rows, p.K2, p.b2.ld, BK, tile_n, false) && make_map(&mp.b2l, p.b2.lo, b2_rows, p.K2, p.b2.ld, BK, tile_n, false) &&
          make_map(&mp.a2h, p.a2.hi, a_rows, p.K2, p.a2.ld, BK, BM, false) && make_map(&mp.a2l, p.a2.lo, a_rows, p.K2, p.a2.ld, BK, BM, false);
   } else if (ok) {
     mp.a2h = mp.a1h; mp.a2l = mp.a1l; mp.b2h = mp.b1h; mp.b2l = mp.b1l;
@@ -1168,12 +1140,9 @@ int launch_gemm_tc(const GemmProblem& p, cudaStream_t stream) {
   if (!ok) return -2;
   TcParams tp{};
   tp.K1 = p.K1; tp.K2 = p.K2; tp.b2_per_seg = p.b2_per_seg; tp.n_out = p.n_out;
-  if (p.b2_identity && (!p.b2_lo_zero || p.b2_per_seg || p.K2 != p.n_out || p.n_out != BN || p.K1 <= 0 || bn != BN)) return -1;
-  // the K2 block variants exist for the residual GEMM mlp.3 (converted A), with the identity as N = 64 MMAs or as a zero-lo
-  // block; the converter always comes with one of them
+  // the zero-lo identity block exists for the residual GEMM mlp.3 (converted A), and the converter always comes with it
   if (p.b2_lo_zero && (p.epi != EPI_BIAS_PLANES || !p.K2 || !p.a_conv)) return -1;
   if (p.a_conv && !p.b2_lo_zero) return -1;
-  const int k2b = p.b2_identity ? K2_DIAG : p.b2_lo_zero ? K2_LO_ZERO : K2_FULL;
   tp.m_tiles = p.rows / BM; tp.n_tiles = p.n_out / tile_n; tp.batch = p.batch;
   tp.taps = p.taps; tp.kb_per_tap = p.kb_per_tap;
   for (int t = 0; t < 9; ++t) tp.tap_off[t] = p.tap_off[t];
@@ -1191,21 +1160,20 @@ int launch_gemm_tc(const GemmProblem& p, cudaStream_t stream) {
   if (p.max_ctas > 0 && grid > p.max_ctas) grid = p.max_ctas;      // test hook: the same tiles on fewer CTAs
   cudaError_t le;
   if (p.a_conv) {
-    le = k2b == K2_DIAG ? launch_variant<EPI_BIAS_PLANES, ACV_NORM_RELU, false, 256, K2_DIAG>(grid, stream, mp, tp)
-                        : launch_variant<EPI_BIAS_PLANES, ACV_NORM_RELU, false, 256, K2_LO_ZERO>(grid, stream, mp, tp);
+    le = launch_variant<EPI_BIAS_PLANES, ACV_NORM_RELU>(grid, stream, mp, tp);
   } else {
     switch (p.epi) {
       case EPI_F32:
         le = bn == 128 ? launch_variant<EPI_F32, ACV_NONE, false, 128>(grid, stream, mp, tp)
-                       : launch_variant<EPI_F32, ACV_NONE, false, 128, K2_FULL, true>(grid, stream, mp, tp);
+                       : launch_variant<EPI_F32, ACV_NONE, false, 128, true>(grid, stream, mp, tp);
         break;
       case EPI_CONV:
         le = bn == 64 ? launch_variant<EPI_CONV, ACV_NONE, false, 64>(grid, stream, mp, tp) : launch_variant<EPI_CONV, ACV_NONE, false, 128>(grid, stream, mp, tp);
         break;
-      case EPI_F32_STATS: le = launch_variant<EPI_F32_STATS, ACV_NONE, false, 128, K2_FULL, true>(grid, stream, mp, tp); break;
+      case EPI_F32_STATS: le = launch_variant<EPI_F32_STATS, ACV_NONE, false, 128, true>(grid, stream, mp, tp); break;
       case EPI_QSCALE: le = launch_variant<EPI_QSCALE>(grid, stream, mp, tp); break;
       case EPI_L2NORM: le = launch_variant<EPI_L2NORM>(grid, stream, mp, tp); break;
-      case EPI_SCORE_SUMS: le = launch_variant<EPI_SCORE_SUMS, ACV_NONE, false, 128, K2_FULL, true>(grid, stream, mp, tp); break;
+      case EPI_SCORE_SUMS: le = launch_variant<EPI_SCORE_SUMS, ACV_NONE, false, 128, true>(grid, stream, mp, tp); break;
       case EPI_SCORE_CONF: le = launch_variant<EPI_SCORE_CONF>(grid, stream, mp, tp); break;
       case EPI_QKV: le = p.a_hi_only ? launch_variant<EPI_QKV, ACV_NONE, true>(grid, stream, mp, tp) : launch_variant<EPI_QKV>(grid, stream, mp, tp); break;
       case EPI_BIAS_PLANES: le = launch_variant<EPI_BIAS_PLANES>(grid, stream, mp, tp); break;

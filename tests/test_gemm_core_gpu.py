@@ -376,19 +376,14 @@ def _mlp3_problem(lib, K1, seed=0):
 
 
 @pytest.mark.parametrize("K1", [64, 128, 192, 256, 448])
-def test_converter_identity_block(lib, K1):
+def test_converter_zero_lo_identity_block(lib, K1):
     """mlp.3: [ReLU((h - mu_seg) rstd_seg) | x] . [W1 | I]^T + b with each segment's own statistics, rows past the valid count
-    exactly 0; the identity as a zero-lo block and as 64 x 64 diagonal blocks: bit-identical."""
+    exactly 0; the identity as a zero-lo block, bit-identical under every tile schedule."""
     L, f, keep, (hid, mu, rstd, x, w1, bias) = _mlp3_problem(lib, K1)
-    outs = {}
-    for mode in (2, 3):
-        name = f"converter K1={K1} identity {'zero-lo' if mode == 2 else 'diagonal'}"
-        outs[mode] = schedules(lib, name, {**f, "b2_mode": mode},
-                               {"out_hi": torch.empty(L.rows, 256, dtype=torch.float16, device=DEV),
-                                "out_lo": torch.empty(L.rows, 256, dtype=torch.float16, device=DEV)})
-    for k in ("out_hi", "out_lo"):
-        assert torch.equal(_bytes(outs[2][k]), _bytes(outs[3][k])), f"converter K1={K1}: the identity forms differ ({k})"
-    dev = gr.plane_value(outs[2]["out_hi"], outs[2]["out_lo"])
+    outs = schedules(lib, f"converter K1={K1}", {**f, "b2_mode": 2},
+                     {"out_hi": torch.empty(L.rows, 256, dtype=torch.float16, device=DEV),
+                      "out_lo": torch.empty(L.rows, 256, dtype=torch.float16, device=DEV)})
+    dev = gr.plane_value(outs["out_hi"], outs["out_lo"])
     r, allowed = gr.mlp3_reference(hid.double(), mu.double()[:, :K1], rstd.double()[:, :K1], x[2], w1[2], bias.double(), L)
     v = L.valid_mask(DEV)
     report(f"converter K1={K1}", x_out=gr.ratio((dev - r).abs()[v], allowed[v]), pad_rows=ref._pad_ratio(dev, v))
@@ -592,13 +587,14 @@ def test_pdl_chain(lib):
 
 
 def test_refused_combinations(lib):
-    """The converter without an identity block, an identity block without the converter, and the SIMT backend on an epilogue are
-    refused (no instantiation exists for them)."""
+    """The converter without an identity block, an identity block without the converter, the SIMT backend on an epilogue and
+    an unknown b2_mode are refused (no instantiation exists for them)."""
     L, f, keep, _ = _mlp3_problem(lib, 64)
     outs = {"out_hi": torch.empty(L.rows, 256, dtype=torch.float16, device=DEV),
             "out_lo": torch.empty(L.rows, 256, dtype=torch.float16, device=DEV)}
     INVALID = -1
     assert lib.opb_debug_gemm(_lib.gemm_desc(**{**f, **outs, "b2_mode": 0}), None) == INVALID
-    no_conv = {**f, **outs, "b2_mode": 3, "a_raw": 0, "a1_hi": f["a2_hi"], "a1_lo": f["a2_lo"], "a1_ld": 256}
+    no_conv = {**f, **outs, "b2_mode": 2, "a_raw": 0, "a1_hi": f["a2_hi"], "a1_lo": f["a2_lo"], "a1_ld": 256}
     assert lib.opb_debug_gemm(_lib.gemm_desc(**no_conv), None) == INVALID
     assert lib.opb_debug_gemm(_lib.gemm_desc(**{**f, **outs, "b2_mode": 2, "backend": 1}), None) == INVALID
+    assert lib.opb_debug_gemm(_lib.gemm_desc(**{**f, **outs, "b2_mode": 3}), None) == INVALID

@@ -470,24 +470,6 @@ def test_programmatic_dependent_launch_is_transparent():
         assert torch.equal(outs[0][k], outs[1][k]), k
 
 
-def test_identity_block_as_diagonal_tiles_is_bit_identical():
-    """The residual enters the mlp.3 GEMM as an identity K-block.  Running k-block j as N = 64 MMAs on accumulator columns
-    [64 j, 64 j + 64) against the 64 x 64 diagonal block skips only products with exact zeros: bit-identical to full-width MMAs."""
-    lib = _lib.load()
-    hp = dict(synthetic.DEFAULT_HPARAMS)
-    sd = synthetic.make_state_dict(0, damped=False)
-    data = _cuda(synthetic.make_batch(6, [3, 4, 5], 333, 700, 8))
-    outs = []
-    for on in (1, 0):
-        m = _module(sd, hp)
-        m(data)                                          # creates the handle
-        assert lib.opb_debug_set_identity_diag(m._handle, on) == 0
-        m(data)
-        outs.append({k: v.clone() for k, v in m.last_batched.items()})
-    for k in outs[0]:
-        assert torch.equal(outs[0][k], outs[1][k]), k
-
-
 def test_kv_projection_two_vs_three_passes():
     """The k,v projection runs as A_hi.(B_hi + B_lo) (its output is one fp16 plane; the dropped A_lo term is below that rounding
     and averages out over the segment's rows).  Against the full three-pass product: same matches, conf within 2e-6; both

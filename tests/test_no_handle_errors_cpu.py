@@ -96,6 +96,7 @@ CASES = [
     ("opb_calc_optical_flow_pyr_lk", _lk(workspace_bytes=1000), "workspace_bytes >= (int64_t)B * (int64_t)L.pair_bytes"),
     ("opb_flow_compact", (P, P, P, P, 65536, 32768, P, P, P, P, P, P), "(int64_t)B * cap <= (int64_t)INT32_MAX"),
     ("opb_debug_gemm", (_desc(backend=2),), "d->backend <= 1"),
+    ("opb_debug_gemm", (_desc(b2_mode=3),), "d->b2_mode <= 2"),
     ("opb_debug_gemm", (_desc(backend=1, epi=_lib.EPI_QSCALE),), "p.epi == EPI_F32"),
     # confidence
     ("opb_ransac_epnp_cv", (P, P, P, P, 1, 100, 5.0, 1.5, P, P, P, P, P), "confidence <= 1.0"),

@@ -38,7 +38,6 @@ def step(i):
 SWITCHES = {
     "pdl": lambda v: lib.opb_debug_set_pdl(v),
     "kv_2pass": lambda v: lib.opb_debug_set_kv_passes(model._handle, 2 if v else 3),
-    "identity_diag": lambda v: lib.opb_debug_set_identity_diag(model._handle, v),
 }
 pairs = int(sys.argv[1]) if len(sys.argv) > 1 else 12
 for w in range(30):          # reach the power-capped steady state first

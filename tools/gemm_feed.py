@@ -9,11 +9,11 @@
     ring refills, launch).  The slope is reported as executed TFLOP/s (three fp16 passes per product), as the shared-memory
     fill per SM (96 KB land in a CTA's ring per k-block: A hi/lo + B hi/lo) and as that fill summed over the SMs.
 (b) the mlp.3-shaped GEMM (converter variant: A = ReLU(IN(hid)) formed from raw fp32 in the core, plus the identity K-block)
-    at rows = 262144 (32 frames of 1024 + 7168 rows), n_out = 256 and K1 = 256 / 512 / 768 / 1024, with the identity block as
-    N = 64 diagonal MMAs and at full width.  The same line fit; the slope counts the three passes of the K1 part only, the
-    identity block is in the intercept.  Both (a) and (b) go through opb_debug_gemm's problem descriptor.
-(c) the benchmarked call (match_frames, B = 32, N2D = 1024, N3D = 7000) with the profiling hook on, with the identity block
-    in both forms: ms per step and share of the step for every GEMM and the large helper kernels.
+    at rows = 262144 (32 frames of 1024 + 7168 rows), n_out = 256 and K1 = 256 / 512 / 768 / 1024.  The same line fit; the
+    slope counts the three passes of the K1 part only, the identity block is in the intercept.  Both (a) and (b) go through
+    opb_debug_gemm's problem descriptor.
+(c) the benchmarked call (match_frames, B = 32, N2D = 1024, N3D = 7000) with the profiling hook on: ms per step and share of
+    the step for every GEMM and the large helper kernels.
 
 --lib loads another build of the library (A/B between builds in one process).  Needs a GPU; there is no CPU path.
 """
@@ -129,42 +129,37 @@ def mlp3_slope(lib, window):
     bias = torch.randn(256, device=dev, generator=g)
     nparam = (segs + max(MLP3_K1S) // 512) * 512
     mu, rstd = 0.1 * torch.randn(nparam, device=dev, generator=g), 1 + 0.1 * torch.rand(nparam, device=dev, generator=g)
-    res = {}
-    for diag in (1, 0):
-        pts = []
-        for K1 in MLP3_K1S:
-            hid = torch.randn(rows, K1, device=dev, generator=g)
-            w1 = planes(256, K1)
-            # every row valid: frames of n_pad + m_pad rows with N = n_pad, M = m_pad
-            desc = _lib.gemm_desc(epi=_lib.EPI_BIAS_PLANES, rows=rows, n_out=256, K1=K1, K2=256, b1_hi=w1[0], b1_lo=w1[1], b1_ld=K1,
-                                  a2_hi=x[0], a2_lo=x[1], a2_ld=256, b2_hi=eye[0], b2_lo=eye[1], b2_ld=256, b2_mode=3 if diag else 2,
-                                  a_raw=hid, a_raw_ld=K1, mu=mu, rstd=rstd, B=MLP3_FRAMES, N=MLP3_NPAD, M=MLP3_MPAD,
-                                  n_pad=MLP3_NPAD, m_pad=MLP3_MPAD, bias=bias, out_hi=out[0], out_lo=out[1], out_ld=256)
+    pts = []
+    for K1 in MLP3_K1S:
+        hid = torch.randn(rows, K1, device=dev, generator=g)
+        w1 = planes(256, K1)
+        # every row valid: frames of n_pad + m_pad rows with N = n_pad, M = m_pad
+        desc = _lib.gemm_desc(epi=_lib.EPI_BIAS_PLANES, rows=rows, n_out=256, K1=K1, K2=256, b1_hi=w1[0], b1_lo=w1[1], b1_ld=K1,
+                              a2_hi=x[0], a2_lo=x[1], a2_ld=256, b2_hi=eye[0], b2_lo=eye[1], b2_ld=256, b2_mode=2,
+                              a_raw=hid, a_raw_ld=K1, mu=mu, rstd=rstd, B=MLP3_FRAMES, N=MLP3_NPAD, M=MLP3_MPAD,
+                              n_pad=MLP3_NPAD, m_pad=MLP3_MPAD, bias=bias, out_hi=out[0], out_lo=out[1], out_ld=256)
 
-            def launch():
-                rc = lib.opb_debug_gemm(desc, None)
-                if rc != 0:
-                    raise RuntimeError(f"opb_debug_gemm (mlp.3) rc={rc}")
+        def launch():
+            rc = lib.opb_debug_gemm(desc, None)
+            if rc != 0:
+                raise RuntimeError(f"opb_debug_gemm (mlp.3) rc={rc}")
 
-            pts.append((K1,) + time_launches(launch, window))
-            del hid, w1
-        Ks = np.array([p[0] for p in pts], float)
-        ts = np.array([p[1] for p in pts], float)
-        slope, icept = np.polyfit(Ks, ts, 1)
-        tflops = 3 * 2.0 * rows * 256 / (slope * 1e-3) / 1e12
-        form = "N = 64 diagonal MMAs" if diag else "full width"
-        print(f"(b) mlp.3-shaped GEMM, rows={rows} n_out=256 K2=256 identity block {form}")
-        for K1, ms, n in pts:
-            print(f"    K1={K1:5d}  {ms:8.3f} ms/launch  ({n} launches)")
-        print(f"    main loop  {tflops:6.1f} TFLOP/s executed (K1 part)   intercept {icept:8.3f} ms per launch   "
-              f"fit residual max {np.abs(ts - (slope * Ks + icept)).max():.4f} ms")
-        res["diag" if diag else "full"] = {"slope_tflops_executed": tflops, "intercept_ms": icept,
-                                            "points": [{"K1": K1, "ms": ms} for K1, ms, _ in pts]}
-    return res
+        pts.append((K1,) + time_launches(launch, window))
+        del hid, w1
+    Ks = np.array([p[0] for p in pts], float)
+    ts = np.array([p[1] for p in pts], float)
+    slope, icept = np.polyfit(Ks, ts, 1)
+    tflops = 3 * 2.0 * rows * 256 / (slope * 1e-3) / 1e12
+    print(f"(b) mlp.3-shaped GEMM, rows={rows} n_out=256 K2=256")
+    for K1, ms, n in pts:
+        print(f"    K1={K1:5d}  {ms:8.3f} ms/launch  ({n} launches)")
+    print(f"    main loop  {tflops:6.1f} TFLOP/s executed (K1 part)   intercept {icept:8.3f} ms per launch   "
+          f"fit residual max {np.abs(ts - (slope * Ks + icept)).max():.4f} ms")
+    return {"slope_tflops_executed": tflops, "intercept_ms": icept, "points": [{"K1": K1, "ms": ms} for K1, ms, _ in pts]}
 
 
-def step_profile(identity_diag, runs=5):
-    from onepose_b200 import GATsSuperGlue, _lib, synthetic
+def step_profile(runs=5):
+    from onepose_b200 import GATsSuperGlue, synthetic
     dev = torch.device("cuda")
     hp = dict(synthetic.DEFAULT_HPARAMS)
     model = GATsSuperGlue(hp).eval()
@@ -174,9 +169,7 @@ def step_profile(identity_diag, runs=5):
     db, leaves = synthetic.make_object(0, M, 8)
     q = torch.from_numpy(np.stack([synthetic.make_frame(f, db, N)[0] for f in range(B)], 0)).to(dev)
     model.set_object(torch.from_numpy(db).to(dev), torch.from_numpy(leaves).to(dev), reserve=(B, N))
-    model.match_frames(q)                                   # creates the handle
-    _lib.check(_lib.load().opb_debug_set_identity_diag(model._handle, identity_diag), model._handle)
-    for _ in range(3):
+    for _ in range(4):
         model.match_frames(q)
     torch.cuda.synchronize()
     model.set_profiling(True)
@@ -190,8 +183,7 @@ def step_profile(identity_diag, runs=5):
             acc[p][0] += e["ms"]; acc[p][1] += e["flops"]; acc[p][2] = e["launches"]
     model.set_profiling(False)
     total /= runs
-    form = "N = 64 diagonal MMAs" if identity_diag else "full width"
-    print(f"(c) match_frames B={B} N2D={N} N3D={M}, identity block {form}, profiling on (an event after every launch), "
+    print(f"(c) match_frames B={B} N2D={N} N3D={M}, profiling on (an event after every launch), "
           f"mean of {runs} steps: {total:.3f} ms/step")
     print(f"    {'entry':22s} {'launches':>8s} {'ms/step':>8s} {'share':>6s} {'TFLOP/s alg.':>12s}  what")
     out = {"step_ms": total, "entries": {}}
@@ -223,8 +215,7 @@ def main():
     if not args.no_mlp3:
         mlp3_slope(lib, args.window)
     if not args.no_step:
-        for identity_diag in (1, 0):
-            step_profile(identity_diag)
+        step_profile()
 
 
 if __name__ == "__main__":
