@@ -493,6 +493,37 @@ int opb_flow_compact(const uint8_t* status, const float* pts2d, const float* pts
 int opb_flow_reprojection(const double* K, const double* pose, const double* pts2d, const double* pts3d, const int32_t* offsets, int32_t B,
                           double* dist, void* stream);
 
+/* ---- the tracker's flow-only state machine (csrc/track.cu) ----
+ * BATracker's per-frame logic around flow_track in the live demo's order (inference_demo.py:253-299, track_interval 5) with
+ * track(frame, flow_track_only=True): update_kf's gate, add_kf's first pose, motion_prediction and track()'s choice of the
+ * pose (src/tracker/ba_tracker.py:105-145, :147-149, :275-293, :727-802).  One thread per track in fp64, on the caller's
+ * stream, no allocation and no host synchronisation.  Bundle adjustment is not part of it.
+ *
+ * Per-track state, device memory the caller owns (onepose_b200.track.init_state makes it):
+ *   frame            int64 [B]        frames seen (the demo's id); 0 for a new or reset track
+ *   hist             f64 [B, 3, 16]   the last up to 3 reported poses (pose_list[-3:]), row-major 4x4, oldest first
+ *   hist_len         int32 [B]        poses in hist, 0..3
+ *   init_cnt         int32 [B]        init_cnt, 3 for a new track
+ *   use_motion_cnt   int32 [B]        use_motion_cnt, 0 for a new track
+ * A track is at its first frame when frame <= 0 or hist_len <= 0.  Poses are row-major 4x4 f64 [B, 16]. */
+enum { OPB_TRACK_GATE_NONE = 0, OPB_TRACK_GATE_ADD = 1, OPB_TRACK_GATE_ACCEPT = 2, OPB_TRACK_GATE_REJECT = 3 };
+enum { OPB_TRACK_FLOW = 0, OPB_TRACK_MOTION = 1, OPB_TRACK_PRED = 2, OPB_TRACK_INIT = 3, OPB_TRACK_KEYFRAME = 4 };
+/* The keyframe decision of this frame, per track: GATE_ADD at the first frame (update_kf accepts with no keyframe, then add_kf;
+ * hist becomes [pose_pred], hist_len 1); at frame % 5 == 0 GATE_REJECT if cm_degree_5_metric(pose_pred, last reported pose)
+ * has trans > 10 cm or rot > 10 deg, else GATE_ACCEPT (the frame's inlier pairs become the keyframe); GATE_NONE otherwise.
+ * pose_pred f64 [B, 16] (the frame's matcher pose), gate int32 [B] out.  Only the first frame writes hist / hist_len. */
+int opb_track_gate(const double* pose_pred, int32_t B, const int64_t* frame, double* hist, int32_t* hist_len, int32_t* gate, void* stream);
+/* track()'s steps 2-6 after flow_track, per track: with d = cm_degree_5_metric(last reported pose, pose_flow) and pose_mo =
+ * pose_pred while hist_len < 3, else motion_prediction(hist): pose_mo if ((d.trans > 10 or d.rot > 10) and use_motion_cnt < 3)
+ * or kpt_dist > 10 (use_motion_cnt + 1); else pose_flow if d.trans < 20 and d.rot < 20 (use_motion_cnt = 0); else pose_mo
+ * (use_motion_cnt + 1).  Then while init_cnt > 0 it is decremented and pose_pred reported instead.  The reported pose is
+ * appended to hist; a comparison with NaN is false.  At the first frame (no track() call in the demo) pose_out = pose_pred,
+ * branch KEYFRAME and only frame changes.  frame += 1 for every track.
+ * pose_pred, pose_flow f64 [B, 16] (flow_track's pose_init_homo), kpt_dist f64 [B]; pose_out f64 [B, 16] and branch int32 [B]
+ * out (FLOW, MOTION, PRED: pose_mo while the history is short, INIT: the init override, KEYFRAME). */
+int opb_track_select(const double* pose_pred, const double* pose_flow, const double* kpt_dist, int32_t B, int64_t* frame, double* hist,
+                     int32_t* hist_len, int32_t* init_cnt, int32_t* use_motion_cnt, double* pose_out, int32_t* branch, void* stream);
+
 /* ---- adjacent producer: SuperPoint key-point extractor (SURVEY 8f N4) ----
  * Replaces SuperPoint.forward (reference src/models/extractors/SuperPoint/superpoint.py:140-197): shared VGG-style encoder
  * (:142-152), score head + 65-way softmax + 8x8 pixel shuffle (:155-160), simple_nms (:47-61, :161), threshold / border /

@@ -121,6 +121,8 @@ SYMBOLS = {
                                                C.c_double, C.c_double, _I, _P, C.c_int64, _P, _P, _P, _P]),
     "opb_flow_compact": (C.c_int, [_P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P, _P]),
     "opb_flow_reprojection": (C.c_int, [_P, _P, _P, _P, _P, _I, _P, _P]),
+    "opb_track_gate": (C.c_int, [_P, _I, _P, _P, _P, _P, _P]),
+    "opb_track_select": (C.c_int, [_P, _P, _P, _I, _P, _P, _P, _P, _P, _P, _P, _P]),
     "opb_debug_set_pdl": (C.c_int, [_I]),
     "opb_debug_set_ws_fill": (C.c_int, [_I]),
     "opb_debug_set_kv_passes": (C.c_int, [_P, _I]),
