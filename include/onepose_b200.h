@@ -300,6 +300,25 @@ int opb_gather_matches_objects(const int64_t* matches0, const float* mscores0, c
                                const int32_t* kp3_first, const int32_t* kp3_count, int32_t B, int32_t N, double* pts2d, double* pts3d,
                                float* mconf, int32_t* query_index, int32_t* offsets, void* stream);
 
+/* ---- colour camera frames to the grey frames every frame consumer below takes (csrc/frames.cu) ----
+ * The reference reads its frames as cv2.imread(path, cv2.IMREAD_GRAYSCALE) of the colour PNGs parse_scanned_data.py writes
+ * (NormalizedDataset, src/datasets/normalized_dataset.py:25-34; read_gray_scale, src/utils/data_utils.py:275-276;
+ * local_feature_2D_detector.py:12, :155, :173).  opb_grey_frames makes those grey pixels from colour pixels in device memory
+ * -- a camera's or cv2.VideoCapture's frames -- and optionally NormalizedDataset's `image / 255.`.  On the caller's current
+ * device and stream; asynchronous, no host synchronisation, no allocation.
+ *   frames            device uint8 [F, H, W, C]  8-bit pixels, C = 3 or 4 by `order`; frame f starts at frames + f * frame_pitch,
+ *                     its row y at + y * row_pitch (bytes; row_pitch >= W * C; frame_pitch 0, one frame for all F, or
+ *                     >= H * row_pitch).  F <= 65535, H, W <= 32767 (the crop's bounds)
+ *   order             OPB_ORDER_BGR, _RGB, _BGRA or _RGBA: the channels of a pixel in memory order; alpha is ignored
+ *   grey              device uint8 [F, H, W] out, with its own pitches: grey_row_pitch >= W, grey_frame_pitch >= H * grey_row_pitch
+ *   image             device fp32 [F, 1, H, W] out (dense), or NULL: grey / 255 as a float32 division, numpy's `image / 255.`
+ * grey = (9797 * R + 19234 * G + 3737 * B) >> 15, OpenCV 4.13's IMREAD_GRAYSCALE of a colour 8-bit PNG, bit for bit on every
+ * colour (the model is tests/grey_reference.py).  It is not cv2.cvtColor(COLOR_BGR2GRAY), which differs by one level on half
+ * of the colours.  The outputs must not overlap the frames or each other. */
+enum { OPB_ORDER_BGR = 0, OPB_ORDER_RGB = 1, OPB_ORDER_BGRA = 2, OPB_ORDER_RGBA = 3 };
+int opb_grey_frames(const uint8_t* frames, int64_t frame_pitch, int64_t row_pitch, int32_t F, int32_t H, int32_t W, int32_t order, uint8_t* grey,
+                    int64_t grey_frame_pitch, int64_t grey_row_pitch, float* image, void* stream);
+
 /* ---- between one frame's pose and the next frame's extractor input: the pose-guided crop ----
  * The reference's live loop (inference_demo.py:193-247) crops every frame after the first around the object's box under the
  * previous pose: previous_pose_detect (src/local_feature_2D_detector/local_feature_2D_detector.py:232-259), host numpy +

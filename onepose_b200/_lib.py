@@ -107,6 +107,7 @@ SYMBOLS = {
     "opb_debug_cv_subsets": (C.c_int, [_I, _I, _I, _P, _P]),
     "opb_gather_matches": (C.c_int, [_P, _P, _P, _P, _I, _I, _I, _P, _P, _P, _P, _P, _P]),
     "opb_gather_matches_objects": (C.c_int, [_P, _P, _P, _P, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P]),
+    "opb_grey_frames": (C.c_int, [_P, C.c_int64, C.c_int64, _I, _I, _I, _I, _P, C.c_int64, C.c_int64, _P, _P]),
     "opb_boxes_from_poses": (C.c_int, [_P, _P, _P, _I, _I, _P, _P, _P]),
     "opb_crop_resize": (C.c_int, [_P, C.c_int64, C.c_int64, _I, _I, _I, _P, _P, _I, _P, _P, _P, _P, _P]),
     "opb_crop_resize_indexed": (C.c_int, [_P, C.c_int64, C.c_int64, _I, _I, _I, _P, _I, _P, _P, _I, _P, _P, _P, _P, _P]),
