@@ -382,6 +382,57 @@ int opb_crop_resize_indexed(const uint8_t* frames, int64_t frame_pitch, int64_t 
  * A rejected box (as for opb_crop_resize) gives a zero image, a zero transform and K_crop = K. */
 int opb_warp_crop_u8(const uint8_t* frames, int64_t frame_pitch, int64_t row_pitch, int32_t B, int32_t H, int32_t W, const int32_t* box,
                      const double* K, int32_t out_h, int32_t out_w, uint8_t* out, double* trans, double* K_crop, void* stream);
+/* opb_crop_resize's two warps on colour frames, into uint8: the crops parse_scanned_data.py's parse_video writes to color/
+ * (:151-159, cv2.warpAffine of the BGR frame, then of its first-stage crop).
+ *   frames        device uint8 [n_frames, H, W, C], C = 3 or 4, packed pixels; frame f starts at frames + f * frame_pitch, its
+ *                 row y at + y * row_pitch (bytes; row_pitch >= W * C, frame_pitch >= 0)
+ *   frame_index   device int32 [B], or NULL: crop b reads frame frame_index[b] (an index outside [0, n_frames) is rejected as a
+ *                 rejected box is), or frame b, with n_frames == B
+ *   image         device uint8 [B, S, S, C] out: every channel warped as cv2.warpAffine warps a C-channel 8-bit image
+ *   box, K, crop_size, K_crop, trans, status as in opb_crop_resize, per crop.
+ * Channel c of crop b equals, bit for bit, opb_crop_resize's pixels (times 255) of plane c of the same frame: cv2 warps every
+ * channel with the grey warp's positions and weights.  A rejected box gives a zero crop, zero transforms and K_crop = K. */
+int opb_crop_resize_colour(const uint8_t* frames, int64_t frame_pitch, int64_t row_pitch, int32_t n_frames, int32_t H, int32_t W, int32_t C,
+                           const int32_t* frame_index, int32_t B, const int32_t* box, const double* K, int32_t crop_size, uint8_t* image,
+                           double* K_crop, double* trans, int32_t* status, void* stream);
+
+/* ---- an annotated scan's poses, boxes and crop geometry (csrc/scan.cu) ----
+ * parse_scanned_data.py's data_process_anno (:184-240) and parse_video (:129-181) turn an ARKit scan -- ARposes.txt, Box.txt,
+ * Frames.txt and the video -- into the object poses, boxes and 512 x 512 colour crops inference.py evaluates against.  The two
+ * calls below, with opb_crop_resize_colour between them, do its arithmetic on the caller's current device and stream: device
+ * pointers, asynchronous, no host synchronisation, no allocation.  fp64 with every product and sum rounded on its own in numpy's
+ * index order; the model is tests/scan_reference.py.
+ *
+ * data_process_anno's loop (downsample_rate = 1) over n_rows ARposes rows, in one launch:
+ *   K          device f64 [9]              the averaged intrinsics (K_homo = [K | 0])
+ *   arposes    device f64 [n_rows, 8]      (timestamp, x, y, z, qw, qx, qy, qz) per row, comment and blank lines removed
+ *   T_ow       device f64 [16]             Box.txt's object-to-world transform, row-major
+ *   corners    device f64 [n_corners, 3]   the object's box corners (8 from Box.txt); n_corners <= 1024
+ *   pose       device f64 [n_out, 16] out  T_oc of the kept rows in order, row-major; zeros in slots past the kept count
+ *   proj       device f64 [n_out, n_corners, 2] out, or NULL: reproj(K_homo, T_oc, corners) of the kept rows; zeros past them
+ *   box        device int32 [n_out, 4] out [x0, y0, x1, y1], the projection's min / max truncated towards zero (parse_video's
+ *                                          astype(int)); [0, 0, 0, 0] past the kept rows, or for a NaN extreme
+ *   row        device int32 [n_out] out, or NULL: the ARposes row of each slot; -1 past the kept rows
+ *   keep       device int32 [n_rows] out, or NULL: 1 for a kept row, 0 for a skipped one
+ *   count      device int32 [1] out: the number of kept rows
+ * Per row: R = quat2mat(q) (transforms3d's non-normalising formula: s = 2 / |q|^2, the identity for |q|^2 < float64 eps),
+ * R @ diag(1, -1, -1), T_cw = [R p; 0 1], T_oc = inv(T_cw) @ T_ow, the projection of the corners and its min / max.  A row is
+ * skipped when x0 < -1000, y0 < -1000, x1 > 3000 or y1 > 3000 (a NaN extreme fails these tests and is kept, as in numpy).  A
+ * skipped row does not advance the reference's index, and parse_video stops at the first index without a box file, so video
+ * frame i pairs with the i-th kept row and frames past the kept count get nothing: slot i of the outputs is frame i's. */
+int opb_scan_poses(const double* K, const double* arposes, int32_t n_rows, const double* T_ow, const double* corners, int32_t n_corners,
+                   int32_t n_out, double* pose, double* proj, int32_t* box, int32_t* row, int32_t* keep, int32_t* count, void* stream);
+/* parse_video's crop-to-frame transform and box in crop coordinates for F frames, one thread per frame:
+ *   trans      device f64 [F, 2, 6]         T1 and T2 of opb_crop_resize_colour
+ *   K_crop     device f64 [F, 9]            its K_crop
+ *   pose       device f64 [F, 16]           T_oc (opb_scan_poses' pose)
+ *   corners    device f64 [n_corners, 3]    n_corners <= 1024
+ *   status     device int32 [F]             opb_crop_resize_colour's status
+ *   M          device f64 [F, 9] out        inv(T2_homo @ T1_homo), the crop-to-frame transform written to M/
+ *   box_crop   device f64 [F, 4] out        min / max of reproj(K_crop_homo, T_oc, corners), not truncated (bbox/)
+ * Both are zero for a frame of status 0. */
+int opb_scan_crop_geometry(const double* trans, const double* K_crop, const double* pose, const double* corners, int32_t n_corners,
+                           const int32_t* status, int32_t F, double* M, double* box_crop, void* stream);
 
 /* ---- the first frame, and every frame after a lost pose: detection by 2D-2D matching against reference views ----
  * LocalFeatureObjectDetector.detect (local_feature_2D_detector.py:76-147, 196-230) between the caller's 2D-2D matcher and the

@@ -112,6 +112,9 @@ SYMBOLS = {
     "opb_crop_resize": (C.c_int, [_P, C.c_int64, C.c_int64, _I, _I, _I, _P, _P, _I, _P, _P, _P, _P, _P]),
     "opb_crop_resize_indexed": (C.c_int, [_P, C.c_int64, C.c_int64, _I, _I, _I, _P, _I, _P, _P, _I, _P, _P, _P, _P, _P]),
     "opb_warp_crop_u8": (C.c_int, [_P, C.c_int64, C.c_int64, _I, _I, _I, _P, _P, _I, _I, _P, _P, _P, _P]),
+    "opb_crop_resize_colour": (C.c_int, [_P, C.c_int64, C.c_int64, _I, _I, _I, _I, _P, _I, _P, _P, _I, _P, _P, _P, _P, _P]),
+    "opb_scan_poses": (C.c_int, [_P, _P, _I, _P, _P, _I, _I, _P, _P, _P, _P, _P, _P, _P]),
+    "opb_scan_crop_geometry": (C.c_int, [_P, _P, _P, _P, _I, _P, _I, _P, _P, _P]),
     "opb_estimate_affine_partial": (C.c_int, [_P, _P, _P, _I, C.c_double, _I, C.c_double, _I, _P, _P, _P, _P, _P]),
     "opb_boxes_from_matches": (C.c_int, [_P, _P, _P, _I, _I, _P, _P, _I, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P, _P]),
     "opb_boxes_from_matches_objects": (C.c_int, [_P, _P, _P, _I, _I, _P, _P, _I, _P, _P, _I, _I, _P, _P, _I, _I, _I, _I, _P, _P, _P, _P, _P,

@@ -78,6 +78,19 @@ def _frames_args(frames: torch.Tensor):
     return dev, B, H, W
 
 
+def _colour_frames_args(frames: torch.Tensor):
+    dev = _lib.cuda_device(frames)
+    if frames.dtype != torch.uint8 or frames.dim() != 4 or frames.shape[-1] not in (3, 4):
+        raise ValueError(f"frames must be uint8 [B, H, W, C] with C = 3 or 4, got {frames.dtype} {list(frames.shape)}")
+    B, H, W, C = (int(v) for v in frames.shape)
+    if not 0 < B <= MAX_FRAMES or not 0 < H <= MAX_SIDE or not 0 < W <= MAX_SIDE:
+        raise ValueError(f"frames must be 1..{MAX_FRAMES} images of 1..{MAX_SIDE} pixels a side, got {list(frames.shape)}")
+    row_pitch = frames.stride(1) if H > 1 else W * C          # the stride of a dimension of size 1 addresses nothing
+    if frames.stride(3) != 1 or (W > 1 and frames.stride(2) != C) or row_pitch < W * C:
+        raise ValueError(f"frames must have packed pixels (strides [.., .., {C}, 1]) and rows that do not overlap, got strides {frames.stride()}")
+    return dev, B, H, W, C, row_pitch
+
+
 def _boxes(boxes: torch.Tensor, B: int, dev) -> torch.Tensor:
     if boxes.dtype != torch.int32 or tuple(boxes.shape) != (B, 4):
         raise ValueError(f"boxes must be int32 [{B}, 4], got {boxes.dtype} {list(boxes.shape)}")
@@ -130,6 +143,39 @@ def crop_frames(frames: torch.Tensor, boxes: torch.Tensor, K: torch.Tensor, crop
     else:
         _lib.call(dev, "opb_crop_resize_indexed", frames, frames.stride(0), frames.stride(1), F, H, W, frame_index, B, boxes, K, S, out["image"],
                   out["K_crop"], out["trans"], out["status"])
+    return out
+
+
+def crop_frames_colour(frames: torch.Tensor, boxes: torch.Tensor, K: torch.Tensor, crop_size: int = 512, frame_index=None) -> dict:
+    """``crop_frames``' two warps on colour frames, kept in uint8: the crops ``parse_scanned_data.py``'s ``parse_video`` writes
+    (``:151-159``), ``cv2.warpAffine`` of the BGR frame and then of its first-stage crop.  frames uint8 [B,H,W,C] CUDA with C = 3
+    or 4 (packed pixels; any row and frame stride), boxes int32 [B,4], K [3,3] or [B,3,3], crop_size S (S % 8 == 0).
+
+    Returns device tensors: image uint8 [B,S,S,C], channel c equal bit for bit to ``cv2.warpAffine`` of the C-channel image
+    (which warps each channel plane as the grey warp does), and K_crop, trans and status exactly as ``crop_frames`` returns
+    them.  A rejected box gives a zero crop.  ``frame_index`` is ``crop_frames``': frames is then [F,H,W,C] and crop b reads frame
+    frame_index[b].  No host synchronisation.
+
+    The reference turns a crop grey only after it: ``cv2.imwrite`` of the colour crop, then ``IMREAD_GRAYSCALE``.  Making the
+    frame grey first and cropping the grey frame gives other pixels, so ``frames.grey_frames(image)`` is the extractor's
+    input for a scanned sequence, not ``crop_frames(grey_frames(frames))``."""
+    dev, B, H, W, C, row_pitch = _colour_frames_args(frames)
+    S = int(crop_size)
+    if S <= 0 or S % 8 or S > MAX_SIDE:
+        raise ValueError(f"crop_size must be a positive multiple of 8 up to {MAX_SIDE}, got {crop_size!r}")
+    F = B
+    if frame_index is not None:
+        frame_index = torch.as_tensor(frame_index)
+        B = int(frame_index.shape[0]) if frame_index.dim() == 1 else 0
+        if not 0 < B <= MAX_FRAMES:
+            raise ValueError(f"frame_index must be an integer [B] sequence or tensor with 1 <= B <= {MAX_FRAMES}")
+        frame_index = _indices(frame_index, B, F, "frame_index", dev)
+    boxes = _boxes(boxes, B, dev)
+    K = _per_frame(K, B, (3, 3), "K", dev)
+    out = {"image": torch.empty(B, S, S, C, dtype=torch.uint8, device=dev), "K_crop": torch.empty(B, 3, 3, dtype=torch.float64, device=dev),
+           "trans": torch.empty(B, 2, 2, 3, dtype=torch.float64, device=dev), "status": torch.empty(B, dtype=torch.int32, device=dev)}
+    _lib.call(dev, "opb_crop_resize_colour", frames, frames.stride(0), row_pitch, F, H, W, C, frame_index, B, boxes, K, S, out["image"],
+              out["K_crop"], out["trans"], out["status"])
     return out
 
 

@@ -3,6 +3,7 @@
 //   previous_pose_detect   local_feature_2D_detector.py:232-259   reproj -> min / max -> astype(int32)        opb_boxes_from_poses
 //   crop_img_by_bbox       :160-186   get_K_crop_resize x 2, get_image_crop_resize x 2, then / 255           opb_crop_resize
 //                          the same where crop b reads frame frame_index[b] (several boxes per frame)   opb_crop_resize_indexed
+//   parse_scanned_data.py   :151-159   the same two warps on colour frames, kept in uint8                    opb_crop_resize_colour
 //   get_image_crop_resize / get_K_crop_resize   data_utils.py:233-272   one cv2.warpAffine, T @ K             opb_warp_crop_u8
 //
 // The pixels are OpenCV's, bit for bit.  cv2.warpAffine(INTER_LINEAR) on 8-bit data with a constant border is integer
@@ -175,14 +176,22 @@ __device__ void invert_transform(const double* T, double* m) {
   m[5] = sub(mul(-m[3], T[2]), mul(m[4], T[5]));
 }
 
-// One pixel of cv2.warpAffine(src, T, INTER_LINEAR), border constant 0, for 8-bit data; m = invert_transform(T), src(x, y) is
-// called for positions inside [0, sw) x [0, sh) only.  Source coordinates in 1/1024 (rint = round half to even), reduced to
-// 1/32; the four weights are cv2's int16 table entries rint(w * 32768) of the float32 products (1 - fx/32 | fx/32) *
-// (1 - fy/32 | fy/32): those products are exact, so an entry is 32 * (32 - fx | fx) * (32 - fy | fy) and sums to 32768 as it
-// stands -- but for fx = fy = 0, where 32768 saturates to 32767 and cv2's fix-up puts the 1 on a neighbour, which cannot change
-// the rounded pixel (|p1 - p0| < 16384).  tests/test_crop_reference_cpu.py checks both statements.
-template <class Src>
-__device__ __forceinline__ int warp_pixel(const double* m, int x, int y, int sw, int sh, Src src) {
+// The C channel values of one pixel, in memory order.
+template <int C>
+struct Px {
+  int v[C];
+};
+
+// One pixel of cv2.warpAffine(src, T, INTER_LINEAR), border constant 0, for 8-bit data of C channels; m = invert_transform(T),
+// src(x, y) gives the Px<C> at a position inside [0, sw) x [0, sh) and is called for those only.  Source coordinates in 1/1024
+// (rint = round half to even), reduced to 1/32; the four weights are cv2's int16 table entries rint(w * 32768) of the float32
+// products (1 - fx/32 | fx/32) * (1 - fy/32 | fy/32): those products are exact, so an entry is 32 * (32 - fx | fx) * (32 - fy |
+// fy) and sums to 32768 as it stands -- but for fx = fy = 0, where 32768 saturates to 32767 and cv2's fix-up puts the 1 on a
+// neighbour, which cannot change the rounded pixel (|p1 - p0| < 16384).  tests/test_crop_reference_cpu.py checks both
+// statements.  cv2 warps a multi-channel image with the same positions and weights for every channel, so channel c is the grey
+// warp of plane c (tests/test_scan_reference_cpu.py checks it against cv2).
+template <int C, class Src>
+__device__ __forceinline__ Px<C> warp_pixel(const double* m, int x, int y, int sw, int sh, Src src) {
   const long long ad = __double2ll_rn(mul(mul(m[0], (double)x), 1024.0)), bd = __double2ll_rn(mul(mul(m[3], (double)x), 1024.0));
   const long long X0 = __double2ll_rn(mul(add(mul(m[1], (double)y), m[2]), 1024.0)) + 16;
   const long long Y0 = __double2ll_rn(mul(add(mul(m[4], (double)y), m[5]), 1024.0)) + 16;
@@ -190,15 +199,22 @@ __device__ __forceinline__ int warp_pixel(const double* m, int x, int y, int sw,
   const int sx = (int)min(max(X >> 5, -32768LL), 32767LL), sy = (int)min(max(Y >> 5, -32768LL), 32767LL);   // saturate_cast<short>
   const int fx = (int)(X & 31), fy = (int)(Y & 31);
   const bool x0 = sx >= 0 && sx < sw, x1 = sx + 1 >= 0 && sx + 1 < sw, y0 = sy >= 0 && sy < sh, y1 = sy + 1 >= 0 && sy + 1 < sh;
-  int acc = 0;
-  if (y0 && x0) acc += (32 - fx) * (32 - fy) * src(sx, sy);
-  if (y0 && x1) acc += fx * (32 - fy) * src(sx + 1, sy);
-  if (y1 && x0) acc += (32 - fx) * fy * src(sx, sy + 1);
-  if (y1 && x1) acc += fx * fy * src(sx + 1, sy + 1);
-  return (acc * 32 + (1 << 14)) >> 15;
+  Px<C> acc{};
+  auto tap = [&](int w, int u, int v) {
+    const Px<C> p = src(u, v);
+    for (int c = 0; c < C; ++c) acc.v[c] += w * p.v[c];
+  };
+  if (y0 && x0) tap((32 - fx) * (32 - fy), sx, sy);
+  if (y0 && x1) tap(fx * (32 - fy), sx + 1, sy);
+  if (y1 && x0) tap((32 - fx) * fy, sx, sy + 1);
+  if (y1 && x1) tap(fx * fy, sx + 1, sy + 1);
+  for (int c = 0; c < C; ++c) acc.v[c] = (acc.v[c] * 32 + (1 << 14)) >> 15;
+  return acc;
 }
 
-// Output pixels of crop b = blockIdx.y from frame f (read only when frame_ok); see crop_warp_kernel below.
+// Output pixels of crop b = blockIdx.y from frame f (read only when frame_ok), C channels a pixel; see crop_warp_kernel below.
+// out_u8 is [B][out_h][out_w][C]; out_f32 (C = 1 only) [B][out_h][out_w].
+template <int C>
 __device__ __forceinline__ void crop_warp(int f, bool frame_ok, const uint8_t* __restrict__ frames, long long frame_pitch, long long row_pitch,
                                           int H, int W, const int32_t* __restrict__ box, const double* __restrict__ trans, int stages, int out_h,
                                           int out_w, uint8_t* __restrict__ out_u8, float* __restrict__ out_f32) {
@@ -213,19 +229,25 @@ __device__ __forceinline__ void crop_warp(int f, bool frame_ok, const uint8_t* _
   if (idx >= (long long)out_h * out_w) return;
   const int x = (int)(idx % out_w), y = (int)(idx / out_w);
   const uint8_t* frame = frames + (size_t)f * frame_pitch;
-  auto pixel = [&](int u, int v) { return (int)__ldg(frame + (size_t)v * row_pitch + u); };
-  int val = 0;
+  auto pixel = [&](int u, int v) {
+    const uint8_t* q = frame + (size_t)v * row_pitch + (size_t)u * C;
+    Px<C> p;
+    for (int c = 0; c < C; ++c) p.v[c] = (int)__ldg(q + c);
+    return p;
+  };
+  Px<C> val{};
   if (ok) {
     if (stages == 1) {
-      val = warp_pixel(m[0], x, y, W, H, pixel);
+      val = warp_pixel<C>(m[0], x, y, W, H, pixel);
     } else {
       const double* m1 = m[0];
-      val = warp_pixel(m[1], x, y, bx[2] - bx[0], bx[3] - bx[1], [&](int u, int v) { return warp_pixel(m1, u, v, W, H, pixel); });
+      val = warp_pixel<C>(m[1], x, y, bx[2] - bx[0], bx[3] - bx[1], [&](int u, int v) { return warp_pixel<C>(m1, u, v, W, H, pixel); });
     }
   }
   const size_t o = (size_t)b * out_h * out_w + (size_t)idx;
-  if (out_u8) out_u8[o] = (uint8_t)val;
-  else out_f32[o] = __fdiv_rn((float)val, 255.f);
+  if (out_u8)
+    for (int c = 0; c < C; ++c) out_u8[o * C + c] = (uint8_t)val.v[c];
+  else out_f32[o] = __fdiv_rn((float)val.v[0], 255.f);
 }
 
 // One thread per output pixel of frame blockIdx.y.  stages as in crop_transforms_kernel, whose trans this reads.  The result
@@ -233,7 +255,7 @@ __device__ __forceinline__ void crop_warp(int f, bool frame_ok, const uint8_t* _
 __global__ void __launch_bounds__(kWarpThreads) crop_warp_kernel(const uint8_t* __restrict__ frames, long long frame_pitch, long long row_pitch, int H,
                                                                  int W, const int32_t* __restrict__ box, const double* __restrict__ trans, int stages,
                                                                  int out_h, int out_w, uint8_t* __restrict__ out_u8, float* __restrict__ out_f32) {
-  crop_warp(blockIdx.y, true, frames, frame_pitch, row_pitch, H, W, box, trans, stages, out_h, out_w, out_u8, out_f32);
+  crop_warp<1>(blockIdx.y, true, frames, frame_pitch, row_pitch, H, W, box, trans, stages, out_h, out_w, out_u8, out_f32);
 }
 
 // crop_warp_kernel for crop_img_by_bbox into fp32 where crop blockIdx.y reads frame frame_index[blockIdx.y] of n_frames; an
@@ -244,7 +266,19 @@ __global__ void __launch_bounds__(kWarpThreads) crop_warp_indexed_kernel(const u
                                                                          const double* __restrict__ trans, int out_size, float* __restrict__ out) {
   const int b = blockIdx.y;
   const bool in = frame_in_range(frame_index, b, n_frames);
-  crop_warp(in ? frame_index[b] : 0, in, frames, frame_pitch, row_pitch, H, W, box, trans, 2, out_size, out_size, nullptr, out);
+  crop_warp<1>(in ? frame_index[b] : 0, in, frames, frame_pitch, row_pitch, H, W, box, trans, 2, out_size, out_size, nullptr, out);
+}
+
+// crop_img_by_bbox's two warps into uint8 for frames of C channels: crop blockIdx.y reads frame frame_index[blockIdx.y] of
+// n_frames (an index outside that range gives zeros), or frame blockIdx.y when frame_index is null.
+template <int C>
+__global__ void __launch_bounds__(kWarpThreads) crop_warp_colour_kernel(const uint8_t* __restrict__ frames, long long frame_pitch, long long row_pitch,
+                                                                        int n_frames, int H, int W, const int32_t* __restrict__ frame_index,
+                                                                        const int32_t* __restrict__ box, const double* __restrict__ trans, int out_size,
+                                                                        uint8_t* __restrict__ out) {
+  const int b = blockIdx.y;
+  const bool in = !frame_index || frame_in_range(frame_index, b, n_frames);
+  crop_warp<C>(frame_index ? (in ? frame_index[b] : 0) : b, in, frames, frame_pitch, row_pitch, H, W, box, trans, 2, out_size, out_size, out, nullptr);
 }
 
 // One thread per frame: vis_utils.reproj (:209-236) of n points, (K_homo @ pose_homo) @ X then the division by the third row, and
@@ -337,4 +371,29 @@ extern "C" int opb_warp_crop_u8(const uint8_t* frames, int64_t frame_pitch, int6
   if (frames)
     if (int rc = opb::check_frames(__func__, frame_pitch, row_pitch, B, H, W)) return rc;
   return opb::launch_crop(__func__, frames, frame_pitch, row_pitch, B, H, W, box, K, 1, out_h, out_w, out, nullptr, trans, K_crop, nullptr, stream);
+}
+
+extern "C" int opb_crop_resize_colour(const uint8_t* frames, int64_t frame_pitch, int64_t row_pitch, int32_t n_frames, int32_t H, int32_t W, int32_t C,
+                                      const int32_t* frame_index, int32_t B, const int32_t* box, const double* K, int32_t crop_size, uint8_t* image,
+                                      double* K_crop, double* trans, int32_t* status, void* stream) {
+  REQUIRE(__func__, frames && box && K && image && K_crop && trans && status);
+  REQUIRE(__func__, C == 3 || C == 4);
+  if (int rc = opb::check_frames(__func__, frame_pitch, row_pitch, B, H, W)) return rc;
+  REQUIRE(__func__, row_pitch >= (int64_t)W * C);
+  REQUIRE(__func__, n_frames > 0 && (frame_index != nullptr || n_frames == B));
+  REQUIRE(__func__, crop_size > 0 && crop_size % 8 == 0 && crop_size <= opb::kMaxSide);
+  cudaStream_t st = (cudaStream_t)stream;
+  if (frame_index)
+    LAUNCH_NH(__func__, opb::crop_transforms_indexed_kernel, (unsigned)((B + 127) / 128), 128, 0, st, box, frame_index, n_frames, K, B, crop_size,
+              trans, K_crop, status);
+  else
+    LAUNCH_NH(__func__, opb::crop_transforms_kernel, (unsigned)((B + 127) / 128), 128, 0, st, box, K, B, 2, crop_size, crop_size, trans, K_crop, status);
+  const dim3 grid((unsigned)(((long long)crop_size * crop_size + opb::kWarpThreads - 1) / opb::kWarpThreads), (unsigned)B);
+  if (C == 3)
+    LAUNCH_NH(__func__, opb::crop_warp_colour_kernel<3>, grid, opb::kWarpThreads, 0, st, frames, frame_pitch, row_pitch, n_frames, H, W, frame_index, box,
+              trans, crop_size, image);
+  else
+    LAUNCH_NH(__func__, opb::crop_warp_colour_kernel<4>, grid, opb::kWarpThreads, 0, st, frames, frame_pitch, row_pitch, n_frames, H, W, frame_index, box,
+              trans, crop_size, image);
+  return OPB_OK;
 }
