@@ -563,6 +563,59 @@ int opb_flow_compact(const uint8_t* status, const float* pts2d, const float* pts
 int opb_flow_reprojection(const double* K, const double* pose, const double* pts2d, const double* pts3d, const int32_t* offsets, int32_t B,
                           double* dist, void* stream);
 
+/* ---- an object's SfM post-processing (csrc/sfm.cu) ----
+ * run.py postprocess (:142-163) after COLMAP's triangulation: get_tkl and filter_3d, merge, and the 3D half of get_kpt_ann.
+ * Caller's current device and stream, device pointers, asynchronous, no host synchronisation, no allocation: each step sizes
+ * one caller-provided workspace (256-byte aligned) with its *_workspace_bytes query.  A count one step finds (kept points,
+ * groups, observations) is written to a device int64 that the next step reads; `cap` arguments bound what a step may hold.
+ *
+ * opb_sfm_filter_points: P points in ascending id order, ids int64 [P], xyz f64 [P, 3], track_len int64 [P] (COLMAP's
+ * point2D_idxs lengths); corners f64 [8, 3]; max_num_kp3d >= 0.
+ *   track_length  out: get_tkl's threshold, the smallest length L present with at most max_num_kp3d points longer than L (the
+ *                 group at L is kept whole, so more than max_num_kp3d points can pass)
+ *   kept_ids, kept_xyz   int64 [P], fp32 [P, 3] out: the points of length >= track_length strictly inside the box, in order;
+ *                 filter_by_3d_box in fp32: m = (p - c4) . v for v = c5 - c4, c0 - c4, c7 - c4, kept when 0 < m < v . v,
+ *                 each product and sum rounded on its own, the sums left to right
+ *   n_kept        out: the kept count */
+int opb_sfm_filter_workspace_bytes(int32_t P, int64_t* bytes);
+int opb_sfm_filter_points(const int64_t* ids, const double* xyz, const int64_t* track_len, int32_t P, int32_t max_num_kp3d,
+                          const double* corners, void* workspace, int64_t workspace_bytes, int64_t* kept_ids, float* kept_xyz,
+                          int64_t* track_length, int64_t* n_kept, void* stream);
+/* opb_sfm_merge_points: merge (filter_points.py:86-117) of the first min(*n, cap) rows of xyz fp32 [cap, 3] with ids int64.
+ * Point i neighbours j when scipy's pdist of their rows widened to fp64 (dx*dx + dy*dy, + dz*dz, correctly rounded sqrt) is
+ * below dist_threshold (> 0); j neighbours itself.  The greedy pass walks j in order: j is skipped when any neighbour is already
+ * in a group, otherwise its neighbours, ascending, are the next group.  A point can be dropped without being in any group.
+ *   merged_xyz     f64 [cap, 3] out   np.mean of the group's fp32 rows (fp32 sum in member order, fp32 divide), widened
+ *   group_offsets  int32 [cap + 1] out  group g's members are group_offsets[g] .. group_offsets[g + 1] - 1
+ *   member_ids, member_index   int64 / int32 [cap] out: each member's id and row
+ *   slot_of        int32 [cap] out    row i's member position, or INT32_MAX for a row in no group
+ *   n_groups, n_members   out: the groups and their members (group_offsets[n_groups]); nothing is written past row
+ *                  min(*n, cap) - 1 of member_ids, member_index or slot_of */
+int opb_sfm_merge_workspace_bytes(int32_t cap, int64_t* bytes);
+int opb_sfm_merge_points(const float* xyz, const int64_t* ids, const int64_t* n, int32_t cap, double dist_threshold, void* workspace,
+                         int64_t workspace_bytes, double* merged_xyz, int32_t* group_offsets, int64_t* member_ids, int32_t* member_index,
+                         int32_t* slot_of, int64_t* n_groups, int64_t* n_members, void* stream);
+/* opb_sfm_gather_observations: the observations of the merge groups in get_kpt_ann's order.  Image f (the caller's order) holds
+ * features 0 .. counts[f] - 1 (counts[f] <= cap) whose COLMAP point ids are point3d_ids int64 [F, cap] (-1: none); F * cap
+ * <= INT32_MAX.  A feature observes member m when its id is kept_ids[i] (ascending, the first min(*n_kept, kept_cap)) and
+ * slot_of[i] = m (opb_sfm_merge_points' outputs).
+ *   order    int32 [F * cap] out   the observing features as f * cap + k, ordered by member position and, within a member,
+ *                                  by (image, feature); one image may observe a point twice
+ *   idxs     int64 [kept_cap] out  each group's observation count
+ *   total    out: the number of observations (the valid prefix of order)
+ *   missing  out: the position of the first member without an observation (the reference's KeyError), or a value above
+ *            every position */
+int opb_sfm_gather_workspace_bytes(int32_t F, int32_t cap, int32_t kept_cap, int64_t* bytes);
+int opb_sfm_gather_observations(const int64_t* point3d_ids, const int32_t* counts, int32_t F, int32_t cap, const int64_t* kept_ids,
+                                const int64_t* n_kept, int32_t kept_cap, const int32_t* slot_of, const int32_t* group_offsets,
+                                const int64_t* n_groups, void* workspace, int64_t workspace_bytes, int32_t* order, int64_t* idxs,
+                                int64_t* total, int64_t* missing, void* stream);
+/* opb_sfm_gather_features: rows 0 .. total - 1 of the collected features, widened to f64: out_descriptors [total, D] row r =
+ * descriptors[f, :, k] and out_scores [total] = scores[f, k] for order[r] = f * cap + k.  scores fp32 [F, cap], descriptors
+ * fp32 [F, D, cap] (SuperPoint's padded outputs). */
+int opb_sfm_gather_features(const int32_t* order, int64_t total, int32_t F, int32_t cap, int32_t D, const float* scores,
+                            const float* descriptors, double* out_descriptors, double* out_scores, void* stream);
+
 /* ---- the tracker's flow-only state machine (csrc/track.cu) ----
  * BATracker's per-frame logic around flow_track in the live demo's order (inference_demo.py:253-299, track_interval 5) with
  * track(frame, flow_track_only=True): update_kf's gate, add_kf's first pose, motion_prediction and track()'s choice of the

@@ -127,6 +127,13 @@ SYMBOLS = {
     "opb_flow_reprojection": (C.c_int, [_P, _P, _P, _P, _P, _I, _P, _P]),
     "opb_track_gate": (C.c_int, [_P, _I, _P, _P, _P, _P, _P]),
     "opb_track_select": (C.c_int, [_P, _P, _P, _I, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "opb_sfm_filter_workspace_bytes": (C.c_int, [_I, C.POINTER(C.c_int64)]),
+    "opb_sfm_filter_points": (C.c_int, [_P, _P, _P, _I, _I, _P, _P, C.c_int64, _P, _P, _P, _P, _P]),
+    "opb_sfm_merge_workspace_bytes": (C.c_int, [_I, C.POINTER(C.c_int64)]),
+    "opb_sfm_merge_points": (C.c_int, [_P, _P, _P, _I, C.c_double, _P, C.c_int64, _P, _P, _P, _P, _P, _P, _P, _P]),
+    "opb_sfm_gather_workspace_bytes": (C.c_int, [_I, _I, _I, C.POINTER(C.c_int64)]),
+    "opb_sfm_gather_observations": (C.c_int, [_P, _P, _I, _I, _P, _P, _I, _P, _P, _P, _P, C.c_int64, _P, _P, _P, _P, _P]),
+    "opb_sfm_gather_features": (C.c_int, [_P, C.c_int64, _I, _I, _I, _P, _P, _P, _P, _P]),
     "opb_debug_set_pdl": (C.c_int, [_I]),
     "opb_debug_set_ws_fill": (C.c_int, [_I]),
     "opb_debug_set_kv_passes": (C.c_int, [_P, _I]),
