@@ -49,6 +49,8 @@ struct ObjectState {      // per-object constants: the handle's current object (
   bool prologue_ready = false;
 };
 
+constexpr int kCurrentObject = -1;   // key of opb_set_object's object in opb_matcher::objects; opb_add_object's ids count up from 0
+
 }  // namespace opb
 
 using namespace opb;
@@ -56,7 +58,6 @@ using namespace opb;
 struct opb_matcher : Handle {
   opb_config cfg{};
   bool weights_ready = false;
-  bool object_ready = false;
   int num_sms = 132;      // multiprocessors of the device (opb_create reads it; 132 on an H100 SXM)
   // packed weights
   AttnLayerW attn[8];
@@ -65,9 +66,7 @@ struct opb_matcher : Handle {
   PlaneBuf wf;            // final_proj [256,256]
   DevBuf bf;
   PlaneBuf eye;           // [256,256] identity, fp16-split (residual as an identity K-block of the mlp.3 GEMM)
-  // per-object constants
-  ObjectState cur;                              // opb_set_object's object (valid while object_ready)
-  std::map<int, ObjectState> objects;           // opb_add_object registrations, by id
+  std::map<int, ObjectState> objects;           // opb_add_object registrations by id; opb_set_object's object under kCurrentObject
   int next_object_id = 0;
   // workspace (chunk)
   int chunk_frames = 0;   // user override
@@ -446,8 +445,30 @@ static int load_object(opb_matcher* m, ObjectState& o, const float* desc3d_db, c
   return 0;
 }
 
+// opb_set_object / opb_add_object (`fn`; `need`: its argument conditions; `id_ok`: false for a null id pointer): loads an object
+// into the entry under `key`, reusing the buffers of an entry already there.  A failed load leaves no entry under `key`.
+static int load_entry(opb_matcher* m, const char* fn, const char* need, int key, const float* desc3d_db, const float* desc2d_db, int M, int Lf,
+                      bool id_ok, cudaStream_t st) {
+  if (!m->weights_ready) return fail(m, OPB_E_STATE, "opb_%s before opb_finalize_weights", fn);
+  if (!desc3d_db || !desc2d_db || !id_ok || M <= 0 || Lf <= 0 || Lf > 32)
+    return fail(m, OPB_E_INVALID, "%s: need %s (got M=%d, L=%d)", fn, need, M, Lf);
+  DeviceGuard dg(m->device);
+  CK(m, dg.err);
+  ObjectState& o = m->objects[key];
+  if (int rc = ordered(m, st, [&] { return load_object(m, o, desc3d_db, desc2d_db, M, Lf, st); })) {
+    cudaDeviceSynchronize();                       // work in flight may still read the entry's buffers
+    m->objects.erase(key);
+    return rc;
+  }
+  return OPB_OK;
+}
+
+static ObjectState* find_object(opb_matcher* m, int key) { return m->objects.count(key) ? &m->objects.at(key) : nullptr; }
+
+// An object of opb_add_object by the id a caller passed: no such id reaches the current object's reserved key.
+static ObjectState* registered(opb_matcher* m, int id) { return id == kCurrentObject ? nullptr : find_object(m, id); }
+
 static void invalidate_prologues(opb_matcher* m) {
-  m->cur.prologue_ready = false;
   for (auto& kv : m->objects) kv.second.prologue_ready = false;
 }
 
@@ -654,63 +675,40 @@ int opb_finalize_weights(opb_matcher* m) {
   if (int rc = upload_f32(m, m->wa3, wa3)) return rc;
   CK(m, cudaDeviceSynchronize());
   m->weights_ready = true;
-  m->object_ready = false;  // s2 and the prologue depend on the weights: the current object is set again, registered objects
-  invalidate_prologues(m);  // recompute theirs on their next use
-  for (auto& kv : m->objects) kv.second.s2_ready = false;
+  m->objects.erase(kCurrentObject);   // s2 and the prologue depend on the weights: the current object is set again, registered
+  for (auto& kv : m->objects) kv.second.s2_ready = kv.second.prologue_ready = false;   // objects recompute theirs on their next use
   return OPB_OK;
 }
 
 int opb_set_object(opb_matcher* m, const float* desc3d_db, const float* desc2d_db, int32_t M, int32_t Lf, void* stream) {
   if (!m) return OPB_E_INVALID;
-  if (!m->weights_ready) return fail(m, OPB_E_STATE, "opb_set_object before opb_finalize_weights");
-  if (!desc3d_db || !desc2d_db || M <= 0 || Lf <= 0 || Lf > 32)
-    return fail(m, OPB_E_INVALID, "set_object: need M > 0 and 1 <= num_leaf <= 32 (got M=%d, L=%d)", M, Lf);
-  DeviceGuard dg(m->device);
-  CK(m, dg.err);
-  const cudaStream_t st = (cudaStream_t)stream;
-  m->object_ready = false;
-  if (int rc = ordered(m, st, [&] { return load_object(m, m->cur, desc3d_db, desc2d_db, M, Lf, st); })) return rc;
-  m->object_ready = true;
-  return OPB_OK;
+  return load_entry(m, "set_object", "M > 0 and 1 <= num_leaf <= 32", kCurrentObject, desc3d_db, desc2d_db, M, Lf, /*id_ok=*/true, (cudaStream_t)stream);
 }
 
 int opb_add_object(opb_matcher* m, const float* desc3d_db, const float* desc2d_db, int32_t M, int32_t Lf, void* stream, int32_t* object_id) {
   if (!m) return OPB_E_INVALID;
-  if (!m->weights_ready) return fail(m, OPB_E_STATE, "opb_add_object before opb_finalize_weights");
-  if (!desc3d_db || !desc2d_db || !object_id || M <= 0 || Lf <= 0 || Lf > 32)
-    return fail(m, OPB_E_INVALID, "add_object: need M > 0, 1 <= num_leaf <= 32 and an id pointer (got M=%d, L=%d)", M, Lf);
-  DeviceGuard dg(m->device);
-  CK(m, dg.err);
-  const cudaStream_t st = (cudaStream_t)stream;
-  const int id = m->next_object_id;
-  ObjectState& o = m->objects[id];
-  if (int rc = ordered(m, st, [&] { return load_object(m, o, desc3d_db, desc2d_db, M, Lf, st); })) {
-    cudaDeviceSynchronize();
-    m->objects.erase(id);
-    return rc;
-  }
-  m->next_object_id++;
-  *object_id = id;
-  return OPB_OK;
+  const int rc = load_entry(m, "add_object", "M > 0, 1 <= num_leaf <= 32 and an id pointer", m->next_object_id, desc3d_db, desc2d_db, M, Lf,
+                            object_id != nullptr, (cudaStream_t)stream);
+  if (rc == OPB_OK) *object_id = m->next_object_id++;
+  return rc;
 }
 
 int opb_remove_object(opb_matcher* m, int32_t object_id) {
   if (!m) return OPB_E_INVALID;
-  auto it = m->objects.find(object_id);
-  if (it == m->objects.end()) return fail(m, OPB_E_INVALID, "remove_object: unknown object id %d", object_id);
+  if (!registered(m, object_id)) return fail(m, OPB_E_INVALID, "remove_object: unknown object id %d", object_id);
   DeviceGuard dg(m->device);
   CK(m, dg.err);
   CK(m, cudaDeviceSynchronize());                  // calls in flight may still read the object's buffers
-  m->objects.erase(it);
+  m->objects.erase(object_id);
   return OPB_OK;
 }
 
 int opb_reserve_workspace(opb_matcher* m, int32_t frames, int32_t N) {
   if (!m || frames <= 0 || N <= 0) return OPB_E_INVALID;
-  if (!m->object_ready && m->objects.empty()) return fail(m, OPB_E_STATE, "opb_reserve_workspace needs an object (the workspace depends on M)");
+  if (m->objects.empty()) return fail(m, OPB_E_STATE, "opb_reserve_workspace needs an object (the workspace depends on M)");
   DeviceGuard dg(m->device);
   CK(m, dg.err);
-  int m_pad = m->object_ready ? m->cur.m_pad : 0;   // sized for the largest object the handle knows
+  int m_pad = 0;                                   // sized for the largest object the handle knows
   for (auto& kv : m->objects) m_pad = std::max(m_pad, kv.second.m_pad);
   return ensure_workspace(m, chunk_of(m, frames), N, m_pad);
 }
@@ -732,13 +730,14 @@ int opb_set_chunk_frames(opb_matcher* m, int32_t frames) {
 int opb_forward(opb_matcher* m, const float* q, const int32_t* n2d_lengths, int32_t B, int32_t N, int64_t* m0, int64_t* m1, float* s0, float* s1,
                 float* conf, void* stream) {
   if (!m) return OPB_E_INVALID;
-  if (!m->weights_ready || !m->object_ready) return fail(m, OPB_E_STATE, "opb_forward needs weights and an object (finalize_weights, set_object)");
+  ObjectState* cur = find_object(m, kCurrentObject);
+  if (!m->weights_ready || !cur) return fail(m, OPB_E_STATE, "opb_forward needs weights and an object (finalize_weights, set_object)");
   if (!q || !m0 || !m1 || !s0 || !s1 || B <= 0 || N <= 0) return fail(m, OPB_E_INVALID, "opb_forward: bad argument (B=%d, N=%d)", B, N);
   DeviceGuard dg(m->device);
   CK(m, dg.err);
   const cudaStream_t st = (cudaStream_t)stream;
-  std::vector<ObjectState*> fobj((size_t)B, &m->cur);      // every frame uses the current object
-  return ordered(m, st, [&] { return forward_frames(m, fobj.data(), q, n2d_lengths, B, N, m->cur.M, m0, m1, s0, s1, conf, st); });
+  std::vector<ObjectState*> fobj((size_t)B, cur);           // every frame uses the current object
+  return ordered(m, st, [&] { return forward_frames(m, fobj.data(), q, n2d_lengths, B, N, cur->M, m0, m1, s0, s1, conf, st); });
 }
 
 int opb_forward_objects(opb_matcher* m, const int32_t* object_ids_host, const float* q, const int32_t* n2d_lengths, int32_t B, int32_t N,
@@ -750,9 +749,8 @@ int opb_forward_objects(opb_matcher* m, const int32_t* object_ids_host, const fl
   std::vector<ObjectState*> fobj((size_t)B);
   int m_max = 0;
   for (int b = 0; b < B; ++b) {
-    auto it = m->objects.find(object_ids_host[b]);
-    if (it == m->objects.end()) return fail(m, OPB_E_INVALID, "opb_forward_objects: unknown object id %d (frame %d)", object_ids_host[b], b);
-    fobj[b] = &it->second;
+    fobj[b] = registered(m, object_ids_host[b]);
+    if (!fobj[b]) return fail(m, OPB_E_INVALID, "opb_forward_objects: unknown object id %d (frame %d)", object_ids_host[b], b);
     if (fobj[b]->Lf != fobj[0]->Lf)
       return fail(m, OPB_E_INVALID, "opb_forward_objects: frames %d and 0 use objects with different leaf counts (%d, %d)", b, fobj[b]->Lf,
                   fobj[0]->Lf);
@@ -827,12 +825,13 @@ int opb_get_profile_entry(opb_matcher* m, const char* prefix, double* ms_out, do
 int opb_forward_host(opb_matcher* m, const float* qh, const int32_t* n2d_lengths_host, int32_t B, int32_t N, int64_t* m0h, int64_t* m1h, float* s0h,
                      float* s1h, float* confh, int32_t materialize_conf, void* stream) {
   if (!m) return OPB_E_INVALID;
-  if (!m->object_ready) return fail(m, OPB_E_STATE, "opb_forward_host needs an object");
+  const ObjectState* cur = find_object(m, kCurrentObject);
+  if (!cur) return fail(m, OPB_E_STATE, "opb_forward_host needs an object");
   if (!qh || !m0h || !m1h || !s0h || !s1h || B <= 0 || N <= 0) return fail(m, OPB_E_INVALID, "opb_forward_host: bad argument");
   DeviceGuard dg(m->device);
   CK(m, dg.err);
   const cudaStream_t st = (cudaStream_t)stream;
-  const size_t M = m->cur.M;
+  const size_t M = cur->M;
   const bool want_conf = confh != nullptr || materialize_conf != 0;
   DevBuf* stg[] = {&m->st_q, &m->st_m0, &m->st_m1, &m->st_s0, &m->st_s1, &m->st_conf, &m->st_len};
   for (auto* b : stg) b->grew = false;

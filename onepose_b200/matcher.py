@@ -22,6 +22,7 @@ import torch.nn as nn
 from . import _lib
 
 GNN_LAYERS = ["GATs", "self", "cross"] * 4          # GATs_SuperGlue.py:162
+_CURRENT = -1                                       # key of the current object (set_object) in _objects; add_object's ids are >= 0
 
 
 class _GATsParams(nn.Module):
@@ -105,13 +106,12 @@ class GATsSuperGlue(nn.Module):
         self._handle = None
         self._handle_device = None
         self._weights_key = None
-        self._M = None
         self._obj_key = None           # (data_ptr, _version, shape) of the caller tensors the current object was packed from
         self._obj_ref = None           # strong reference to those tensors: their storage cannot be recycled under the key
         self._obj_copy = None          # private copy of the packed object (exact comparison on a key miss)
         self._chunk_frames = 0
         self._hoist = True
-        self._objects = {}             # registered object id -> M (add_object)
+        self._objects = {}             # M of each registered object by id (add_object), and of the current one under _CURRENT
         self.last_batched = None       # batched outputs of the last forward (all B frames)
 
     # ------------------------------------------------------------------ handle / weights
@@ -135,8 +135,8 @@ class GATsSuperGlue(nn.Module):
         h = C.c_void_p()
         _lib.check(self._lib.opb_create(C.byref(cfg), C.byref(h)))
         self._handle, self._handle_device = h, device
-        self._weights_key = self._obj_key = self._obj_ref = self._obj_copy = self._M = None
-        self._objects = {}             # registrations live on the handle
+        self._weights_key = self._obj_key = self._obj_ref = self._obj_copy = None
+        self._objects = {}             # objects live on the handle
         if self._chunk_frames:
             _lib.check(self._lib.opb_set_chunk_frames(self._handle, self._chunk_frames), self._handle)
         if not self._hoist:
@@ -151,7 +151,8 @@ class GATsSuperGlue(nn.Module):
             _lib.check(self._lib.opb_load_weight(self._handle, name.encode(), w.data_ptr(), w.numel()), self._handle)
         _lib.check(self._lib.opb_finalize_weights(self._handle), self._handle)
         self._weights_key = key
-        self._obj_key = self._obj_ref = self._obj_copy = self._M = None
+        self._obj_key = self._obj_ref = self._obj_copy = None
+        self._objects.pop(_CURRENT, None)      # a weight reload keeps the registered objects, not the current one
 
     def set_hoist(self, enable: bool):
         """Evaluate the frame-invariant GNN layers once per call (default) or per frame like the reference."""
@@ -170,6 +171,16 @@ class GATsSuperGlue(nn.Module):
         """Upload per-object constants once (what inference.py:113-130 builds per sequence).
         descriptors3d_db [256, M], descriptors2d_db [256, M*L], CUDA fp32.  reserve = (frames, N): size the
         workspace now instead of on the first call."""
+        d3, d2, M, L, st = self._prepare_object(descriptors3d_db, descriptors2d_db)
+        _lib.check(self._lib.opb_set_object(self._handle, d3.data_ptr(), d2.data_ptr(), M, L, st), self._handle)
+        self._objects[_CURRENT] = M
+        self._obj_key = self._obj_ref = self._obj_copy = None
+        if reserve is not None:
+            _lib.check(self._lib.opb_reserve_workspace(self._handle, int(reserve[0]), int(reserve[1])), self._handle)
+
+    def _prepare_object(self, descriptors3d_db: torch.Tensor, descriptors2d_db: torch.Tensor):
+        """(d3, d2, M, L, stream) of an object to load: fp32 contiguous CUDA tensors, with the handle on their device and its
+        weights current."""
         d3 = descriptors3d_db.float().contiguous()
         d2 = descriptors2d_db.float().contiguous()
         if not d3.is_cuda:
@@ -179,16 +190,10 @@ class GATsSuperGlue(nn.Module):
         M = d3.shape[1]
         if M == 0 or d2.shape[1] % M:
             raise ValueError(f"descriptors2d_db has {d2.shape[1]} columns, not a multiple of M={M}")
-        st = torch.cuda.current_stream(d3.device).cuda_stream
-        _lib.check(self._lib.opb_set_object(self._handle, d3.data_ptr(), d2.data_ptr(), M, d2.shape[1] // M, st),
-                   self._handle)
-        self._M = M
-        self._obj_key = self._obj_ref = self._obj_copy = None
-        if reserve is not None:
-            _lib.check(self._lib.opb_reserve_workspace(self._handle, int(reserve[0]), int(reserve[1])), self._handle)
+        return d3, d2, M, d2.shape[1] // M, torch.cuda.current_stream(d3.device).cuda_stream
 
     def _require_object(self):
-        if self._handle is None or self._M is None:
+        if self._handle is None or _CURRENT not in self._objects:
             raise RuntimeError("no object set: call set_object(descriptors3d_db, descriptors2d_db) first (or use forward(data))")
 
     def _check_device(self, q: torch.Tensor):
@@ -208,7 +213,12 @@ class GATsSuperGlue(nn.Module):
         self._check_device(descriptors2d_query)
         q = descriptors2d_query.float().contiguous()
         B, _, N = q.shape
-        M = self._M
+        return self._match(q, B, N, self._objects[_CURRENT], return_conf, lengths, out,
+                           lambda lens, *res: self._lib.opb_forward(self._handle, q.data_ptr(), lens, B, N, *res))
+
+    def _match(self, q, B, N, M, return_conf, lengths, out, call):
+        """match_frames / match_objects for B frames of N queries, M-wide rows: the result tensors (views of `out` or fresh),
+        `lengths` on the device, then call(lengths, matches0, matches1, scores0, scores1, conf, stream), all pointers."""
         dev = q.device
 
         def buf(name, shape, dtype):
@@ -224,28 +234,17 @@ class GATsSuperGlue(nn.Module):
             if lengths.numel() != B:
                 raise ValueError("lengths must have one entry per frame")
         st = torch.cuda.current_stream(dev).cuda_stream
-        _lib.check(self._lib.opb_forward(self._handle, q.data_ptr(), lengths.data_ptr() if lengths is not None else None, B, N,
-                                         m0.data_ptr(), m1.data_ptr(), s0.data_ptr(), s1.data_ptr(),
-                                         conf.data_ptr() if conf is not None else None, st), self._handle)
+        _lib.check(call(lengths.data_ptr() if lengths is not None else None, m0.data_ptr(), m1.data_ptr(), s0.data_ptr(), s1.data_ptr(),
+                        conf.data_ptr() if conf is not None else None, st), self._handle)
         return {"matches0": m0, "matches1": m1, "matching_scores0": s0, "matching_scores1": s1, "conf_matrix": conf}
 
     # ------------------------------------------------------------------ several objects per call
     def add_object(self, descriptors3d_db: torch.Tensor, descriptors2d_db: torch.Tensor) -> int:
         """Register an object (descriptors3d_db [256, M], descriptors2d_db [256, M*L], CUDA fp32) next to the current one and
         return its id for match_objects.  Its frame-invariant GNN layers run on its first use; reloading the weights keeps it."""
-        d3 = descriptors3d_db.float().contiguous()
-        d2 = descriptors2d_db.float().contiguous()
-        if not d3.is_cuda:
-            raise RuntimeError("onepose_b200 has no CPU path: tensors must be on a CUDA device")
-        self._ensure_handle(d3.device)
-        self._sync_weights()
-        M = d3.shape[1]
-        if M == 0 or d2.shape[1] % M:
-            raise ValueError(f"descriptors2d_db has {d2.shape[1]} columns, not a multiple of M={M}")
-        st = torch.cuda.current_stream(d3.device).cuda_stream
+        d3, d2, M, L, st = self._prepare_object(descriptors3d_db, descriptors2d_db)
         oid = C.c_int32()
-        _lib.check(self._lib.opb_add_object(self._handle, d3.data_ptr(), d2.data_ptr(), M, d2.shape[1] // M, st, C.byref(oid)),
-                   self._handle)
+        _lib.check(self._lib.opb_add_object(self._handle, d3.data_ptr(), d2.data_ptr(), M, L, st, C.byref(oid)), self._handle)
         self._objects[oid.value] = M
         return oid.value
 
@@ -274,34 +273,19 @@ class GATsSuperGlue(nn.Module):
         if len(ids) != B:
             raise ValueError(f"object_ids has {len(ids)} entries for {B} frames")
         for i in ids:
-            if i not in self._objects:
+            if i == _CURRENT or i not in self._objects:
                 raise ValueError(f"unknown object id {i}")
         M = max(self._objects[i] for i in ids)
         if out is not None and "matches1" in out and out["matches1"].dim() == 2:
             if out["matches1"].shape[1] < M:
                 raise ValueError(f"out['matches1'] is {out['matches1'].shape[1]} wide, below the call's largest M = {M}")
             M = int(out["matches1"].shape[1])
-        dev = q.device
-
-        def buf(name, shape, dtype):
-            return _out_view(out, name, shape, dtype, dev)
-
-        m0 = buf("matches0", (B, N), torch.int64)
-        m1 = buf("matches1", (B, M), torch.int64)
-        s0 = buf("matching_scores0", (B, N), torch.float32)
-        s1 = buf("matching_scores1", (B, M), torch.float32)
-        conf = buf("conf_matrix", (B, N, M), torch.float32) if return_conf else None
-        if lengths is not None:
-            lengths = lengths.to(device=dev, dtype=torch.int32).contiguous()
-            if lengths.numel() != B:
-                raise ValueError("lengths must have one entry per frame")
         ids_host = (C.c_int32 * B)(*ids)
-        st = torch.cuda.current_stream(dev).cuda_stream
-        _lib.check(self._lib.opb_poll_range(self._handle), self._handle)
-        _lib.check(self._lib.opb_forward_objects(self._handle, ids_host, q.data_ptr(), lengths.data_ptr() if lengths is not None else None,
-                                                 B, N, M, m0.data_ptr(), m1.data_ptr(), s0.data_ptr(), s1.data_ptr(),
-                                                 conf.data_ptr() if conf is not None else None, st), self._handle)
-        return {"matches0": m0, "matches1": m1, "matching_scores0": s0, "matching_scores1": s1, "conf_matrix": conf}
+
+        def call(lens, *res):
+            _lib.check(self._lib.opb_poll_range(self._handle), self._handle)
+            return self._lib.opb_forward_objects(self._handle, ids_host, q.data_ptr(), lens, B, N, M, *res)
+        return self._match(q, B, N, M, return_conf, lengths, out, call)
 
     def match_frames_host(self, q_host: torch.Tensor, out: dict | None = None, lengths: torch.Tensor | None = None,
                           materialize_conf: bool = True):
@@ -311,7 +295,7 @@ class GATsSuperGlue(nn.Module):
         out["conf_matrix"] (fp32, B * N * M elements) receives a copy of it."""
         self._require_object()
         B, _, N = q_host.shape
-        M = self._M
+        M = self._objects[_CURRENT]
         if out is None:
             pin = dict(pin_memory=True)
             out = {"matches0": torch.empty(B, N, dtype=torch.int64, **pin), "matches1": torch.empty(B, M, dtype=torch.int64, **pin),

@@ -264,6 +264,53 @@ def test_registry_remove_add_reload_and_argument_checks():
     m.check_range()
 
 
+def test_current_object_beside_registered_ones():
+    """With a current object set next to a registered one: id -1 (the current object's key inside the handle) is an unknown id
+    to opb_forward_objects and opb_remove_object, and a weight reload unsets the current object (opb_forward refuses until the
+    next opb_set_object) while the registered object gives the same results as before it."""
+    hp = dict(synthetic.DEFAULT_HPARAMS)
+    sd = synthetic.make_state_dict(2)
+    m = _module(sd, hp)
+    N = 64
+    cur = [torch.from_numpy(t).cuda() for t in synthetic.make_object(84, 150, 8)]
+    m.set_object(*cur)
+    a = _add(m, 85, 120, 8)
+    q = torch.cat([_q([9], synthetic.make_object(84, 150, 8)[0], N), _q([10], synthetic.make_object(85, 120, 8)[0], N)])
+    before_cur = {k: v.clone() for k, v in m.match_frames(q).items()}
+    before_reg = {k: v.clone() for k, v in m.match_objects(q, [a, a]).items()}
+    lib, h = m._lib, m._handle
+    o = {k: torch.zeros(2 * 150 * N, dtype=t).cuda() for k, t in (("m0", torch.int64), ("m1", torch.int64), ("s0", torch.float32),
+                                                                   ("s1", torch.float32))}
+    st = torch.cuda.current_stream().cuda_stream
+
+    def forward_objects(ids):
+        arr = (C.c_int32 * 2)(*ids)
+        return lib.opb_forward_objects(h, arr, q.data_ptr(), None, 2, N, 150, o["m0"].data_ptr(), o["m1"].data_ptr(), o["s0"].data_ptr(),
+                                       o["s1"].data_ptr(), None, st)
+    for ids in ([-1, a], [a, -1]):
+        assert forward_objects(ids) == -1, ids
+        assert b"unknown object id -1" in lib.opb_last_error(h), ids
+    assert lib.opb_remove_object(h, -1) == -1
+    assert b"unknown object id -1" in lib.opb_last_error(h)
+    with pytest.raises(ValueError, match="unknown object id -1"):
+        m.match_objects(q, [-1, a])
+    assert forward_objects([a, a]) == 0
+    # weight reload with the same weights, straight through the C ABI
+    assert lib.opb_finalize_weights(h) == 0
+    assert lib.opb_forward(h, q.data_ptr(), None, 2, N, o["m0"].data_ptr(), o["m1"].data_ptr(), o["s0"].data_ptr(), o["s1"].data_ptr(),
+                           None, st) == -3                  # OPB_E_STATE: no current object
+    with pytest.raises(_lib.OpbError, match="OPB_E_STATE"):
+        m.match_frames(q)
+    after_reg = m.match_objects(q, [a, a])
+    for k in before_reg:
+        assert torch.equal(after_reg[k], before_reg[k]), k
+    assert lib.opb_set_object(h, cur[0].data_ptr(), cur[1].data_ptr(), 150, 8, st) == 0
+    after_cur = m.match_frames(q)
+    for k in before_cur:
+        assert torch.equal(after_cur[k], before_cur[k]), k
+    m.check_range()
+
+
 def test_workspace_fill_does_not_change_bits():
     hp = dict(synthetic.DEFAULT_HPARAMS)
     sd = synthetic.make_state_dict(4)
