@@ -615,6 +615,47 @@ int opb_sfm_gather_observations(const int64_t* point3d_ids, const int32_t* count
  * fp32 [F, D, cap] (SuperPoint's padded outputs). */
 int opb_sfm_gather_features(const int32_t* order, int64_t total, int32_t F, int32_t cap, int32_t D, const float* scores,
                             const float* descriptors, double* out_descriptors, double* out_scores, void* stream);
+/* opb_sfm_assign_pairs: each image's assign matrix (count_features and get_assign_matrix, feature_process.py:95-135,
+ * :197-230).  Image f holds features 0 .. counts[f] - 1 with COLMAP point ids point3d_ids int64 [F, cap] (-1: none), cap <=
+ * OPB_SFM_ASSIGN_MAX_CAP (one image is one block's shared memory).  A feature's id is kept when it is in kept_ids int64 [M]
+ * (ascending, distinct) and then belongs to group kept_group[i] (0 <= group < M).  Per image, in the order of each group's first
+ * feature k0: (the last feature whose id is k0's, the group) -- one pair per group.
+ *   pairs        int64 [2, F * cap] out   row 0 the features, row 1 the groups; image f's pairs are columns offsets[f] ..
+ *                                         offsets[f + 1] - 1 (columns past offsets[F] are not written)
+ *   offsets      int64 [F + 1] out
+ *   num_matches  int64 [F] out */
+#define OPB_SFM_ASSIGN_MAX_CAP 8192
+int opb_sfm_assign_workspace_bytes(int32_t F, int32_t cap, int64_t* bytes);
+int opb_sfm_assign_pairs(const int64_t* point3d_ids, const int32_t* counts, int32_t F, int32_t cap, const int64_t* kept_ids,
+                         const int32_t* kept_group, int32_t M, void* workspace, int64_t workspace_bytes, int64_t* pairs, int64_t* offsets,
+                         int64_t* num_matches, void* stream);
+
+/* ---- the JSON text of the per-image 2D annotation files (csrc/json_text.cu) ----
+ * save_2d_anno_for_each_image's json.dump (feature_process.py:233-262): {"keypoints2d": [n, 2], "descriptors2d": [D, n],
+ * "scores2d": [n, 1], "assign_matrix": [2, k], "num_matches": k} with ", " and ": ", each fp32 feature as float.__repr__ of the
+ * widened double (NaN, Infinity, -Infinity as json writes them) and the integers as int.__repr__.
+ *
+ * opb_json_float_repr: float.__repr__ of (double)x[i] into out [n, 24] (NUL-padded) and its length into len int32 [n].
+ * opb_json_float_repr_host: the same routine on the host, on host memory.
+ *
+ * A chunk of Fc <= 65535 images: images int64 [Fc, 4] = (feature row f, n, k >= 1, pair offset) per image, device memory; image c's
+ * numbers are keypoints fp32 [F, cap, 2] row f, descriptors fp32 [F, D, cap] row f, scores fp32 [F, cap] row f, both rows of
+ * pairs int64 [2, pair_stride] from the pair offset (opb_sfm_assign_pairs' layout) and k.  Its text is 3n + Dn + 2k + 1 items
+ * (a number and the text before it; the last one closes the object); item_off int64 [Fc + 1] gives the chunk's first item of
+ * each image, items = item_off[Fc], and max_items >= every image's item count, at most OPB_ANNO2D_MAX_IMAGE_ITEMS.
+ * opb_anno2d_text_lengths sizes every item into the workspace and writes offsets int64 [Fc + 1] (device): image c's text is
+ * bytes offsets[c] .. offsets[c + 1] - 1 of the chunk's.  opb_anno2d_text_write then writes the text to out (offsets[Fc] bytes)
+ * from the same arguments, the workspace that opb_anno2d_text_lengths filled and its offsets. */
+#define OPB_ANNO2D_MAX_IMAGE_ITEMS (1 << 24)
+int opb_json_float_repr(const float* x, int64_t n, char* out, int32_t* len, void* stream);
+int opb_json_float_repr_host(const float* x, int64_t n, char* out, int32_t* len);
+int opb_anno2d_text_workspace_bytes(int32_t Fc, int64_t items, int64_t* bytes);
+int opb_anno2d_text_lengths(const int64_t* images, const int64_t* item_off, int32_t Fc, int64_t items, int64_t max_items, int32_t D,
+                            int32_t cap, const float* keypoints, const float* descriptors, const float* scores, const int64_t* pairs,
+                            int64_t pair_stride, void* workspace, int64_t workspace_bytes, int64_t* offsets, void* stream);
+int opb_anno2d_text_write(const int64_t* images, const int64_t* item_off, int32_t Fc, int64_t max_items, int32_t D, int32_t cap,
+                          const float* keypoints, const float* descriptors, const float* scores, const int64_t* pairs, int64_t pair_stride,
+                          const void* workspace, const int64_t* offsets, char* out, void* stream);
 
 /* ---- the tracker's flow-only state machine (csrc/track.cu) ----
  * BATracker's per-frame logic around flow_track in the live demo's order (inference_demo.py:253-299, track_interval 5) with

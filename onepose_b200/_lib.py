@@ -134,6 +134,13 @@ SYMBOLS = {
     "opb_sfm_gather_workspace_bytes": (C.c_int, [_I, _I, _I, C.POINTER(C.c_int64)]),
     "opb_sfm_gather_observations": (C.c_int, [_P, _P, _I, _I, _P, _P, _I, _P, _P, _P, _P, C.c_int64, _P, _P, _P, _P, _P]),
     "opb_sfm_gather_features": (C.c_int, [_P, C.c_int64, _I, _I, _I, _P, _P, _P, _P, _P]),
+    "opb_sfm_assign_workspace_bytes": (C.c_int, [_I, _I, C.POINTER(C.c_int64)]),
+    "opb_sfm_assign_pairs": (C.c_int, [_P, _P, _I, _I, _P, _P, _I, _P, C.c_int64, _P, _P, _P, _P]),
+    "opb_json_float_repr": (C.c_int, [_P, C.c_int64, _P, _P, _P]),
+    "opb_json_float_repr_host": (C.c_int, [_P, C.c_int64, _P, _P]),
+    "opb_anno2d_text_workspace_bytes": (C.c_int, [_I, C.c_int64, C.POINTER(C.c_int64)]),
+    "opb_anno2d_text_lengths": (C.c_int, [_P, _P, _I, C.c_int64, C.c_int64, _I, _I, _P, _P, _P, _P, C.c_int64, _P, C.c_int64, _P, _P]),
+    "opb_anno2d_text_write": (C.c_int, [_P, _P, _I, C.c_int64, _I, _I, _P, _P, _P, _P, C.c_int64, _P, _P, _P, _P]),
     "opb_debug_set_pdl": (C.c_int, [_I]),
     "opb_debug_set_ws_fill": (C.c_int, [_I]),
     "opb_debug_set_kv_passes": (C.c_int, [_P, _I]),

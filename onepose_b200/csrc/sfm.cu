@@ -5,6 +5,8 @@
 //   filter_points.merge       :86-117   close points merged greedily, np.mean of each group        opb_sfm_merge_points
 //   feature_process.get_kpt_ann         each group's observations, group-major (:95-188, :320-363)  opb_sfm_gather_observations
 //                                       and their descriptors and scores in that order               opb_sfm_gather_features
+//   feature_process.count_features      each image's 2D-3D pairs, one per group (:95-135, :197-230) opb_sfm_assign_pairs
+//                   + get_assign_matrix
 // Every count (kept points, groups, observations) stays on the device: a later step reads it from the scalar an earlier one
 // wrote, and launches for the capacity the caller sized.  The arithmetic is the reference's, one rounding per operation
 // (__fadd_rn and friends, no fused multiply-add); the model is tests/sfm_reference.py and DESIGN §5.13 states the rules.
@@ -12,6 +14,8 @@
 #include <math.h>
 #include <stdint.h>
 
+#include <cub/block/block_radix_sort.cuh>
+#include <cub/block/block_scan.cuh>
 #include <cub/device/device_radix_sort.cuh>
 
 #include "../../include/onepose_b200.h"
@@ -250,6 +254,109 @@ __global__ void gather_features_kernel(const int32_t* __restrict__ order, int64_
   if (threadIdx.x == 0) out_scores[r] = (double)scores[t];
 }
 
+// ---- the 2D-3D pairs of each image ----
+
+// count_features keeps, per image, {kept id: its last feature index} in the order of each id's first feature; get_assign_matrix
+// walks that and pairs an id with its group unless the group was paired before in the image.  So group g's pair comes from the
+// id of g's first feature k0 in the image: (the last feature with that id, g), and the pairs are in the order of k0.
+// One block per image, features k = 16 * thread + i (blocked): a radix sort of (group << 13 | k) puts each group's features in
+// feature order, a max-scan of the segment heads finds every feature's k0, and the features with k0's id raise its last index.
+constexpr int kAssignThreads = 512, kAssignItems = 16, kAssignBits = 13;
+static_assert(kAssignThreads * kAssignItems == OPB_SFM_ASSIGN_MAX_CAP && (1 << kAssignBits) == OPB_SFM_ASSIGN_MAX_CAP, "assign tile");
+using AssignSort = cub::BlockRadixSort<uint64_t, kAssignThreads, kAssignItems>;
+using AssignScan = cub::BlockScan<int, kAssignThreads>;
+struct AssignSmem {
+  union {
+    typename AssignSort::TempStorage sort;
+    uint64_t keys[OPB_SFM_ASSIGN_MAX_CAP];      // the sorted keys
+  } a;
+  typename AssignScan::TempStorage scan;
+  int32_t rank[OPB_SFM_ASSIGN_MAX_CAP];         // feature k: its id's index among the kept ids, -1 without a kept id
+  int32_t group[OPB_SFM_ASSIGN_MAX_CAP];        // at a group's first feature k0: the group
+  int32_t last[OPB_SFM_ASSIGN_MAX_CAP];         // at k0: the last feature with k0's id; -1 elsewhere
+};
+constexpr uint64_t kNoKey = ~0ull;
+
+__global__ void __launch_bounds__(kAssignThreads) assign_pairs_kernel(const int64_t* __restrict__ point3d_ids,
+                                                                      const int32_t* __restrict__ counts, int cap,
+                                                                      const int64_t* __restrict__ kept_ids,
+                                                                      const int32_t* __restrict__ kept_group, int M, int end_bit,
+                                                                      int64_t* __restrict__ packed, int64_t* __restrict__ num_matches) {
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  AssignSmem& sm = *reinterpret_cast<AssignSmem*>(smem_raw);
+  const int f = blockIdx.x, n = min(counts[f], cap);
+  uint64_t key[kAssignItems];
+  for (int i = 0; i < kAssignItems; ++i) {
+    const int k = threadIdx.x * kAssignItems + i;
+    int32_t rank = -1;
+    key[i] = kNoKey;
+    if (k < n) {
+      const int64_t id = point3d_ids[(size_t)f * cap + k];
+      int lo = 0, hi = M;
+      while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (kept_ids[mid] < id) lo = mid + 1;
+        else hi = mid;
+      }
+      if (id != -1 && lo < M && kept_ids[lo] == id) {
+        rank = lo;
+        key[i] = (uint64_t)kept_group[lo] << kAssignBits | (uint64_t)k;
+      }
+    }
+    sm.rank[k] = rank;
+    sm.last[k] = -1;
+  }
+  __syncthreads();
+  AssignSort(sm.a.sort).Sort(key, 0, end_bit);
+  __syncthreads();
+  for (int i = 0; i < kAssignItems; ++i) sm.a.keys[threadIdx.x * kAssignItems + i] = key[i];
+  __syncthreads();
+  int head[kAssignItems];
+  for (int i = 0; i < kAssignItems; ++i) {
+    const int p = threadIdx.x * kAssignItems + i;
+    head[i] = key[i] != kNoKey && (p == 0 || sm.a.keys[p - 1] >> kAssignBits != key[i] >> kAssignBits) ? p : -1;
+  }
+  AssignScan(sm.scan).InclusiveScan(head, head, cub::Max());
+  for (int i = 0; i < kAssignItems; ++i) {
+    if (key[i] == kNoKey) continue;
+    const int p = threadIdx.x * kAssignItems + i;
+    const int k = (int)(key[i] & (OPB_SFM_ASSIGN_MAX_CAP - 1)), k0 = (int)(sm.a.keys[head[i]] & (OPB_SFM_ASSIGN_MAX_CAP - 1));
+    if (p == head[i]) sm.group[k0] = (int32_t)(key[i] >> kAssignBits);
+    if (sm.rank[k] == sm.rank[k0]) atomicMax(&sm.last[k0], k);
+  }
+  __syncthreads();
+  int slot[kAssignItems], total;
+  for (int i = 0; i < kAssignItems; ++i) slot[i] = sm.last[threadIdx.x * kAssignItems + i] >= 0;
+  AssignScan(sm.scan).ExclusiveSum(slot, slot, total);
+  for (int i = 0; i < kAssignItems; ++i) {
+    const int k = threadIdx.x * kAssignItems + i;
+    if (sm.last[k] >= 0) packed[(size_t)f * cap + slot[i]] = (int64_t)sm.last[k] << 32 | sm.group[k];
+  }
+  if (threadIdx.x == 0) num_matches[f] = total;
+}
+
+// offsets[0 .. F] of the images' pairs (one thread: F is the number of images)
+__global__ void assign_offsets_kernel(const int64_t* __restrict__ num_matches, int F, int64_t* __restrict__ offsets) {
+  int64_t s = 0;
+  for (int f = 0; f < F; ++f) {
+    offsets[f] = s;
+    s += num_matches[f];
+  }
+  offsets[F] = s;
+}
+
+// Image f's pairs from its padded row to columns offsets[f] .. of pairs [2, pair_stride]: the feature, then the group.
+__global__ void assign_compact_kernel(const int64_t* __restrict__ packed, const int64_t* __restrict__ num_matches,
+                                      const int64_t* __restrict__ offsets, int cap, int64_t pair_stride, int64_t* __restrict__ pairs) {
+  const int f = blockIdx.x;
+  const int64_t o = offsets[f];
+  for (int i = threadIdx.x; i < num_matches[f]; i += blockDim.x) {
+    const int64_t v = packed[(size_t)f * cap + i];
+    pairs[o + i] = v >> 32;
+    pairs[pair_stride + o + i] = v & 0xffffffff;
+  }
+}
+
 // Workspace of opb_sfm_filter_points: the sorted lengths, then CUB's temporary storage.
 int filter_temp_bytes(int P, size_t* bytes) {
   *bytes = 0;
@@ -371,5 +478,32 @@ extern "C" int opb_sfm_gather_features(const int32_t* order, int64_t total, int3
   if (total > 0)
     LAUNCH_NH(__func__, opb::gather_features_kernel, (unsigned)total, 128, 0, (cudaStream_t)stream, order, total, cap, D, scores, descriptors,
               out_descriptors, out_scores);
+  return OPB_OK;
+}
+
+extern "C" int opb_sfm_assign_workspace_bytes(int32_t F, int32_t cap, int64_t* bytes) {
+  REQUIRE(__func__, bytes && F > 0 && cap > 0 && cap <= OPB_SFM_ASSIGN_MAX_CAP && (int64_t)F * cap <= (int64_t)INT32_MAX);
+  *bytes = (int64_t)opb::align256((size_t)F * cap * 8);
+  return OPB_OK;
+}
+
+extern "C" int opb_sfm_assign_pairs(const int64_t* point3d_ids, const int32_t* counts, int32_t F, int32_t cap, const int64_t* kept_ids,
+                                    const int32_t* kept_group, int32_t M, void* workspace, int64_t workspace_bytes, int64_t* pairs,
+                                    int64_t* offsets, int64_t* num_matches, void* stream) {
+  REQUIRE(__func__, point3d_ids && counts && kept_ids && kept_group && workspace && pairs && offsets && num_matches);
+  REQUIRE(__func__, F > 0 && cap > 0 && cap <= OPB_SFM_ASSIGN_MAX_CAP && M > 0 && (int64_t)F * cap <= (int64_t)INT32_MAX);
+  REQUIRE(__func__, ((uintptr_t)workspace & 255) == 0);
+  REQUIRE(__func__, workspace_bytes >= (int64_t)opb::align256((size_t)F * cap * 8));
+  int group_bits = 0;                   // groups are below M: below the all-ones key of a feature without a kept id
+  while (group_bits < 31 && (1ll << group_bits) <= (int64_t)M) ++group_bits;
+  const size_t smem = sizeof(opb::AssignSmem);
+  CK(opb::no_handle_error, cudaFuncSetAttribute(opb::assign_pairs_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  cudaStream_t st = (cudaStream_t)stream;
+  int64_t* packed = (int64_t*)workspace;
+  LAUNCH_NH(__func__, opb::assign_pairs_kernel, (unsigned)F, opb::kAssignThreads, smem, st, point3d_ids, counts, (int)cap, kept_ids, kept_group,
+            (int)M, opb::kAssignBits + group_bits, packed, num_matches);
+  LAUNCH_NH(__func__, opb::assign_offsets_kernel, 1, 1, 0, st, (const int64_t*)num_matches, (int)F, offsets);
+  LAUNCH_NH(__func__, opb::assign_compact_kernel, (unsigned)F, 256, 0, st, (const int64_t*)packed, (const int64_t*)num_matches,
+            (const int64_t*)offsets, (int)cap, (int64_t)F * cap, pairs);
   return OPB_OK;
 }

@@ -9,12 +9,18 @@ images' device features to the arrays of ``anno_3d_average.npz``, ``anno_3d_coll
 The readers parse COLMAP's binary model on the host (its documented layout).  ``postprocess`` runs the steps on the caller's
 stream; the counts stay on the device until one read, after the last step that sizes an output, brings the counts, ``idxs`` and
 the groups to the host in one copy.
-COLMAP triangulation, the 2D annotations (``anno_2d.json`` and its assign matrices, used for training only) and the PLY
-visualisation are not part of it.
+
+The 2D half of get_kpt_ann (feature_process.py:95-135, :197-294) follows from ``postprocess``'s groups:
+
+    count_features + get_assign_matrix     opb_sfm_assign_pairs                             assign_matrices
+    save_2d_anno (per-image JSON text)     opb_anno2d_text_lengths, opb_anno2d_text_write   save_anno_2d
+
+COLMAP triangulation and the PLY visualisation are not part of it.
 """
 from __future__ import annotations
 
 import ctypes
+import json
 import os
 import struct
 
@@ -121,6 +127,28 @@ def _device_features(features, F: int):
     return sc.contiguous(), de.contiguous()
 
 
+def _point_id_table(images, n_obs, cap: int) -> np.ndarray:
+    """Image f's COLMAP point ids in row f of an int64 [F, cap] table, -1 past its count."""
+    F = len(images)
+    flat = np.concatenate([np.asarray(p, np.int64) for _, p in images])
+    starts = np.cumsum(n_obs) - n_obs
+    pid = np.full((F, cap), -1, np.int64)
+    pid[np.repeat(np.arange(F), n_obs), np.arange(len(flat)) - np.repeat(starts, n_obs)] = flat
+    return pid
+
+
+def _images(images, image_names):
+    if isinstance(images, (str, os.PathLike)):
+        images = read_images_bin(os.path.join(images, "images.bin"))
+    if image_names is not None:
+        by_name = dict(images)
+        missing = [n for n in image_names if n not in by_name]
+        if missing:
+            raise ValueError(f"images {missing[:3]} are not in the model")
+        images = [(n, by_name[n]) for n in image_names]
+    return images
+
+
 def postprocess(points3d, images, features, box_corners, max_num_kp3d: int = 2500, dist_threshold: float = 1e-3,
                 image_names=None) -> dict:
     """run.py postprocess on the device.
@@ -171,10 +199,7 @@ def postprocess(points3d, images, features, box_corners, max_num_kp3d: int = 250
         raise ValueError(f"opb_sfm_gather_observations: an image has {n_obs.max()} features, above the features' cap {cap}")
     if F * cap > INT32_MAX:
         raise ValueError(f"opb_sfm_gather_observations: F * cap = {F * cap} is above {INT32_MAX}")
-    flat = np.concatenate([np.asarray(p, np.int64) for _, p in images])
-    starts = np.cumsum(n_obs) - n_obs
-    pid = np.full((F, cap), -1, np.int64)         # image f's point ids in row f, -1 past its count
-    pid[np.repeat(np.arange(F), n_obs), np.arange(len(flat)) - np.repeat(starts, n_obs)] = flat
+    pid = _point_id_table(images, n_obs, cap)
 
     order = np.argsort(ids, kind="stable")        # filter_by_track_length walks the ids sorted
     with torch.cuda.device(dev):
@@ -240,3 +265,135 @@ def save_anno(anno_dir, result: dict) -> None:
     np.savez(os.path.join(anno_dir, "anno_3d_collect.npz"), keypoints3d=xyz, descriptors3d=host(result["descriptors3d_collect"]),
              scores3d=host(result["scores3d_collect"]))
     np.save(os.path.join(anno_dir, "idxs.npy"), np.asarray(result["idxs"], dtype=np.int64))
+
+
+ANNO2D_CHUNK_BYTES = 1 << 30       # the default bound of save_anno_2d's device text buffer
+_ITEM_BOUND = 27                   # bytes of an item at most: ", " or "], [" and a 23-character float repr
+_OBJECT_BOUND = 128                # the section keys, their brackets and num_matches' closing brace
+
+
+def _assign_device(result: dict, images, features, image_names):
+    """opb_sfm_assign_pairs on postprocess's groups: (device, pairs int64 [2, F * cap] on the device, offsets [F + 1] and
+    num_matches [F] on the host, the number of features of each image, cap)."""
+    images = _images(images, image_names)
+    F = len(images)
+    if F == 0:
+        raise ValueError("opb_sfm_assign_pairs: no images")
+    sc, _ = _device_features(features, F)
+    dev, cap = sc.device, int(sc.shape[1])
+    n_obs = np.array([len(p) for _, p in images], np.int64)
+    if n_obs.max() > cap:
+        raise ValueError(f"opb_sfm_assign_pairs: an image has {n_obs.max()} features, above the features' cap {cap}")
+    ids = np.asarray(result["group_ids"], np.int64)
+    off = np.asarray(result["group_offsets"], np.int64)
+    if ids.size == 0 or off.shape != (off.size,) or off[0] != 0 or off[-1] != ids.size or (np.diff(off) < 0).any():
+        raise ValueError("opb_sfm_assign_pairs: result must hold postprocess's group_ids and group_offsets")
+    group = np.repeat(np.arange(off.size - 1, dtype=np.int32), np.diff(off))
+    order = np.argsort(ids, kind="stable")          # id_mapping's table, searched by id
+    kept, kept_group = ids[order], group[order]
+    if (np.diff(kept) == 0).any():
+        raise ValueError("opb_sfm_assign_pairs: a COLMAP point id is in two groups")
+    pid = _point_id_table(images, n_obs, cap)
+    with torch.cuda.device(dev):
+        up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).pin_memory().to(dev, non_blocking=True)  # noqa: E731
+        d_pid, d_counts, d_kept, d_group = up(pid), up(n_obs.astype(np.int32)), up(kept), up(kept_group)
+        pairs = torch.empty(2, F * cap, dtype=torch.int64, device=dev)
+        counts = torch.empty(2 * F + 1, dtype=torch.int64, device=dev)     # offsets [F + 1], then num_matches [F]: one read
+        ws = _ws(dev, "opb_sfm_assign_workspace_bytes", F, cap)
+        _lib.call(dev, "opb_sfm_assign_pairs", d_pid, d_counts, F, cap, d_kept, d_group, int(kept.size), ws, ws.numel(), pairs,
+                  counts[:F + 1], counts[F + 1:])
+        h = counts.cpu().numpy()
+    return dev, pairs, h[:F + 1].copy(), h[F + 1:].copy(), n_obs, cap
+
+
+def assign_matrices(result: dict, images, features, image_names=None):
+    """count_features + get_assign_matrix (feature_process.py:95-135, :197-230) on the device.
+
+    result        postprocess's result (its group_ids and group_offsets)
+    images, features, image_names   as given to postprocess, in the same order
+
+    Returns (the assign matrices, num_matches int64 [F]): image f's matrix is int64 [2, k_f], row 0 its features and row 1 their
+    groups (the rows of keypoints3d), one pair per group seen in the image, in the order of the group's first feature; the
+    feature is the last one with that first feature's COLMAP point id.  An image without a kept point has a [2, 0] matrix."""
+    dev, pairs, offsets, num, _, _ = _assign_device(result, images, features, image_names)
+    h = pairs[:, :int(offsets[-1])].cpu().numpy()
+    return [h[:, offsets[f]:offsets[f + 1]].copy() for f in range(len(num))], num
+
+
+def _chunks(bounds: np.ndarray, limit: int):
+    """Runs of consecutive images whose text bounds sum to at most ``limit`` bytes."""
+    out, start, total = [], 0, 0
+    for i, b in enumerate(bounds):
+        if b > limit:
+            raise ValueError(f"save_anno_2d: one image's text may take {int(b)} bytes, above max_chunk_bytes = {limit}")
+        if total + b > limit:
+            out.append((start, i))
+            start, total = i, 0
+        total += int(b)
+    out.append((start, len(bounds)))
+    return out
+
+
+def save_anno_2d(anno_dir, img_paths, result: dict, images, features, image_names=None, detection: str = "superpoint",
+                 max_chunk_bytes: int = ANNO2D_CHUNK_BYTES) -> list:
+    """save_2d_anno (feature_process.py:233-294) on the device: for every image with a pair, ``anno_<detection>/<name>.json``
+    beside the image's directory (<dirname(dirname(img_path))>/anno_<detection>/, .png -> .json), byte for byte as json.dump
+    writes {"keypoints2d", "descriptors2d", "scores2d", "assign_matrix", "num_matches"}; then ``<anno_dir>/anno_2d.json``, the
+    list of {"anno_id", "anno_file", "img_file", "pose_file"} (/color/ -> /poses_ba/, .png -> .txt) over the written images.
+
+    img_paths     the images' paths in the features' order (run.py's img_lists)
+    features      forward_padded's dict: keypoints [F, cap, 2], scores [F, cap], descriptors [F, D, cap] (fp32, CUDA)
+    max_chunk_bytes   the bound of the device text buffer: the images go in chunks whose text fits it, one host read each
+
+    Returns the index list that anno_2d.json holds."""
+    img_paths = [str(p) for p in img_paths]
+    dev, pairs, offsets, num, n_obs, cap = _assign_device(result, images, features, image_names)
+    F = len(num)
+    if len(img_paths) != F:
+        raise ValueError(f"save_anno_2d: {len(img_paths)} image paths for {F} images")
+    sc, de = _device_features(features, F)
+    kp = features.get("keypoints")
+    if not isinstance(kp, torch.Tensor) or kp.device != sc.device or kp.dtype != torch.float32 or tuple(kp.shape) != (F, cap, 2):
+        raise ValueError(f"save_anno_2d: features['keypoints'] must be a CUDA fp32 tensor [{F}, {cap}, 2] on the scores' device")
+    kp = kp.contiguous()
+    D = int(de.shape[1])
+    written = np.nonzero(num > 0)[0]
+    items = 3 * n_obs[written] + D * n_obs[written] + 2 * num[written] + 1
+    files = []
+    for f in written:
+        p = img_paths[f]
+        d = os.path.join(os.path.dirname(os.path.dirname(p)), f"anno_{detection}")
+        os.makedirs(d, exist_ok=True)
+        files.append(os.path.join(d, os.path.basename(p).replace(".png", ".json")))
+    if int(max_chunk_bytes) <= 0:
+        raise ValueError(f"save_anno_2d: max_chunk_bytes must be > 0, got {max_chunk_bytes}")
+    with torch.cuda.device(dev):
+        for c0, c1 in (_chunks(_ITEM_BOUND * items + _OBJECT_BOUND, int(max_chunk_bytes)) if written.size else []):
+            Fc = c1 - c0
+            w = written[c0:c1]
+            desc = np.stack([w, n_obs[w], num[w], offsets[w]], axis=1).astype(np.int64)
+            item_off = np.concatenate([[0], np.cumsum(items[c0:c1])]).astype(np.int64)
+            up = lambda a: torch.from_numpy(np.ascontiguousarray(a)).pin_memory().to(dev, non_blocking=True)  # noqa: E731
+            d_desc, d_item_off = up(desc), up(item_off)
+            n_items, max_items = int(item_off[-1]), int(items[c0:c1].max())
+            ws = _ws(dev, "opb_anno2d_text_workspace_bytes", Fc, n_items)
+            text_off = torch.empty(Fc + 1, dtype=torch.int64, device=dev)
+            _lib.call(dev, "opb_anno2d_text_lengths", d_desc, d_item_off, Fc, n_items, max_items, D, cap, kp, de, sc, pairs, F * cap, ws,
+                      ws.numel(), text_off)
+            t = text_off.cpu().numpy()                                   # the chunk's one synchronisation
+            text = torch.empty(max(int(t[-1]), 1), dtype=torch.uint8, device=dev)
+            _lib.call(dev, "opb_anno2d_text_write", d_desc, d_item_off, Fc, max_items, D, cap, kp, de, sc, pairs, F * cap, ws, text_off,
+                      text)
+            host = torch.empty(text.numel(), dtype=torch.uint8, pin_memory=True)
+            host.copy_(text, non_blocking=True)
+            torch.cuda.current_stream(dev).synchronize()
+            buf = memoryview(host.numpy())
+            for i in range(Fc):
+                with open(files[c0 + i], "wb") as fh:
+                    fh.write(buf[t[i]:t[i + 1]])
+    annotations = [{"anno_id": i + 1, "anno_file": files[i], "img_file": img_paths[f],
+                    "pose_file": img_paths[f].replace("/color/", "/poses_ba/").replace(".png", ".txt")} for i, f in enumerate(written)]
+    os.makedirs(anno_dir, exist_ok=True)
+    with open(os.path.join(anno_dir, "anno_2d.json"), "w") as fh:
+        json.dump(annotations, fh)
+    return annotations
