@@ -657,6 +657,28 @@ int opb_anno2d_text_write(const int64_t* images, const int64_t* item_off, int32_
                           const float* keypoints, const float* descriptors, const float* scores, const int64_t* pairs, int64_t pair_stride,
                           const void* workspace, const int64_t* offsets, char* out, void* stream);
 
+/* ---- PNG files of camera frames and crops (csrc/png.cu) ----
+ * The bytes cv2.imencode('.png', frame) (OpenCV 4.13's default call) writes for 8-bit frames, as parse_scanned_data.py's
+ * cv2.imwrite of color/ and color_full/ does (:173, :177, :264-273): SUB-filtered rows (NONE when W = 1), zlib 1.3's level 1
+ * Z_RLE deflate at memLevel 8 with libpng's window and header, IDAT chunks of 8192 bytes with their CRC-32, no ancillary
+ * chunks.  The model is tests/png_reference.py and DESIGN §5.15 states the rules.
+ *
+ * opb_png_encode: F frames of one shape in one call, on the caller's stream, with no allocation and no host synchronisation.
+ *   frames     device uint8 [F, H, W, C], C = 1 (grey), 3 (BGR) or 4 (BGRA) in cv2's channel order; frame f starts at frames +
+ *              f * frame_pitch, its row y at + y * row_pitch (bytes; row_pitch >= W * C; frame_pitch 0, one frame for all F, or
+ *              >= H * row_pitch).  F <= OPB_PNG_MAX_FRAMES, H * (1 + W * C) <= 2^28.
+ *   workspace  device, 256-byte aligned, at least opb_png_workspace_bytes(F, H, W, C); its contents on entry do not matter
+ *   out        device uint8 [F, out_pitch]: frame f's file at out + f * out_pitch, out_pitch >= opb_png_frame_bytes(H, W, C)
+ *              (zlib's deflateBound of the H * (1 + W * C) filtered bytes, 12 bytes per IDAT chunk and 45 for the signature,
+ *              IHDR and IEND); bytes past a file's size are not written
+ *   sizes      device int64 [F] out: each file's size in bytes, or -1 for a file that would not fit its slot (nothing of it is
+ *              then written) */
+#define OPB_PNG_MAX_FRAMES 65535
+int opb_png_workspace_bytes(int32_t F, int32_t H, int32_t W, int32_t C, int64_t* bytes);
+int opb_png_frame_bytes(int32_t H, int32_t W, int32_t C, int64_t* bytes);
+int opb_png_encode(const uint8_t* frames, int64_t frame_pitch, int64_t row_pitch, int32_t F, int32_t H, int32_t W, int32_t C,
+                   void* workspace, int64_t workspace_bytes, uint8_t* out, int64_t out_pitch, int64_t* sizes, void* stream);
+
 /* ---- the tracker's flow-only state machine (csrc/track.cu) ----
  * BATracker's per-frame logic around flow_track in the live demo's order (inference_demo.py:253-299, track_interval 5) with
  * track(frame, flow_track_only=True): update_kf's gate, add_kf's first pose, motion_prediction and track()'s choice of the
