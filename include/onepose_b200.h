@@ -679,6 +679,44 @@ int opb_png_frame_bytes(int32_t H, int32_t W, int32_t C, int64_t* bytes);
 int opb_png_encode(const uint8_t* frames, int64_t frame_pitch, int64_t row_pitch, int32_t F, int32_t H, int32_t W, int32_t C,
                    void* workspace, int64_t workspace_bytes, uint8_t* out, int64_t out_pitch, int64_t* sizes, void* stream);
 
+/* ---- PNG files read as cv2.imread / cv2.imdecode read them (csrc/png_decode.cu) ----
+ * Every stage of the reference reads its frames and crops with cv2.imread: NormalizedDataset (src/datasets/
+ * normalized_dataset.py:25-34) and the SfM feature extraction with IMREAD_GRAYSCALE, the detector's views and queries
+ * (local_feature_2D_detector.py:155, :173), data_utils.read_gray_scale.  opb_png_decode gives OpenCV 4.13's pixels (libpng 1.6,
+ * zlib 1.3) for 8-bit grey (colour type 0), RGB (2) and RGBA (6) files that are not interlaced: any zlib stream (stored, fixed
+ * and dynamic blocks, any window) in any split into IDAT chunks, every row filter.  DESIGN §5.16 states the rules and the model
+ * is tests/png_decode_reference.py.
+ *
+ * F files of one width and height in one call, on the caller's stream, with no allocation and no host synchronisation.
+ *   data       device bytes of the files back to back; file f is data[offsets[f] .. offsets[f + 1])
+ *   offsets    device int64 [F + 1], non-decreasing from 0, offsets[F] <= the total_bytes the workspace was sized for (a file
+ *              outside it reports OPB_PNG_NOT_PNG; offsets that decrease anywhere make every file report OPB_PNG_NOT_PNG)
+ *   F, H, W    F <= OPB_PNG_MAX_FRAMES, H * (1 + 4 W) <= 2^28; every file's IHDR must give W x H
+ *   mode       OPB_PNG_READ_GREY: IMREAD_GRAYSCALE, uint8 [H, W] pixels (a grey file's own, else
+ *              (9797 R + 19234 G + 3737 B) >> 15 with alpha ignored, as opb_grey_frames);
+ *              OPB_PNG_READ_BGR: IMREAD_COLOR, uint8 [H, W, 3] BGR (grey replicated, alpha dropped)
+ *   workspace  device, 256-byte aligned, at least opb_png_decode_workspace_bytes(F, H, W, total_bytes); contents on entry do
+ *              not matter
+ *   out        device: file f's pixel (y, x) at out + f * out_frame_pitch + y * out_row_pitch + x * (1 or 3) (out_row_pitch >=
+ *              W * (1 or 3), out_frame_pitch >= H * out_row_pitch when F > 1)
+ *   image      NULL, or with OPB_PNG_READ_GREY device fp32 [F, 1, H, W] (dense): grey / 255 as a float32 division
+ *   status     device int32 [F] out: OPB_PNG_* below.  A file whose status is not OPB_PNG_OK has none of its out / image
+ *              pixels written; cv2.imdecode returns None for every such file, and an image for every OPB_PNG_OK file.
+ * Statuses: OPB_PNG_NOT_PNG (signature, chunk structure, order or an unhandled critical chunk), OPB_PNG_BAD_CRC (a critical
+ * chunk's CRC-32; an ancillary chunk's is only a warning), OPB_PNG_UNSUPPORTED (another bit depth, colour type, interlace, or
+ * a colour file read grey with gAMA != 1.0, sRGB or iCCP, where libpng converts in linear light), OPB_PNG_BAD_SHAPE (IHDR is not
+ * W x H), OPB_PNG_BAD_DEFLATE (what zlib rejects), OPB_PNG_BAD_ADLER, OPB_PNG_TOO_LITTLE_DATA (the stream ends before the
+ * last row), OPB_PNG_BAD_FILTER (a row filter byte > 4). */
+enum { OPB_PNG_READ_GREY = 0, OPB_PNG_READ_BGR = 1 };
+enum {
+  OPB_PNG_OK = 0, OPB_PNG_NOT_PNG = 1, OPB_PNG_BAD_CRC = 2, OPB_PNG_UNSUPPORTED = 3, OPB_PNG_BAD_SHAPE = 4, OPB_PNG_BAD_DEFLATE = 5,
+  OPB_PNG_BAD_ADLER = 6, OPB_PNG_TOO_LITTLE_DATA = 7, OPB_PNG_BAD_FILTER = 8
+};
+int opb_png_decode_workspace_bytes(int32_t F, int32_t H, int32_t W, int64_t total_bytes, int64_t* bytes);
+int opb_png_decode(const uint8_t* data, const int64_t* offsets, int32_t F, int32_t H, int32_t W, int32_t mode, void* workspace,
+                   int64_t workspace_bytes, uint8_t* out, int64_t out_frame_pitch, int64_t out_row_pitch, float* image,
+                   int32_t* status, void* stream);
+
 /* ---- the tracker's flow-only state machine (csrc/track.cu) ----
  * BATracker's per-frame logic around flow_track in the live demo's order (inference_demo.py:253-299, track_interval 5) with
  * track(frame, flow_track_only=True): update_kf's gate, add_kf's first pose, motion_prediction and track()'s choice of the

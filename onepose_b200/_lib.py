@@ -144,6 +144,8 @@ SYMBOLS = {
     "opb_png_workspace_bytes": (C.c_int, [_I, _I, _I, _I, C.POINTER(C.c_int64)]),
     "opb_png_frame_bytes": (C.c_int, [_I, _I, _I, C.POINTER(C.c_int64)]),
     "opb_png_encode": (C.c_int, [_P, C.c_int64, C.c_int64, _I, _I, _I, _I, _P, C.c_int64, _P, C.c_int64, _P, _P]),
+    "opb_png_decode_workspace_bytes": (C.c_int, [_I, _I, _I, C.c_int64, C.POINTER(C.c_int64)]),
+    "opb_png_decode": (C.c_int, [_P, _P, _I, _I, _I, _I, _P, C.c_int64, _P, C.c_int64, C.c_int64, _P, _P, _P]),
     "opb_debug_set_pdl": (C.c_int, [_I]),
     "opb_debug_set_ws_fill": (C.c_int, [_I]),
     "opb_debug_set_kv_passes": (C.c_int, [_P, _I]),

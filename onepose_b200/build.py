@@ -14,7 +14,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libonepose_b200.so")
-SOURCES = ["api.cu", "crop.cu", "detect.cu", "flow.cu", "frames.cu", "gemm_simt.cu", "gemm_tc.cu", "json_text.cu", "kv_state_tc.cu", "png.cu", "pnp_ransac.cu", "scan.cu", "sfm.cu", "superpoint.cu", "track.cu"]
+SOURCES = ["api.cu", "crop.cu", "detect.cu", "flow.cu", "frames.cu", "gemm_simt.cu", "gemm_tc.cu", "json_text.cu", "kv_state_tc.cu", "png.cu", "png_decode.cu", "pnp_ransac.cu", "scan.cu", "sfm.cu", "superpoint.cu", "track.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-shared",

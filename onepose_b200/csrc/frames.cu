@@ -15,6 +15,7 @@
 #include <stdint.h>
 
 #include "../../include/onepose_b200.h"
+#include "grey.cuh"
 #include "host_util.cuh"
 
 namespace opb {
@@ -24,11 +25,6 @@ constexpr int kMaxSide = 32767;      // the crop's bounds (crop.cu): the frames 
 constexpr int kMaxFrames = 65535;
 constexpr int kThreads = 256;
 constexpr int kGroup = 4;            // pixels per thread
-
-__device__ __forceinline__ uint32_t grey_of(uint32_t c0, uint32_t c1, uint32_t c2, bool red_first) {
-  const uint32_t r = red_first ? c0 : c2, b = red_first ? c2 : c0;
-  return (9797u * r + 19234u * c1 + 3737u * b) >> 15;
-}
 
 // Frame blockIdx.y; thread -> (row, group of kGroup pixels).  C channels per pixel, red first (RGB / RGBA) or third (BGR / BGRA).
 template <int C>

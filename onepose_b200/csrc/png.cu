@@ -20,6 +20,7 @@
 
 #include "../../include/onepose_b200.h"
 #include "host_util.cuh"
+#include "png_common.cuh"
 
 namespace opb {
 namespace {
@@ -120,49 +121,6 @@ __device__ __forceinline__ uint8_t filtered_byte(const Args& a, const uint8_t* s
   const uint8_t* p = src + y * a.row_pitch + (int64_t)x * a.C + sc;
   return a.W > 1 && x > 0 ? (uint8_t)(p[0] - p[-a.C]) : p[0];
 }
-
-template <typename T, typename Op>
-__device__ T block_reduce(T v, Op op, T* sh) {                // every thread gets the result; sh holds 32 values
-  for (int d = 16; d; d >>= 1) v = op(v, __shfl_xor_sync(0xffffffffu, v, d));
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  __syncthreads();
-  if (lane == 0) sh[warp] = v;
-  __syncthreads();
-  v = sh[0];
-  for (int w = 1; w < nw; ++w) v = op(v, sh[w]);
-  return v;
-}
-
-// Exclusive scan of v over the block in thread order, or from the last thread when reverse; *total gets the whole.  Every
-// thread calls it; blockDim.x is a multiple of 32 and sh holds 32 values.
-template <typename T, typename Op>
-__device__ T block_scan(T v, Op op, T identity, T* sh, T* total, bool reverse = false) {
-  const int nw = blockDim.x >> 5;
-  const int r = reverse ? blockDim.x - 1 - threadIdx.x : threadIdx.x;   // rank in scan order
-  const int lane = r & 31, warp = r >> 5;
-  T inc = v;
-  for (int d = 1; d < 32; d <<= 1) {
-    const T u = reverse ? __shfl_down_sync(0xffffffffu, inc, d) : __shfl_up_sync(0xffffffffu, inc, d);
-    if (lane >= d) inc = op(inc, u);
-  }
-  T exc = reverse ? __shfl_down_sync(0xffffffffu, inc, 1) : __shfl_up_sync(0xffffffffu, inc, 1);
-  if (lane == 0) exc = identity;
-  __syncthreads();
-  if (lane == 31) sh[warp] = inc;
-  __syncthreads();
-  T carry = identity, all = identity;
-  for (int w = 0; w < nw; ++w) {
-    if (w < warp) carry = op(carry, sh[w]);
-    all = op(all, sh[w]);
-  }
-  if (total) *total = all;
-  return op(carry, exc);
-}
-
-struct Max { __device__ int32_t operator()(int32_t a, int32_t b) const { return a > b ? a : b; } };
-struct Min { __device__ int32_t operator()(int32_t a, int32_t b) const { return a < b ? a : b; } };
-struct Sum32 { __device__ int32_t operator()(int32_t a, int32_t b) const { return a + b; } };
-struct Sum64 { __device__ unsigned long long operator()(unsigned long long a, unsigned long long b) const { return a + b; } };
 
 __global__ void __launch_bounds__(kTileThreads) png_filter_kernel(Args a) {
   __shared__ unsigned long long sh64[32];
@@ -613,8 +571,7 @@ __global__ void png_offsets_kernel(Args a, int F, int64_t out_pitch, int64_t* si
   }
   or_byte(z, 0, cmf);
   or_byte(z, 1, flg);
-  const unsigned long long A = (1 + a.fr[f].s1) % 65521, Bs = ((unsigned long long)a.n % 65521 + a.fr[f].s2 % 65521) % 65521;
-  const unsigned adler = (unsigned)((Bs << 16) | A);
+  const unsigned adler = adler_of_sums(a.fr[f].s1, a.fr[f].s2, a.n);
   for (int i = 0; i < 4; ++i) or_byte(z, zlen - 4 + i, (adler >> (24 - 8 * i)) & 0xff);
 }
 
@@ -687,39 +644,6 @@ __global__ void __launch_bounds__(kPackThreads) png_pack_kernel(Args a) {
   if (threadIdx.x == 0) or_bits(z, off + 3 + B.hdr_bits + total, lcode[256]);
 }
 
-// ---- CRC-32 (zlib's crc32 and crc32_combine: multmodp / x2nmodp) ----
-
-constexpr uint32_t kPoly = 0xedb88320u;
-__device__ uint32_t multmodp(uint32_t a, uint32_t b) {
-  uint32_t m = 1u << 31, p = 0;
-  for (;;) {
-    if (a & m) {
-      p ^= b;
-      if ((a & (m - 1)) == 0) break;
-    }
-    m >>= 1;
-    b = b & 1 ? (b >> 1) ^ kPoly : b >> 1;
-  }
-  return p;
-}
-__device__ uint32_t x2nmodp(const uint32_t* x2n, int64_t n, unsigned k) {
-  uint32_t p = 1u << 31;
-  while (n) {
-    if (n & 1) p = multmodp(x2n[k & 31], p);
-    n >>= 1;
-    ++k;
-  }
-  return p;
-}
-__device__ uint32_t crc_bytes(const uint32_t* table, uint32_t crc, const uint8_t* p, int64_t n) {
-  crc = ~crc;
-  for (int64_t i = 0; i < n; ++i) crc = table[(crc ^ p[i]) & 0xff] ^ (crc >> 8);
-  return ~crc;
-}
-__device__ __forceinline__ void put_be32(uint8_t* p, uint32_t v) {
-  p[0] = (uint8_t)(v >> 24), p[1] = (uint8_t)(v >> 16), p[2] = (uint8_t)(v >> 8), p[3] = (uint8_t)v;
-}
-
 // One warp per IDAT chunk of each frame: its length, type, bytes and CRC; chunk 0 adds signature and IHDR, the last IEND.
 __global__ void __launch_bounds__(32) png_frame_kernel(Args a, uint8_t* out, int64_t out_pitch) {
   __shared__ uint32_t table[256], x2n[32];
@@ -729,17 +653,7 @@ __global__ void __launch_bounds__(32) png_frame_kernel(Args a, uint8_t* out, int
   if (zlen < 0) return;
   const int64_t nchunks = (zlen + kChunk - 1) / kChunk;
   if (c >= nchunks) return;
-  for (int i = lane; i < 256; i += 32) {
-    uint32_t v = (uint32_t)i;
-    for (int b = 0; b < 8; ++b) v = v & 1 ? (v >> 1) ^ kPoly : v >> 1;
-    table[i] = v;
-  }
-  if (lane == 0) {
-    uint32_t p = 1u << 30;                 // x^1
-    x2n[0] = p;
-    for (int n = 1; n < 32; ++n) x2n[n] = p = multmodp(p, p);
-  }
-  __syncwarp();
+  crc_tables(table, x2n, lane);
   uint8_t* o = out + f * out_pitch;
   const uint8_t* z = a.zbuf + f * a.zcap + (int64_t)c * kChunk;
   const int64_t left = zlen - (int64_t)c * kChunk;
@@ -751,17 +665,8 @@ __global__ void __launch_bounds__(32) png_frame_kernel(Args a, uint8_t* out, int
     ch[4] = 'I', ch[5] = 'D', ch[6] = 'A', ch[7] = 'T';
   }
   __syncwarp();
-  // lane l: CRC of bytes [l * seg, (l + 1) * seg) of type + data, joined in order by crc32_combine
-  const int total = len + 4, seg = (total + 31) / 32;
-  const int b0 = min(total, lane * seg), b1 = min(total, b0 + seg);
-  part[lane] = crc_bytes(table, 0, ch + 4 + b0, b1 - b0);
-  __syncwarp();
+  const uint32_t crc = warp_crc(table, x2n, part, ch + 4, len + 4, lane);
   if (lane == 0) {
-    uint32_t crc = part[0];
-    for (int l = 1; l < 32; ++l) {
-      const int n = min(total, (l + 1) * seg) - min(total, l * seg);
-      if (n > 0) crc = multmodp(x2nmodp(x2n, n, 3), crc) ^ part[l];
-    }
     put_be32(ch + 8 + len, crc);
     if (c == 0) {
       const uint8_t sig[8] = {0x89, 'P', 'N', 'G', '\r', '\n', 0x1a, '\n'};
