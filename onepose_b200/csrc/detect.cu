@@ -28,6 +28,7 @@
 #include <stdint.h>
 
 #include "../../include/onepose_b200.h"
+#include "block.cuh"
 #include "cv_rng.cuh"
 #include "host_util.cuh"
 
@@ -519,22 +520,16 @@ __device__ __forceinline__ void boxes_block(int b, const float* __restrict__ ref
     const int i = i0 + tid;
     const long long m = i < nr ? match(win, i) : -1;
     const bool f = m >= 0 && m < nq;
-    const unsigned bal = __ballot_sync(0xffffffffu, f);
-    if (lane == 0) warp_n[warp] = __popc(bal);
-    __syncthreads();
-    int off = n, total = 0;
-    for (int w = 0; w < kAffWarps; ++w) {
-      off += w < warp ? warp_n[w] : 0;
-      total += warp_n[w];
-    }
+    int total;
+    const int off = n + block_rank(f, warp_n, &total);
     if (f) {
       const float* r = ref_kp + ((size_t)win * cap_ref + i) * 2;
       const float* p = q_kp + ((size_t)q * cap_q + m) * 2;
-      pairs[off + __popc(bal & ((1u << lane) - 1u))] = make_float4(r[0], r[1], p[0], p[1]);
+      pairs[off] = make_float4(r[0], r[1], p[0], p[1]);
     }
     n += total;
-    __syncthreads();
   }
+  // affine_ransac passes a barrier before it reads pairs
   affine_ransac(SharedPairs{pairs}, n, prm, tr.at(b), sh, nullptr);
   if (tid != 0) return;
   for (int k = 0; k < 6; ++k) affine[(size_t)b * 6 + k] = sh.H[k];

@@ -16,6 +16,7 @@
 #include <stdint.h>
 
 #include "../../include/onepose_b200.h"
+#include "block.cuh"
 #include "host_util.cuh"
 
 namespace opb {
@@ -366,29 +367,20 @@ __global__ void __launch_bounds__(kCompactThreads) compact_kernel(const uint8_t*
                                                                   const float* __restrict__ pts3d, const int32_t* __restrict__ counts, int B, int cap,
                                                                   double* __restrict__ out2d, double* __restrict__ out3d, int32_t* __restrict__ offsets,
                                                                   int32_t* __restrict__ n_tracked, float* __restrict__ pad2d, float* __restrict__ pad3d) {
-  __shared__ int warp_tot[kCompactThreads / 32];
-  __shared__ int base_s;
-  const int t = threadIdx.x, lane = t & 31, wid = t >> 5;
-  if (t == 0) base_s = 0;
-  __syncthreads();
+  __shared__ int sh[kCompactThreads / 32];
+  const int t = threadIdx.x;
+  int base = 0;
   for (int b = 0; b < B; ++b) {
     const int n = min(max(counts[b], 0), cap);
-    const int start = base_s;
+    const int start = base;
     if (t == 0) offsets[b] = start;
     for (int c = 0; c < n; c += kCompactThreads) {
       const int r = c + t;
       const size_t row = (size_t)b * cap + r;
       const bool keep = r < n && status[row] == 1;
-      const unsigned m = __ballot_sync(0xffffffffu, keep);
-      if (lane == 0) warp_tot[wid] = __popc(m);
-      __syncthreads();
-      int before = 0, all = 0;
-      for (int w = 0; w < kCompactThreads / 32; ++w) {
-        before += w < wid ? warp_tot[w] : 0;
-        all += warp_tot[w];
-      }
+      int total;
+      const int rank = base - start + block_rank(keep, sh, &total);
       if (keep) {
-        const int rank = base_s - start + before + __popc(m & ((1u << lane) - 1));
         const size_t o = (size_t)start + rank, q = (size_t)b * cap + rank;
         for (int k = 0; k < 2; ++k) {
           out2d[2 * o + k] = pts2d[2 * row + k];
@@ -399,20 +391,17 @@ __global__ void __launch_bounds__(kCompactThreads) compact_kernel(const uint8_t*
           pad3d[3 * q + k] = pts3d[3 * row + k];
         }
       }
-      __syncthreads();
-      if (t == 0) base_s += all;
-      __syncthreads();
+      base += total;
     }
-    const int kept = base_s - start;
+    const int kept = base - start;
     for (int r = kept + t; r < cap; r += kCompactThreads) {
       const size_t q = (size_t)b * cap + r;
       for (int k = 0; k < 2; ++k) pad2d[2 * q + k] = 0.f;
       for (int k = 0; k < 3; ++k) pad3d[3 * q + k] = 0.f;
     }
     if (t == 0) n_tracked[b] = kept;
-    __syncthreads();
   }
-  if (t == 0) offsets[B] = base_s;
+  if (t == 0) offsets[B] = base;
 }
 
 // One thread per track: tracking_utils.project(pts3d, K, pose) -- X R^T + t, then K, then x / z -- and the mean distance to

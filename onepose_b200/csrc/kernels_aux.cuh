@@ -5,6 +5,7 @@
 // griddep_sync() (programmatic dependent launch, see common.cuh).  split_planes, join_planes and the adjacent producers
 // (exclusive_scan_i64, segmented_mean*, gather_*) do not: they are launched without PDL.
 #pragma once
+#include "block.cuh"
 #include "common.cuh"
 #include "gemm_tc.cuh"
 #include "host_util.cuh"
@@ -588,21 +589,13 @@ __global__ void conf_fill_tail(float* __restrict__ conf, long long rows, int ld,
 // ---------------------------------------------------------------------------------------
 // Exclusive prefix sum of the track lengths: one block, each thread scans a contiguous chunk, then a block scan of the chunk sums.
 __global__ void __launch_bounds__(1024) exclusive_scan_i64(const long long* __restrict__ in, long long* __restrict__ out, int n) {
-  __shared__ long long sums[1024];
+  __shared__ long long sh[32];
   const int t = threadIdx.x;
   const int per = (n + 1023) / 1024;
   const int lo = min(t * per, n), hi = min(lo + per, n);
-  long long acc = 0;
+  long long acc = 0, total;
   for (int i = lo; i < hi; ++i) acc += in[i];
-  sums[t] = acc;
-  __syncthreads();
-  for (int off = 1; off < 1024; off <<= 1) {
-    const long long v = t >= off ? sums[t - off] : 0;
-    __syncthreads();
-    sums[t] += v;
-    __syncthreads();
-  }
-  long long run = t ? sums[t - 1] : 0;
+  long long run = block_scan(acc, SumS64(), 0ll, sh, &total);
   for (int i = lo; i < hi; ++i) { out[i] = run; run += in[i]; }
 }
 

@@ -632,9 +632,8 @@ __global__ void __launch_bounds__(kPackThreads) png_pack_kernel(Args a) {
     code_of(tok[i], nb);
     mine += nb;
   }
-  struct S64 { __device__ int64_t operator()(int64_t x, int64_t y) const { return x + y; } };
   int64_t total;
-  int64_t pos = off + 3 + B.hdr_bits + block_scan(mine, S64(), (int64_t)0, sh, &total);
+  int64_t pos = off + 3 + B.hdr_bits + block_scan(mine, SumS64(), (int64_t)0, sh, &total);
   for (int32_t i = my0; i < my1; ++i) {
     int nb;
     const unsigned long long v = code_of(tok[i], nb);

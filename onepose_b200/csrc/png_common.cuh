@@ -1,53 +1,12 @@
-// Pieces the PNG writer (png.cu) and reader (png_decode.cu) share: block-wide reductions and scans, zlib's CRC-32 with
-// crc32_combine (multmodp / x2nmodp) and a warp's CRC of one chunk, and Adler-32 from its two sums.
+// Pieces the PNG writer (png.cu) and reader (png_decode.cu) share: zlib's CRC-32 with crc32_combine (multmodp / x2nmodp) and a
+// warp's CRC of one chunk, and Adler-32 from its two sums.  Both also use the block-wide scans of block.cuh.
 #pragma once
 #include <stdint.h>
 
+#include "block.cuh"
+
 namespace opb {
 namespace {
-
-template <typename T, typename Op>
-__device__ T block_reduce(T v, Op op, T* sh) {                // every thread gets the result; sh holds 32 values
-  for (int d = 16; d; d >>= 1) v = op(v, __shfl_xor_sync(0xffffffffu, v, d));
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nw = blockDim.x >> 5;
-  __syncthreads();
-  if (lane == 0) sh[warp] = v;
-  __syncthreads();
-  v = sh[0];
-  for (int w = 1; w < nw; ++w) v = op(v, sh[w]);
-  return v;
-}
-
-// Exclusive scan of v over the block in thread order, or from the last thread when reverse; *total gets the whole.  Every
-// thread calls it; blockDim.x is a multiple of 32 and sh holds 32 values.
-template <typename T, typename Op>
-__device__ T block_scan(T v, Op op, T identity, T* sh, T* total, bool reverse = false) {
-  const int nw = blockDim.x >> 5;
-  const int r = reverse ? blockDim.x - 1 - threadIdx.x : threadIdx.x;   // rank in scan order
-  const int lane = r & 31, warp = r >> 5;
-  T inc = v;
-  for (int d = 1; d < 32; d <<= 1) {
-    const T u = reverse ? __shfl_down_sync(0xffffffffu, inc, d) : __shfl_up_sync(0xffffffffu, inc, d);
-    if (lane >= d) inc = op(inc, u);
-  }
-  T exc = reverse ? __shfl_down_sync(0xffffffffu, inc, 1) : __shfl_up_sync(0xffffffffu, inc, 1);
-  if (lane == 0) exc = identity;
-  __syncthreads();
-  if (lane == 31) sh[warp] = inc;
-  __syncthreads();
-  T carry = identity, all = identity;
-  for (int w = 0; w < nw; ++w) {
-    if (w < warp) carry = op(carry, sh[w]);
-    all = op(all, sh[w]);
-  }
-  if (total) *total = all;
-  return op(carry, exc);
-}
-
-struct Max { __device__ int32_t operator()(int32_t a, int32_t b) const { return a > b ? a : b; } };
-struct Min { __device__ int32_t operator()(int32_t a, int32_t b) const { return a < b ? a : b; } };
-struct Sum32 { __device__ int32_t operator()(int32_t a, int32_t b) const { return a + b; } };
-struct Sum64 { __device__ unsigned long long operator()(unsigned long long a, unsigned long long b) const { return a + b; } };
 
 // ---- CRC-32 (zlib's crc32 and crc32_combine: multmodp / x2nmodp) ----
 

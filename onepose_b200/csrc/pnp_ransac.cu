@@ -19,6 +19,7 @@
 #include <stdint.h>
 
 #include "../../include/onepose_b200.h"
+#include "block.cuh"
 #include "cv_rng.cuh"
 #include "host_util.cuh"
 
@@ -361,17 +362,6 @@ __device__ int best_hypothesis(const double* __restrict__ hyp, int b, int H, uns
   return (int)(bk >> 32);
 }
 
-// block-wide sum of one int per thread, returned to every thread
-template <int kThreads>
-__device__ __forceinline__ int block_count(int c, int* red /*shared [kThreads / 32]*/) {
-  for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
-  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = c;
-  __syncthreads();
-  int s = 0;
-  for (int w = 0; w < kThreads / 32; ++w) s += red[w];
-  return s;
-}
-
 __device__ __forceinline__ void write_pose(const Pose& T, double* dst) {
   for (int r = 0; r < 3; ++r) {
     for (int k = 0; k < 3; ++k) dst[r * 4 + k] = T.R[r * 3 + k];
@@ -498,9 +488,9 @@ __global__ void __launch_bounds__(kRefineThreads) pnp_select_refine(const double
       inlier_mask[f.o0 + i] = in;
       cnt += in;
     }
-    cnt = block_count<kRefineThreads>(cnt, cnt_w);
+    cnt = block_reduce(cnt, Sum32(), cnt_w);
     if (cnt >= 4) break;
-    __syncthreads();                                 // every thread has read T and cnt_w
+    __syncthreads();                                 // every thread has read T
     if (tid == 0) T = load_record(hyp + ((size_t)b * H + best_h) * kHypStride);
     __syncthreads();
   }
@@ -1281,7 +1271,7 @@ __global__ void __launch_bounds__(kGatherThreads) gather_count(const int64_t* __
   const int64_t* m0 = matches0 + (size_t)b * N;
   int cnt = 0;
   for (int n = tid; n < N; n += kGatherThreads) cnt += is_match(m0[n], M) ? 1 : 0;
-  cnt = block_count<kGatherThreads>(cnt, cnt_w);
+  cnt = block_reduce(cnt, Sum32(), cnt_w);
   if (tid == 0) {
     offsets[b + 1] = cnt;
     if (b == 0) offsets[0] = 0;
@@ -1291,34 +1281,15 @@ __global__ void __launch_bounds__(kGatherThreads) gather_count(const int64_t* __
 // one block: inclusive scan of offsets[1..B] in place (offsets[0] = 0), tiles of 1024 with a running carry
 constexpr int kScanThreads = 1024;
 __global__ void __launch_bounds__(kScanThreads) gather_scan(int B, int* __restrict__ offsets) {
-  __shared__ int warp_sum[kScanThreads / 32];
-  __shared__ int carry;
-  const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
-  if (tid == 0) carry = 0;
+  __shared__ int sh[kScanThreads / 32];
+  int carry = 0;
   for (int base = 0; base < B; base += kScanThreads) {
-    const int i = base + tid;
-    int v = i < B ? offsets[i + 1] : 0;
-    for (int o = 1; o < 32; o <<= 1) {
-      const int u = __shfl_up_sync(0xffffffffu, v, o);
-      if (lane >= o) v += u;
-    }
-    if (lane == 31) warp_sum[warp] = v;
-    __syncthreads();
-    if (warp == 0) {
-      int s = warp_sum[lane];
-      for (int o = 1; o < 32; o <<= 1) {
-        const int u = __shfl_up_sync(0xffffffffu, s, o);
-        if (lane >= o) s += u;
-      }
-      warp_sum[lane] = s;                            // inclusive prefix over warps
-    }
-    __syncthreads();
-    const int c = carry;
-    v += c + (warp > 0 ? warp_sum[warp - 1] : 0);
-    if (i < B) offsets[i + 1] = v;
-    __syncthreads();                                 // every thread has read carry and warp_sum
-    if (tid == kScanThreads - 1) carry = v;
-    __syncthreads();
+    const int i = base + (int)threadIdx.x;
+    const int v = i < B ? offsets[i + 1] : 0;
+    int total;
+    const int exc = block_scan(v, Sum32(), 0, sh, &total);
+    if (i < B) offsets[i + 1] = carry + exc + v;
+    carry += total;
   }
 }
 
@@ -1328,8 +1299,8 @@ __global__ void __launch_bounds__(kGatherThreads) gather_compact(const int64_t* 
                                                                  const int* __restrict__ kp3_first, const int* __restrict__ kp3_count,
                                                                  const int* __restrict__ offsets, double* __restrict__ pts2d, double* __restrict__ pts3d,
                                                                  float* __restrict__ mconf, int* __restrict__ query_index) {
-  __shared__ int warp_cnt[kGatherThreads / 32];
-  const int b = blockIdx.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  __shared__ int sh[kGatherThreads / 32];
+  const int b = blockIdx.x, tid = threadIdx.x;
   const int M = frame_kp3_count(kp3_count, b, M_all);
   const float* kp3d = kp3d_all + (kp3_first ? (size_t)kp3_first[b] * 3 : 0);
   const size_t row0 = (size_t)b * N;
@@ -1338,18 +1309,10 @@ __global__ void __launch_bounds__(kGatherThreads) gather_compact(const int64_t* 
     const int n = base + tid;
     const int64_t m = n < N ? matches0[row0 + n] : -1;
     const bool valid = is_match(m, M);
-    const unsigned ballot = __ballot_sync(0xffffffffu, valid);
-    if (lane == 0) warp_cnt[warp] = __popc(ballot);
-    __syncthreads();
-    int before = 0, total = 0;
-#pragma unroll
-    for (int w = 0; w < kGatherThreads / 32; ++w) {
-      const int c = warp_cnt[w];
-      before += w < warp ? c : 0;
-      total += c;
-    }
+    int total;
+    const int rank = block_rank(valid, sh, &total);
     if (valid) {
-      const size_t o = (size_t)(pos + before + __popc(ballot & ((1u << lane) - 1u)));
+      const size_t o = (size_t)(pos + rank);
       const float* k2 = kp2d + (row0 + n) * 2;
       const float* k3 = kp3d + (size_t)m * 3;
       pts2d[o * 2 + 0] = (double)k2[0];
@@ -1361,7 +1324,6 @@ __global__ void __launch_bounds__(kGatherThreads) gather_compact(const int64_t* 
       if (query_index) query_index[o] = n;
     }
     pos += total;
-    __syncthreads();                                 // warp_cnt is rewritten by the next tile
   }
 }
 

@@ -9,6 +9,7 @@
 #include <stdint.h>
 
 #include "../../include/onepose_b200.h"
+#include "block.cuh"
 #include "host_util.cuh"
 
 namespace opb {
@@ -102,26 +103,6 @@ __device__ void corner_extent(const double P[3][4], const double* corners, int n
   }
 }
 
-// Inclusive sum of v over the block (kScanThreads threads); *total gets the block's sum.  Every thread must call it.
-__device__ int block_inclusive_sum(int v, int* total) {
-  __shared__ int warp_sum[kScanThreads / 32];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int d = 1; d < 32; d <<= 1) {
-    const int u = __shfl_up_sync(0xffffffffu, v, d);
-    if (lane >= d) v += u;
-  }
-  if (lane == 31) warp_sum[warp] = v;
-  __syncthreads();
-  int before = 0, all = 0;
-  for (int w = 0; w < kScanThreads / 32; ++w) {
-    before += w < warp ? warp_sum[w] : 0;
-    all += warp_sum[w];
-  }
-  __syncthreads();
-  *total = all;
-  return v + before;
-}
-
 // One block walks the rows in order, kScanThreads at a time: each thread computes its row's pose and the extent of its
 // projected corners, the skip rule decides keep, and a block scan gives each kept row its slot, the number of kept rows before
 // it.  Slots below n_out get the pose, projections, box and source row; slots from the kept count to n_out are cleared.
@@ -130,6 +111,7 @@ __global__ void __launch_bounds__(kScanThreads) scan_poses_kernel(const double* 
                                                                   int n_out, double* __restrict__ pose, double* __restrict__ proj,
                                                                   int32_t* __restrict__ box, int32_t* __restrict__ row_of, int32_t* __restrict__ keep,
                                                                   int32_t* __restrict__ count) {
+  __shared__ int sh[kScanThreads / 32];
   double Tow[16], Kc[9];
   for (int i = 0; i < 16; ++i) Tow[i] = T_ow[i];
   for (int i = 0; i < 9; ++i) Kc[i] = K[i];
@@ -146,7 +128,7 @@ __global__ void __launch_bounds__(kScanThreads) scan_poses_kernel(const double* 
       if (keep) keep[r] = kept ? 1 : 0;
     }
     int total;
-    const int slot = base + block_inclusive_sum(kept ? 1 : 0, &total) - 1;
+    const int slot = base + block_rank(kept, sh, &total);
     if (kept && slot < n_out) {
       double* Po = pose + (size_t)slot * 16;
       for (int rr = 0; rr < 3; ++rr)

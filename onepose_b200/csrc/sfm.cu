@@ -19,6 +19,7 @@
 #include <cub/device/device_radix_sort.cuh>
 
 #include "../../include/onepose_b200.h"
+#include "block.cuh"
 #include "host_util.cuh"
 
 namespace opb {
@@ -37,26 +38,6 @@ __device__ __forceinline__ float dot3(const float* a, const float* b) {
   return __fadd_rn(__fadd_rn(__fmul_rn(a[0], b[0]), __fmul_rn(a[1], b[1])), __fmul_rn(a[2], b[2]));
 }
 
-// Inclusive sum of v over the block (kFilterThreads threads); *total gets the block's sum.  Every thread must call it.
-__device__ int block_inclusive_sum(int v, int* total) {
-  __shared__ int warp_sum[kFilterThreads / 32];
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int d = 1; d < 32; d <<= 1) {
-    const int u = __shfl_up_sync(0xffffffffu, v, d);
-    if (lane >= d) v += u;
-  }
-  if (lane == 31) warp_sum[warp] = v;
-  __syncthreads();
-  int before = 0, all = 0;
-  for (int w = 0; w < kFilterThreads / 32; ++w) {
-    before += w < warp ? warp_sum[w] : 0;
-    all += warp_sum[w];
-  }
-  __syncthreads();
-  *total = all;
-  return v + before;
-}
-
 // One block walks the points in ascending id order.  get_tkl's threshold is the smallest length L present with at most
 // max_num_kp3d points longer than L: the sorted lengths' entry max(P - 1 - max_num_kp3d, 0).  A point is kept when its length
 // is at least that and it lies strictly inside the box; a block scan gives each kept point its slot.
@@ -65,6 +46,7 @@ __global__ void __launch_bounds__(kFilterThreads) filter_kernel(const double* __
                                                                 int k0, const double* __restrict__ corners, int64_t* __restrict__ kept_ids,
                                                                 float* __restrict__ kept_xyz, int64_t* __restrict__ track_length,
                                                                 int64_t* __restrict__ n_kept) {
+  __shared__ int sh[kFilterThreads / 32];
   const int64_t tl = sorted_len[k0];
   float c4[3], v[3][3], vv[3];
   const int axis_corner[3] = {5, 0, 7};                       // v45, v40, v47
@@ -91,7 +73,7 @@ __global__ void __launch_bounds__(kFilterThreads) filter_kernel(const double* __
       }
     }
     int total;
-    const int slot = base + block_inclusive_sum(kept ? 1 : 0, &total) - 1;
+    const int slot = base + block_rank(kept, sh, &total);
     if (kept) {
       kept_ids[slot] = ids[i];
       for (int a = 0; a < 3; ++a) kept_xyz[(size_t)slot * 3 + a] = p[a];

@@ -17,6 +17,7 @@
 #include <vector>
 
 #include "../../include/onepose_b200.h"
+#include "block.cuh"
 #include "common.cuh"
 #include "gemm_common.cuh"
 #include "gemm_tc.cuh"
@@ -261,7 +262,7 @@ __device__ __forceinline__ bool sp_keep(float s, int pix, int H, int W, float th
 }
 
 __global__ void __launch_bounds__(256) sp_count(const float* __restrict__ nms, int H, int W, float thr, int border, int* __restrict__ blk_counts) {
-  __shared__ int wsum[8];
+  __shared__ int sh[8];
   griddep_sync();
   const int b = blockIdx.y, HW = H * W;
   const int p0 = blockIdx.x * kSelChunk + threadIdx.x * 8;
@@ -271,20 +272,13 @@ __global__ void __launch_bounds__(256) sp_count(const float* __restrict__ nms, i
     const int p = p0 + e;
     if (p < HW && sp_keep(nms[(long long)b * HW + p], p, H, W, thr, border)) ++c;
   }
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) c += __shfl_xor_sync(0xffffffffu, c, o);
-  if ((threadIdx.x & 31) == 0) wsum[threadIdx.x >> 5] = c;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    int s = 0;
-    for (int i = 0; i < 8; ++i) s += wsum[i];
-    blk_counts[b * gridDim.x + blockIdx.x] = s;
-  }
+  c = block_reduce(c, Sum32(), sh);
+  if (threadIdx.x == 0) blk_counts[b * gridDim.x + blockIdx.x] = c;
 }
 
 __global__ void __launch_bounds__(256) sp_compact(const float* __restrict__ nms, int H, int W, float thr, int border, const int* __restrict__ blk_counts,
                                                   int* __restrict__ cand_idx, float* __restrict__ cand_score, int* __restrict__ totals) {
-  __shared__ int wsum[8];
+  __shared__ int sh[8];
   __shared__ int base_s;
   griddep_sync();
   const int b = blockIdx.y, HW = H * W;
@@ -304,18 +298,9 @@ __global__ void __launch_bounds__(256) sp_compact(const float* __restrict__ nms,
     sv[e] = p < HW ? nms[(long long)b * HW + p] : 0.f;
     if (p < HW && sp_keep(sv[e], p, H, W, thr, border)) keep |= 1u << e;
   }
-  const int c = __popc(keep);
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  int incl = c;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const int n = __shfl_up_sync(0xffffffffu, incl, o);
-    if (lane >= o) incl += n;
-  }
-  if (lane == 31) wsum[wid] = incl;
-  __syncthreads();
-  int off = base_s + incl - c;
-  for (int i = 0; i < wid; ++i) off += wsum[i];
+  int tot;
+  const int exc = block_scan(__popc(keep), Sum32(), 0, sh, &tot);
+  int off = base_s + exc;                                       // read after the scan's barriers
 #pragma unroll
   for (int e = 0; e < 8; ++e)
     if (keep & (1u << e)) {
