@@ -940,6 +940,14 @@ int opb_debug_kv_state_h(const void* kvh, int32_t frames, int32_t n, int32_t m_p
                          int32_t* n_groups, void* stream);
 /* fp32 [rows, cols] -> fp16-split planes: hi = fp16(64 x), lo = fp16(64 x - hi). */
 int opb_debug_split(const float* x, void* hi, void* lo, size_t n, void* stream);
+/* The block-wide primitives of csrc/block.cuh on their own: one block of `threads` threads (a multiple of 32 in [32, 1024])
+ * walks `tiles` consecutive tiles of `threads` inputs `in` and calls one primitive per tile, always with the same shared
+ * scratch.  prim 0 block_reduce, 1 block_scan (exclusive; reverse = 1: from the last thread), 2 block_rank (`in` as int32
+ * keep flags, nonzero = keep; op 0 only).  op picks the operator and the element type: 0 Sum32, 1 Max, 2 Min (int32),
+ * 3 Sum64 (uint64, wrapping), 4 SumS64 (int64).  value and total [tiles][threads] get, per thread and tile, what that thread
+ * got: the reduction (in both), the exclusive prefix and the scan's total, or the rank and the block's count. */
+int opb_debug_block(int32_t prim, int32_t op, int32_t reverse, int32_t threads, int32_t tiles, const void* in, void* value, void* total,
+                    void* stream);
 
 #ifdef __cplusplus
 }

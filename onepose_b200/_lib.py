@@ -152,6 +152,7 @@ SYMBOLS = {
     "opb_debug_gemm": (C.c_int, [C.POINTER(OpbDebugGemmDesc), _P]),
     "opb_debug_kv_state_h": (C.c_int, [_P, _I, _I, _I, _I, _P, C.POINTER(_I), _P]),
     "opb_debug_split": (C.c_int, [_P, _P, _P, C.c_size_t, _P]),
+    "opb_debug_block": (C.c_int, [_I, _I, _I, _I, _I, _P, _P, _P, _P]),
     "opb_debug_set_stop": (C.c_int, [_P, _I, _I]),
     "opb_debug_set_stop_pass": (C.c_int, [_P, _I, _I]),
     "opb_debug_invalidate_prologues": (C.c_int, [_P]),

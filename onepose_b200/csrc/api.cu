@@ -539,6 +539,38 @@ static int segmented(const char* fn, const double* x, const int64_t* seg_len, in
   return rc;
 }
 
+// opb_debug_block's kernels: one block walks `tiles` tiles of blockDim.x inputs and calls one primitive of block.cuh per tile,
+// always with the same sh, as the library's tile loops do.  Per thread and tile: what the primitive returned, and the total.
+template <typename T, typename Op>
+__global__ void debug_block_scan(int prim, Op op, T identity, bool reverse, int tiles, const T* __restrict__ in, T* __restrict__ value,
+                                 T* __restrict__ total) {
+  __shared__ T sh[32];
+  for (int t = 0; t < tiles; ++t) {
+    const size_t i = (size_t)t * blockDim.x + threadIdx.x;
+    T all;
+    const T v = prim == 0 ? (all = block_reduce(in[i], op, sh)) : block_scan(in[i], op, identity, sh, &all, reverse);
+    value[i] = v;
+    total[i] = all;
+  }
+}
+
+__global__ void debug_block_rank(int tiles, const int32_t* __restrict__ keep, int32_t* __restrict__ value, int32_t* __restrict__ total) {
+  __shared__ int sh[32];
+  for (int t = 0; t < tiles; ++t) {
+    const size_t i = (size_t)t * blockDim.x + threadIdx.x;
+    int all;
+    value[i] = block_rank(keep[i] != 0, sh, &all);
+    total[i] = all;
+  }
+}
+
+template <typename T, typename Op>
+static int debug_block_launch(int prim, Op op, T identity, bool reverse, int threads, int tiles, const void* in, void* value, void* total,
+                              cudaStream_t st) {
+  return launched("opb_debug_block", "debug_block_scan",
+                  launch_k(false, debug_block_scan<T, Op>, 1, threads, 0, st, prim, op, identity, reverse, tiles, (const T*)in, (T*)value, (T*)total));
+}
+
 }  // namespace opb
 
 // =========================================================================================
@@ -1099,6 +1131,28 @@ int opb_debug_kv_state_h(const void* kvh, int32_t frames, int32_t n, int32_t m_p
 int opb_debug_split(const float* x, void* hi, void* lo, size_t n, void* stream) {
   LAUNCH_NH(__func__, split_planes, (unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream, x, (__half*)hi, (__half*)lo, (long long)n);
   return OPB_OK;
+}
+
+int opb_debug_block(int32_t prim, int32_t op, int32_t reverse, int32_t threads, int32_t tiles, const void* in, void* value, void* total,
+                    void* stream) {
+  REQUIRE(__func__, in && value && total);
+  REQUIRE(__func__, threads >= 32 && threads <= 1024 && threads % 32 == 0 && tiles > 0);
+  REQUIRE(__func__, prim >= 0 && prim <= 2 && op >= 0 && op <= 4);
+  REQUIRE(__func__, prim != 2 || op == 0);
+  REQUIRE(__func__, reverse == 0 || (prim == 1 && reverse == 1));
+  cudaStream_t st = (cudaStream_t)stream;
+  const bool rev = reverse != 0;
+  if (prim == 2) {
+    LAUNCH_NH(__func__, debug_block_rank, 1, threads, 0, st, tiles, (const int32_t*)in, (int32_t*)value, (int32_t*)total);
+    return OPB_OK;
+  }
+  switch (op) {
+    case 0: return debug_block_launch<int32_t>(prim, Sum32(), 0, rev, threads, tiles, in, value, total, st);
+    case 1: return debug_block_launch<int32_t>(prim, Max(), INT32_MIN, rev, threads, tiles, in, value, total, st);
+    case 2: return debug_block_launch<int32_t>(prim, Min(), INT32_MAX, rev, threads, tiles, in, value, total, st);
+    case 3: return debug_block_launch<unsigned long long>(prim, Sum64(), 0ull, rev, threads, tiles, in, value, total, st);
+    default: return debug_block_launch<long long>(prim, SumS64(), 0ll, rev, threads, tiles, in, value, total, st);
+  }
 }
 
 }  // extern "C"

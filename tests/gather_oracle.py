@@ -26,3 +26,23 @@ def gather_matches(matches0, keypoints2d, keypoints3d, matching_scores0=None):
     return {"pts2d": np.concatenate(p2).reshape(-1, 2), "pts3d": np.concatenate(p3).reshape(-1, 3),
             "mconf": np.concatenate(conf).astype(np.float32) if matching_scores0 is not None else None,
             "query_index": np.concatenate(qi).astype(np.int32), "offsets": np.array(off, np.int32)}
+
+
+def gather_objects_numpy(matches0, keypoints2d, keypoints3d, object_ids, matching_scores0=None):
+    """numpy restatement of the mixed gather (``opb_gather_matches_objects``): frame b keeps entries 0 <= m < M_b of its object
+    and reads that object's key points (the reference's kpts3d[matches[valid]] per frame), frame-major, ascending query index.
+    keypoints3d maps object id -> [M_b, 3]; same outputs as ``gather_matches``."""
+    p2, p3, conf, qi, off = [], [], [], [], [0]
+    for b, oid in enumerate(object_ids):
+        kp3 = keypoints3d[oid]
+        m = matches0[b]
+        valid = (m > -1) & (m < len(kp3))
+        p2.append(keypoints2d[b][valid].astype(np.float64))
+        p3.append(kp3[m[valid]].astype(np.float64))
+        if matching_scores0 is not None:
+            conf.append(matching_scores0[b][valid])
+        qi.append(np.nonzero(valid)[0].astype(np.int32))
+        off.append(off[-1] + int(valid.sum()))
+    return {"pts2d": np.concatenate(p2).reshape(-1, 2), "pts3d": np.concatenate(p3).reshape(-1, 3),
+            "mconf": np.concatenate(conf).astype(np.float32) if matching_scores0 is not None else None,
+            "query_index": np.concatenate(qi).astype(np.int32), "offsets": np.array(off, np.int32)}

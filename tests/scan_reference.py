@@ -70,11 +70,14 @@ def skipped(reproj_box3d):
     return bool(x0 < -1000 or y0 < -1000 or x1 > 3000 or y1 > 3000)
 
 
-def process_poses(K, box_lines, arposes_lines):
+def process_poses(K, box_lines, arposes_lines, corners=None):
     """data_process_anno's loop (:202-238, downsample_rate 1) -> ({index: (T_oc, reproj_box3d, row)}, keep per data row), where
-    row counts the data rows (comment and blank lines removed) as read_arposes does."""
+    row counts the data rows (comment and blank lines removed) as read_arposes does.  corners [n, 3] replaces get_bbox3d's 8
+    corners in reproj and the skip rule (opb_scan_poses takes any n up to 1024)."""
     fx, fy, cx, cy = K[0, 0], K[1, 1], K[0, 2], K[1, 2]
     _, bbox_3d_homo = get_bbox3d(box_lines)
+    if corners is not None:
+        bbox_3d_homo = np.concatenate([np.asarray(corners, np.float64).reshape(-1, 3), np.ones((len(corners), 1))], axis=1)
     K_homo = np.array([[fx, 0, cx, 0], [0, fy, cy, 0], [0, 0, 1, 0]])
     saved, keep = {}, []
     lines = [l.strip() for l in arposes_lines]

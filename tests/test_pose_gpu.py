@@ -8,7 +8,7 @@ import pytest
 import torch
 
 from onepose_b200 import GATsSuperGlue, SuperPoint, _lib, pnp, synthetic
-from tests.gather_oracle import gather_matches as gather_oracle
+from tests.gather_oracle import gather_matches as gather_oracle, gather_objects_numpy
 from tests.golden_util import GOLDEN_DIR
 
 pytestmark = pytest.mark.gpu
@@ -77,6 +77,134 @@ def test_gather_matches_without_query_points():
     with pytest.raises(ValueError):
         pnp.gather_matches(torch.zeros(2, 4, dtype=torch.int64, device="cuda"), torch.zeros(2, 5, 2, device="cuda"),
                            torch.zeros(5, 3, device="cuda"))
+
+
+# ---- past the first tile of the gather's scans: offsets over more than 1024 frames, compaction past 256 entries ----
+
+EDGE_FRAMES = list(range(1022, 1027)) + list(range(2046, 2051))
+OBJECT_M = [1, 300, 700]                 # the objects of the mixed gather
+FILL = 0xA5
+
+
+def _tile_edge_matches(rs, Mb, N, fill):
+    """matches0 [B, N] for frames of Mb[b] 3D key points: "empty" (T = 0), "full" (every entry a match), or "mixed": -1, matches,
+    indices >= M_b and below -1, with the frames at 1022-1026 and 2046-2050 (the edges of gather_scan's 1024-frame tiles)
+    alternately empty and fully matched."""
+    B = len(Mb)
+    valid = (rs.rand(B, N) * Mb[:, None]).astype(np.int64)
+    if fill == "empty":
+        return np.full((B, N), -1, np.int64)
+    if fill == "full":
+        return valid
+    u = rs.rand(B, N)
+    m0 = np.full((B, N), -1, np.int64)
+    m0[u < 0.5] = valid[u < 0.5]
+    beyond = (u >= 0.5) & (u < 0.6)
+    m0[beyond] = (Mb[:, None] + rs.randint(0, 5, (B, N)))[beyond]
+    neg = (u >= 0.6) & (u < 0.65)
+    m0[neg] = -rs.randint(2, 1 << 40, size=int(neg.sum()))
+    for k, b in enumerate(e for e in EDGE_FRAMES if e < B):
+        m0[b] = -1 if (k + N) % 2 else valid[b]
+    return m0
+
+
+def _inputs(rs, m0, Mb):
+    kp2 = rs.uniform(0, 512, size=(*m0.shape, 2)).astype(np.float32)
+    kp2[(m0 < 0) | (m0 >= Mb[:, None])] = np.nan              # rows of unmatched entries must never be read
+    return kp2, rs.rand(*m0.shape).astype(np.float32)
+
+
+def _filled(shape, dtype):
+    n = int(np.prod(shape)) * torch.empty(0, dtype=dtype).element_size()
+    return torch.full((n,), FILL, dtype=torch.uint8, device="cuda").view(dtype).reshape(shape)
+
+
+def _gather_abi(name, m0, sc, kp2, mid, B, N, ref):
+    """Entry point `name` (arguments m0, sc, kp2, *mid, then the outputs) into outputs whose bytes are FILL first, each with 8
+    spare rows past its capacity: offsets equal the oracle's int32 cumsum exactly, every row below T is byte-equal, and no row at
+    or past T, nor an offset past B, is written."""
+    cap = B * N + 8
+    out = {"pts2d": _filled((cap, 2), torch.float64), "pts3d": _filled((cap, 3), torch.float64), "mconf": _filled((cap,), torch.float32),
+           "query_index": _filled((cap,), torch.int32), "offsets": _filled((B + 1 + 8,), torch.int32)}
+    _lib.call(torch.device("cuda"), name, m0, sc, kp2, *mid, out["pts2d"], out["pts3d"], out["mconf"], out["query_index"], out["offsets"])
+    off = out["offsets"].cpu()
+    assert np.array_equal(off[:B + 1].numpy(), ref["offsets"]) and bool((off[B + 1:].view(torch.uint8) == FILL).all())
+    T = int(ref["offsets"][-1])
+    for key in ("pts2d", "pts3d", "mconf", "query_index"):
+        v = out[key].cpu()
+        assert v[:T].numpy().tobytes() == ref[key].tobytes(), key
+        assert bool((v[T:].contiguous().view(torch.uint8) == FILL).all()), key
+
+
+GATHER_CASES = [(B, N, fill) for B in (1023, 1024, 1025, 2048, 2049) for N in (1, 255, 256, 257) for fill in ("mixed", "empty", "full")]
+GATHER_CASES.append((70000, 3, "mixed"))
+
+
+@pytest.mark.parametrize("B,N,fill", GATHER_CASES, ids=[f"B{c[0]}-N{c[1]}-{c[2]}" for c in GATHER_CASES])
+def test_gather_past_one_scan_tile(B, N, fill):
+    """gather_matches and gather_matches_objects at more than 1024 frames (gather_scan carries a running total from tile to
+    tile) and at N around gather_compact's 256-entry tiles, against the numpy oracles, through the Python API and through the C
+    ABI into pre-filled outputs."""
+    rs = np.random.RandomState(B * 1000 + N * 3 + len(fill))
+    M = 7000
+    Mb = np.full(B, M)
+    m0 = _tile_edge_matches(rs, Mb, N, fill)
+    kp2, sc = _inputs(rs, m0, Mb)
+    kp3 = (0.05 * rs.randn(M, 3)).astype(np.float32)
+    ref = gather_oracle(m0, kp2, kp3, sc)
+    kept = ((m0 >= 0) & (m0 < M)).sum(1)
+    assert np.array_equal(ref["offsets"], np.concatenate([[0], np.cumsum(kept)]).astype(np.int32))
+    assert (ref["offsets"][-1] == 0) == (fill == "empty") and (ref["offsets"][-1] == B * N) == (fill == "full")
+    d = [torch.from_numpy(x).cuda() for x in (m0, kp2, kp3, sc)]
+    _assert_same(pnp.gather_matches(d[0], d[1], d[2], d[3]), ref)
+    _gather_abi("opb_gather_matches", d[0], d[3], d[1], (d[2], B, N, M), B, N, ref)
+
+    ids = rs.randint(0, len(OBJECT_M), B)                      # frames of three objects, mixed
+    Mb = np.array(OBJECT_M)[ids]
+    m0 = _tile_edge_matches(rs, Mb, N, fill)
+    kp2, sc = _inputs(rs, m0, Mb)
+    objs = {i: (0.05 * rs.randn(m, 3)).astype(np.float32) for i, m in enumerate(OBJECT_M)}
+    ref = gather_objects_numpy(m0, kp2, objs, ids.tolist(), sc)
+    d = [torch.from_numpy(x).cuda() for x in (m0, kp2, sc)]
+    _assert_same(pnp.gather_matches_objects(d[0], d[1], {i: torch.from_numpy(v).cuda() for i, v in objs.items()}, ids.tolist(), d[2]), ref)
+    kp3_all = torch.from_numpy(np.concatenate([objs[i] for i in range(len(OBJECT_M))])).cuda()
+    first = np.concatenate([[0], np.cumsum(OBJECT_M)[:-1]])[ids].astype(np.int32)
+    tab = [torch.from_numpy(t).cuda() for t in (first, Mb.astype(np.int32))]
+    _gather_abi("opb_gather_matches_objects", d[0], d[2], d[1], (kp3_all, tab[0], tab[1], B, N), B, N, ref)
+
+
+def test_poses_from_matches_past_one_scan_tile():
+    """poses_from_matches on 1100 frames of 0 to 12 pairs (make_pnp_scene's points and outliers, as test_pose_domain_gpu.py's
+    _scene makes them; the frames at 1022-1026 empty or full) against ransac_pnp_batch on the numpy-gathered lists with the same
+    seed: pose, inlier mask and inlier counts bit for bit."""
+    B, N, seed = 1100, 12, 5
+    rs = np.random.RandomState(3)
+    n_b = rs.randint(0, N + 1, B)
+    n_b[1022:1027] = [0, N, 0, N, 0]
+    K = np.zeros((B, 3, 3))
+    kp2 = np.full((B, N, 2), np.nan, np.float32)
+    kp3 = np.zeros((B * N, 3), np.float32)
+    m0 = np.full((B, N), -1, np.int64)
+    for b in range(B):
+        K[b], uv, P, _ = synthetic.make_pnp_scene(b, max(int(n_b[b]), 1))
+        slots = np.sort(rs.choice(N, n_b[b], replace=False))
+        kp2[b, slots] = uv[:n_b[b]]
+        kp3[b * N:b * N + n_b[b]] = P[:n_b[b]]
+        m0[b, slots] = b * N + np.arange(n_b[b])
+    m0[m0 < 0] = np.where(rs.rand(int((m0 < 0).sum())) < 0.5, -1, B * N + 3)    # unmatched: -1 or past M
+    sc = rs.rand(B, N).astype(np.float32)
+    d = [torch.from_numpy(x).cuda() for x in (K, kp2, kp3, m0, sc)]
+    res = pnp.poses_from_matches(d[0], d[1], d[2], d[3], d[4], seed=seed)
+    ref = gather_oracle(m0, kp2, kp3, sc)
+    off = torch.from_numpy(ref["offsets"]).cuda()
+    pose, mask, cnt = pnp.ransac_pnp_batch(d[0], torch.from_numpy(ref["pts2d"]).cuda(), torch.from_numpy(ref["pts3d"]).cuda() * 1000.0, off,
+                                           seed=seed)
+    pose[:, :, 3] /= 1000.0
+    T = int(ref["offsets"][-1])
+    assert torch.equal(res["offsets"], off)
+    assert torch.equal(res["pose"], pose) and torch.equal(res["n_inliers"], cnt) and torch.equal(res["inlier_mask"][:T], mask)
+    few = torch.from_numpy(n_b < 4).cuda()                     # fewer than 4 pairs: the identity pose and no inliers
+    assert not cnt[few].any() and int((cnt > 0).sum()) > 400
 
 
 def _matcher(desc3d, desc2d_db):

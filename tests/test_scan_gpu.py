@@ -188,6 +188,176 @@ def test_refusals_name_their_entry_point_and_condition():
         scan.object_poses(K, rows, torch.eye(4), torch.zeros(0, 3))
 
 
+# ---- past the kernel's first 256-row tile: a real capture has one ARposes row per video frame ----
+
+K0 = np.array([[500.0, 0, 320], [0, 500.0, 240], [0, 0, 1]])
+BOX = ["header\n", "0.0,0.0,0.0,0.1,0.1,0.1,1.0,0.0,0.0,0.0\n"]
+# the moves of test_each_skip_bound_and_the_pairing_on_the_device, and a camera at the box corner (0.05, 0.05, 0.05): that
+# corner projects to 0 / 0, so the extent is NaN, which compares false against every bound and the row is kept
+SKIPS = {"x0": "2.2,0.0,0.5", "y0": "0.0,-2.2,0.5", "x1": "-2.9,0.0,0.5", "y1": "0.0,2.9,0.5"}
+SCAN_N = [255, 256, 257, 511, 512, 513, 1000, 4097]
+PATTERNS = ["all", "none", "alternating", "runs", "nan"]
+
+
+def _move(kind, i, skips=SKIPS):
+    if kind == "in":            # kept, a pose of its own on every row, and no corner that projects to a whole pixel (where
+        # astype(int) would turn an ulp of difference between two correct fp64 evaluations into a pixel)
+        x, y, z = (0.01 + 0.002 * (i * 0.6180339887498949 % 1), 0.02 - 0.002 * (i * 0.41421356237309515 % 1),
+                   0.5 + 0.01 * (i * 0.7320508075688772 % 1))
+        return f"{x!r},{y!r},{z!r}"
+    if kind == "nan":
+        return "0.05,0.05,0.05"
+    return skips[kind]
+
+
+def _kinds(n, pattern):
+    """Per row "in", "nan" or one of the skip moves.  runs: skipped runs [m - 37, m) below odd multiples m of 256 and [m, m + 53)
+    from even ones (0 included), so runs end and start exactly on tile boundaries.  nan: NaN extents at rows 0, 255, 256, 511,
+    512, 767, 768 and n - 1, among rows of which every third is skipped."""
+    skip = list(SKIPS)
+    k = [skip[i % 4] if pattern == "none" or (pattern == "alternating" and i % 2) or (pattern == "nan" and i % 3 == 1) else "in"
+         for i in range(n)]
+    if pattern == "runs":
+        for m in range(0, n + 1, 256):
+            for i in (range(m - 37, m) if (m // 256) % 2 else range(m, m + 53)):
+                if 0 <= i < n:
+                    k[i] = skip[i % 4]
+    if pattern == "nan":
+        for i in (0, 255, 256, 511, 512, 767, 768, n - 1):
+            if i < n:
+                k[i] = "nan"
+    return k
+
+
+def _scan_case(kinds, K=K0, corners=None, skips=SKIPS):
+    """(rows f64 [n, 8], T_ow, corners, the model's saved slots and keep) for rows of the given kinds."""
+    lines = [f"{i * 0.1},{_move(k, i, skips)},1.0,0.0,0.0,0.0\n" for i, k in enumerate(kinds)]
+    with np.errstate(all="ignore"):
+        saved, keep = sr.process_poses(K, BOX, lines, corners)
+    assert keep.tolist() == [int(k in ("in", "nan")) for k in kinds]
+    rows = np.array([[float(e) for e in ln.split(",")] for ln in lines])
+    return rows, sr.parse_box(BOX), sr.get_bbox3d(BOX)[0] if corners is None else corners, saved, keep
+
+
+def _ref_box(p):
+    """The kernel's box of projected corners p: [x0, y0, x1, y1] truncated towards zero (astype(int) of the min / max), or 0
+    when an extent is not a finite int32 (NaN: numpy's min / max propagate it)."""
+    with np.errstate(all="ignore"):
+        ext = np.concatenate([p.min(0), p.max(0)])
+    return np.trunc(ext).astype(np.int32) if np.all(np.isfinite(ext)) else np.zeros(4, np.int32)
+
+
+def _check_slots(got, saved, keep, n_out):
+    """got (numpy) of opb_scan_poses with n_out slots against the model: keep, the full kept count, and per slot below
+    min(count, n_out) the row, pose (1e-12), projections (1e-7; NaN and infinities where the model has them) and box; slots from
+    the count to n_out cleared."""
+    c = len(saved)
+    m = min(c, n_out)
+    assert got["keep"].tolist() == keep.tolist() and int(got["count"][0]) == c
+    assert got["row"][:m].tolist() == [saved[i][2] for i in range(m)]
+    if m:
+        np.testing.assert_allclose(got["pose"][:m], np.stack([saved[i][0] for i in range(m)]), atol=1e-12, rtol=0)
+        ref = np.stack([saved[i][1] for i in range(m)])
+        p = got["proj"][:m]
+        assert np.array_equal(np.isnan(p), np.isnan(ref)) and np.array_equal(np.isinf(p), np.isinf(ref))
+        fin = np.isfinite(ref)
+        np.testing.assert_allclose(p[fin], ref[fin], atol=1e-7, rtol=0)
+        assert np.array_equal(got["box"][:m], np.stack([_ref_box(saved[i][1]) for i in range(m)]))
+    assert not got["pose"][c:n_out].any() and not got["proj"][c:n_out].any() and not got["box"][c:n_out].any()
+    assert (got["row"][c:n_out] == -1).all()
+
+
+def _numpy(out):
+    return {k: v.cpu().numpy() for k, v in out.items()}
+
+
+@pytest.mark.parametrize("pattern", PATTERNS)
+@pytest.mark.parametrize("n", SCAN_N)
+def test_object_poses_past_one_tile(n, pattern):
+    kinds = _kinds(n, pattern)
+    rows, T_ow, corners, saved, keep = _scan_case(kinds)
+    out = _numpy(scan.object_poses(K0, rows, T_ow, corners, device=DEV))
+    _check_slots(out, saved, keep, n)
+    if pattern == "none":
+        assert int(out["count"][0]) == 0 and (out["row"] == -1).all()
+    if pattern == "nan":
+        nan_slots = [i for i in range(len(saved)) if kinds[saved[i][2]] == "nan"]
+        assert len(nan_slots) == sum(k == "nan" for k in kinds) and not out["box"][nan_slots].any()
+
+
+PAD = 8                      # spare rows past n_out and past n_rows that the call must leave alone
+FILL = 0xA5
+
+
+def _filled(shape, dtype):
+    """A device tensor of the given shape whose bytes are all FILL."""
+    n = int(np.prod(shape)) * torch.empty(0, dtype=dtype).element_size()
+    return torch.full((n,), FILL, dtype=torch.uint8, device=DEV).view(dtype).reshape(shape)
+
+
+def _untouched(t):
+    return bool((t.contiguous().view(torch.uint8) == FILL).all())
+
+
+@pytest.mark.parametrize("n,pattern", [(1000, "runs"), (4097, "alternating"), (513, "nan"), (600, "all")])
+def test_scan_poses_writes_its_slots_only(n, pattern):
+    """opb_scan_poses into outputs filled with a byte pattern first, with PAD rows past n_out (and past n_rows for keep): n_out
+    below the kept count and above it, each across a multiple of 256 from it, equal to it, 1, and past n_rows.  count is the full
+    kept count whatever n_out is, slots from it to n_out are cleared, and nothing past n_out / n_rows is written."""
+    rows, T_ow, corners, saved, keep = _scan_case(_kinds(n, pattern))
+    c, nc = len(saved), len(corners)
+    assert c >= 256
+    lo = c // 256 * 256                                   # a multiple of 256 at or below the count
+    args = [torch.from_numpy(np.ascontiguousarray(a)).to(DEV) for a in (K0, rows, T_ow, corners)]
+    for n_out in sorted({1, lo - 1, c - 1, c, c + 1, lo + 257, n + 300}):
+        out = {"pose": _filled((n_out + PAD, 4, 4), torch.float64), "proj": _filled((n_out + PAD, nc, 2), torch.float64),
+               "box": _filled((n_out + PAD, 4), torch.int32), "row": _filled((n_out + PAD,), torch.int32),
+               "keep": _filled((n + PAD,), torch.int32), "count": _filled((1 + PAD,), torch.int32)}
+        _lib.call(torch.device(DEV), "opb_scan_poses", args[0], args[1], n, args[2], args[3], nc, n_out, out["pose"], out["proj"],
+                  out["box"], out["row"], out["keep"], out["count"])
+        got = _numpy({k: v[:n if k == "keep" else 1 if k == "count" else n_out] for k, v in out.items()})
+        _check_slots(got, saved, keep, n_out)
+        for k, v in out.items():
+            assert _untouched(v[n if k == "keep" else 1 if k == "count" else n_out:]), (n_out, k)
+
+
+@pytest.mark.parametrize("nc", [1, 9, 1024])
+def test_object_poses_with_any_number_of_corners(nc):
+    """n_corners of 1, 9 and the bound 1024, over 600 rows with skipped runs across the tile boundaries, against the model's
+    reproj and skip rule over the same corners."""
+    rs = np.random.RandomState(nc)
+    corners = rs.uniform(-0.05, 0.05, (nc, 3))
+    far = {"x0": "3.0,0.0,0.5", "y0": "0.0,-3.0,0.5", "x1": "-6.0,0.0,0.5", "y1": "0.0,6.0,0.5"}   # past the bounds from any corner
+    rows, T_ow, corners, saved, keep = _scan_case(_kinds(600, "runs"), corners=corners, skips=far)
+    out = _numpy(scan.object_poses(K0, rows, T_ow, corners, device=DEV))
+    assert out["proj"].shape == (600, nc, 2)
+    _check_slots(out, saved, keep, 600)
+
+
+def test_annotate_past_one_tile():
+    """annotate of F = 600 small frames (32 x 48, crop_size 8) and 800 ARposes rows of which fewer than F are kept: the pairing,
+    status, poses, boxes and crops against the model's parse_video, and frames past the kept count cleared, across three tiles."""
+    K = np.array([[40.0, 0, 24], [0, 40.0, 16], [0, 0, 1]])     # the kept boxes fall inside the 48 x 32 frame
+    F, S, n = 600, 8, 800
+    far = {"x0": "30.0,0.0,0.5", "y0": "0.0,-30.0,0.5", "x1": "-80.0,0.0,0.5", "y1": "0.0,80.0,0.5"}
+    kinds = ["in" if i % 5 in (0, 2, 3) or 250 <= i < 270 else list(far)[i % 4] for i in range(n)]
+    rows, T_ow, corners, saved, keep = _scan_case(kinds, K, skips=far)
+    assert 256 < len(saved) < F
+    frames_np = np.stack([sr.colour_frame(32, 48, f) for f in range(F)])
+    ref = sr.parse_video(list(frames_np), saved, K, sr.get_bbox3d(BOX)[1], S)
+    ann = scan.annotate(torch.from_numpy(frames_np).to(DEV), K, rows, T_ow, corners, crop_size=S)
+    status = ann["status"].cpu().numpy()
+    assert status.tolist() == [int(r is not None) for r in ref]
+    c = len(saved)
+    assert int(status.sum()) == c
+    img, pose, box = (ann[k].cpu().numpy() for k in ("image", "pose", "box"))
+    for f in range(c):
+        np.testing.assert_allclose(pose[f], ref[f]["pose"], atol=1e-12, rtol=0)
+        assert np.array_equal(box[f], ref[f]["box"]) and np.array_equal(img[f], ref[f]["image"]), f
+    for k in ("pose", "box", "image", "M", "box_crop"):
+        assert not ann[k][c:].any(), k
+
+
 # ---- the evaluation step on the crops ----
 
 def _chain(image_u8, K_crop, pose, sp, mm, kp3):
